@@ -14,6 +14,10 @@ same through Engine.train_step with pinned-host inputs (H2D inside the timed reg
 of the loss every step; roofline = dominant training kernel class (per-op CUDA-event times from
 se_run_ops_timed); retrieval = all-pairs distance N=50000, D=100 in Gpairs/s with its HBM roofline;
 cpu_baseline = the float32 CPU restatement of the Keras reference (oracle/) timed on the host cores.
+
+--dump-outputs DIR writes what the last timed training step and the last timed retrieval call computed as DIR/<name>.npy
+(float32 / float64; fixed seeded samples of the large arrays, < 64 MB in all): the inputs are seeded, so two builds run
+with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -31,7 +35,7 @@ if ROOT not in sys.path:
 
 ARCH = 'resnet-110-fc'
 PER_GPU_BATCH = 128
-METRIC = 'images/sec training ResNet-110 CIFAR-100 at 1/2/4/8 B200; retrieval Gpairs/s'
+METRIC = 'images/sec training ResNet-110 CIFAR-100 at 1/2/4/8 H100; retrieval Gpairs/s'
 # the same string on both arms (native / --impl reference): the driver compares config.workload
 WORKLOAD = ('CIFAR-100 ResNet-110 (%s) cosine loss vs cifar100.unitsphere, SGD momentum 0.9 + clipnorm 10 + L2 2e-4, '
             'batch %d/GPU, synthetic 32x32x3' % (ARCH, PER_GPU_BATCH))
@@ -47,21 +51,6 @@ WORKLOADS = {
 }
 
 
-def traffic_lookup(kernel):
-    """dram bytes per launch of a kernel class from the committed ncu --set full summaries (profiles/*_traffic.json)."""
-    import glob
-    best = None
-    for fn in sorted(glob.glob(os.path.join(ROOT, 'profiles', '*_traffic.json'))):
-        try:
-            with open(fn) as f:
-                d = json.load(f)
-        except (OSError, ValueError):
-            continue
-        if kernel in d:
-            best = d[kernel]['dram_bytes_per_launch']
-    return best
-
-
 def peaks():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
@@ -69,7 +58,8 @@ def peaks():
             d = json.load(f)
         return {'hbm_gbs': d['hbm_gbs'], 'tflops_burst': d['bf16_tflops'], 'tflops_sustained': d['bf16_tflops_sustained'],
                 'source': 'measured (MEASURED_PEAKS.json)'}
-    return {'hbm_gbs': 6650.0, 'tflops_burst': 1590.0, 'tflops_sustained': 1400.0, 'source': 'fallback (B200_PROFILING.md)'}
+    # NVIDIA's H100 SXM data sheet (dense BF16, HBM3 at 700 W): ceilings, not measured rates
+    return {'hbm_gbs': 3350.0, 'tflops_burst': 989.0, 'tflops_sustained': 989.0, 'source': 'H100 SXM data sheet (not measured)'}
 
 
 class ClockSampler:
@@ -123,7 +113,7 @@ def cpu_reference_arm(steps, warmup, sample_batch=None, budget_s=150.0):
     from oracle import models as omodels
     from oracle import train as otrain
     emb = np.load(os.path.join(ROOT, 'tests', 'golden', 'class_matrices.npz'))['cifar100_embedding']
-    # torch.distributed.run exports OMP_NUM_THREADS=1, and "every core" (128 on the B200 host) makes the tiny convs of
+    # torch.distributed.run exports OMP_NUM_THREADS=1, and "every core" of a large host makes the tiny convs of
     # ResNet-110 ~400x slower through OpenMP oversubscription: probe a few thread counts with one small step each and
     # keep the fastest -- the number reported as `cores`.
     ncpu = max(1, os.cpu_count() or 1)
@@ -182,7 +172,7 @@ def run_reference(args):
 
 # ----------------------------------------------------------------------------------------------- GPU arm
 def tc_coverage(graph, batch, mode, L):
-    """How many convolutions of the network run on the tcgen05 kernels in `mode`, per direction (se_conv2d_path: the
+    """How many convolutions of the network run on the tensor-core kernels in `mode`, per direction (se_conv2d_path: the
     library's own host-side planning).  Never raises: a reporting extra must not break the bench."""
     try:
         lib = L.load()
@@ -249,12 +239,11 @@ def profile_step(eng, L, pk):
     if c['flops'] > 0 and c['flops'] / (tf32_peak * 1e12) > c['bytes'] / (pk['hbm_gbs'] * 1e9):
         achieved = c['flops'] / avg_s / 1e12
         roof = {'bound': 'tensor', 'kernel': name, 'achieved': achieved, 'peak': tf32_peak, 'unit': 'TFLOP/s',
-                'frac': achieved / tf32_peak, 'traffic': None}
+                'frac': achieved / tf32_peak}
     else:
         achieved = c['bytes'] / avg_s / 1e9 if c['bytes'] else 0.0
         roof = {'bound': 'hbm', 'kernel': name, 'achieved': achieved, 'peak': pk['hbm_gbs'], 'unit': 'GB/s',
-                'frac': achieved / pk['hbm_gbs'], 'traffic': None}
-    roof['traffic'] = traffic_lookup(name)
+                'frac': achieved / pk['hbm_gbs']}
     roof.update({'avg_launch_us': 1e6 * avg_s, 'launches_per_step': c['n'], 'share_of_step': c['ms'] / total,
                  'peak_source': pk['source'] + (', sustained bf16 / 2 (TF32)' if roof['bound'] == 'tensor' else ''),
                  'algorithmic_bytes_per_launch': c['bytes'], 'algorithmic_flops_per_launch': c['flops']})
@@ -263,8 +252,9 @@ def profile_step(eng, L, pk):
     return roof, breakdown, total, conv_flops
 
 
-def bench_retrieval(L, rank, world, dev, n, d, reps, mode, pk_hbm=6567.4):
-    """All-pairs distance (evaluate_retrieval.py:56-63), rows sharded over ranks, no exchange step."""
+def bench_retrieval(L, rank, world, dev, n, d, reps, mode, pk_hbm, dump=None):
+    """All-pairs distance (evaluate_retrieval.py:56-63), rows sharded over ranks, no exchange step.  `dump`: dict that
+    receives the outputs of the last timed calls (see --dump-outputs)."""
     import torch
     from semantic_embeddings_b200.evaluate_retrieval import pairwise_distances
     rng = np.random.RandomState(0)
@@ -286,6 +276,8 @@ def bench_retrieval(L, rank, world, dev, n, d, reps, mode, pk_hbm=6567.4):
     torch.cuda.synchronize(dev)
     ms = float(np.mean([a.elapsed_time(b) for a, b in evs]))
     chk = float(out[0, :8].sum().item())
+    if dump is not None and rows > 0:
+        dump['retrieval_distances_sample'] = seeded_sample(out)
     # ranking step (evaluate_retrieval.py:67 restricted to the clip_ahp+1 = 251 ranks the metrics read): se_row_topk
     rank_ms = None
     if rows > 0 and n <= 52000:
@@ -310,9 +302,11 @@ def bench_retrieval(L, rank, world, dev, n, d, reps, mode, pk_hbm=6567.4):
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         for _ in range(3):
-            _, _, fused = pairwise_topk(k=k, feat_dev=fd)
+            tk_idx, _, fused = pairwise_topk(k=k, feat_dev=fd)
         b.record()
         torch.cuda.synchronize(dev)
+        if dump is not None:
+            dump['retrieval_top%d_index' % k] = seeded_sample(torch.as_tensor(tk_idx))
         extra['fused_topk'] = {'ms': a.elapsed_time(b) / 3.0, 'k': k, 'fused': bool(fused),
                                'gpairs_per_s': float(n) * n / (a.elapsed_time(b) / 3.0 / 1000.0) / 1e9,
                                'kernels': 'pairwise_tc_kernel<2> on a 4096-column sample (per-row thresholds in its epilogue), '
@@ -432,6 +426,14 @@ def run_native(args):
     ms_res, _ = timed(resident, args.steps, False)
     ms_e2e, last_loss = timed(from_host, args.steps, True)
     clocks = sampler.stop() if rank == 0 else None
+    dump = {} if (args.dump_outputs and rank == 0) else None
+    if dump is not None:
+        # what a caller of the timed step receives: per-sample loss / accuracy, the embeddings of the batch, and the
+        # parameters the step left (the profiling run below executes more steps)
+        dump['train_loss_per_sample'] = eng.loss_buf.clone()
+        dump['train_acc_per_sample'] = eng.acc_buf.clone()
+        dump['train_embeddings'] = eng.act['head_out'].clone()
+        dump['train_parameters_after_step'] = seeded_sample(eng.P)
 
     gb = B * world
     value = gb * args.steps / (ms_res / 1000.0)
@@ -444,7 +446,8 @@ def run_native(args):
     retrieval = None
     if not args.skip_retrieval and args.workload == 'config2':
         n, d = args.retrieval_n, 100
-        ms_r, rows, chk, rank_ms, r_extra = bench_retrieval(L, rank, world, dev, n, d, 5, mode, pk['hbm_gbs'])
+        ms_r, rows, chk, rank_ms, r_extra = bench_retrieval(L, rank, world, dev, n, d, 5, mode, pk['hbm_gbs'],
+                                                            dump if rank == 0 else None)
         if world > 1:
             t = torch.tensor([ms_r], device=dev)
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -456,9 +459,8 @@ def run_native(args):
         retrieval = {'value': gpairs, 'unit': 'Gpairs/s', 'N': n, 'D': d, 'ms': ms_r, 'rows_per_gpu': rows,
                      'roofline': {'bound': 'hbm', 'kernel': 'pairwise_dist', 'achieved': ach, 'peak': pk['hbm_gbs'],
                                   'unit': 'GB/s', 'frac': ach / pk['hbm_gbs'],
-                                  'traffic': traffic_lookup('pairwise_dist') if (n == 50000 and world == 1) else None,
                                   'algorithmic_bytes_per_launch': per_gpu_bytes, 'peak_source': pk['source']},
-                     'arithmetic': 'tcgen05 kind::f16, split-fp16 x3 (fp32-level accuracy)' if (mode != L.SE_MODE_F32 and caps & 8) else 'fp32 FFMA'}
+                     'arithmetic': 'wgmma f16, split-fp16 x3 (fp32-level accuracy)' if (mode != L.SE_MODE_F32 and caps & 8) else 'fp32 FFMA'}
         retrieval.update(r_extra)
         if rank_ms is not None:
             # per-row top-251 of this rank's row block; bound: one read of the block (4 bytes per pair)
@@ -481,13 +483,13 @@ def run_native(args):
             'ms_per_step': ms_res / args.steps, 'higher_is_better': True, 'scaling': args.scaling, 'vs_baseline': None,
             'dtype': (args.mode if tc else 'f32'), 'data': 'synthetic',
             'config': {'workload': wl['name'] if (args.workload != 'config2' or B != PER_GPU_BATCH) else WORKLOAD, 'per_gpu_batch': B, 'global_batch': gb, 'parallelism': 'dp%d' % world,
-                       'arith_mode': args.mode, 'tc_capabilities': caps, 'tcgen05_layers': tc_coverage(eng.g, B, mode, L),
+                       'arith_mode': args.mode, 'tc_capabilities': caps, 'tensor_core_layers': tc_coverage(eng.g, B, mode, L),
                        'cuda_graph': not args.no_graph,
                        'gradient_exchange': ('none' if world == 1 else
                                              ('NCCL inside the library: %d bucketed all-reduces overlapped with the backward '
                                               'pass, captured in the step graph' % eng.grad_buckets) if eng.comm_native
                                              else 'torch.distributed all_reduce of the flat buffer between two graphs'),
-                       'l2_policy': 'activations+gradients touched per step (~%.1f GB) exceed the 126 MB L2; '
+                       'l2_policy': 'activations+gradients touched per step (~%.1f GB) exceed the 50 MB L2; '
                                     'retrieval output 10 GB' % (eng_bytes(eng) / 1e9)},
             'e2e': {'value': e2e, 'unit': 'images/s', 'ms_per_step': ms_e2e / args.steps,
                     'h2d_bytes_per_step': int(xs_host[0].numel() * 4 + ys_host[0].numel() * 4),
@@ -501,8 +503,33 @@ def run_native(args):
             'retrieval': retrieval, 'cpu_baseline': cpu, 'clocks': clocks, 'peaks': pk,
         }
         print(json.dumps(line))
+    if dump is not None:
+        write_dump(args.dump_outputs, dump)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_SAMPLE = 4 << 20      # elements kept of an output larger than this (16 MB in float32)
+
+
+def seeded_sample(t):
+    """A copy of a tensor's values, flattened; above DUMP_SAMPLE elements a fixed seeded sample of them (same positions
+    on every run with the same shapes)."""
+    import torch
+    flat = t.detach().reshape(-1)
+    if flat.numel() > DUMP_SAMPLE:
+        g = torch.Generator().manual_seed(flat.numel())
+        idx = torch.randint(0, flat.numel(), (DUMP_SAMPLE,), generator=g).sort().values
+        flat = flat[idx.to(flat.device)]
+    return flat.clone()
+
+
+def write_dump(dirname, arrays):
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a.detach().cpu().numpy() if hasattr(a, 'detach') else a)
+        a = a.astype(np.float64 if (a.dtype.kind in 'iu' or a.dtype == np.float64) else np.float32)   # indices stay exact
+        np.save(os.path.join(dirname, name + '.npy'), a)
 
 
 def eng_bytes(eng):
@@ -519,7 +546,7 @@ def main():
     ap.add_argument('--steps', type=int, default=100)
     ap.add_argument('--warmup', type=int, default=5)
     ap.add_argument('--impl', default='native', choices=['native', 'reference'])
-    # tf32x3 = tcgen05 tiles with error compensation (meets the 1e-4 parity gate; the mode the training CLI runs);
+    # tf32x3 = tensor-core tiles with error compensation (meets the 1e-4 parity gate; the mode the training CLI runs);
     # tf32 = single-pass (outside the gate, for comparison only); f32 = fp32 FFMA kernels
     ap.add_argument('--mode', default='tf32x3', choices=['tf32x3', 'tf32', 'f32'])
     ap.add_argument('--batch', type=int, default=0, help='per-GPU batch (default: the workload\'s)')
@@ -533,6 +560,8 @@ def main():
     ap.add_argument('--skip-retrieval', action='store_true')
     ap.add_argument('--skip-cpu-baseline', action='store_true')
     ap.add_argument('--no-graph', action='store_true')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the outputs of the last timed step / retrieval call to DIR/<name>.npy')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == 'reference':

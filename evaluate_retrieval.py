@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Drop-in for the reference's evaluate_retrieval.py (same flags, same feature pickles, same table / CSV output) on the
-B200 kernels.  Reference: evaluate_retrieval.py:157-208.
+H100 kernels.  Reference: evaluate_retrieval.py:157-208.
 
   pairwise_retrieval + ClassHierarchy.hierarchical_precision (:186-195)
         -> semantic_embeddings_b200.evaluate_retrieval.retrieval_metrics: distance rows (se_pairwise_dist), full rankings

@@ -1,4 +1,4 @@
-/* se_b200.h -- C ABI of the B200-native hot path of cvjena/semantic-embeddings.
+/* se_b200.h -- C ABI of the H100-native hot path of cvjena/semantic-embeddings.
  *
  * The reference (/root/reference, pure Python on Keras 2.2 / TF 1.x) has no FFI layer: its
  * device work is whatever the Keras graph of learn_image_embeddings.py and the numpy calls of
@@ -20,9 +20,9 @@
  *     communicator with its stream.  Kernels keep no state between calls.
  *   - activations are float32 NHWC; conv kernels are float32 HWIO (Keras layout); dense
  *     kernels are (in,out).  `mode` selects the arithmetic of contraction kernels:
- *     SE_MODE_F32 = fp32 FFMA; SE_MODE_TF32 = tcgen05 kind::tf32 (operands truncated to a
- *     10-bit mantissa, fp32 accumulate in TMEM: ~1e-3 relative, outside the reference's fp32
- *     semantics, kept for comparison); SE_MODE_TF32X3 = tcgen05 kind::tf32 with error
+ *     SE_MODE_F32 = fp32 FFMA; SE_MODE_TF32 = TF32 wgmma (operands read with a
+ *     10-bit mantissa, fp32 accumulate: ~1e-3 relative, outside the reference's fp32
+ *     semantics, kept for comparison); SE_MODE_TF32X3 = TF32 wgmma with error
  *     compensation (every operand split into hi + lo, hi*hi + hi*lo + lo*hi in one fp32
  *     accumulator: fp32-level results, the mode the training path runs and is benchmarked in).
  *     Shapes the tensor path does not cover fall back to the fp32 kernels -- never to the CPU.
@@ -62,7 +62,7 @@ int64_t se_launch_count(void);
 int se_device_sm_count(void);
 /* one-time per-process setup (device query, shared-memory attributes); call before capturing CUDA graphs */
 int se_init(void);
-/* bit mask of the tcgen05 kernels compiled in: 1 conv fwd, 2 conv dgrad, 4 conv wgrad, 8 pairwise */
+/* bit mask of the tensor-core kernels compiled in: 1 conv fwd, 2 conv dgrad, 4 conv wgrad, 8 pairwise */
 int se_tc_capabilities(void);
 
 /* ------------------------------------------------------------------ convolution / dense
@@ -70,7 +70,7 @@ int se_tc_capabilities(void);
  * models/wide_residual_network.py:9,20,28,31,46,53 and keras.applications.ResNet50 (utils.py:237).
  * Explicit zero padding (pad_t, pad_l) and output size: the host computes TF 'SAME'
  * (pad_before = total//2, so k=3,s=2 on an even input gives pad 0 before / 1 after).
- * In SE_MODE_TF32 / SE_MODE_TF32X3 the tcgen05 kernels take: 3x3 / stride 1 / pad 1 on image widths 4..56 (weight
+ * In SE_MODE_TF32 / SE_MODE_TF32X3 the tensor-core kernels take: 3x3 / stride 1 / pad 1 on image widths 4..56 (weight
  * gradient: ..64), 1x1 / stride 1 / pad 0 on any image size (>= 128 pixels per call), 1x1 / stride 2 / pad 0 with
  * Wo <= 32 -- channel counts in multiples of 16 (the GEMM K dimension: 16 or a multiple of 32); backward data and weight
  * gradient of 3x3 / stride 2 / pad 0 on even image sizes with >= 128 channels on both sides (nine strided 1x1 GEMMs).
@@ -89,7 +89,7 @@ typedef struct {
  * (float64, caller zeroes) -- the BatchNormalization statistics of the next layer. */
 int se_conv2d_fwd(const se_conv_desc* d, const float* x, const float* w, const float* bias,
                   const float* residual, float* y, int relu, double* stats, int mode, void* stream);
-/* same, with an optional transposed copy w_t = [kh][kw][Cout][Cin] of the kernel: the tcgen05 forward path
+/* same, with an optional transposed copy w_t = [kh][kw][Cout][Cin] of the kernel: the tensor-core forward path
  * (SE_MODE_TF32) consumes K-major operands; without w_t the call uses the fp32 kernels. */
 int se_conv2d_fwd_ex(const se_conv_desc* d, const float* x, const float* w, const float* w_t, const float* bias,
                      const float* residual, float* y, int relu, double* stats, int mode, void* stream);
@@ -114,11 +114,15 @@ int se_transpose_filters(const float* P, float* PT, const int64_t* table, int n,
 /* dx = beta*dx + conv^T(dy, w)   (gradient wrt the input; autodiff of the above) */
 int se_conv2d_dgrad(const se_conv_desc* d, const float* dy, const float* w, float* dx, float beta,
                     int mode, void* stream);
-/* dw += x (*) dy ; dbias += sum_pixels dy   (dbias may be NULL). Accumulates: caller zeroes. */
+/* dw += x (*) dy ; dbias += sum_pixels dy   (dbias may be NULL). Accumulates: caller zeroes.
+ * Split-K partial sums go through a workspace of the library, one per device and stream (se_init prepares the one of
+ * se_run_ops' side stream), and are added in a fixed order: the same result on every run.  When a request does not fit
+ * the 32 MB workspace, or a stream's first call is inside a graph capture, the partial sums are added with atomics
+ * instead (same values up to the order of float additions). */
 int se_conv2d_wgrad(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias,
                     int mode, void* stream);
 /* Which kernel family takes this layer in `mode` (pure host-side planning: no device work, callable without a GPU):
- * 1 = a tcgen05 kernel, 0 = an fp32 kernel; direction 0 forward, 1 backward data, 2 weight gradient.  (Forward: given the
+ * 1 = a tensor-core kernel, 0 = an fp32 kernel; direction 0 forward, 1 backward data, 2 weight gradient.  (Forward: given the
  * auxiliary kernel copies of se_conv_aux; with BatchNorm statistics wider than 384 channels the sums come from a separate
  * se_bn_stats pass, see se_conv2d_fwd_aux.) */
 int se_conv2d_path(const se_conv_desc* d, int mode, int direction);

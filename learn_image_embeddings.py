@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Drop-in for the reference's learn_image_embeddings.py (same flags, same embedding / feature pickles) on the
-B200-native engine.  Reference: learn_image_embeddings.py:54-275.
+H100-native engine.  Reference: learn_image_embeddings.py:54-275.
 
 What each part of the reference script maps to:
   model construction + compile (:123-150, 224-236)  -> semantic_embeddings_b200.utils.build_network + engine.Engine
@@ -17,7 +17,7 @@ Deviations, all stated at run time when they apply:
   * --gpus N > 1: launch with `python -m torch.distributed.run --nproc-per-node N learn_image_embeddings.py ...`
     (one process per GPU, NCCL all-reduce; the reference's in-graph towers have the same arithmetic);
   * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles, datasets/cifar.py) and 'synthetic[:n]';
-  * --arith selects the arithmetic of the convolutions: tf32x3 (default: tcgen05 tiles with error compensation, fp32-level
+  * --arith selects the arithmetic of the convolutions: tf32x3 (default: tensor-core tiles with error compensation, fp32-level
     results), f32 (fp32 FFMA kernels), tf32 (single-pass TF32, ~1e-3 relative deviation: NOT the reference's arithmetic).
 """
 import argparse

@@ -1,6 +1,6 @@
-"""B200-native hot path of cvjena/semantic-embeddings: training of hierarchy-based semantic image
+"""H100-native hot path of cvjena/semantic-embeddings: training of hierarchy-based semantic image
 embeddings (CNN -> L2-normalise -> 1-cosine loss against a fixed class-embedding matrix) and the
-all-pairs retrieval distance matrix, as hand-written sm_100a CUDA behind a C ABI
+all-pairs retrieval distance matrix, as hand-written sm_90a CUDA behind a C ABI
 (include/se_b200.h, libse_b200.so).  Host modules mirror the reference's Python interface:
 
   utils.py              build_network, l2norm, inv_correlation, nn_accuracy, get_lr_schedule  (reference utils.py)

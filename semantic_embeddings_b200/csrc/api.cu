@@ -46,7 +46,7 @@ int sm_count() {
 int conv_fwd_simt(const se_conv_desc*, const float*, const float*, const float*, const float*, float*, int, double*, cudaStream_t);
 int conv_dgrad_simt(const se_conv_desc*, const float*, const float*, float*, float, cudaStream_t);
 int conv_wgrad_simt(const se_conv_desc*, const float*, const float*, float*, float*, cudaStream_t);
-// conv_tc.cu (tcgen05 kind::tf32); each returns SE_ERR_UNSUPPORTED for shapes it does not cover
+// conv_tc.cu / conv_wgrad_tc.cu (wgmma TF32); each returns SE_ERR_UNSUPPORTED for shapes it does not cover
 int conv_fwd_tc(const se_conv_desc*, const float*, const float*, const float*, const float*, const float*, float*, int, double*,
                 cudaStream_t);
 int conv_dgrad_tc(const se_conv_desc*, const float*, const float*, const float*, float*, float, cudaStream_t);
@@ -71,7 +71,7 @@ static int check_desc(const se_conv_desc* d) {
 
 using namespace se;
 
-extern "C" const char* se_version(void) { return "se_b200 0.1 (sm_100a)"; }
+extern "C" const char* se_version(void) { return "se_b200 0.1 (sm_90a)"; }
 extern "C" const char* se_last_error(void) { return g_err; }
 extern "C" int64_t se_launch_count(void) { return g_launches.load(); }
 extern "C" int se_device_sm_count(void) { return sm_count(); }
@@ -79,6 +79,7 @@ namespace se { int init_conv_simt(); int init_pairwise_tc(); int init_conv_tc();
 // One-time per-process setup that must not happen inside a CUDA-graph capture: device query and the
 // cudaFuncSetAttribute calls of every kernel that needs more than 48 KB of dynamic shared memory.
 static bool side_stream_ready();
+static int prepare_side_workspace();
 
 extern "C" int se_init(void) {
   sm_count();
@@ -87,6 +88,7 @@ extern "C" int se_init(void) {
   if (rc == SE_OK) rc = se::init_conv_tc();
   if (rc == SE_OK) rc = se::init_conv_wgrad_tc();
   if (rc == SE_OK) side_stream_ready();      // side stream + fork/join events of se_run_ops exist before any graph capture
+  if (rc == SE_OK) rc = prepare_side_workspace();   // and the weight-gradient workspace of that stream
   return rc;
 }
 namespace se { int tc_capabilities(); }
@@ -235,7 +237,7 @@ extern "C" int se_sgd_apply_devlr(float* p, const float* g, float* v, int64_t n,
 // Weight gradients are off the critical path of the backward pass (nothing reads dW before the optimizer), so a
 // multi-op plan issues them on a second, lowest-priority stream: fork after the op that produced dY, join at the end of
 // the plan.  Inside a CUDA-graph capture this becomes a parallel branch.  The backward-data / BatchNorm-backward
-// chain and the wgrad kernels are sized to be co-resident on an SM (shared memory, TMEM columns, registers; see
+// chain and the wgrad kernels can share an SM (shared memory, registers; see
 // conv_tc.cu / conv_wgrad_tc.cu), so the side branch fills the latency bubbles of the main chain.  SE_NO_SIDE_STREAM=1
 // keeps everything on one stream.
 static cudaStream_t g_side = nullptr;
@@ -255,6 +257,9 @@ static bool side_stream_ready() {
   }
   return true;
 }
+
+namespace se { int wgrad_workspace_prepare(cudaStream_t st); }
+static int prepare_side_workspace() { return g_side ? se::wgrad_workspace_prepare(g_side) : SE_OK; }
 
 namespace se {
 cudaStream_t comm_stream();

@@ -1,4 +1,4 @@
-// Shared helpers of the se_b200 CUDA library (sm_100a only).
+// Shared helpers of the se_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,6 +16,14 @@ int bn_bwd(const float* x, const float* y, const float* dout, int64_t rows, int 
            float* dbeta, double* scratch, int early, void* stream);
 void count_launch(int n = 1);
 int sm_count();
+// weight gradients without atomics (conv_wgrad_tc.cu): split-K partial sums go to slices of a workspace of the library
+// (one per device and stream) and wgrad_reduce adds the slices into dW / dbias in slice order, so the result is the same
+// on every run.  Slice k holds [T = kh*kw*Cin*Cout] dW partials at ws + k*T; the bias partials follow all slices,
+// [splits][Cout].  wgrad_workspace sets *ws = nullptr when `floats` do not fit (or the stream first appears inside a graph
+// capture): the kernels then add their partial sums into dW / dbias with atomics ("direct mode").
+int wgrad_workspace(long long floats, cudaStream_t st, float** ws);
+long long wgrad_fit_splits(long long want, long long T, int Cout);   // split count whose slices fit (want if none fit)
+int wgrad_reduce(const float* ws, int splits, long long T, int Cout, float* dw, float* dbias, cudaStream_t st);
 
 inline int check_launch(const char* what) {
   cudaError_t e = cudaGetLastError();
@@ -37,7 +45,7 @@ inline int check_launch(const char* what) {
 
 // Programmatic dependent launch (PDL).  Every kernel of this library is launched with the
 // programmatic-stream-serialization attribute and starts with pdl_grid_sync(): the dependent grid may become resident
-// (barrier init, TMEM allocation, descriptor prefetch) while the preceding grid drains, and it blocks in
+// (barrier init, descriptor prefetch) while the preceding grid drains, and it blocks in
 // griddepcontrol.wait -- which returns only when ALL prerequisite grids have completed and flushed their writes --
 // before it touches global memory.  Invariant that keeps this safe at any chain depth: no kernel reads or writes
 // global memory before its griddepcontrol.wait.  SE_NO_PDL=1 turns the attribute off (kernels then serialise fully).

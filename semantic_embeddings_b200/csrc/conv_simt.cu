@@ -1,6 +1,6 @@
 // fp32 FFMA convolution kernels ("parity mode", SE_MODE_F32) -- implicit GEMM over NHWC / HWIO.
 //
-// These are the exact-fp32 counterpart of the tcgen05 path (conv_tc.cu) and the fallback for the
+// These are the exact-fp32 counterpart of the tensor-core path (conv_tc.cu) and the fallback for the
 // shapes that path does not cover (Cin=3 stem, stride-2 layers, 7x7, dense layers).  They stand for
 // the Conv2D / Dense ops of the reference graph (models/cifar_resnet.py:96-105,218,233;
 // models/plainnet.py:52,67,70,76; models/wide_residual_network.py:9-53,96) and their autodiff
@@ -9,6 +9,8 @@
 //   forward : Y[m, co]   = sum_{tap,ci} X[pix(m,tap), ci] * W[tap, ci, co]      M = N*Ho*Wo
 //   dgrad   : dX[m, ci]  = sum_{tap,co} dY[opix(m,tap), co] * W[tap, ci, co]    M = N*H*W
 //   wgrad   : dW[tap,ci,co] = sum_m X[pix(m,tap), ci] * dY[m, co]               reduction over pixels
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace se {
@@ -287,7 +289,7 @@ conv_dgrad_kernel(ConvP p, const float* __restrict__ dy, const float* __restrict
 template <int BM, int BN, int TM, int TN>
 __global__ void __launch_bounds__((BM / TM) * (BN / TN))
 conv_wgrad_kernel(ConvP p, const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dw,
-                  float* __restrict__ dbias, long long pix_per_split) {
+                  float* __restrict__ dbias, long long pix_per_split, int direct) {
   pdl_grid_sync();
   constexpr int NT = (BM / TM) * (BN / TN);
   constexpr int CG = BN / TN;
@@ -300,6 +302,7 @@ conv_wgrad_kernel(ConvP p, const float* __restrict__ x, const float* __restrict_
   const int tid = threadIdx.x;
   const int tn = tid % CG, tm = tid / CG;
   const int KK = p.kh * p.kw * p.Cin;
+  const long long T = (long long)KK * p.Cout;   // dw / dbias: workspace slices, one per split (wgrad_reduce), or direct
   const int m0 = blockIdx.x * BM;  // kk tile
   const int n0 = blockIdx.y * BN;  // cout tile
   const long long P = (long long)p.N * p.Ho * p.Wo;
@@ -369,10 +372,15 @@ conv_wgrad_kernel(ConvP p, const float* __restrict__ x, const float* __restrict_
 #pragma unroll
     for (int j = 0; j < TN; ++j) {
       int co = n0 + tn * TN + j;
-      if (co < p.Cout) atomicAdd(&dw[(long long)kk * p.Cout + co], acc[i][j]);
+      if (co >= p.Cout) continue;
+      if (direct) atomicAdd(&dw[(long long)kk * p.Cout + co], acc[i][j]);
+      else dw[blockIdx.z * T + (long long)kk * p.Cout + co] = acc[i][j];
     }
   }
-  if (do_bias && n0 + tid < p.Cout) atomicAdd(&dbias[n0 + tid], bsum);
+  if (do_bias && n0 + tid < p.Cout) {
+    if (direct) atomicAdd(&dbias[n0 + tid], bsum);
+    else dbias[(long long)blockIdx.z * p.Cout + n0 + tid] = bsum;
+  }
 }
 
 // ---------------------------------------------------------------------------------------- wgrad 3x3 stride 1 'same'
@@ -384,7 +392,7 @@ conv_wgrad_kernel(ConvP p, const float* __restrict__ x, const float* __restrict_
 template <int NCI, int NCO>
 __global__ void __launch_bounds__(256)
 conv_wgrad3x3_kernel(ConvP p, const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dw,
-                     float* __restrict__ dbias, int TH, int tiles_per_img, int num_tiles) {
+                     float* __restrict__ dbias, int TH, int tiles_per_img, int num_tiles, int direct) {
   pdl_grid_sync();
   constexpr int CI_T = 2, CO_T = 2;
   constexpr int CIT = NCI * CI_T, COT = NCO * CO_T;
@@ -526,11 +534,16 @@ conv_wgrad3x3_kernel(ConvP p, const float* __restrict__ x, const float* __restri
 #pragma unroll
           for (int b = 0; b < CO_T; ++b) {
             int ci = ci0 + tci + NCI * a, co = co0 + tco + NCO * b;
-            atomicAdd(&dw[((long long)(r * 3 + s) * p.Cin + ci) * p.Cout + co], acc[r][s][a][b]);
+            const long long o = ((long long)(r * 3 + s) * p.Cin + ci) * p.Cout + co;
+            if (direct) atomicAdd(&dw[o], acc[r][s][a][b]);
+            else dw[blockIdx.x * 9LL * p.Cin * p.Cout + o] = acc[r][s][a][b];
           }
-    if (dbias != nullptr && tci == 0 && blockIdx.y == 0) {
+    if (dbias != nullptr && tci == 0 && blockIdx.y == 0) {   // dw / dbias: workspace slices, one per CTA column (wgrad_reduce)
 #pragma unroll
-      for (int b = 0; b < CO_T; ++b) atomicAdd(&dbias[co0 + tco + NCO * b], bacc[b]);
+      for (int b = 0; b < CO_T; ++b) {
+        if (direct) atomicAdd(&dbias[co0 + tco + NCO * b], bacc[b]);
+        else dbias[(long long)blockIdx.x * p.Cout + co0 + tco + NCO * b] = bacc[b];
+      }
     }
   }
 }
@@ -742,25 +755,31 @@ static int launch_wgrad3x3(const ConvP& p, const float* x, const float* dy, floa
   int tiles_per_img = ceil_div(p.H, TH);
   int num_tiles = p.N * tiles_per_img;
   int cy = p.Cin / CIT, cz = p.Cout / COT;
-  int gx = min(num_tiles, max(1, (2 * sm_count()) / (cy * cz)));
+  const long long T = 9LL * p.Cin * p.Cout;
+  int gx = (int)wgrad_fit_splits(min(num_tiles, max(1, (2 * sm_count()) / (cy * cz))), T, p.Cout);
   auto kern = conv_wgrad3x3_kernel<NCI, NCO>;
   if (smem > WGRAD3X3_MAX_SMEM) return SE_ERR_UNSUPPORTED;
   if (smem > 48 * 1024) {   // attribute normally raised by se_init(); direct C-ABI callers get it lazily
     static bool inited = false;
     if (!inited) { int rc = init_conv_simt(); if (rc) return rc; inited = true; }
   }
-  launch(kern, dim3(gx, cy, cz), dim3(256), smem, st, p, x, dy, dw, dbias, TH, tiles_per_img, num_tiles);
-  return check_launch("conv_wgrad3x3_kernel");
+  float* ws = nullptr;
+  int rc = wgrad_workspace(gx * (T + p.Cout), st, &ws);
+  if (rc) return rc;
+  launch(kern, dim3(gx, cy, cz), dim3(256), smem, st, p, x, dy, ws ? ws : dw, ws ? (dbias ? ws + gx * T : nullptr) : dbias, TH,
+         tiles_per_img, num_tiles, ws ? 0 : 1);
+  rc = check_launch("conv_wgrad3x3_kernel");
+  return (rc || !ws) ? rc : wgrad_reduce(ws, gx, T, p.Cout, dw, dbias, st);
 }
 
 // Weight gradient of a 3x3 / stride 1 / 'same' convolution with very few input channels (the RGB stem,
 // models/cifar_resnet.py:218 `conv0`): the 27 x Cout outputs are far too small for the tiled GEMM above (64x64 tiles
 // at 1/6 occupancy, 293-way split-K: 123 us).  Here one thread owns (k = (tap, ci) or the bias row, 4 output channels)
 // for one of PG pixel groups of a 8-row tile staged in shared memory: 2 shared loads per 4 FMAs, a shared-memory
-// combine of the pixel groups, then one atomic per output and CTA.  Persistent over the tiles.
+// combine of the pixel groups, then one partial per output and CTA.  Persistent over the tiles.
 __global__ void __launch_bounds__(512)
 conv_wgrad_stem_kernel(ConvP p, const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dw,
-                       float* __restrict__ dbias, int TH, int PG, int num_tiles) {
+                       float* __restrict__ dbias, int TH, int PG, int num_tiles, int direct) {
   pdl_grid_sync();
   extern __shared__ __align__(16) float ssm[];
   const int Wp = p.W + 2;
@@ -809,8 +828,11 @@ conv_wgrad_stem_kernel(ConvP p, const float* __restrict__ x, const float* __rest
       const float4 o = *reinterpret_cast<const float4*>(red + ((g - 1) * per_pg + rem) * 4);
       a0 += o.x; a1 += o.y; a2 += o.z; a3 += o.w;
     }
-    float* dst = (k < KK) ? dw + (long long)k * p.Cout + 4 * cq : (dbias ? dbias + 4 * cq : nullptr);
-    if (dst) { atomicAdd(dst, a0); atomicAdd(dst + 1, a1); atomicAdd(dst + 2, a2); atomicAdd(dst + 3, a3); }
+    // dw / dbias: workspace slices, one per CTA (wgrad_reduce), or direct
+    const long long sl = direct ? 0 : blockIdx.x;
+    float* dst = (k < KK) ? dw + sl * KK * p.Cout + (long long)k * p.Cout + 4 * cq : (dbias ? dbias + sl * p.Cout + 4 * cq : nullptr);
+    if (dst && direct) { atomicAdd(dst, a0); atomicAdd(dst + 1, a1); atomicAdd(dst + 2, a2); atomicAdd(dst + 3, a3); }
+    else if (dst) *reinterpret_cast<float4*>(dst) = make_float4(a0, a1, a2, a3);
   }
 }
 
@@ -827,9 +849,15 @@ static int launch_wgrad_stem(const ConvP& p, const float* x, const float* dy, fl
                        (size_t)max(PG - 1, 1) * per_pg * 4) * sizeof(float);
   if (smem > 48 * 1024) return SE_ERR_UNSUPPORTED;
   const int num_tiles = p.N * (p.H / TH);
-  const int grid = min(num_tiles, 2 * sm_count());
-  launch(conv_wgrad_stem_kernel, dim3(grid), dim3(threads), smem, st, p, x, dy, dw, dbias, TH, PG, num_tiles);
-  return check_launch("conv_wgrad_stem_kernel");
+  const long long T = 9LL * p.Cin * p.Cout;
+  const int grid = (int)wgrad_fit_splits(min(num_tiles, 2 * sm_count()), T, p.Cout);
+  float* ws = nullptr;
+  int rc = wgrad_workspace(grid * (T + p.Cout), st, &ws);
+  if (rc) return rc;
+  launch(conv_wgrad_stem_kernel, dim3(grid), dim3(threads), smem, st, p, x, dy, ws ? ws : dw, ws ? (dbias ? ws + grid * T : nullptr) : dbias,
+         TH, PG, num_tiles, ws ? 0 : 1);
+  rc = check_launch("conv_wgrad_stem_kernel");
+  return (rc || !ws) ? rc : wgrad_reduce(ws, grid, T, p.Cout, dw, dbias, st);
 }
 
 int conv_wgrad_simt(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st) {
@@ -855,10 +883,17 @@ int conv_wgrad_simt(const se_conv_desc* d, const float* x, const float* dy, floa
   // split the pixel reduction so that the grid fills the machine about twice
   long long want = max(1LL, (long long)(2 * sm_count()) / ((long long)gx * gy));
   long long splits = min(want, ceil_div<long long>(P, 4 * BK));
+  const long long T = (long long)KK * p.Cout;
+  splits = max(1LL, wgrad_fit_splits(splits, T, p.Cout));
   long long per = ceil_div<long long>(ceil_div<long long>(P, splits), BK) * BK;
   splits = ceil_div<long long>(P, per);
-  launch(conv_wgrad_kernel<BM, BN, TM, TN>, dim3(gx, gy, (unsigned)splits), dim3((BM / TM) * (BN / TN)), 0, st, p, x, dy, dw, dbias, per);
-  return check_launch("conv_wgrad_kernel");
+  float* ws = nullptr;
+  int rc = wgrad_workspace(splits * (T + p.Cout), st, &ws);
+  if (rc) return rc;
+  launch(conv_wgrad_kernel<BM, BN, TM, TN>, dim3(gx, gy, (unsigned)splits), dim3((BM / TM) * (BN / TN)), 0, st, p, x, dy,
+         ws ? ws : dw, ws ? (dbias ? ws + splits * T : nullptr) : dbias, per, ws ? 0 : 1);
+  rc = check_launch("conv_wgrad_kernel");
+  return (rc || !ws) ? rc : wgrad_reduce(ws, (int)splits, T, p.Cout, dw, dbias, st);
 }
 
 }  // namespace se

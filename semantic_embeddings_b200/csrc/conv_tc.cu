@@ -1,37 +1,29 @@
-// tcgen05 (kind::tf32) implicit-GEMM convolution for 3x3 / stride 1 / 'same' layers -- the bulk of every
+// Tensor-core (wgmma, TF32) implicit-GEMM convolution for 3x3 / stride 1 / 'same' layers -- the bulk of every
 // reference architecture (models/cifar_resnet.py:96-105, models/wide_residual_network.py:20-53,
 // models/plainnet.py:52,70) -- and for the 1x1 layers (stride 1 and 2) of keras.applications.ResNet50 (utils.py:237) and
 // of the wide-ResNet shortcuts (wide_residual_network.py:28): forward and data gradient.  fp32 NHWC activations are read
-// as TF32 operands straight from HBM/L2 (no conversion pass), fp32 accumulation in TMEM.
+// as TF32 operands straight from HBM/L2 (no conversion pass), fp32 accumulation in registers.
 //
-// The description below is the 3x3 case with image rows that divide 32 (template GEN = 0: every 3x3 layer of the CIFAR
-// networks).  GEN = 1 adds, with the same pipeline: 1x1 as a GEMM over the flat pixel list (one accumulator block, no
-// taps), 1x1 / stride 2 through tensor maps of the sub-sampled view x[:, ::2, ::2, :], and 3x3 on any row width up to 56
-// ("padded row slots" and strips: see ConvTcParams and plan_geometry).
-//
-//   GEMM view   P[m, (s, n)] = sum_{r, k} A_r[m, k] * B_r[(s, n), k]      y[h, w, n] = sum_s P[(h, w + s - 1), (s, n)]
-//     m : 128 output pixels of one tile = a (W x Hb x Nb) box of the NHWC tensor
-//     A_r : the same box shifted VERTICALLY by the filter row (r-1); TMA zero-fills the rows above / below the
-//           image, which is the 'same' padding -- no im2col buffer, no index arithmetic in the kernel
-//     the three horizontal taps s are stacked along N (N_mma = 3 * BNc) so that the input tile is fetched 3x
-//     instead of 9x; the horizontal shift is applied to the OUTPUT in the epilogue: a thread owns pixel w of
-//     a row and takes P[., s=0] from lane-1 and P[., s=2] from lane+1 (zero at the image border) -- possible
-//     because a warp's 32 TMEM lanes are 32 consecutive pixels of whole image rows (W divides 32)
+//   GEMM view   y[m, n] = sum_{tap, k} A_tap[m, k] * B_tap[n, k]
+//     m : 128 output pixels of one tile = a (Wb x Hb x Nb) box of the NHWC tensor (powers of two; pixels past the
+//         image are zero-filled on load and skipped on store)
+//     A_tap : the same box shifted by the filter tap (r - 1, s - 1); TMA zero-fills what lies outside the image, which
+//             is the 'same' padding -- no im2col buffer, no index arithmetic on the load path
 //     forward : k = input channel,  n = output channel, B = transposed kernel copy [tap][co][ci]
-//     dgrad   : k = output channel, n = input channel,  B = the HWIO kernel itself [8-tap][ci][co]
+//     dgrad   : k = output channel, n = input channel,  B = the HWIO kernel itself [8 - tap][ci][co]
 //               (dX = conv(dY, W rotated by 180 degrees and transposed))
+//   1x1 / stride 1 layers are the same GEMM over the flat pixel list (tiles of 128 consecutive pixels), 1x1 / stride 2
+//   layers address the input (forward) or the output (backward data) through the sub-sampled view x[:, ::2, ::2, :].
 //
-// Persistent, warp-specialised (384 threads): warp 0 TMA producer (weights resident in shared memory when they fit,
-// else one filter row x channel block per pipeline stage; it only ARRIVES at the prologue barrier so its first loads do
-// not wait for the TMEM allocation), warp 1 MMA issuer (elect.sync inside a provably uniform branch: descriptors stay
-// in uniform registers, no R2UR waterfalls; M=128, N=3*BNc<=240, K=8 per instruction, two tiles interleaved), warp 2
-// TMEM allocator, warps 4-11 two epilogue groups that share the (tile, 32-column block) work items: tcgen05.ld ->
-// combine taps -> bias (from shared memory) / residual / ReLU -> 32x16 blocks staged in shared memory in the TMA
-// SWIZZLE_64B layout -> ONE bulk tensor store per block (cp.reduce add for the accumulating dgrad); BatchNorm sum and
-// sum-of-squares of the stored values via a shuffle butterfly into per-warp slots, float64 across CTAs.
-// Backward-data launches are sized (shared memory, TMEM columns, 128 registers) to share the SM with the weight-
-// gradient kernel that se_run_ops runs on its side stream; layers with few pixel tiles split the output channels over
-// two CTAs.  No integer division per tile in the epilogue (pixel index = tile * 128 + lane).
+// Warp-specialised (384 threads): warp 0 issues the TMA loads of a ring of (tap, channel block) stages, the two
+// consumer warpgroups (threads 128..383) each own 64 rows of the tile and issue m64nBNk8 wgmma on them; the epilogue
+// (bias / residual / ReLU / BatchNorm sums, or the accumulate of the data gradient) runs on the accumulator registers.
+//
+// X3 = error-compensated arithmetic ("3xTF32"): every fp32 operand is the sum of hi = its mantissa truncated to 10
+// bits and lo = x - hi, and the product is accumulated as A_hi*B_hi + A_hi*B_lo + A_lo*B_hi in the same fp32
+// accumulator (the dropped A_lo*B_lo and the truncation of lo are ~2^-21 relative: fp32-level results from
+// tensor-core tiles).  Weights: lo is a second B tile written once per step by se_split_filters.  Activations: the
+// consumer threads split each stage in shared memory (A -> hi in place, lo into a second A tile) before its MMAs.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -42,651 +34,204 @@ namespace se {
 using namespace tc;
 
 constexpr int CT_BM = 128;
-constexpr int CT_MAX_STAGES = 8;
-constexpr int CT_MAX_ACC = 8;
-constexpr int CT_STAGE_OUT = 4096;          // per epilogue warp: two 32-pixel x 16-channel sub-buffers (2 KB each)
-constexpr int CT_SMEM_BUDGET = 200 * 1024 - 8 * CT_STAGE_OUT;
+constexpr int CT_THREADS = 384;        // warpgroup 0: TMA producer (one thread), warpgroups 1 and 2: MMA + epilogue
+constexpr int CT_MAX_STAGES = 6;
+constexpr int CT_SMEM_BUDGET = 200 * 1024;
 
 struct ConvTcParams {
-  int N, H, W;              // image batch / size (input == output size)
-  int Kc, Nc;               // GEMM K channels (A tensor channels), GEMM N channels (output tensor channels)
+  int N, H, W;              // extent of the grid the pixel tiles cover (images, rows, pixels)
+  int Kc, Nc, BN;           // GEMM K channels (A tensor channels), GEMM N channels, output channels per tile
   int Wb, Hb, Nb;           // pixel box, Wb*Hb*Nb == 128
-  int tiles_m, tiles_n, BN;
+  int tw, th;               // tiles along a row / along the rows of an image
   int cblk, kblocks;        // channels per pipeline stage (16 or 32), Kc / cblk
-  int rg;                   // filter rows per pipeline stage (3 = the whole 3x3 window of one channel block, or 1)
-  int flip;                 // 1: dgrad (tap index reversed when addressing B)
+  int taps, pad, flip;      // filter size (3 or 1), 'same' padding rows (1 or 0), 1: dgrad (tap order reversed for B)
+  int stages, stage_bytes, a_bytes, b_bytes;
+  long long o_sn, o_sh, o_sw;   // output (and residual) element strides of an image, a row, a pixel
+  int ovh, ovw;             // rows / pixels of the output view that exist (a strided view may be one short)
   int relu;
   float beta;               // dgrad: out = beta*out + D
-  int stages, stage_bytes, a_bytes, acc_stride, tmem_cols, nacc, b_merged;
-  int stage_out;            // output staging bytes per epilogue warp: 4096 (two sub-buffers) or 2048
-  int res, res_b_bytes, nt; // resident-weights mode: B loaded once per CTA, MMAs of `nt` tiles interleaved
-  int res_bl_off;           // X3: byte offset of the resident low-part weights inside the resident block
-  int single;               // resident-weights mode, whole image rows: ONE input box of Hb+2 rows per tile; the three filter
-                            // rows read it at offsets of a_tap bytes (descriptor start addresses) instead of three shifted boxes
-  int a_tap;                // bytes between the A slabs of consecutive filter rows inside a stage (a_bytes, or W * row_bytes)
-  int a_stage_bytes;        // bytes of input data in a resident-mode stage (what TMA fills and the splitters rewrite)
-  int taps;                 // filter size: 3 (3x3, three horizontal partial sums per pixel) or 1 (1x1: a plain GEMM)
-  int flat;                 // 1x1: the A tensor is addressed as a flat [pixels][channels] matrix, tile = 128 consecutive pixels
-  int tpi;                  // pixel tiles per image (Nb == 1)
-  // "padded" tiles (image widths that do not divide 32): a tile is 128 / Wb row slots of Wb lanes; an image row is cut
-  // into NS strips of Ws output pixels, each loaded as a Wb-pixel box that starts one pixel early for strips > 0 (the
-  // left neighbour) and runs past the strip (the right neighbour; zero-filled by TMA past the image border).  Slots are
-  // ordered (strip, row) for whole-row tiles, (image, row) for whole-image tiles; rows / images past the tensor are
-  // zero-filled on load and clipped on store (4-d output map, box = Ws pixels x rpw rows).
-  int padded, NS, Ws, rpw;
-  int pad;                  // rows of 'same' padding above the image: 1 (3x3) or 0 (1x1)
   const float* bias;
   const float* residual;
   float* out;
   double* stats;
-  long long* trace;         // debug: per-role clock64 timeline of CTA 0 (SE_CT_TRACE_PTR)
-  int debug;                // bit 0: no tiles (fixed overhead only), bit 1: skip A loads, bit 2: skip epilogue stores/stats
 };
 
-constexpr int CT_THREADS = 384;   // warp 0 TMA, warp 1 MMA, warp 2 TMEM alloc, warps 4-7 / 8-11 two epilogue groups
-constexpr int CT_THREADS_X3 = 416; // + warps 3 and 12: operand splitters of the error-compensated mode (see conv_tc_kernel);
-                                   // 13 warps x 128 registers leave room for the co-resident weight-gradient kernel
-constexpr int CT_NCONV = 64;       // splitter threads
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a, uint64_t b, int acc) {
+  if constexpr (BN == 16) wgmma_tf32_n16(d, a, b, acc);
+  else if constexpr (BN == 32) wgmma_tf32_n32(d, a, b, acc);
+  else if constexpr (BN == 64) wgmma_tf32_n64(d, a, b, acc);
+  else wgmma_tf32_n128(d, a, b, acc);
+}
 
-// x -> x - tf32_trunc(x): the part of an fp32 operand that kind::tf32 (which reads the upper 19 bits of the word,
-// i.e. truncates the mantissa to 10 bits) does not see.  Exact in fp32 (the difference has <= 13 significant bits).
-__device__ __forceinline__ float tf32_lo(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
-// bytes is a multiple of 8 * 16 * nthreads for every tile shape of this kernel except the smallest (handled by the tail)
-__device__ __forceinline__ void split_lo_inplace(uint8_t* base, int bytes, int tid, int nthreads) {
-  float4* q = reinterpret_cast<float4*>(base);
-  const int n = bytes >> 4;
-  int i = tid;
-  for (; i + 7 * nthreads < n; i += 8 * nthreads) {      // eight independent 16-byte loads in flight per thread
-    float4 v[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = q[i + j * nthreads];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      v[j].x = tf32_lo(v[j].x); v[j].y = tf32_lo(v[j].y); v[j].z = tf32_lo(v[j].z); v[j].w = tf32_lo(v[j].w);
-      q[i + j * nthreads] = v[j];
-    }
-  }
-  for (; i < n; i += nthreads) {
-    float4 v = q[i];
-    v.x = tf32_lo(v.x); v.y = tf32_lo(v.y); v.z = tf32_lo(v.z); v.w = tf32_lo(v.w);
-    q[i] = v;
+// in place: x -> tf32_hi(x), and lo = x - hi into a second tile (X3 only)
+__device__ __forceinline__ void split_tile(uint8_t* hi, uint8_t* lo, int bytes, int tid, int nthreads) {
+  float4* h = reinterpret_cast<float4*>(hi);
+  float4* l = reinterpret_cast<float4*>(lo);
+  for (int i = tid; i < (bytes >> 4); i += nthreads) {
+    const float4 v = h[i];
+    if (lo) l[i] = make_float4(tf32_lo(v.x), tf32_lo(v.y), tf32_lo(v.z), tf32_lo(v.w));
+    h[i] = make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w));
   }
 }
 
-// column sums of a 32 x NC block held one row per lane (v[j] = column j of this lane's row):
-// after the butterfly lane L holds the total of column L (NC == 32) or L >> 1 (NC == 16).
-template <int NC>
-__device__ __forceinline__ float butterfly_colsum(float (&v)[NC], int lane) {
-#pragma unroll
-  for (int off = 16, cnt = NC / 2; cnt >= 1; off >>= 1, cnt >>= 1) {
-    const bool up = (lane & off) != 0;
-#pragma unroll
-    for (int k = 0; k < cnt; ++k) {
-      float send = up ? v[k] : v[k + cnt];
-      float keep = up ? v[k + cnt] : v[k];
-      v[k] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
-  }
-  if (NC == 16) v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
-  return v[0];
-}
-
-template <int NC>
-__device__ __forceinline__ void tmem_ld_cols(uint32_t taddr, uint32_t (&v)[NC]);
-template <>
-__device__ __forceinline__ void tmem_ld_cols<32>(uint32_t taddr, uint32_t (&v)[32]) { tmem_ld_32x32(taddr, v); }
-template <>
-__device__ __forceinline__ void tmem_ld_cols<16>(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-#define CT_TRACE(role, ev)                                                                 \
-  do {                                                                                     \
-    if (p.trace && blockIdx.x == 0 && tr_n < 250) {                                        \
-      p.trace[(role) * 512 + 2 * tr_n] = (ev);                                             \
-      p.trace[(role) * 512 + 2 * tr_n + 1] = clock64();                                    \
-      ++tr_n;                                                                              \
-    }                                                                                      \
-  } while (0)
-
-// One block of NC output channels of one pixel: combine the three horizontal partial sums, apply the epilogue
-// ops, store, and (optionally) fold the stored values into the BatchNorm statistics.
-template <int NC, int GEN>
-__device__ __forceinline__ void conv_tc_load_combine(const ConvTcParams& p, uint32_t t_addr, int lblk, int c0, bool has_left,
-                                                     bool has_right, float (&o)[NC]) {
-  // GEN == 0: the 3x3 layers whose image rows divide 32 (every layer of the CIFAR networks) -- the generic features below
-  // fold to constants and their code disappears from that instantiation
-  const int k_taps = GEN ? p.taps : 3, k_NS = GEN ? p.NS : 1, k_pad = GEN ? p.pad : 1;
-  const bool k_padded = GEN && p.padded, k_flat = GEN && p.flat;
-  (void)k_taps; (void)k_NS; (void)k_pad; (void)k_padded; (void)k_flat;
-  if (k_taps == 1) {                              // 1x1: the accumulator is the result
-    uint32_t v1[NC];
-    tmem_ld_cols<NC>(t_addr + c0, v1);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < NC; ++j) o[j] = __uint_as_float(v1[j]);
-    return;
-  }
-  uint32_t v[NC], vl[NC], vr[NC];                 // centre (s=1), left (s=0) and right (s=2) partial sums
-  tmem_ld_cols<NC>(t_addr + lblk * p.BN + c0, vl);
-  tmem_ld_cols<NC>(t_addr + p.BN + c0, v);
-  tmem_ld_cols<NC>(t_addr + (2 - lblk) * p.BN + c0, vr);
-  tmem_ld_wait();
-#pragma unroll
-  for (int j = 0; j < NC; ++j) {
-    // y[w] = P0[w-1] + P1[w] + P2[w+1]: the neighbours' partial sums come from the adjacent lanes
-    float l = __shfl_up_sync(0xffffffffu, __uint_as_float(vl[j]), 1);
-    float r = __shfl_down_sync(0xffffffffu, __uint_as_float(vr[j]), 1);
-    float c = __uint_as_float(v[j]);
-    if (has_left) c += l;
-    if (has_right) c += r;
-    o[j] = c;
-  }
-}
-
-// Output staging: a warp's 32 pixels x 16 channels sit in shared memory as 32 rows of 64 bytes in the TMA
-// SWIZZLE_64B layout (16-byte chunk c of row r at chunk c ^ ((r >> 1) & 3): the 8 lanes of a store phase hit 8
-// different bank groups), and leave with ONE bulk tensor store -- full 32-byte sectors, out-of-range rows clipped by
-// the hardware.  Direct 16-byte stores from the one-row-per-lane register layout cost one memory transaction per lane
-// and instruction and were what the epilogue spent most of its time on.
-__device__ __forceinline__ void stage_put(uint8_t* sub, int lane, int q, float4 val) {
-  *reinterpret_cast<float4*>(sub + lane * 64 + ((q ^ ((lane >> 1) & 3)) << 4)) = val;
-}
-
-template <int NC, int GEN>
-__device__ __forceinline__ void conv_tc_epilogue_block(const ConvTcParams& p, const CUtensorMap* map_o, uint32_t t_addr, int lblk,
-                                                       int c0, int tn, bool valid, bool has_left, bool has_right, int row0,
-                                                       uint8_t* stg, const float* exrow, const float* s_bias, float* sw,
-                                                       int lane, long long* dbg = nullptr, int srow = -1, int sc1 = 0,
-                                                       int sc3 = 0) {
-  // GEN == 0: the 3x3 layers whose image rows divide 32 (every layer of the CIFAR networks) -- the generic features below
-  // fold to constants and their code disappears from that instantiation
-  const int k_taps = GEN ? p.taps : 3, k_NS = GEN ? p.NS : 1, k_pad = GEN ? p.pad : 1;
-  const bool k_padded = GEN && p.padded, k_flat = GEN && p.flat;
-  (void)k_taps; (void)k_NS; (void)k_pad; (void)k_padded; (void)k_flat;
-  // srow: staging row of this lane (-1: none -- a lane outside its strip); padded mode stores at (channel, sc1, row0, sc3)
-  if (!k_padded) srow = lane;
-  // exrow: residual row of this pixel (forward only)
-  const bool live = valid && !(p.debug & 4);
-  if (dbg) dbg[0] = clock64();
-  float o[NC];
-  conv_tc_load_combine<NC, GEN>(p, t_addr, lblk, c0, has_left, has_right, o);
-  if (dbg) dbg[1] = clock64();
-#pragma unroll
-  for (int q = 0; q < NC / 4; ++q) {
-    float4 val = make_float4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]);
-    if (live) {
-      const float4 b = *reinterpret_cast<const float4*>(s_bias + tn * p.BN + c0 + 4 * q);
-      val.x += b.x; val.y += b.y; val.z += b.z; val.w += b.w;
-      if (exrow) {   // read-only path load: free to be scheduled ahead of the shared-memory stores of this block
-        const float4 e = __ldg(reinterpret_cast<const float4*>(exrow + c0) + q);
-        val.x += e.x; val.y += e.y; val.z += e.z; val.w += e.w;
-      }
-      if (p.relu) { val.x = fmaxf(val.x, 0.f); val.y = fmaxf(val.y, 0.f); val.z = fmaxf(val.z, 0.f); val.w = fmaxf(val.w, 0.f); }
-    } else {
-      val = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    if (srow >= 0) stage_put(stg + (q >> 2) * 2048, srow, q & 3, val);
-    o[4 * q] = val.x; o[4 * q + 1] = val.y; o[4 * q + 2] = val.z; o[4 * q + 3] = val.w;
-  }
-  fence_proxy_async();                          // the staged values -> visible to the bulk-copy engine
-  __syncwarp();
-  if (lane == 0 && !(p.debug & 4)) {
-#pragma unroll
-    for (int h = 0; h < NC / 16; ++h) {
-      if (k_padded) {
-        if (p.beta != 0.f) tma_reduce_add_4d(map_o, stg + h * 2048, tn * p.BN + c0 + 16 * h, sc1, row0, sc3);
-        else tma_store_4d(map_o, stg + h * 2048, tn * p.BN + c0 + 16 * h, sc1, row0, sc3);
-      } else if (p.beta != 0.f) tma_reduce_add_2d(map_o, stg + h * 2048, tn * p.BN + c0 + 16 * h, row0);   // dgrad accumulate
-      else tma_store_2d(map_o, stg + h * 2048, tn * p.BN + c0 + 16 * h, row0);
-    }
-    tma_store_commit();
-  }
-  if (dbg) dbg[2] = clock64();
-  if (sw && !(p.debug & 4)) {
-    float o2[NC];
-#pragma unroll
-    for (int j = 0; j < NC; ++j) o2[j] = o[j] * o[j];
-    const float cs = butterfly_colsum<NC>(o, lane), cq = butterfly_colsum<NC>(o2, lane);
-    const int col = (NC == 32) ? lane : (lane >> 1);
-    if (NC == 32 || (lane & 1) == 0) {
-      // each (warp, channel) slot is owned by exactly one lane: plain read-modify-write, no atomics
-      sw[tn * p.BN + c0 + col] += cs;
-      sw[p.Nc + tn * p.BN + c0 + col] += cq;
-    }
-  }
-  if (dbg) dbg[3] = clock64();
-}
-
-// X3 = error-compensated arithmetic ("3xTF32"): every fp32 operand is the sum of the part kind::tf32 reads (hi =
-// mantissa truncated to 10 bits) and a remainder lo = x - hi (<= 13 significant bits, of which tf32 keeps the top 10),
-// and the product is accumulated as A_hi*B_hi + A_hi*B_lo + A_lo*B_hi in the same fp32 TMEM accumulator (the dropped
-// A_lo*B_lo and the truncation of lo are ~2^-21 relative: fp32-level results from tensor-core tiles).  Weights: lo is
-// a second (resident or streamed) B tile written once per step by se_split_filters.  Activations: no second tile --
-// pass 1 issues A*B_hi and A*B_lo on the tile as TMA delivered it (the hardware truncation IS the hi part), the
-// splitter warps (3 and 12) then rewrite the tile IN PLACE as lo, and pass 2 issues A_lo*B_hi.  The MMA thread runs
-// the two passes as two cursors over the same stage sequence (whichever is ready goes next), so pass 1 of the next
-// tile overlaps the split of the previous one.
-template <int X3, int GEN>
-__global__ void __maxnreg__(128)
+template <int BN, int X3>
+__global__ void __launch_bounds__(CT_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-               const __grid_constant__ CUtensorMap map_bl, const __grid_constant__ CUtensorMap map_o, ConvTcParams p) {
-  // GEN == 0: the 3x3 layers whose image rows divide 32 (every layer of the CIFAR networks) -- the generic features below
-  // fold to constants and their code disappears from that instantiation
-  const int k_taps = GEN ? p.taps : 3, k_NS = GEN ? p.NS : 1, k_pad = GEN ? p.pad : 1;
-  const bool k_padded = GEN && p.padded, k_flat = GEN && p.flat;
-  (void)k_taps; (void)k_NS; (void)k_pad; (void)k_padded; (void)k_flat;
+               const __grid_constant__ CUtensorMap map_bl, ConvTcParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* res_b = smem;                                   // resident weights (res mode), else empty
-  uint8_t* tiles = smem + p.res_b_bytes;
-  uint8_t* stg_all = tiles + (size_t)p.stages * p.stage_bytes;          // output staging: [8 epilogue warps][4 KB]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(stg_all + 8 * p.stage_out);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + CT_MAX_STAGES;
-  uint64_t* t_full = bars + 2 * CT_MAX_STAGES;
-  uint64_t* t_empty = t_full + CT_MAX_ACC;
-  uint64_t* b_full = t_empty + CT_MAX_ACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(b_full + 1);
-  uint64_t* hi_done = bars + 2 * CT_MAX_STAGES + 2 * CT_MAX_ACC + 4;       // X3: pass-1 MMAs of a stage have read it
-  uint64_t* lo_ready = hi_done + CT_MAX_STAGES;                            // X3: the stage now holds the lo parts
-  float* s_bias = reinterpret_cast<float*>(lo_ready + CT_MAX_STAGES);      // [Nc] (zeros without a bias)
-  float* s_stats = s_bias + p.Nc;                                                              // [8 warps][2 * Nc]
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * p.stage_bytes);
+  uint64_t* empty = full + CT_MAX_STAGES;
+  float* s_stats = reinterpret_cast<float*>(empty + CT_MAX_STAGES);     // [8 consumer warps][2][BN]
 
-  const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
-  const int total_tiles = p.tiles_m * p.tiles_n;
-  const int per_cta = (total_tiles + gridDim.x - 1) / gridDim.x;
-  const int t_begin = blockIdx.x * per_cta;
-  const int t_end = (p.debug & 1) ? t_begin : min(total_tiles, t_begin + per_cta);
+  const int tid = threadIdx.x;
+  const int tm = blockIdx.x, tn = blockIdx.y;
+  const int tw_i = tm % p.tw, rest = tm / p.tw;
+  const int w0 = tw_i * p.Wb, h0 = (rest % p.th) * p.Hb, n0 = (rest / p.th) * p.Nb;
   const int row_bytes = p.cblk * 4;
-  const int tiles_per_img = p.tpi;
-  const int strip_bytes = p.a_bytes / k_NS;                 // one strip of a filter row's A slab
-  const int b_rows = k_taps * p.BN;                         // B rows of one filter row: (s, n)
+  const int nk = p.taps * p.taps * p.kblocks;
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&map_a); prefetch_tmap(&map_b); prefetch_tmap(&map_o);
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int a = 0; a < p.nacc; ++a) { mbar_init(&t_full[a], 1); mbar_init(&t_empty[a], 128 * ((p.BN + 31) >> 5)); }
-    mbar_init(b_full, 1);
-    if (X3) for (int s = 0; s < p.stages; ++s) { mbar_init(&hi_done[s], 1); mbar_init(&lo_ready[s], CT_NCONV); }
+  if (tid == 0) {
+    prefetch_tmap(&map_a); prefetch_tmap(&map_b);
+    if (X3) prefetch_tmap(&map_bl);
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     fence_barrier_init();
-    fence_proxy_async();
   }
-  // The producer warp only ARRIVES at the prologue barrier (its mbarrier initialisation is what the others need):
-  // its first TMA loads go out without waiting for the TMEM allocation and the statistics zeroing of the other warps.
-  uint32_t tmem_base = 0;
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("barrier.arrive 3, %0;" ::"r"(X3 ? CT_THREADS_X3 : CT_THREADS) : "memory");   // named barrier 3: never shared with the final __syncthreads
-  } else {
-    if (warp == 2) tmem_alloc(tmem_slot, p.tmem_cols);
-    if (p.stats) for (int i = threadIdx.x - 32; i < 16 * p.Nc; i += (X3 ? CT_THREADS_X3 : CT_THREADS) - 32) s_stats[i] = 0.f;
-    fence_before_sync();
-    asm volatile("barrier.sync 3, %0;" ::"r"(X3 ? CT_THREADS_X3 : CT_THREADS) : "memory");
-    fence_after_sync();
-    tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);   // provably warp-uniform (see tc.cuh elect_one)
-  }
+  __syncthreads();
   pdl_wait();                               // nothing above touches global memory (see common.cuh)
 
-  if (warp == 0 && elect_one()) {
+  if (tid < 128) {
     // ===================== TMA producer
-    int stage = 0, phase = 0, tr_n = 0;
-    CT_TRACE(0, 0);
-    const uint32_t tx = p.rg * (p.a_bytes + (X3 ? 2 : 1) * b_rows * row_bytes);
-    if (p.res && t_begin < t_end) {
-      // weights once per CTA: three boxes of 3*BN rows (one per filter row; see the tap order note below)
-      mbar_expect_tx(b_full, (X3 ? 2 : 1) * 3 * b_rows * row_bytes);
-      for (int r = 0; r < 3; ++r) {
-        const int tap0 = p.flip ? 8 - (r * 3 + 2) : r * 3;
-        tma_load_2d(res_b + r * b_rows * row_bytes, &map_b, b_full, 0, tap0 * p.Nc);
-        if (X3) tma_load_2d(res_b + p.res_bl_off + r * b_rows * row_bytes, &map_bl, b_full, 0, tap0 * p.Nc);
-      }
-    }
-    for (int t = t_begin; p.res && t < t_end; ++t) {
-      // one stage per tile: the three vertically shifted input boxes
-      const int tm = t;
-      int n0, h0;
-      if (p.Nb == 1) { n0 = tm / tiles_per_img; h0 = (tm % tiles_per_img) * p.Hb; }
-      else { n0 = tm * p.Nb; h0 = 0; }
-      mbar_wait(&empty[stage], phase ^ 1);
-      CT_TRACE(0, 1);
-      mbar_expect_tx(&full[stage], p.a_stage_bytes);
-      uint8_t* sa = tiles + (size_t)stage * p.stage_bytes;
-      if (p.single) tma_load_4d(sa, &map_a, &full[stage], 0, 0, h0 - 1, n0);      // rows h0-1 .. h0+Hb: halo rows included
-      else for (int r = 0; r < 3; ++r)
-        for (int s = 0; s < k_NS; ++s)
-          tma_load_4d(sa + r * p.a_bytes + s * strip_bytes, &map_a, &full[stage], 0, s * p.Ws - (s > 0), h0 + r - 1, n0);
-      CT_TRACE(0, 2);
-      if (++stage == p.stages) { stage = 0; phase ^= 1; }
-    }
-    for (int t = t_begin; !p.res && t < t_end; ++t) {
-      const int tm = t / p.tiles_n, tn = t % p.tiles_n;
-      int n0, h0;
-      if (p.Nb == 1) { n0 = tm / tiles_per_img; h0 = (tm % tiles_per_img) * p.Hb; }
-      else { n0 = tm * p.Nb; h0 = 0; }
-      for (int rb = 0; rb < k_taps; rb += p.rg) {
-        for (int kb = 0; kb < p.kblocks; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          CT_TRACE(0, 1);
-          mbar_expect_tx(&full[stage], (p.debug & 2) ? tx - p.rg * p.a_bytes : tx);
-          uint8_t* sa = tiles + (size_t)stage * p.stage_bytes;
-          uint8_t* sb = sa + p.rg * p.a_bytes;
-          for (int rr = 0; rr < p.rg; ++rr) {
-            const int r = rb + rr;
-            if (k_flat) tma_load_4d(sa + rr * p.a_bytes, &map_a, &full[stage], kb * p.cblk, tm * CT_BM, 0, 0);
-            else if (!(p.debug & 2))
-              for (int s = 0; s < k_NS; ++s)
-                tma_load_4d(sa + rr * p.a_bytes + s * strip_bytes, &map_a, &full[stage], kb * p.cblk, s * p.Ws - (s > 0),
-                            h0 + r - k_pad, n0);
-            uint8_t* sbr = sb + rr * b_rows * row_bytes;
-            if (p.b_merged) {
-              // one box of 3*BN rows: taps (r,0),(r,1),(r,2) are consecutive row blocks of B.  For dgrad the tap
-              // index is reversed, so the box starts at tap 8-(3r+2) and holds the s-blocks in the order 2,1,0.
-              const int tap0 = p.flip ? k_taps * k_taps - 1 - (r * k_taps + k_taps - 1) : r * k_taps;
-              tma_load_2d(sbr, &map_b, &full[stage], kb * p.cblk, tap0 * p.Nc);
-              if (X3) tma_load_2d(sbr + p.rg * b_rows * row_bytes, &map_bl, &full[stage], kb * p.cblk, tap0 * p.Nc);
-            } else {
-              for (int s = 0; s < k_taps; ++s) {
-                const int tap = r * k_taps + s;
-                const int btap = p.flip ? k_taps * k_taps - 1 - tap : tap;
-                tma_load_2d(sbr + s * p.BN * row_bytes, &map_b, &full[stage], kb * p.cblk, btap * p.Nc + tn * p.BN);
-                if (X3)
-                  tma_load_2d(sbr + p.rg * b_rows * row_bytes + s * p.BN * row_bytes, &map_bl, &full[stage], kb * p.cblk,
-                              btap * p.Nc + tn * p.BN);
-              }
-            }
-          }
-          CT_TRACE(0, 2);
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1 && elect_one()) {
-    // ===================== MMA issuer
-    const uint32_t idesc = umma_idesc(2 /*tf32*/, CT_BM, k_taps * p.BN);
-    const uint32_t sbo = 8 * row_bytes;
-    int stage = 0, phase = 0, tr_n = 0;
-    CT_TRACE(1, 0);
-    if (X3 && t_begin < t_end) {
-      // ---- error-compensated mode, pass 1 (A*B_hi, A*B_lo on the tile as TMA delivered it).  A "unit" is one pipeline
-      // stage: a whole tile (resident weights) or one (filter-row group, channel block) of a tile.  Pass 2 (A_lo*B_hi
-      // once the splitters have rewritten the stage) is issued by a second thread (warp 2): each thread's instruction
-      // stream -- barrier waits, descriptor arithmetic, commits -- is what bounds small layers, so it is split in two;
-      // the order pass 1 -> split -> pass 2 of a stage is carried by the hi_done / lo_ready barriers.
-      const uint32_t dhi = umma_desc_hi_kmajor(sbo, row_bytes);
-      const uint32_t tiles_lo = ((smem_u32(tiles) & 0x3FFFFu) >> 4) | (1u << 16);     // descriptor low words: address >> 4
-      const uint32_t bres_lo = ((smem_u32(res_b) & 0x3FFFFu) >> 4) | (1u << 16);
-      const int kst = p.cblk / 8;
-      const int rows_u = p.res ? 3 : p.rg;                         // filter rows per unit
-      const int upt = p.res ? 1 : (k_taps / p.rg) * p.kblocks;     // units per tile
-      const int U = (t_end - t_begin) * upt;
-      const uint32_t a_step = (uint32_t)(p.res ? p.a_tap : p.a_bytes) >> 4, b_step = (uint32_t)(b_rows * row_bytes) >> 4;
-      const uint32_t stage_step = (uint32_t)p.stage_bytes >> 4;
-      const uint32_t lo_delta = p.res ? (uint32_t)p.res_bl_off >> 4 : (uint32_t)p.rg * b_step;
-      if (p.res) mbar_wait(b_full, 0);
-      int s1 = 0, ph1 = 0, k1 = 0, a1 = 0, aph1 = 0;
-      for (int u1 = 0; u1 < U; ++u1) {
-        if (k1 == 0) mbar_wait(&t_empty[a1], aph1 ^ 1);
-        mbar_wait(&full[s1], ph1);
-        fence_after_sync();
-        CT_TRACE(1, 2);
-        const uint32_t d_tmem = tmem_base + a1 * p.acc_stride;
-        uint32_t da_r = tiles_lo + s1 * stage_step;
-        uint32_t db_r = p.res ? bres_lo : da_r + p.rg * a_step;
-        for (int rr = 0; rr < rows_u; ++rr) {
-          uint32_t da = da_r, db = db_r;
-          for (int ks = 0; ks < kst; ++ks) {
-            const uint64_t qa = ((uint64_t)dhi << 32) | da, qh = ((uint64_t)dhi << 32) | db,
-                           ql = ((uint64_t)dhi << 32) | (db + lo_delta);
-            if ((k1 | rr | ks) == 0) mma_tf32_c<false>(d_tmem, qa, qh, idesc);
-            else mma_tf32_c<true>(d_tmem, qa, qh, idesc);
-            mma_tf32_c<true>(d_tmem, qa, ql, idesc);
-            da += 2; db += 2;                                      // next 8 channels: 32 bytes
-          }
-          da_r += a_step; db_r += b_step;
-        }
-        mma_commit(&hi_done[s1]);
-        CT_TRACE(1, 3);
-        if (++s1 == p.stages) { s1 = 0; ph1 ^= 1; }
-        if (++k1 == upt) { k1 = 0; if (++a1 == p.nacc) { a1 = 0; aph1 ^= 1; } }
-      }
-    }
-    if (!X3 && p.res && t_begin < t_end) {
-      // Small layers are bound by the instruction stream of this single issuing thread: everything that does
-      // not change inside a group of tiles is hoisted, descriptors are (constant high word | address), and the
-      // MMAs of up to four tiles are interleaved (independent accumulators back to back).
-      mbar_wait(b_full, 0);
-      const uint32_t dhi = umma_desc_hi_kmajor(sbo, row_bytes);
-      const uint32_t bres = smem_u32(res_b);
-      const uint32_t tiles_u32 = smem_u32(tiles);
-      const int kst = p.cblk / 8;
-      int s_idx = 0, s_ph = 0, a_idx = 0, a_ph = 0;
-      for (int g0 = t_begin; g0 < t_end; g0 += p.nt) {
-        const int nj = min(p.nt, t_end - g0);
-        uint32_t a_addr[4], d_addr[4];
-        uint64_t* e_bar[4];
-        uint64_t* f_bar[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          if (j < nj) {
-            mbar_wait(&t_empty[a_idx], a_ph ^ 1);
-            mbar_wait(&full[s_idx], s_ph);
-            a_addr[j] = tiles_u32 + s_idx * p.stage_bytes;
-            d_addr[j] = tmem_base + a_idx * p.acc_stride;
-            e_bar[j] = &empty[s_idx];
-            f_bar[j] = &t_full[a_idx];
-            if (++s_idx == p.stages) { s_idx = 0; s_ph ^= 1; }
-            if (++a_idx == p.nacc) { a_idx = 0; a_ph ^= 1; }
-          }
-        }
-        CT_TRACE(1, 2);
-        fence_after_sync();
-        for (int r = 0; r < 3; ++r) {
-          for (int ks = 0; ks < kst; ++ks) {
-            const uint64_t db = umma_desc_join(dhi, bres + r * b_rows * row_bytes + ks * 32);
-            const uint32_t aoff = r * p.a_tap + ks * 32;
-            if ((r | ks) == 0) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                if (j < nj) mma_tf32_c<false>(d_addr[j], umma_desc_join(dhi, a_addr[j] + aoff), db, idesc);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                if (j < nj) mma_tf32_c<true>(d_addr[j], umma_desc_join(dhi, a_addr[j] + aoff), db, idesc);
-            }
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          if (j < nj) { mma_commit(e_bar[j]); mma_commit(f_bar[j]); }
-        }
-        CT_TRACE(1, 3);
-      }
-    }
-    for (int t = t_begin; !X3 && !p.res && t < t_end; ++t) {
-      const int i = t - t_begin, acc = i % p.nacc, acc_phase = (i / p.nacc) & 1;
-      mbar_wait(&t_empty[acc], acc_phase ^ 1);
-      CT_TRACE(1, 1);
-      fence_after_sync();
-      const uint32_t d_tmem = tmem_base + acc * p.acc_stride;
-      uint32_t first = 1;
-      for (int it = 0; it < (k_taps / p.rg) * p.kblocks; ++it) {
-        mbar_wait(&full[stage], phase);
-        CT_TRACE(1, 2);
-        fence_after_sync();
-        const uint32_t a0 = smem_u32(tiles + (size_t)stage * p.stage_bytes);
-        const uint32_t b0 = a0 + p.rg * p.a_bytes;
-        const uint32_t dhi = umma_desc_hi_kmajor(sbo, row_bytes);
-        for (int rr = 0; rr < p.rg; ++rr) {
-          for (int ks = 0; ks < p.cblk / 8; ++ks) {
-            const uint64_t da = umma_desc_join(dhi, a0 + rr * p.a_bytes + ks * 32);
-            const uint64_t db = umma_desc_join(dhi, b0 + rr * b_rows * row_bytes + ks * 32);
-            if (first) mma_tf32_c<false>(d_tmem, da, db, idesc);
-            else mma_tf32_c<true>(d_tmem, da, db, idesc);
-            first = 0;
-          }
-        }
-        mma_commit(&empty[stage]);
-        CT_TRACE(1, 3);
+    if (tid == 0) {
+      int stage = 0, phase = 0;
+      const uint32_t tx = (p.a_bytes + p.b_bytes) * (X3 ? 2 : 1) - (X3 ? p.a_bytes : 0);
+      for (int it = 0; it < nk; ++it) {
+        const int tap = it / p.kblocks, kb = it - tap * p.kblocks;
+        const int r = tap / p.taps, s = tap - r * p.taps;
+        const int btap = p.flip ? p.taps * p.taps - 1 - tap : tap;
+        mbar_wait(&empty[stage], phase ^ 1);
+        mbar_expect_tx(&full[stage], tx);
+        uint8_t* sa = smem + (size_t)stage * p.stage_bytes;
+        uint8_t* sb = sa + p.a_bytes;
+        tma_load_4d(sa, &map_a, &full[stage], kb * p.cblk, w0 + s - p.pad, h0 + r - p.pad, n0);
+        tma_load_2d(sb, &map_b, &full[stage], kb * p.cblk, btap * p.Nc + tn * BN);
+        if (X3) tma_load_2d(sb + p.b_bytes, &map_bl, &full[stage], kb * p.cblk, btap * p.Nc + tn * BN);
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
-      mma_commit(&t_full[acc]);
     }
-  } else if (X3 && warp == 2 && elect_one()) {
-    // ===================== MMA issuer, pass 2 of the error-compensated mode: A_lo * B_hi
-    if (t_begin < t_end) {
-      const uint32_t idesc = umma_idesc(2 /*tf32*/, CT_BM, k_taps * p.BN);
-      const uint32_t dhi = umma_desc_hi_kmajor(8 * row_bytes, row_bytes);
-      const uint32_t tiles_lo = ((smem_u32(tiles) & 0x3FFFFu) >> 4) | (1u << 16);
-      const uint32_t bres_lo = ((smem_u32(res_b) & 0x3FFFFu) >> 4) | (1u << 16);
-      const int kst = p.cblk / 8;
-      const int rows_u = p.res ? 3 : p.rg;
-      const int upt = p.res ? 1 : (k_taps / p.rg) * p.kblocks;
-      const int U = (t_end - t_begin) * upt;
-      const uint32_t a_step = (uint32_t)(p.res ? p.a_tap : p.a_bytes) >> 4, b_step = (uint32_t)(b_rows * row_bytes) >> 4;
-      const uint32_t stage_step = (uint32_t)p.stage_bytes >> 4;
-      int s2 = 0, ph2 = 0, k2 = 0, a2 = 0, tr_n = 0;
-      for (int u2 = 0; u2 < U; ++u2) {
-        mbar_wait(&lo_ready[s2], ph2);
-        fence_after_sync();
-        CT_TRACE(4, 4);
-        const uint32_t d_tmem = tmem_base + a2 * p.acc_stride;
-        uint32_t da_r = tiles_lo + s2 * stage_step;
-        uint32_t db_r = p.res ? bres_lo : da_r + p.rg * a_step;
-        for (int rr = 0; rr < rows_u; ++rr) {
-          uint32_t da = da_r, db = db_r;
-          for (int ks = 0; ks < kst; ++ks) {
-            mma_tf32_c<true>(d_tmem, ((uint64_t)dhi << 32) | da, ((uint64_t)dhi << 32) | db, idesc);
-            da += 2; db += 2;
-          }
-          da_r += a_step; db_r += b_step;
-        }
-        mma_commit(&empty[s2]);
-        if (++k2 == upt) { k2 = 0; mma_commit(&t_full[a2]); if (++a2 == p.nacc) a2 = 0; }
-        CT_TRACE(4, 5);
-        if (++s2 == p.stages) { s2 = 0; ph2 ^= 1; }
-      }
-    }
-  } else if (X3 && (warp == 3 || warp >= 12)) {
-    // ===================== operand splitters (X3): stage by stage, in the producer's order
-    const int tid_c = (warp == 3 ? 0 : 32) + lane;
-    const int upt = p.res ? 1 : (k_taps / p.rg) * p.kblocks;
-    const int U = max(0, t_end - t_begin) * upt;
-    const int bytes = p.res ? p.a_stage_bytes : p.rg * p.a_bytes;
-    int stage = 0, phase = 0;
-    int tr_n = (tid_c == 0) ? 0 : 1000;
-    for (int u = 0; u < U; ++u) {
-      mbar_wait(&full[stage], phase);              // (the TMA writes of this stage are visible to this thread)
-      mbar_wait(&hi_done[stage], phase);           // pass-1 MMAs have finished reading the raw tile
-      CT_TRACE(3, 1);
-      split_lo_inplace(tiles + (size_t)stage * p.stage_bytes, bytes, tid_c, CT_NCONV);
-      fence_proxy_async();                         // generic-proxy writes -> visible to the tensor core
-      mbar_arrive(&lo_ready[stage]);
-      CT_TRACE(3, 2);
-      if (++stage == p.stages) { stage = 0; phase ^= 1; }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue: two groups of 4 warps; a warp owns one TMEM lane quarter
-    const int q4 = warp & 3, grp = (warp - 4) >> 2;
-    int tr_n = (warp == 4 && lane == 0) ? 0 : 1000;
-    CT_TRACE(2, 0);
-    float* sw = p.stats ? s_stats + (warp - 4) * 2 * p.Nc : nullptr;
-    for (int i = threadIdx.x - 128; i < p.Nc; i += 256) s_bias[i] = p.bias ? p.bias[i] : 0.f;
-    named_bar_sync(1, 256);
-    uint8_t* stg_w = stg_all + (warp - 4) * p.stage_out;
-    const bool two_sub = p.stage_out >= 4096 && p.BN == 16;
-    int sbuf = 0;                                      // 16-channel layers alternate the two sub-buffers
-    const int lblk = (p.b_merged && p.flip) ? 2 : 0;   // column block holding the s=0 partial sums
-    // per-thread geometry, computed once: integer divisions by run-time values cost ~100 cycles each and used to
-    // make up a third of the per-tile epilogue time.  A tile is 128 consecutive pixels of the NHWC tensor, so the
-    // pixel index is tm*128 + m and only the column position inside the image row (wb) needs a division.
-    const int m = q4 * 32 + lane;                   // row of the tile == TMEM lane
-    const int wb = m % p.Wb;
-    bool has_left = wb > 0, has_right = wb < p.W - 1;
-    const long long total_px = (long long)p.N * p.H * p.W;
-    // padded tiles: this lane's row slot, strip and pixel column (see ConvTcParams)
-    int pd_hr = 0, pd_img = 0, pd_w = 0, pd_w0 = 0, pd_srow = -1, pd_sub = 0;
-    if (k_padded) {
-      const int slot = m / p.Wb;
-      const int strip = (p.Nb == 1) ? slot / p.Hb : 0;
-      pd_hr = slot % p.Hb;
-      pd_img = (p.Nb == 1) ? 0 : slot / p.Hb;
-      const int wo = wb - (strip > 0 ? 1 : 0);
-      pd_w0 = strip * p.Ws;
-      pd_w = pd_w0 + wo;
-      pd_sub = slot % p.rpw;
-      if (wo >= 0 && wo < p.Ws && pd_w < p.W) pd_srow = pd_sub * p.Ws + wo;
-      has_left = pd_w > 0; has_right = pd_w < p.W - 1;
-    }
-    // work items = (tile, 32-column block), dealt alternately to the two groups: with one tile per CTA and 64 output
-    // channels both groups work on that tile instead of one group doing its blocks back to back
-    const int nblk = (p.BN + 31) >> 5;
-    int it = 0, blk = grp;                          // tile index inside the CTA, block inside the tile
-    int acc = 0, acc_phase = 0;                     // accumulator ring position of tile `it`
-    while (blk >= nblk) { blk -= nblk; ++it; if (++acc == p.nacc) { acc = 0; acc_phase ^= 1; } }
-    while (t_begin + it < t_end) {
-      const int t = t_begin + it;
-      int tm = t, tn = 0;
-      if (p.tiles_n != 1) { tm = t / p.tiles_n; tn = t - tm * p.tiles_n; }
-      long long pix = (long long)tm * CT_BM + m;
-      bool valid = pix < total_px;
-      int row0 = tm * CT_BM + q4 * 32;                // first pixel of this warp's 32 rows
-      int sc3 = 0;
-      if (k_padded) {
-        int n, h;
-        if (p.Nb == 1) { n = tm / p.tpi; h = (tm - n * p.tpi) * p.Hb + pd_hr; }
-        else { n = tm * p.Nb + pd_img; h = pd_hr; }
-        valid = pd_srow >= 0 && h < p.H && n < p.N;
-        pix = ((long long)n * p.H + h) * p.W + pd_w;
-        row0 = h - pd_sub;                            // first image row of this warp's slots
-        sc3 = n;
-      }
-      const float* rrow = p.residual ? p.residual + pix * p.Nc + tn * p.BN : nullptr;
-      mbar_wait(&t_full[acc], acc_phase);
-      CT_TRACE(2, 1);
-      fence_after_sync();
-      const uint32_t t_addr = tmem_base + ((uint32_t)(q4 * 32) << 16) + acc * p.acc_stride;
-      const int c0 = blk * 32;
-      long long* dbg = (p.trace && blockIdx.x == 0 && warp == 4 && lane == 0 && t == t_begin && blk == 0) ? p.trace + 2 * 512 + 400 : nullptr;
-      if (c0 + 32 <= p.BN) {
-        if (lane == 0) tma_store_wait_read<0>();      // the bulk stores that read this warp's staging have drained it
-        __syncwarp();
-        conv_tc_epilogue_block<32, GEN>(p, &map_o, t_addr, lblk, c0, tn, valid, has_left, has_right, row0, stg_w, rrow, s_bias, sw, lane, dbg,
-                                   pd_srow, pd_w0, sc3);
-        sbuf = 0;
-      } else {
-        if (lane == 0) { if (two_sub) tma_store_wait_read<1>(); else tma_store_wait_read<0>(); }
-        __syncwarp();
-        conv_tc_epilogue_block<16, GEN>(p, &map_o, t_addr, lblk, c0, tn, valid, has_left, has_right, row0, stg_w + sbuf * 2048, rrow, s_bias,
-                                   sw, lane, dbg, pd_srow, pd_w0, sc3);
-        if (two_sub) sbuf ^= 1;
-      }
-      CT_TRACE(2, 2);
-      fence_before_sync();                          // this item's TMEM reads are complete
-      mbar_arrive(&t_empty[acc]);                   // the barrier expects one arrival per item and thread (128 * nblk)
-      CT_TRACE(2, 3);
-      blk += 2;
-      while (blk >= nblk) { blk -= nblk; ++it; if (++acc == p.nacc) { acc = 0; acc_phase ^= 1; } }
-    }
+    return;
   }
 
-  if (warp >= 4 && lane == 0) tma_store_wait_all<0>();     // bulk stores read shared memory: drain before the CTA exits
-  __syncthreads();
+  // ===================== consumers: warpgroup wg owns rows 64*wg .. 64*wg+63 of the tile
+  const int wg = (tid >> 7) - 1, tid_wg = tid & 127, lane = tid & 31;
+  // X3: each stage's MMAs start a fresh register tile `part` that is then added into `acc` -- the tensor core's own
+  // accumulation loses low bits with every instruction, which over the 3 x 9 x Kc / 8 MMAs of a wide layer exceeds the
+  // fp32-level error budget of this mode
+  float acc[BN / 2], part[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  int stage = 0, phase = 0;
+  for (int it = 0; it < nk; ++it) {
+    mbar_wait(&full[stage], phase);
+    uint8_t* sa = smem + (size_t)stage * p.stage_bytes;
+    uint8_t* sb = sa + p.a_bytes;
+    uint8_t* sbl = sb + p.b_bytes;
+    uint8_t* sal = sbl + p.b_bytes;
+    if (X3) {
+      split_tile(sa, sal, p.a_bytes, tid - 128, 256);
+      split_tile(sb, nullptr, p.b_bytes, tid - 128, 256);
+      fence_proxy_async();                   // generic-proxy writes -> visible to the tensor core
+      named_bar_sync(1, 256);
+    }
+    const uint32_t a0 = smem_u32(sa) + wg * 64 * row_bytes, b0 = smem_u32(sb);
+    wgmma_fence();
+#pragma unroll 1
+    for (int ks = 0; ks < p.cblk / 8; ++ks) {
+      const uint64_t da = wgmma_desc(a0 + ks * 32, row_bytes), db = wgmma_desc(b0 + ks * 32, row_bytes);
+      if (X3) {
+        wgmma_tf32<BN>(part, da, db, ks != 0);
+        wgmma_tf32<BN>(part, da, wgmma_desc(smem_u32(sbl) + ks * 32, row_bytes), 1);
+        wgmma_tf32<BN>(part, wgmma_desc(smem_u32(sal) + wg * 64 * row_bytes + ks * 32, row_bytes), db, 1);
+      } else {
+        wgmma_tf32<BN>(acc, da, db, (it | ks) != 0);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (X3) {
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[stage]);
+    if (++stage == p.stages) { stage = 0; phase ^= 1; }
+  }
+
+  // ===================== epilogue on the registers: the two rows of this thread, BN/8 column pairs each
+  long long off[2];
+  bool valid[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = wg * 64 + fragment_row(2 * h, tid_wg);
+    const int wb = m % p.Wb, hb = (m / p.Wb) % p.Hb, nb = m / (p.Wb * p.Hb);
+    const int n = n0 + nb, y = h0 + hb, x = w0 + wb;
+    valid[h] = n < p.N && y < p.H && x < p.W && y < p.ovh && x < p.ovw;
+    off[h] = valid[h] ? n * p.o_sn + y * p.o_sh + x * p.o_sw : 0;
+  }
+  float csum[BN / 4], csq[BN / 4];
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = tn * BN + 8 * j + 2 * (lane & 3);
+    float2 b = make_float2(0.f, 0.f);
+    if (p.bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+    float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float2 v = make_float2(acc[4 * j + 2 * h] + b.x, acc[4 * j + 2 * h + 1] + b.y);
+      if (valid[h]) {
+        float2* o = reinterpret_cast<float2*>(p.out + off[h] + col);
+        if (p.residual) {
+          const float2 e = __ldg(reinterpret_cast<const float2*>(p.residual + off[h] + col));
+          v.x += e.x; v.y += e.y;
+        }
+        if (p.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
+        if (p.beta != 0.f) { const float2 prev = *o; v.x += p.beta * prev.x; v.y += p.beta * prev.y; }
+        *o = v;
+        s0 += v.x; s1 += v.y; q0 += v.x * v.x; q1 += v.y * v.y;
+      }
+    }
+    csum[2 * j] = s0; csum[2 * j + 1] = s1; csq[2 * j] = q0; csq[2 * j + 1] = q1;
+  }
   if (p.stats) {
-    for (int i = threadIdx.x; i < 2 * p.Nc; i += blockDim.x) {
+    // column sums over the 8 row groups of the warp (lanes with the same lane & 3), then over the 8 warps in warp order;
+    // the per-CTA sums are added across CTAs with float64 atomics (arrival order, float64 rounding)
+#pragma unroll
+    for (int j = 0; j < BN / 4; ++j) {
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) {
+        csum[j] += __shfl_xor_sync(0xffffffffu, csum[j], o);
+        csq[j] += __shfl_xor_sync(0xffffffffu, csq[j], o);
+      }
+    }
+    float* sw = s_stats + ((tid - 128) >> 5) * 2 * BN;
+    if (lane < 4) {
+#pragma unroll
+      for (int j = 0; j < BN / 4; ++j) {
+        const int c = 8 * (j >> 1) + 2 * lane + (j & 1);
+        sw[c] = csum[j];
+        sw[BN + c] = csq[j];
+      }
+    }
+    named_bar_sync(2, 256);
+    for (int i = tid - 128; i < 2 * BN; i += 256) {
       double v = 0.0;
 #pragma unroll
-      for (int wv = 0; wv < 8; ++wv) v += (double)s_stats[wv * 2 * p.Nc + i];
-      if (v != 0.0) atomicAdd(&p.stats[i], v);
+      for (int w = 0; w < 8; ++w) v += (double)s_stats[w * 2 * BN + i];
+      if (v != 0.0) atomicAdd(&p.stats[(i >= BN ? p.Nc : 0) + tn * BN + (i % BN)], v);
     }
   }
-  if (warp == 2) tmem_dealloc(tmem_base, p.tmem_cols);
 }
 
 // [tap][ci][co] (HWIO) -> [tap][co][ci] for every listed conv kernel of a flat parameter buffer, in one launch
@@ -718,50 +263,22 @@ transpose_filters_kernel(const float* __restrict__ P, float* __restrict__ PT, fl
 }
 
 // ---------------------------------------------------------------------------------------- host side
-// Pixel-tile geometry of a W x H image (see ConvTcParams).  Exact tiles when W divides 32 and whole rows / images fill
-// 128 pixels; otherwise padded tiles: rows (or strips of rows wider than 30 pixels) in power-of-two lane groups.
-struct ConvTcGeom { int Wb, Hb, Nb, tpi, padded, NS, Ws, rpw; };
 static int pow2_ge(int v) { int q = 1; while (q < v) q <<= 1; return q; }
-static bool plan_geometry(int W, int H, ConvTcGeom* g) {
-  static const bool no_pad = getenv("SE_CT_NO_PADDED") != nullptr;
-  g->NS = 1; g->Ws = W; g->padded = 0; g->rpw = 1;
-  if (W < 4) return false;
-  if (W <= 32 && (W & (W - 1)) == 0 && ((W * H >= 128) ? (H % (128 / W) == 0) : (128 % (W * H) == 0))) {
-    g->Wb = W;
-    if (W * H >= 128) { g->Hb = 128 / W; g->Nb = 1; g->tpi = H / g->Hb; }
-    else { g->Hb = H; g->Nb = 128 / (W * H); g->tpi = 1; }
-    return true;
-  }
-  if (no_pad) return false;
-  g->padded = 1;
-  if (W <= 32) {
-    g->Wb = max(8, pow2_ge(W));                // 8-pixel (1024-byte at 32 channels) slabs keep every box swizzle-aligned
-    g->rpw = 32 / g->Wb;
-    const int slots = 128 / g->Wb;             // row slots per tile
-    if (H >= slots || pow2_ge(H) >= slots) { g->Hb = slots; g->Nb = 1; g->tpi = (H + slots - 1) / slots; }
-    else { g->Hb = pow2_ge(H); g->Nb = slots / g->Hb; g->tpi = 1; }
-    if (g->Hb % g->rpw != 0) return false;
-    return true;
-  }
-  // wide rows: strips of Ws <= 28 outputs in 32-lane boxes (one pixel of left context for strips > 0, >= 3 spare lanes)
-  if (W > 56) return false;
-  g->Wb = 32; g->NS = 2; g->Ws = (W + 1) / 2; g->Hb = 2; g->Nb = 1; g->tpi = (H + 1) / 2;
-  return true;
-}
+
+// image sizes the 3x3 tiles take: rows of 4..56 pixels (every layer of the reference networks at their input sizes)
+static bool geometry_ok(int W) { return W >= 4 && W <= 56; }
 
 static bool tc_shape_ok(const se_conv_desc* d, int Kc, int Nc) {
   if (d->kh != 3 || d->kw != 3 || d->stride != 1 || d->pad_t != 1 || d->pad_l != 1 || d->Ho != d->H || d->Wo != d->W)
     return false;
   if (Kc % 16 != 0 || Nc % 16 != 0) return false;
   if (Kc > 16 && Kc % 32 != 0) return false;
-  ConvTcGeom g;
-  return plan_geometry(d->W, d->H, &g);
+  return geometry_ok(d->W);
 }
 
 // 1x1 / stride 1 / no padding: a GEMM over the flat pixel list, any image size
 static bool tc_shape_ok_1x1(const se_conv_desc* d, int Kc, int Nc) {
-  static const bool off = getenv("SE_CT_NO_1X1") != nullptr;
-  if (off || d->kh != 1 || d->kw != 1 || d->stride != 1 || d->pad_t != 0 || d->pad_l != 0 || d->Ho != d->H || d->Wo != d->W)
+  if (d->kh != 1 || d->kw != 1 || d->stride != 1 || d->pad_t != 0 || d->pad_l != 0 || d->Ho != d->H || d->Wo != d->W)
     return false;
   if (Kc % 16 != 0 || Nc % 16 != 0) return false;
   if (Kc > 16 && Kc % 32 != 0) return false;
@@ -771,216 +288,125 @@ static bool tc_shape_ok_1x1(const se_conv_desc* d, int Kc, int Nc) {
 // 1x1 / stride 2 / no padding (the first convolution and the projection shortcut of a ResNet-50 stage, the shortcuts of
 // wide_residual_network.py:28): the GEMM of the 1x1 case over the (Ho, Wo) grid, the input (forward) or the output
 // (backward data) addressed through a tensor map of the sub-sampled VIEW x[:, ::2, ::2, :] (pixel and row strides
-// doubled) -- no gather pass.  Tiles are rows of the output grid (padded-tile geometry).
+// doubled) -- no gather pass.
 static bool tc_shape_ok_1x1_s2(const se_conv_desc* d, int Kc, int Nc) {
-  static const bool off = getenv("SE_CT_NO_1X1") != nullptr || getenv("SE_CT_NO_S2") != nullptr;
-  if (off || d->kh != 1 || d->kw != 1 || d->stride != 2 || d->pad_t != 0 || d->pad_l != 0 || d->Ho != (d->H + 1) / 2 ||
+  if (d->kh != 1 || d->kw != 1 || d->stride != 2 || d->pad_t != 0 || d->pad_l != 0 || d->Ho != (d->H + 1) / 2 ||
       d->Wo != (d->W + 1) / 2)
     return false;
   if (Kc % 16 != 0 || Nc % 16 != 0) return false;
   if (Kc > 16 && Kc % 32 != 0) return false;
-  ConvTcGeom g;
-  return d->Wo <= 32 && plan_geometry(d->Wo, d->Ho, &g) && g.Hb % (32 / g.Wb) == 0;
+  return d->Wo <= 32 && geometry_ok(d->Wo);
 }
 
-// output channels per N tile: the MMA N is taps*BNc (<= 240 for 3x3, 128 for 1x1) and two accumulators must fit the
-// 512 TMEM columns
-static int pick_bn(int Nc, int taps) {
-  const int top = taps == 1 ? 128 : 80;
-  if (Nc <= top) return Nc;
-  for (int bn = top; bn >= 16; bn -= 16)
+// output channels per tile: the widest wgmma N that divides the channel count (<= 128; <= 64 in the error-compensated
+// mode, whose second accumulator tile would not fit the registers at 128)
+static int pick_bn(int Nc, int x3) {
+  for (int bn = x3 ? 64 : 128; bn >= 16; bn >>= 1)
     if (Nc % bn == 0) return bn;
-  return 16;
+  return 0;
 }
 
-size_t conv_wgrad_tc_smem(const se_conv_desc* d, int* tmem_cols, int x3);   // conv_wgrad_tc.cu
-constexpr int WG_COOP_SMEM_MAX = 120 * 1024;
+template <int BN>
+static void conv_tc_go(int x3, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& ma, const CUtensorMap& mb,
+                       const CUtensorMap& mbl, const ConvTcParams& p) {
+  if (x3) launch(conv_tc_kernel<BN, 1>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
+  else launch(conv_tc_kernel<BN, 0>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
+}
 
 static int conv_tc_launch(const se_conv_desc* d, const float* a_tensor, int Kc, const float* bmat, int Nc, int flip,
                           const float* bias, const float* residual, float* out, int relu, float beta, double* stats,
                           cudaStream_t st, const float* bmat_lo = nullptr, int taps = 3, int s2 = 0, int x3_plan = -1,
                           int out_view_w = 0, int out_view_h = 0) {
   // out_view_w / out_view_h (s2 backward data only, 0 = Wo x Ho): extent of the sub-sampled output view that starts at
-  // `out` -- a caller that passes dx + (r*W + s)*Cin writes dx[:, r::2, s::2, :], whose last column / row may not exist
-  // (they are clipped by the bulk store): one tap of a 3x3 / stride 2 data gradient, conv_dgrad_tc below
-  // x3_plan >= 0: plan only (se_conv2d_path) -- the shape / shared-memory / TMEM decisions below for arithmetic mode
-  // x3_plan, no pointers touched, nothing launched: SE_OK when this kernel would take the layer
+  // `out` -- a caller that passes dx + (r*W + s)*Cin writes dx[:, r::2, s::2, :], whose last column / row may not exist:
+  // one tap of a 3x3 / stride 2 data gradient, conv_dgrad_tc below
+  // x3_plan >= 0: plan only (se_conv2d_path) -- the shape / shared-memory decisions below for arithmetic mode x3_plan,
+  // no pointers touched, nothing launched: SE_OK when this kernel would take the layer
   // s2 (1x1 / stride 2): tiles over the (Ho, Wo) grid; forward reads the sub-sampled view of a_tensor, backward data
   // (flip) writes the sub-sampled view of out (after zeroing it: the other three quarters of dx are zero)
   ConvTcParams p;
   const int gW = s2 ? d->Wo : d->W, gH = s2 ? d->Ho : d->H;      // the grid the pixel tiles cover
   const int x3 = x3_plan >= 0 ? x3_plan : (bmat_lo ? 1 : 0);   // error-compensated mode: bmat_lo = the low parts of bmat (se_split_filters)
   const long long total_px = (long long)d->N * gH * gW;
-  p.taps = taps; p.flat = taps == 1 && !s2; p.pad = taps == 3 ? 1 : 0;
+  const bool flat = taps == 1 && !s2;
+  p.taps = taps; p.pad = taps == 3 ? 1 : 0; p.flip = flip;
   p.N = d->N; p.H = gH; p.W = gW; p.Kc = Kc; p.Nc = Nc;
-  p.Wb = gW; p.tpi = 1; p.padded = 0; p.NS = 1; p.Ws = gW; p.rpw = 1;
-  if (p.flat) {
+  if (flat) {
     // a 128-pixel tile is a run of the flat [N*H*W][C] matrix: the kernel sees one "image" of 1 x total_px pixels
     if (total_px > 0x7fffffffLL) return SE_ERR_UNSUPPORTED;
     p.N = 1; p.H = 1; p.W = (int)total_px; p.Wb = CT_BM; p.Hb = 1; p.Nb = 1;
   } else {
-    ConvTcGeom g;
-    if (!plan_geometry(gW, gH, &g)) return SE_ERR_UNSUPPORTED;
-    p.Wb = g.Wb; p.Hb = g.Hb; p.Nb = g.Nb; p.tpi = g.tpi; p.padded = g.padded; p.NS = g.NS; p.Ws = g.Ws; p.rpw = g.rpw;
-    if (s2 && flip && !p.padded) {
-      // the strided output view needs the 4-d store of the padded path: the same tiles, described as row slots
-      p.padded = 1; p.rpw = 32 / p.Wb;
-      if (p.Hb % p.rpw != 0) return SE_ERR_UNSUPPORTED;
-    }
+    p.Wb = min(pow2_ge(gW), CT_BM);
+    p.Hb = min(CT_BM / p.Wb, pow2_ge(gH));
+    p.Nb = CT_BM / (p.Wb * p.Hb);
   }
-  p.BN = pick_bn(Nc, taps);
-  if (p.BN % 16 != 0 || Nc % p.BN != 0) return SE_ERR_UNSUPPORTED;
-  p.tiles_n = Nc / p.BN;
-  if (p.flat) p.tiles_m = (int)ceil_div<long long>(total_px, CT_BM);
-  else p.tiles_m = (p.Nb == 1) ? d->N * p.tpi : ceil_div(d->N, p.Nb);
-  // few pixel tiles (64 channels at 8x8: 64 tiles for 148 SMs): split the output channels over two CTAs per tile --
-  // each then streams half of the 9*Cin*Cout weights, the dominant traffic of such a layer, and half of the epilogue
-  static const bool no_nsplit = getenv("SE_CT_NO_NSPLIT") != nullptr;
-  if (!no_nsplit && 2 * p.tiles_m * p.tiles_n <= sm_count() && p.BN >= 64 && (p.BN / 2) % 16 == 0) {
-    p.BN /= 2;
-    p.tiles_n *= 2;
-  }
+  p.tw = ceil_div(p.W, p.Wb); p.th = ceil_div(p.H, p.Hb);
+  const long long tiles_m = (long long)p.tw * p.th * ceil_div(p.N, p.Nb);
+  p.BN = pick_bn(Nc, x3);
+  if (p.BN == 0 || tiles_m > 0x7fffffffLL || Nc / p.BN > 65535) return SE_ERR_UNSUPPORTED;
   p.cblk = Kc >= 32 ? 32 : 16;
   p.kblocks = Kc / p.cblk;
-  p.flip = flip; p.relu = relu; p.beta = beta;
   p.a_bytes = CT_BM * p.cblk * 4;
-  // the whole 3x3 window of a channel block in one pipeline stage when two such stages fit (fewer barrier
-  // round trips per tile: small layers are bound by the single MMA-issuing thread, not by bandwidth)
-  // Backward-data launches leave room for the weight-gradient kernel of the same layer (it runs concurrently on the
-  // side stream of se_run_ops): shared memory = what that kernel leaves, TMEM <= 256 columns -- unless that would
-  // cost this kernel its pipeline, in which case it takes the whole SM as the forward launches do.
-  p.stage_out = CT_STAGE_OUT;
-  int budget = CT_SMEM_BUDGET, tmem_budget = 512;
-  static const bool no_coop = getenv("SE_NO_SIDE_STREAM") != nullptr;
-  if (flip && !no_coop) {
-    int wg_cols = 0;
-    const size_t wg = conv_wgrad_tc_smem(d, &wg_cols, x3);
-    if (wg > 0 && wg <= (size_t)WG_COOP_SMEM_MAX && wg_cols <= 256) {
-      if (pick_bn(Nc, taps) == 16) p.stage_out = 2048;          // one sub-buffer per warp buys the input pipeline a stage
-      budget = 225 * 1024 - (int)wg - 2048 - 8 * p.stage_out;
-      tmem_budget = 256;
-    }
-  }
-  const int full_budget = CT_SMEM_BUDGET;
- retry:
-  p.rg = taps;
-  p.stage_bytes = taps * p.a_bytes + (1 + x3) * ceil_div(taps * taps * p.BN * p.cblk * 4, 1024) * 1024;
-  if (2 * p.stage_bytes > budget) {
-    p.rg = 1;
-    p.stage_bytes = p.a_bytes + (1 + x3) * ceil_div(taps * p.BN * p.cblk * 4, 1024) * 1024;
-  }
-  p.stages = min(CT_MAX_STAGES, budget / p.stage_bytes);
-  if (p.stages < 2) {
-    if (budget != full_budget) { budget = full_budget; tmem_budget = 512; p.stage_out = CT_STAGE_OUT; goto retry; }
-    return SE_ERR_UNSUPPORTED;
-  }
-  // resident-weights mode: every tile of the CTA uses the same 9*BN x Kc weight block
-  p.res = 0; p.res_b_bytes = 0; p.res_bl_off = 0; p.nt = 1; p.single = 0; p.a_tap = p.a_bytes; p.a_stage_bytes = 3 * p.a_bytes;
-  static const char* dbg_nores = getenv("SE_CT_NORES");
-  const int wbytes = (1 + x3) * ceil_div(9 * p.BN * Kc * 4, 1024) * 1024;
-  static const bool no_single = getenv("SE_CT_NO_SINGLE") != nullptr;
-  const int single = (p.Nb == 1 && p.NS == 1 && p.Wb % 8 == 0 && !no_single && taps == 3) ? 1 : 0;
-  const int a_stage = single ? (p.Hb + 2) * p.Wb * p.cblk * 4 : 3 * p.a_bytes;
-  const int res_stage = ceil_div(a_stage, 1024) * 1024;
-  if (!dbg_nores && taps == 3 && p.tiles_n == 1 && p.kblocks == 1 && wbytes <= (1 + x3) * 40 * 1024 &&
-      ((budget - wbytes) / res_stage >= 2 || budget != full_budget)) {
-    p.res = 1; p.res_b_bytes = wbytes; p.res_bl_off = wbytes / 2; p.rg = 3;
-    p.single = single;
-    p.a_tap = single ? p.Wb * p.cblk * 4 : p.a_bytes;
-    p.a_stage_bytes = a_stage;
-    p.stage_bytes = res_stage;
-    p.stages = min(CT_MAX_STAGES, (budget - wbytes) / p.stage_bytes);
-    if (p.stages < 2) { budget = full_budget; tmem_budget = 512; p.stage_out = CT_STAGE_OUT; goto retry; }
-    static const char* dbg_nt = getenv("SE_CT_NT");
-    p.nt = dbg_nt ? atoi(dbg_nt) : 2;   // measured: 2 beats 4 (first epilogue starts earlier) and 1 (MMA bubbles)
-    p.nt = max(1, min(min(p.nt, 4), p.stages - 1));
-  }
-  static const char* dbg_stages = getenv("SE_CT_STAGES");         // tuning knobs for scripts/bench_conv.py
-  static const char* dbg_mode = getenv("SE_CT_DEBUG");
-  if (dbg_stages) p.stages = max(1, min(p.stages, atoi(dbg_stages)));
-  p.debug = dbg_mode ? atoi(dbg_mode) : 0;
-  static const char* dbg_trace = getenv("SE_CT_TRACE_PTR");
-  p.trace = dbg_trace ? reinterpret_cast<long long*>(strtoull(dbg_trace, nullptr, 0)) : nullptr;
-  int stride = 32;
-  while (stride < taps * p.BN) stride <<= 1;
-  if (2 * stride > 512) return SE_ERR_UNSUPPORTED;
-  if (tmem_budget < 512) {
-    // one accumulator is enough only when a CTA has a single tile; otherwise keep the MMA / epilogue overlap
-    const int tiles_per_cta = ceil_div(p.tiles_m * p.tiles_n, min(sm_count(), p.tiles_m * p.tiles_n));
-    if (tmem_budget / stride < min(2, tiles_per_cta)) tmem_budget = 512;
-  }
-  p.acc_stride = stride; p.nacc = min(CT_MAX_ACC, tmem_budget / stride);
-  p.tmem_cols = 32;
-  while (p.tmem_cols < p.nacc * stride) p.tmem_cols <<= 1;
-  p.nt = max(1, min(p.nt, p.nacc));
-  p.b_merged = (p.tiles_n == 1) ? 1 : 0;
+  p.b_bytes = p.BN * p.cblk * 4;
+  p.stage_bytes = (p.a_bytes + p.b_bytes) * (1 + x3);
+  p.stages = min(CT_MAX_STAGES, CT_SMEM_BUDGET / p.stage_bytes);
+  if (p.stages < 2) return SE_ERR_UNSUPPORTED;
+  p.relu = relu; p.beta = beta;
   p.bias = bias; p.residual = residual; p.out = out; p.stats = stats;
-  if (stats && (size_t)16 * Nc * sizeof(float) > 24 * 1024) return SE_ERR_UNSUPPORTED;
-  if (beta != 0.f && (beta != 1.f || residual || relu)) return SE_ERR_UNSUPPORTED;   // accumulate = bulk reduce-add of the raw result
-
-  const size_t smem = (size_t)p.res_b_bytes + (size_t)p.stages * p.stage_bytes + 8 * p.stage_out + (4 * CT_MAX_STAGES + 2 * CT_MAX_ACC + 4) * 8 + Nc * 4 + (stats ? 16 * Nc * 4 : 0) + 1024 + 64;
+  if (stats && (size_t)16 * Nc * sizeof(float) > 24 * 1024) return SE_ERR_UNSUPPORTED;   // wide layers: separate statistics pass
+  if (beta != 0.f && (beta != 1.f || residual || relu)) return SE_ERR_UNSUPPORTED;
+  const size_t smem = 1024 + (size_t)p.stages * p.stage_bytes + 2 * CT_MAX_STAGES * 8 + 16 * p.BN * 4;
   if (smem > 227 * 1024) return SE_ERR_UNSUPPORTED;
   if (x3_plan >= 0) return SE_OK;
+  // output (and residual) addressing: NHWC over the tile grid, or the strided view dx[:, ::2, ::2, :] (s2 backward data)
+  p.o_sw = Nc; p.o_sh = (long long)p.W * Nc; p.o_sn = (long long)p.H * p.W * Nc;
+  p.ovw = p.W; p.ovh = p.H;
+  if (s2 && flip) {
+    p.o_sw = 2LL * Nc; p.o_sh = 2LL * d->W * Nc; p.o_sn = (long long)d->H * d->W * Nc;
+    if (out_view_w) p.ovw = out_view_w;
+    if (out_view_h) p.ovh = out_view_h;
+  }
   CUtensorMap ma, mb, mbl;
   {
-    uint64_t dims[4] = {(uint64_t)Kc, (uint64_t)gW, (uint64_t)gH, (uint64_t)d->N};
-    uint64_t strides[3] = {(uint64_t)Kc * 4, (uint64_t)gW * Kc * 4, (uint64_t)gH * gW * Kc * 4};
+    uint64_t dims[4] = {(uint64_t)Kc, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.N};
+    uint64_t strides[3] = {(uint64_t)Kc * 4, (uint64_t)p.W * Kc * 4, (uint64_t)p.H * p.W * Kc * 4};
     if (s2 && !flip) {      // forward: x[:, ::2, ::2, :]
       strides[0] = (uint64_t)2 * Kc * 4; strides[1] = (uint64_t)2 * d->W * Kc * 4; strides[2] = (uint64_t)d->H * d->W * Kc * 4;
     }
-    uint32_t box[4] = {(uint32_t)p.cblk, (uint32_t)p.Wb, (uint32_t)(p.single ? p.Hb + 2 : p.Hb), (uint32_t)p.Nb};
-    if (p.flat) {
-      dims[1] = (uint64_t)total_px; dims[2] = 1; dims[3] = 1;
-      strides[1] = strides[2] = (uint64_t)total_px * Kc * 4;
-      box[1] = CT_BM; box[2] = 1; box[3] = 1;
-    }
+    uint32_t box[4] = {(uint32_t)p.cblk, (uint32_t)p.Wb, (uint32_t)p.Hb, (uint32_t)p.Nb};
     CUtensorMapSwizzle sw = p.cblk == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
     if (!make_tmap(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(a_tensor), dims, strides, box, sw)) return SE_ERR_CUDA;
     uint64_t bdims[2] = {(uint64_t)Kc, (uint64_t)taps * taps * Nc};
     uint64_t bstrides[1] = {(uint64_t)Kc * 4};
-    uint32_t bbox[2] = {(uint32_t)p.cblk, (uint32_t)(p.b_merged ? taps * p.BN : p.BN)};
+    uint32_t bbox[2] = {(uint32_t)p.cblk, (uint32_t)p.BN};
     if (!make_tmap(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(bmat), bdims, bstrides, bbox, sw)) return SE_ERR_CUDA;
     mbl = mb;
     if (x3 && !make_tmap(&mbl, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(bmat_lo), bdims, bstrides, bbox, sw))
       return SE_ERR_CUDA;
   }
-  CUtensorMap mo;
-  {
-    // output(s) as [pixels][channels]: 32-pixel x 16-channel boxes, SWIZZLE_64B staging (see stage_put)
-    uint64_t odims[2] = {(uint64_t)Nc, (uint64_t)total_px};
-    uint64_t ostrides[1] = {(uint64_t)Nc * 4};
-    uint32_t obox[2] = {16u, 32u};
-    if (p.padded) {
-      // [N][H][W][channels]: one strip of Ws pixels x rpw rows per warp; pixels / rows / images past the tensor are clipped
-      uint64_t odims4[4] = {(uint64_t)Nc, (uint64_t)(out_view_w ? out_view_w : gW), (uint64_t)(out_view_h ? out_view_h : gH), (uint64_t)d->N};
-      uint64_t ostrides4[3] = {(uint64_t)Nc * 4, (uint64_t)gW * Nc * 4, (uint64_t)gH * gW * Nc * 4};
-      if (s2 && flip) {     // backward data: dx[:, ::2, ::2, :]
-        ostrides4[0] = (uint64_t)2 * Nc * 4; ostrides4[1] = (uint64_t)2 * d->W * Nc * 4; ostrides4[2] = (uint64_t)d->H * d->W * Nc * 4;
-      }
-      uint32_t obox4[4] = {16u, (uint32_t)p.Ws, (uint32_t)p.rpw, 1u};
-      if (!make_tmap(&mo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, out, odims4, ostrides4, obox4, CU_TENSOR_MAP_SWIZZLE_64B)) return SE_ERR_CUDA;
-    } else
-    if (!make_tmap(&mo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, out, odims, ostrides, obox, CU_TENSOR_MAP_SWIZZLE_64B)) return SE_ERR_CUDA;
-  }
-  int grid = min(sm_count(), p.tiles_m * p.tiles_n);
   if (s2 && flip && beta == 0.f &&
       cudaMemsetAsync(out, 0, (size_t)d->N * d->H * d->W * Nc * sizeof(float), st) != cudaSuccess) {
     set_error("conv_tc: cudaMemsetAsync failed");
     return SE_ERR_CUDA;
   }
-  const bool gen = taps != 3 || p.padded || p.flat || p.NS != 1;
-  if (x3 && gen) launch(conv_tc_kernel<1, 1>, dim3(grid), dim3(CT_THREADS_X3), smem, st, ma, mb, mbl, mo, p);
-  else if (x3) launch(conv_tc_kernel<1, 0>, dim3(grid), dim3(CT_THREADS_X3), smem, st, ma, mb, mbl, mo, p);
-  else if (gen) launch(conv_tc_kernel<0, 1>, dim3(grid), dim3(CT_THREADS), smem, st, ma, mb, mbl, mo, p);
-  else launch(conv_tc_kernel<0, 0>, dim3(grid), dim3(CT_THREADS), smem, st, ma, mb, mbl, mo, p);
+  const dim3 grid((unsigned)tiles_m, (unsigned)(Nc / p.BN));
+  switch (p.BN) {
+    case 16: conv_tc_go<16>(x3, grid, smem, st, ma, mb, mbl, p); break;
+    case 32: conv_tc_go<32>(x3, grid, smem, st, ma, mb, mbl, p); break;
+    case 64: conv_tc_go<64>(x3, grid, smem, st, ma, mb, mbl, p); break;
+    default: conv_tc_go<128>(x3, grid, smem, st, ma, mb, mbl, p); break;
+  }
   return check_launch("conv_tc_kernel");
 }
 
+template <int BN>
+static bool set_smem_limit() {
+  return cudaFuncSetAttribute(conv_tc_kernel<BN, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess &&
+         cudaFuncSetAttribute(conv_tc_kernel<BN, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess;
+}
+
 int init_conv_tc() {
-  if (cudaFuncSetAttribute(conv_tc_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_tc_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_tc_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_tc_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
+  if (!set_smem_limit<16>() || !set_smem_limit<32>() || !set_smem_limit<64>() || !set_smem_limit<128>()) {
     set_error("init_conv_tc: cannot raise the shared-memory limit");
     return SE_ERR_CUDA;
   }
@@ -1006,10 +432,10 @@ int conv_fwd_tc(const se_conv_desc* d, const float* x, const float* w_t, const f
   return conv_tc_launch(d, x, d->Cin, w_t, d->Cout, 0, bias, residual, y, relu, 0.f, stats, st, w_t_lo, k1 ? 1 : 3, k2);
 }
 
-bool conv3x3s2_tc_ok(const se_conv_desc* d);      // conv1x1_wgrad_tc.cu
+bool conv3x3s2_tc_ok(const se_conv_desc* d);      // conv_wgrad_tc.cu
 
 // 3x3 / stride 2 / no leading padding, wide layers (see conv3x3s2_tc_ok): nine 1x1 / stride 2 data gradients, one per
-// filter tap, each reduce-added into its own sub-sampled view of dx:   dx[:, r::2, s::2, :] += dY W[r, s]^T
+// filter tap, each added into its own sub-sampled view of dx:   dx[:, r::2, s::2, :] += dY W[r, s]^T
 static int conv_dgrad_tc_3x3s2(const se_conv_desc* d, const float* dy, const float* w, const float* w_lo, float* dx, float beta,
                                cudaStream_t st) {
   if (beta != 0.f && beta != 1.f) return SE_ERR_UNSUPPORTED;
@@ -1043,8 +469,7 @@ int conv_dgrad_tc(const se_conv_desc* d, const float* dy, const float* w, const 
   return conv_tc_launch(d, dy, d->Cout, w, d->Cin, 1, nullptr, nullptr, dx, 0, beta, nullptr, st, w_lo, k1 ? 1 : 3, k2);
 }
 
-
-// se_conv2d_path: would the tcgen05 kernel of this file take the layer?  (dir 0 forward, 1 backward data; x3 = 0 / 1)
+// se_conv2d_path: would the tensor-core kernel of this file take the layer?  (dir 0 forward, 1 backward data; x3 = 0 / 1)
 bool conv_tc_would_run(const se_conv_desc* d, int dir, int x3) {
   if (dir == 1 && conv3x3s2_tc_ok(d)) {
     se_conv_desc d1 = *d;
@@ -1078,7 +503,7 @@ int transpose_filters(const float* P, float* PT, float* PL, float* PTL, const lo
   return SE_OK;
 }
 
-// bit 0 conv fwd, bit 1 conv dgrad, bit 2 conv wgrad, bit 3 pairwise: which tcgen05 kernels are compiled in
+// bit 0 conv fwd, bit 1 conv dgrad, bit 2 conv wgrad, bit 3 pairwise: which tensor-core kernels are compiled in
 int tc_capabilities() { return 1 | 2 | 4 | 8; }
 
 }  // namespace se

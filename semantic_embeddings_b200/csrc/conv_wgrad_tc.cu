@@ -1,26 +1,23 @@
-// tcgen05 (kind::tf32) weight gradient of 3x3 / stride 1 / 'same' convolutions:
-//   dW[r, s, ci, co] += sum_pixels X[pixel + (r-1, s-1), ci] * dY[pixel, co]      (autodiff of Conv2D, reference
-//   models/cifar_resnet.py:96-105 etc. under learn_image_embeddings.py:238)
+// Tensor-core (wgmma, TF32) weight gradient of the convolutions the forward kernels take (conv_tc.cu): 3x3 / stride 1
+// / 'same', 1x1 / stride 1 and 2, and the wide 3x3 / stride 2 layers of wide_residual_network.py:20-31:
+//   dW[r, s, ci, co] += sum_pixels X[pixel * stride + (r, s) - pad, ci] * dY[pixel, co]      (autodiff of Conv2D, reference
+//   models/cifar_resnet.py:96-105 etc. under learn_image_embeddings.py:238)          dbias[co] += sum_pixels dY[pixel, co]
 //
-// The reduction dimension is the PIXEL axis, so both operands are "MN-major" for the tensor core (channels are
-// contiguous, pixels are strided): no transposition of activations is needed, the NHWC tiles that TMA drops into
-// shared memory are consumed as they are.  For 32-bit (TF32) operands the tensor core accepts MN-major data only in
-// the SWIZZLE_128B_BASE32B layout (32-byte swizzle granules, atoms of 32 channels x 4 pixels), which TMA produces
-// with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.  Channel counts that are not multiples of 32 (the 16-channel stage of
-// ResNet-110) use the same 32-channel boxes: the out-of-range channels are zero-filled by the hardware and the zero
-// rows / columns of D are simply not written back.
-//
-//   per pixel tile (PT pixels = Hb image rows, or Nb whole images) and per horizontal tap s:
-//     one TMA box of Hb+2 rows x W pixels x 32 input channels, shifted by s-1 pixels (zero-filled halo = 'same' padding);
-//     the three VERTICAL taps r read that same box at row offsets r*W pixels -- a whole number of 1024-byte swizzle
-//     periods (W >= 8), so they are just different descriptor start addresses.  With LBO = one image row, the four
-//     32-row blocks of an M = 128 instruction are the taps r = 0, 1, 2 (and a fourth, ignored, garbage block):
-//        D_s[(r, ci), co] += A_s[(r, ci), pix] * B[co, pix]         3 MMAs per 8 pixels (+1 with an all-ones A for dbias)
-//   Accumulators stay in TMEM across ALL pixel tiles of a CTA (split-K over CTAs); one epilogue at the end adds them
-//   into dW / dbias with 16-byte reductions, each CTA starting at a different column so that the CTAs do not queue on
-//   the same L2 lines.
-// grid = (pixel-tile groups, input-channel chunks of 32, output-channel chunks of <= 128); persistent over its tiles.
+// The reduction dimension is the PIXEL axis, in which both NHWC tensors are strided; TF32 wgmma reads only K-major
+// operands, so each warpgroup loads a chunk of 32 pixels of X (64 input channels, shifted by the filter tap and
+// zero outside the image) and of dY (BN output channels) into registers and writes them TRANSPOSED into shared memory
+// as [channel][32 pixels] rows of 128 bytes in the 128-byte swizzle layout; the next chunk's global loads are in flight
+// while the MMAs of the current one run.  M = 64 input channels, N = BN output channels, K = 8 pixels per instruction.
+// X3 (error-compensated, see conv_tc.cu): the transposing stores write hi and lo parts into two tiles each, and
+// dW = X_hi*dY_hi + X_hi*dY_lo + X_lo*dY_hi.
+// grid = (pixel ranges, 64-channel input blocks x filter taps, output-channel tiles); the two warpgroups of a CTA take
+// alternate chunks of its range (split-K).  Every warpgroup stores its partial sums into its own slice of a library
+// workspace, and a second kernel adds the slices into dW / dbias in a fixed order: the result is the same on every run
+// (float atomics would add the slices in whatever order they arrive).
 #include <stdlib.h>
+
+#include <algorithm>
+#include <mutex>
 
 #include "common.cuh"
 #include "tc.cuh"
@@ -29,434 +26,324 @@ namespace se {
 
 using namespace tc;
 
-// conv_wgrad_pk.cu: the "packed" error-compensated variant for layers with Cin, Cout <= 16 (its own operand layout)
-int init_conv_wgrad_pk();
-size_t conv_wgrad_pk_smem(const se_conv_desc* d, int* tmem_cols);
-int conv_wgrad_pk(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st);
-// conv1x1_wgrad_tc.cu: 1x1 / stride 1 layers (a GEMM over the flat pixel list)
-int init_conv1x1_wgrad_tc();
-bool conv1x1_wgrad_tc_ok(const se_conv_desc* d);
-int conv1x1_wgrad_tc(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias, int x3, cudaStream_t st,
-                     int x_view_w = 0, int x_view_h = 0);
-bool conv3x3s2_tc_ok(const se_conv_desc* d);
-int conv3x3s2_wgrad_tc(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias, int x3, cudaStream_t st);
-static bool wgrad_is_packed(const se_conv_desc* d, int x3) {
-  static const bool no_pack = getenv("SE_WG_NO_PACK") != nullptr;
-  return x3 && d->Cin <= 16 && d->Cout <= 16 && !no_pack;
-}
+constexpr int WG_PX = 32;              // pixels per chunk: one 128-byte swizzle row per channel
+constexpr int WG_MT = 64;              // rows of dW ((filter tap, input channel) pairs) per warpgroup tile
+constexpr int WG_THREADS = 256;
 
 struct WgTcParams {
-  int N, H, W, Cin, Cout;      // W = the row pitch of the shared-memory boxes: the image width rounded up to a power of two >= 8
-                               // (TMA zero-fills the pixels past the image: they add nothing to the sums)
-  int tpi;                     // pixel tiles per image (Nb == 1); the last one may hang over the image (zero-filled rows)
-  int Hb, Nb, PT;              // pixel tile: Hb rows of one image (Nb == 1) or Nb whole images; PT = W*Hb*Nb pixels
-  int img_px;                  // pixels of one image inside the tile (Hb * W)
-  int img_stride;              // bytes between images inside an x buffer ((Hb + 2) * W * 128)
-  int xbuf_bytes;              // one horizontally shifted x buffer (Nb * img_stride)
-  int nnb, ncols;              // dY: 32-channel blocks per CTA, MMA N = 32 * nnb
-  int G;                       // accumulators: 3 horizontal taps (+1 for the bias gradient)
-  int stages, stage_bytes, dy_bytes;
-  int tiles_m;
-  int debug;                   // SE_WG_DEBUG: 1 = no atomics, 2 = load one tap only, 4 = no MMAs (timing experiments)
-  float* dw;
+  int N, H, W, Cin, Cout, Ho, Wo, kw, stride, pad_t, pad_l;
+  int KK;                      // rows of dW: kh * kw * Cin, row = tap * Cin + ci
+  int npx;                     // N * Ho * Wo
+  int chunks;                  // ceil(npx / 32)
+  int per_cta;                 // chunks per CTA (even)
+  float* ws;                   // [2 * gridDim.x][KK * Cout] partial dW, then [2 * gridDim.x][Cout] partial dbias
+  float* dw;                   // direct mode (ws == nullptr): atomics straight into dW / dbias
   float* dbias;
 };
 
-__device__ __forceinline__ float wg_tf32_lo(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
+// Workspaces of the split-K partial sums: one per (device, stream), 32 MB each, allocated outside graph captures (se_init
+// prepares the one of se_run_ops' side stream).  A request that does not fit, or a stream that first appears inside a
+// capture, runs in direct mode instead: the partial sums go into dW with float atomics (correct, not bit-reproducible).
+constexpr long long WG_WS_FLOATS = 8LL << 20;
+struct WgWorkspace { int dev; cudaStream_t st; float* ptr; };
+constexpr int WG_MAX_WS = 32;
+static WgWorkspace g_wg_ws[WG_MAX_WS];
+static int g_wg_nws = 0;
+static std::mutex g_wg_mu;
 
-// X3 = error-compensated arithmetic (see conv_tc.cu): dW = X_hi*dY_hi + X_hi*dY_lo + X_lo*dY_hi in one fp32 accumulator.
-// hi is what kind::tf32 reads of the raw tile (mantissa truncated to 10 bits); the epilogue warps, idle until the last
-// tile, produce the lo parts: warp 2 writes dY_lo into a second (small) dY buffer of the stage as soon as the tile has
-// landed, warps 3-5 rewrite the three X buffers IN PLACE as X_lo once pass 1 (X*dY_hi, X*dY_lo) has read them, then
-// pass 2 issues X_lo*dY_hi.  The MMA warp runs the passes as two cursors over the stage sequence.
-// Layers with Cin, Cout <= 16 use the "packed" variant of conv_wgrad_pk.cu instead (lo parts in the zero-filled channel
-// slots of the 32-channel boxes: no second pass).
-//
-// Measured (B200, 16 -> 16 channels at 32x32, batch 128): consecutive MMAs that share their B descriptor cost ~35 cycles
-// each, an MMA with a new B operand ~100 more (the MN-major B slab is re-staged) -- so dY, the small operand, is B and
-// every k-step issues all MMAs of one B slab back to back.  The alternative layout (one X box, three shifted dY boxes
-// stacked along N) moves fewer bytes but changes B every MMA and was 25 % slower.
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a, uint64_t b, int acc) {
+  if constexpr (BN == 16) wgmma_tf32_n16(d, a, b, acc);
+  else if constexpr (BN == 32) wgmma_tf32_n32(d, a, b, acc);
+  else if constexpr (BN == 64) wgmma_tf32_n64(d, a, b, acc);
+  else wgmma_tf32_n128(d, a, b, acc);
+}
+
+// one channel quadruple of one pixel -> four transposed rows of a [channel][32 pixels] tile (X3: hi and lo tiles)
 template <int X3>
-__global__ void __launch_bounds__(192, 1)
-conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_dy, WgTcParams p) {
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* tiles = smem;
-  uint8_t* ones = tiles + (size_t)p.stages * p.stage_bytes;               // 8 pixels x 32 channels of 1.0f (G == 4)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ones + (p.G == 4 ? 1024 : 0));
-  uint64_t* full = bars;
-  uint64_t* empty = bars + 4;
-  uint64_t* done = bars + 8;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
-  uint64_t* ylo_ready = bars + 10;          // X3: dY_lo of the stage written
-  uint64_t* hi_done = bars + 14;            // X3: pass-1 MMAs have read the stage
-  uint64_t* lo_ready = bars + 18;           // X3: the X buffers of the stage hold X_lo
-
-  const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
-  const int per_cta = (p.tiles_m + gridDim.x - 1) / gridDim.x;
-  const int t_begin = blockIdx.x * per_cta;
-  const int t_end = min(p.tiles_m, t_begin + per_cta);
-  const int ci0 = blockIdx.y * 32;
-  const int co0 = blockIdx.z * p.ncols;
-  const int tiles_per_img = p.tpi;
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < p.G * p.ncols) tmem_cols <<= 1;
-
-  if (p.G == 4) {
-    float4* o = reinterpret_cast<float4*>(ones);
-    for (int i = threadIdx.x; i < 64; i += blockDim.x) o[i] = make_float4(1.f, 1.f, 1.f, 1.f);
-  }
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&map_x); prefetch_tmap(&map_dy);
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(done, 1);
-    if (X3) for (int s = 0; s < p.stages; ++s) { mbar_init(&ylo_ready[s], 32); mbar_init(&hi_done[s], 1); mbar_init(&lo_ready[s], 96); }
-    fence_barrier_init();
-  }
-  fence_proxy_async();                      // generic-proxy writes of the ones tile -> visible to the tensor core
-  if (warp == 1) tmem_alloc(tmem_slot, tmem_cols);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-  pdl_wait();                               // nothing above touches global memory (see common.cuh)
-
-  if (t_begin < t_end) {
-    if (warp == 0) {
-      // ===================== TMA producer (convergent warp, one elected lane issues)
-      int stage = 0, phase = 0;
-      const int ntap = (p.debug & 2) ? 1 : 3;
-      const uint32_t tx = ntap * p.xbuf_bytes + p.dy_bytes;
-      for (int t = t_begin; t < t_end; ++t) {
-        int n0, h0;
-        if (p.Nb == 1) { n0 = t / tiles_per_img; h0 = (t - n0 * tiles_per_img) * p.Hb; }
-        else { n0 = t * p.Nb; h0 = 0; }
-        mbar_wait(&empty[stage], phase ^ 1);
-        uint8_t* sb = tiles + (size_t)stage * p.stage_bytes;
-        if (elect_one()) {
-          mbar_expect_tx(&full[stage], tx);
-          for (int s = 0; s < ntap; ++s) tma_load_4d(sb + s * p.xbuf_bytes, &map_x, &full[stage], ci0, s - 1, h0 - 1, n0);
-          for (int nb = 0; nb < p.nnb; ++nb)
-            tma_load_4d(sb + 3 * p.xbuf_bytes + nb * (p.PT * 128), &map_dy, &full[stage], co0 + nb * 32, 0, h0, n0);
-        }
-        __syncwarp();
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-    } else if (warp == 1) {
-      // ===================== MMA issuer (convergent warp, one elected lane issues)
-      // instruction descriptor: tf32 x tf32 -> f32, A and B both MN-major (bits 15 / 16), M = 128, N = ncols
-      const uint32_t idesc = umma_idesc(2, 128, p.ncols) | (1u << 15) | (1u << 16);
-      // descriptor high word: SBO = 512 B (consecutive 4-pixel atoms), version 1, SWIZZLE_128B_BASE32B
-      const uint32_t hi = (512u >> 4) | (1u << 14) | (1u << 29);
-      const uint32_t lbo_a = (((uint32_t)(p.W * 128) >> 4) & 0x3FFFu) << 16;      // next vertical tap = next image row
-      const uint32_t lbo_b = (((uint32_t)(p.PT * 128) >> 4) & 0x3FFFu) << 16;     // next 32-channel block of dY
-      const uint32_t ones_lo = (smem_u32(ones) & 0x3FFFFu) >> 4;                  // LBO 0, the same 8 pixels for every k-step
-      const uint32_t tiles_u32 = smem_u32(tiles);
-      const int ksteps = (p.debug & 4) ? 0 : p.PT / 8;
-      int stage = 0, phase = 0;
-      uint32_t acc = 0;
-      if (X3 == 1) {
-        const int T = t_end - t_begin;
-        int u1 = 0, s1 = 0, ph1 = 0, u2 = 0, s2 = 0, ph2 = 0;
-        while (u2 < T) {
-          int ok1 = 0;
-          if (u1 < T) ok1 = mbar_try_wait(&full[s1], ph1) && mbar_try_wait(&ylo_ready[s1], ph1);
-          ok1 = __shfl_sync(0xffffffffu, ok1, 0);          // one decision for the warp (elect_one needs convergence)
-          if (ok1) {
-            fence_after_sync();
-            const uint32_t sb = tiles_u32 + (uint32_t)s1 * p.stage_bytes;
-            const uint32_t dyb = sb + 3 * p.xbuf_bytes, dyl = dyb + p.dy_bytes;
-            uint32_t img_off = 0, rem = 0;
-            for (int ks = 0; ks < ksteps; ++ks) {
-              const uint64_t db = ((uint64_t)hi << 32) | (uint64_t)((((dyb + ks * 1024) & 0x3FFFFu) >> 4) | lbo_b);
-              const uint64_t dl = ((uint64_t)hi << 32) | (uint64_t)((((dyl + ks * 1024) & 0x3FFFFu) >> 4) | lbo_b);
-              const uint32_t a0 = sb + img_off + rem * 128;
-              if (elect_one()) {
-                // all MMAs of one B slab back to back (a new B operand costs far more than a new A operand)
+__device__ __forceinline__ void put_t(uint8_t* hi, uint8_t* lo, int c4, int px, float4 v) {
+  const float e[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-                for (int s = 0; s < 3; ++s) {
-                  const uint64_t da = ((uint64_t)hi << 32) | (uint64_t)((((a0 + s * p.xbuf_bytes) & 0x3FFFFu) >> 4) | lbo_a);
-                  mma_tf32(tmem_base + s * p.ncols, da, db, idesc, acc);
-                }
-                if (p.G == 4) mma_tf32(tmem_base + 3 * p.ncols, ((uint64_t)hi << 32) | (uint64_t)ones_lo, db, idesc, acc);
-#pragma unroll
-                for (int s = 0; s < 3; ++s) {
-                  const uint64_t da = ((uint64_t)hi << 32) | (uint64_t)((((a0 + s * p.xbuf_bytes) & 0x3FFFFu) >> 4) | lbo_a);
-                  mma_tf32(tmem_base + s * p.ncols, da, dl, idesc, 1);
-                }
-                if (p.G == 4) mma_tf32(tmem_base + 3 * p.ncols, ((uint64_t)hi << 32) | (uint64_t)ones_lo, dl, idesc, 1);
-              }
-              __syncwarp();
-              acc = 1;
-              rem += 8;
-              if ((int)rem == p.img_px) { rem = 0; img_off += p.img_stride; }
-            }
-            if (elect_one()) mma_commit(&hi_done[s1]);
-            __syncwarp();
-            ++u1;
-            if (++s1 == p.stages) { s1 = 0; ph1 ^= 1; }
-          }
-          int ok2 = 0;
-          if (u2 < u1) ok2 = mbar_try_wait(&lo_ready[s2], ph2);
-          ok2 = __shfl_sync(0xffffffffu, ok2, 0);
-          if (ok2) {
-            fence_after_sync();
-            const uint32_t sb = tiles_u32 + (uint32_t)s2 * p.stage_bytes;
-            const uint32_t dyb = sb + 3 * p.xbuf_bytes;
-            uint32_t img_off = 0, rem = 0;
-            for (int ks = 0; ks < ksteps; ++ks) {
-              const uint64_t db = ((uint64_t)hi << 32) | (uint64_t)((((dyb + ks * 1024) & 0x3FFFFu) >> 4) | lbo_b);
-              const uint32_t a0 = sb + img_off + rem * 128;
-              if (elect_one()) {
-#pragma unroll
-                for (int s = 0; s < 3; ++s) {
-                  const uint64_t da = ((uint64_t)hi << 32) | (uint64_t)((((a0 + s * p.xbuf_bytes) & 0x3FFFFu) >> 4) | lbo_a);
-                  mma_tf32(tmem_base + s * p.ncols, da, db, idesc, 1);
-                }
-              }
-              __syncwarp();
-              rem += 8;
-              if ((int)rem == p.img_px) { rem = 0; img_off += p.img_stride; }
-            }
-            if (elect_one()) mma_commit(&empty[s2]);
-            __syncwarp();
-            ++u2;
-            if (++s2 == p.stages) { s2 = 0; ph2 ^= 1; }
-          }
-        }
-      }
-      for (int t = t_begin; !X3 && t < t_end; ++t) {
-        mbar_wait(&full[stage], phase);
-        fence_after_sync();
-        const uint32_t sb = tiles_u32 + (uint32_t)stage * p.stage_bytes;
-        const uint32_t dyb = sb + 3 * p.xbuf_bytes;
-        uint32_t img_off = 0, rem = 0;               // byte offset of the current image / pixel inside the image
-        for (int ks = 0; ks < ksteps; ++ks) {
-          const uint64_t db = ((uint64_t)hi << 32) | (uint64_t)((((dyb + ks * 1024) & 0x3FFFFu) >> 4) | lbo_b);
-          const uint32_t a0 = sb + img_off + rem * 128;
-          if (elect_one()) {
-#pragma unroll
-            for (int s = 0; s < 3; ++s) {
-              const uint64_t da = ((uint64_t)hi << 32) | (uint64_t)((((a0 + s * p.xbuf_bytes) & 0x3FFFFu) >> 4) | lbo_a);
-              mma_tf32(tmem_base + s * p.ncols, da, db, idesc, acc);
-            }
-            if (p.G == 4) mma_tf32(tmem_base + 3 * p.ncols, ((uint64_t)hi << 32) | (uint64_t)ones_lo, db, idesc, acc);
-          }
-          __syncwarp();
-          acc = 1;
-          rem += 8;
-          if ((int)rem == p.img_px) { rem = 0; img_off += p.img_stride; }
-        }
-        if (elect_one()) mma_commit(&empty[stage]);
-        __syncwarp();
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-      if (elect_one()) mma_commit(done);
-      __syncwarp();
+  for (int j = 0; j < 4; ++j) {
+    const uint32_t o = swizzle_offset(4 * c4 + j, px >> 2, 128) + (px & 3) * 4;
+    if (X3) {
+      *reinterpret_cast<float*>(hi + o) = tf32_hi(e[j]);
+      *reinterpret_cast<float*>(lo + o) = tf32_lo(e[j]);
     } else {
-      // ===================== epilogue: TMEM -> reductions into dW / dbias (4 warps, one lane quarter each)
-      const int q4 = warp & 3;                              // TMEM lane quarter == vertical tap r (quarter 3: bias row)
-      if (X3 == 1) {
-        // operand splitters until the last tile has been issued (then these warps run the epilogue as usual)
-        int stage = 0, phase = 0;
-        for (int t = t_begin; t < t_end; ++t) {
-          uint8_t* sb = tiles + (size_t)stage * p.stage_bytes;
-          mbar_wait(&full[stage], phase);
-          if (warp == 2) {
-            const float4* src = reinterpret_cast<const float4*>(sb + 3 * p.xbuf_bytes);
-            float4* dst = reinterpret_cast<float4*>(sb + 3 * p.xbuf_bytes + p.dy_bytes);
-            const int n = p.dy_bytes >> 4;
-#pragma unroll 4
-            for (int i = lane; i < n; i += 32) {
-              float4 v = src[i];
-              v.x = wg_tf32_lo(v.x); v.y = wg_tf32_lo(v.y); v.z = wg_tf32_lo(v.z); v.w = wg_tf32_lo(v.w);
-              dst[i] = v;
-            }
-            fence_proxy_async();
-            mbar_arrive(&ylo_ready[stage]);
-          } else {
-            mbar_wait(&hi_done[stage], phase);
-            float4* q = reinterpret_cast<float4*>(sb);
-            const int n = (3 * p.xbuf_bytes) >> 4;
-#pragma unroll 4
-            for (int i = (warp - 3) * 32 + lane; i < n; i += 96) {
-              float4 v = q[i];
-              v.x = wg_tf32_lo(v.x); v.y = wg_tf32_lo(v.y); v.z = wg_tf32_lo(v.z); v.w = wg_tf32_lo(v.w);
-              q[i] = v;
-            }
-            fence_proxy_async();
-            mbar_arrive(&lo_ready[stage]);
-          }
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
-      }
-      if (q4 < 3 || p.G == 4) {
-        mbar_wait(done, 0);
-        fence_after_sync();
-        const int ci = ci0 + lane;
-        const int ngrp = p.ncols / 16;
-        const int g_first = (q4 < 3) ? 0 : 3, g_last = (q4 < 3) ? 3 : 4;
-        for (int gi = g_first; gi < g_last; ++gi) {
-          const int g = (q4 < 3) ? (gi + blockIdx.x) % 3 : 3;          // stagger the CTAs over the taps ...
-          float* dst = nullptr;
-          if (g < 3) { if (ci < p.Cin) dst = p.dw + ((long long)(q4 * 3 + g) * p.Cin + ci) * p.Cout + co0; }
-          else if (lane == 0 && blockIdx.y == 0 && p.dbias) dst = p.dbias + co0;
-          for (int j = 0; j < ngrp; ++j) {
-            const int c0 = ((j + blockIdx.x) % ngrp) * 16;             // ... and over the columns
-            const bool col_ok = co0 + c0 < p.Cout;                     // columns past Cout come from zero-filled channels
-            uint32_t v[16];
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                  "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                : "r"(tmem_base + ((uint32_t)(q4 * 32) << 16) + g * p.ncols + c0)
-                : "memory");
-            tmem_ld_wait();
-            if (dst && col_ok && !(p.debug & 1)) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                float4 val = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                                         __uint_as_float(v[4 * q + 3]));
-                atomicAdd(reinterpret_cast<float4*>(dst + c0 + 4 * q), val);
-              }
-            }
-          }
-        }
-      }
+      *reinterpret_cast<float*>(hi + o) = e[j];
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, tmem_cols);
+}
+
+template <int BN, int X3>
+__global__ void __launch_bounds__(WG_THREADS, 1)
+conv_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dy, WgTcParams p) {
+  pdl_grid_sync();
+  constexpr int XQ = WG_PX * WG_MT / 4 / 128;        // float4 loads of X per thread and chunk (4)
+  constexpr int YQ = WG_PX * BN / 4 / 128;           // of dY (1..8)
+  constexpr int X_BYTES = WG_MT * 128, Y_BYTES = BN * 128;
+  constexpr int WG_BYTES = (X_BYTES + Y_BYTES) * (X3 ? 2 : 1);
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  uint8_t* sx = smem + wg * WG_BYTES;
+  uint8_t* sy = sx + X_BYTES;
+  uint8_t* sxl = sy + Y_BYTES;
+  uint8_t* syl = sxl + X_BYTES;
+
+  // rows m0.. of dW are (filter tap, input channel) pairs: narrow layers fill the 64-row tile with several taps
+  const int m0 = blockIdx.y * WG_MT, co0 = blockIdx.z * BN;
+  const bool do_bias = blockIdx.y == 0;
+  const long long split = 2LL * blockIdx.x + wg, T = (long long)p.KK * p.Cout;
+  // this thread's four rows (a channel quadruple of one tap: Cin % 4 == 0) and pixel slots (XQ / YQ of them) in a chunk
+  const int xc4 = t % (WG_MT / 4), xp0 = t / (WG_MT / 4);
+  const int yc4 = t % (BN / 4), yp0 = t / (BN / 4);
+  const int kk = m0 + 4 * xc4;
+  const bool xc_ok = kk < p.KK;
+  const int tap = kk / p.Cin, ci = kk - tap * p.Cin;
+  const int r = tap / p.kw, s = tap - r * p.kw;
+  const int hw = p.Ho * p.Wo;
+  const int c_begin = blockIdx.x * p.per_cta, c_end = min(p.chunks, c_begin + p.per_cta);
+
+  float4 xv[XQ], yv[YQ];
+  auto load = [&](int chunk) {
+#pragma unroll
+    for (int q = 0; q < XQ; ++q) {
+      const int g = chunk * WG_PX + xp0 + q * (128 / (WG_MT / 4));
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (g < p.npx && xc_ok) {
+        const int n = g / hw, rem = g - n * hw, ho = rem / p.Wo, wo = rem - ho * p.Wo;
+        const int hi = ho * p.stride + r - p.pad_t, wi = wo * p.stride + s - p.pad_l;
+        if (hi >= 0 && hi < p.H && wi >= 0 && wi < p.W)
+          v = __ldg(reinterpret_cast<const float4*>(x + (((long long)n * p.H + hi) * p.W + wi) * p.Cin + ci));
+      }
+      xv[q] = v;
+    }
+#pragma unroll
+    for (int q = 0; q < YQ; ++q) {
+      const int g = chunk * WG_PX + yp0 + q * (128 / (BN / 4));
+      yv[q] = g < p.npx ? __ldg(reinterpret_cast<const float4*>(dy + (long long)g * p.Cout + co0) + yc4)
+                        : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  };
+
+  // X3: each chunk's MMAs go into a fresh register tile that is then added into `acc` (see conv_tc.cu)
+  float acc[BN / 2], part[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
+  int c = c_begin + wg;
+  if (c < c_end) load(c);
+  int first = 1;
+  for (; c < c_end; c += 2) {
+#pragma unroll
+    for (int q = 0; q < XQ; ++q) put_t<X3>(sx, sxl, xc4, xp0 + q * (128 / (WG_MT / 4)), xv[q]);
+#pragma unroll
+    for (int q = 0; q < YQ; ++q) {
+      put_t<X3>(sy, syl, yc4, yp0 + q * (128 / (BN / 4)), yv[q]);
+      if (do_bias) { bsum.x += yv[q].x; bsum.y += yv[q].y; bsum.z += yv[q].z; bsum.w += yv[q].w; }
+    }
+    fence_proxy_async();                    // generic-proxy writes -> visible to the tensor core
+    named_bar_sync(1 + wg, 128);
+    if (c + 2 < c_end) load(c + 2);         // next chunk's loads overlap this chunk's MMAs
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < WG_PX / 8; ++ks) {
+      const uint64_t da = wgmma_desc(smem_u32(sx) + ks * 32, 128), db = wgmma_desc(smem_u32(sy) + ks * 32, 128);
+      if (X3) {
+        wgmma_tf32<BN>(part, da, db, ks > 0);
+        wgmma_tf32<BN>(part, da, wgmma_desc(smem_u32(syl) + ks * 32, 128), 1);
+        wgmma_tf32<BN>(part, wgmma_desc(smem_u32(sxl) + ks * 32, 128), db, 1);
+      } else {
+        wgmma_tf32<BN>(acc, da, db, first == 0 || ks > 0);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (X3) {
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+    }
+    named_bar_sync(1 + wg, 128);            // every warp's MMAs have read the tiles before they are rewritten
+    first = 0;
+  }
+  // this warpgroup's slice (zeros when it had no chunk): every element of the slices is written exactly once
+  float* dwt = p.ws ? p.ws + split * T : p.dw;
+#pragma unroll
+  for (int i = 0; i < BN / 2; i += 2) {
+    const int row = m0 + fragment_row(i, t), co = co0 + fragment_col(i, t);
+    if (row >= p.KK) continue;
+    float2* o = reinterpret_cast<float2*>(dwt + (long long)row * p.Cout + co);
+    if (p.ws) *o = make_float2(acc[i], acc[i + 1]);
+    else atomicAdd(o, make_float2(acc[i], acc[i + 1]));
+  }
+  if (do_bias) {
+    // the threads of one channel quadruple add their sums in thread order (the tiles are free: the loop ended on a barrier)
+    float4* sb = reinterpret_cast<float4*>(sx);
+    sb[t] = bsum;
+    named_bar_sync(1 + wg, 128);
+    if (t < BN / 4) {
+      float4 v = sb[t];
+      for (int k = t + BN / 4; k < 128; k += BN / 4) { v.x += sb[k].x; v.y += sb[k].y; v.z += sb[k].z; v.w += sb[k].w; }
+      if (p.ws) reinterpret_cast<float4*>(p.ws + 2LL * gridDim.x * T + split * p.Cout + co0)[t] = v;
+      else if (p.dbias) atomicAdd(reinterpret_cast<float4*>(p.dbias + co0) + t, v);
+    }
+  }
+}
+
+// dW[i] += sum over the slices in slice order; dbias likewise (when given)
+__global__ void __launch_bounds__(256)
+conv_wgrad_reduce_kernel(const float* __restrict__ ws, int splits, long long T, int Cout, float* __restrict__ dw,
+                         float* __restrict__ dbias) {
+  pdl_grid_sync();
+  const long long n = T + (dbias ? Cout : 0);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const bool b = i >= T;
+    const float* src = b ? ws + (long long)splits * T + (i - T) : ws + i;
+    const long long stride = b ? Cout : T;
+    float v = 0.f;
+    for (int k = 0; k < splits; ++k) v += src[k * stride];
+    if (b) dbias[i - T] += v;
+    else dw[i] += v;
+  }
+}
+
+// ---------------------------------------------------------------------------------------- host side
+template <int BN>
+static bool set_smem_limit() {
+  return cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess &&
+         cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess;
 }
 
 int init_conv_wgrad_tc() {
-  if (cudaFuncSetAttribute(conv_wgrad_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_wgrad_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-      init_conv_wgrad_pk() != SE_OK || init_conv1x1_wgrad_tc() != SE_OK) {
+  if (!set_smem_limit<16>() || !set_smem_limit<32>() || !set_smem_limit<64>() || !set_smem_limit<128>()) {
     set_error("init_conv_wgrad_tc: cannot raise the shared-memory limit");
     return SE_ERR_CUDA;
   }
   return SE_OK;
 }
 
-// Geometry + shared-memory plan; SE_OK when the tcgen05 path can run this layer.  `with_bias` adds the ones tile.
-// Co-residency with the backward-data kernel of the same layer (se_run_ops issues wgrad on a side stream): when two
-// pipeline stages fit in ~half of the SM's shared memory the kernel takes only those, and conv_tc.cu sizes the
-// dgrad kernel to the rest (conv_wgrad_tc_smem() is what it asks).
-constexpr int WG_COOP_SMEM = 120 * 1024;
-
-static int plan_wgrad(const se_conv_desc* d, bool with_bias, int x3, WgTcParams* pp, size_t* smem_out) {
-  if (d->kh != 3 || d->kw != 3 || d->stride != 1 || d->pad_t != 1 || d->pad_l != 1 || d->Ho != d->H || d->Wo != d->W)
-    return SE_ERR_UNSUPPORTED;
-  const int Cin = d->Cin, Cout = d->Cout, H = d->H;
-  if (Cin % 16 != 0 || Cout % 16 != 0) return SE_ERR_UNSUPPORTED;
-  // vertical taps are address offsets of r*W pixels: whole 1024-byte swizzle periods need a row pitch that is a multiple
-  // of 8 pixels -- image rows are loaded as boxes of W (pitch) >= d->W pixels, zero-filled past the image
-  if (d->W > 64 || d->W < 4) return SE_ERR_UNSUPPORTED;
-  static const bool no_pad = getenv("SE_CT_NO_PADDED") != nullptr;
-  int W = 8;
-  while (W < d->W) W <<= 1;
-  if (no_pad && (W != d->W)) return SE_ERR_UNSUPPORTED;
-  WgTcParams& p = *pp;
-  p.N = d->N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout;
-  p.G = with_bias ? 4 : 3;
-  // output channels per CTA: at most 128 (4 accumulators x 128 columns = the 512 TMEM columns), in 32-channel blocks
-  const int gz = ceil_div(Cout, 128);
-  p.nnb = ceil_div(ceil_div(Cout, gz), 32);
-  p.ncols = 32 * p.nnb;
-  p.PT = max(64, 2 * W);
-  int Hp = 1;
-  while (Hp < H) Hp <<= 1;
-  if (W * H >= p.PT || W * Hp >= p.PT) {
-    p.Hb = p.PT / W; p.Nb = 1; p.tpi = ceil_div(H, p.Hb);
-    if (no_pad && H % p.Hb != 0) return SE_ERR_UNSUPPORTED;
-  } else {
-    // whole images: Hp >= H row slots each (the rows past the image are zero-filled)
-    p.Hb = Hp; p.Nb = p.PT / (W * Hp); p.tpi = 1;
-    if (no_pad && Hp != H) return SE_ERR_UNSUPPORTED;
+int wgrad_workspace(long long floats, cudaStream_t st, float** ws) {
+  *ws = nullptr;
+  if (floats > WG_WS_FLOATS) return SE_OK;                      // direct mode
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) {
+    set_error("wgrad_workspace: no usable CUDA device");
+    return SE_ERR_CUDA;
   }
-  p.img_px = p.Hb * W;
-  p.img_stride = (p.Hb + 2) * W * 128;
-  p.xbuf_bytes = p.Nb * p.img_stride;
-  p.dy_bytes = p.PT * 128 * p.nnb;
-  p.stage_bytes = ceil_div(3 * p.xbuf_bytes + (1 + x3) * p.dy_bytes, 1024) * 1024;
-  const int fixed = (with_bias ? 1024 : 0) + 24 * 8 + 1024 + 64;
-  if (2 * p.stage_bytes + fixed <= WG_COOP_SMEM) p.stages = 2;
-  else p.stages = min(4, (200 * 1024) / p.stage_bytes);
-  if (p.stages < 1) return SE_ERR_UNSUPPORTED;
-  p.tiles_m = (p.Nb == 1) ? d->N * p.tpi : ceil_div(d->N, p.Nb);
-  *smem_out = (size_t)p.stages * p.stage_bytes + fixed;
+  std::lock_guard<std::mutex> lock(g_wg_mu);
+  for (int i = 0; i < g_wg_nws; ++i)
+    if (g_wg_ws[i].dev == dev && g_wg_ws[i].st == st) { *ws = g_wg_ws[i].ptr; return SE_OK; }
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (g_wg_nws == WG_MAX_WS || cudaStreamIsCapturing(st, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone)
+    return SE_OK;                                               // direct mode: no allocation inside a capture
+  float* ptr = nullptr;
+  if (cudaMalloc(&ptr, WG_WS_FLOATS * sizeof(float)) != cudaSuccess) {
+    set_error("wgrad_workspace: cannot allocate the %lld-byte weight-gradient workspace", WG_WS_FLOATS * 4);
+    return SE_ERR_CUDA;
+  }
+  g_wg_ws[g_wg_nws++] = {dev, st, ptr};
+  *ws = ptr;
   return SE_OK;
 }
 
-// dynamic shared memory the wgrad kernel of this layer will take, and its TMEM columns (0 when it cannot run)
-size_t conv_wgrad_tc_smem(const se_conv_desc* d, int* tmem_cols, int x3) {
-  WgTcParams p;
-  size_t smem = 0;
-  if (wgrad_is_packed(d, x3)) {
-    const size_t pk = conv_wgrad_pk_smem(d, tmem_cols);
-    if (pk > 0) return pk;                    // (0: a shape the packed kernel does not take -- the general kernel runs it)
-  }
-  if (plan_wgrad(d, true, x3, &p, &smem) != SE_OK) return 0;
-  int cols = 32;
-  while (cols < p.G * p.ncols) cols <<= 1;
-  if (tmem_cols) *tmem_cols = cols;
-  return smem;
+int wgrad_workspace_prepare(cudaStream_t st) {
+  float* ws = nullptr;
+  return wgrad_workspace(1, st, &ws);
 }
 
-// se_conv2d_path: would a tcgen05 weight-gradient kernel take the layer?
+long long wgrad_fit_splits(long long want, long long T, int Cout) {
+  const long long fit = WG_WS_FLOATS / (T + Cout);
+  return fit >= 1 ? std::min(want, fit) : want;               // not even one slice fits: direct mode, any split count
+}
+
+int wgrad_reduce(const float* ws, int splits, long long T, int Cout, float* dw, float* dbias, cudaStream_t st) {
+  const long long n = T + (dbias ? Cout : 0);
+  const long long blocks = std::min(ceil_div<long long>(n, 256), 4LL * sm_count());
+  launch(conv_wgrad_reduce_kernel, dim3((unsigned)blocks), dim3(256), 0, st, ws, splits, T, Cout, dw, dbias);
+  return check_launch("conv_wgrad_reduce_kernel");
+}
+
+// 1x1 convolutions (stride 1 or 2, no padding): two thirds of the layers of keras.applications.ResNet50 (reference
+// utils.py:237) and the shortcut projections of wide_residual_network.py:28
+static bool conv1x1_wgrad_tc_ok(const se_conv_desc* d) {
+  if (d->kh != 1 || d->kw != 1 || d->pad_t != 0 || d->pad_l != 0) return false;
+  if (d->stride == 2) {
+    if (d->Ho != (d->H + 1) / 2 || d->Wo != (d->W + 1) / 2 || d->Wo > 32) return false;
+  } else if (d->stride != 1 || d->Ho != d->H || d->Wo != d->W) {
+    return false;
+  }
+  return d->Cin % 4 == 0 && d->Cout % 16 == 0 && (long long)d->N * d->H * d->W >= 32 &&
+         (long long)d->N * d->H * d->W <= 0x7fffffffLL;
+}
+
+// 3x3 / stride 2 / no leading padding (the down-sampling layers of wide_residual_network.py:20-31 on even image sizes:
+// 'same' puts the one padding row / column AFTER the image).  Worth it for wide layers only; the 16..64-channel layers
+// of the CIFAR ResNets stay on the fp32 kernel.  conv_tc.cu runs their data gradient as nine strided 1x1 GEMMs.
+bool conv3x3s2_tc_ok(const se_conv_desc* d) {
+  return d->kh == 3 && d->kw == 3 && d->stride == 2 && d->pad_t == 0 && d->pad_l == 0 && d->H % 2 == 0 && d->W % 2 == 0 &&
+         d->Ho == d->H / 2 && d->Wo == d->W / 2 && d->Wo <= 32 && d->Wo >= 2 && d->Ho >= 2 && d->Cin >= 128 && d->Cout >= 128 &&
+         d->Cin % 16 == 0 && d->Cout % 32 == 0;
+}
+
+static bool conv3x3_wgrad_tc_ok(const se_conv_desc* d) {
+  return d->kh == 3 && d->kw == 3 && d->stride == 1 && d->pad_t == 1 && d->pad_l == 1 && d->Ho == d->H && d->Wo == d->W &&
+         d->Cin % 16 == 0 && d->Cout % 16 == 0 && d->W >= 4 && d->W <= 64;
+}
+
+// se_conv2d_path: would the tensor-core weight-gradient kernel take the layer?
 bool conv_wgrad_tc_would_run(const se_conv_desc* d, int x3) {
-  if (conv1x1_wgrad_tc_ok(d) || conv3x3s2_tc_ok(d)) return true;
-  if (wgrad_is_packed(d, x3) && conv_wgrad_pk_smem(d, nullptr) > 0) return true;
-  WgTcParams p;
-  size_t smem = 0;
-  return plan_wgrad(d, true, x3, &p, &smem) == SE_OK;
+  (void)x3;
+  return conv1x1_wgrad_tc_ok(d) || conv3x3s2_tc_ok(d) || conv3x3_wgrad_tc_ok(d);
+}
+
+template <int BN>
+static void wgrad_go(int x3, dim3 grid, cudaStream_t st, const float* x, const float* dy, const WgTcParams& p) {
+  const size_t smem = 1024 + 2 * (size_t)(WG_MT * 128 + BN * 128) * (x3 ? 2 : 1);
+  if (x3) launch(conv_wgrad_tc_kernel<BN, 1>, grid, dim3(WG_THREADS), smem, st, x, dy, p);
+  else launch(conv_wgrad_tc_kernel<BN, 0>, grid, dim3(WG_THREADS), smem, st, x, dy, p);
 }
 
 int conv_wgrad_tc(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias, int x3, cudaStream_t st) {
+  if (!conv_wgrad_tc_would_run(d, x3)) return SE_ERR_UNSUPPORTED;
   if ((reinterpret_cast<uintptr_t>(dw) & 15) != 0 || (dbias && (reinterpret_cast<uintptr_t>(dbias) & 15) != 0))
     return SE_ERR_UNSUPPORTED;
-  WgTcParams p;
-  size_t smem = 0;
   static bool inited = false;
   if (!inited) { int rc0 = init_conv_wgrad_tc(); if (rc0) return rc0; inited = true; }
-  if (conv1x1_wgrad_tc_ok(d)) return conv1x1_wgrad_tc(d, x, dy, dw, dbias, x3, st);
-  if (conv3x3s2_tc_ok(d)) return conv3x3s2_wgrad_tc(d, x, dy, dw, dbias, x3, st);
-  if (wgrad_is_packed(d, x3)) {
-    const int rc_pk = conv_wgrad_pk(d, x, dy, dw, dbias, st);
-    if (rc_pk != SE_ERR_UNSUPPORTED) return rc_pk;
-  }
-  int rc = plan_wgrad(d, dbias != nullptr, x3, &p, &smem);
-  if (rc != SE_OK) return rc;
-  const int Cin = d->Cin, Cout = d->Cout, W = d->W, H = d->H;
-  const int gz = ceil_div(Cout, 128);
+  const long long npx = (long long)d->N * d->Ho * d->Wo, KK = (long long)d->kh * d->kw * d->Cin;
+  if (npx > 0x7fffffffLL - 64 || KK > 0x7fffffffLL) return SE_ERR_UNSUPPORTED;
+  WgTcParams p;
+  p.N = d->N; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.Cout = d->Cout; p.Ho = d->Ho; p.Wo = d->Wo;
+  p.kw = d->kw; p.stride = d->stride; p.pad_t = d->pad_t; p.pad_l = d->pad_l;
+  p.KK = (int)KK;
+  p.npx = (int)npx;
+  p.chunks = (int)ceil_div<long long>(npx, WG_PX);
   p.dw = dw; p.dbias = dbias;
-  const uint32_t Wbox = (uint32_t)p.W;          // row pitch of the boxes (>= W)
-  static const char* dbg = getenv("SE_WG_DEBUG");
-  p.debug = dbg ? atoi(dbg) : 0;
-
-  CUtensorMap mx, mdy;
-  {
-    uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)d->N};
-    uint64_t strides[3] = {(uint64_t)Cin * 4, (uint64_t)W * Cin * 4, (uint64_t)H * W * Cin * 4};
-    uint32_t box[4] = {32u, Wbox, (uint32_t)(p.Hb + 2), (uint32_t)p.Nb};
-    if (!make_tmap(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(x), dims, strides, box,
-                   CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B))
-      return SE_ERR_CUDA;
-    uint64_t ydims[4] = {(uint64_t)Cout, (uint64_t)W, (uint64_t)H, (uint64_t)d->N};
-    uint64_t ystrides[3] = {(uint64_t)Cout * 4, (uint64_t)W * Cout * 4, (uint64_t)H * W * Cout * 4};
-    uint32_t ybox[4] = {32u, Wbox, (uint32_t)p.Hb, (uint32_t)p.Nb};
-    if (!make_tmap(&mdy, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(dy), ydims, ystrides, ybox,
-                   CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B))
-      return SE_ERR_CUDA;
+  int BN = x3 ? 64 : 128;                   // error-compensated mode: a second accumulator tile, see the kernel
+  while (d->Cout % BN != 0) BN >>= 1;
+  const int gy = (int)ceil_div<long long>(KK, WG_MT), gz = d->Cout / BN;
+  // about eight CTAs per SM over all row / column tiles, each with at least 4 chunks: a warpgroup's chunks are
+  // latency-bound round trips (load, transpose, MMA), so the pixel range is cut finely
+  long long gx = ceil_div<long long>(8LL * sm_count(), (long long)gy * gz);
+  gx = std::max(1LL, std::min(gx, ceil_div<long long>(p.chunks, 4)));
+  const long long T = KK * d->Cout;
+  gx = std::max(1LL, wgrad_fit_splits(2 * gx, T, d->Cout) / 2);      // the slices fit the workspace
+  int rc = wgrad_workspace(2 * gx * (T + d->Cout), st, &p.ws);
+  if (rc) return rc;
+  p.per_cta = (int)ceil_div<long long>(p.chunks, gx);
+  p.per_cta += p.per_cta & 1;
+  gx = ceil_div<long long>(p.chunks, p.per_cta);
+  if (gy > 65535 || gz > 65535) return SE_ERR_UNSUPPORTED;
+  const dim3 grid((unsigned)gx, (unsigned)gy, (unsigned)gz);
+  switch (BN) {
+    case 16: wgrad_go<16>(x3, grid, st, x, dy, p); break;
+    case 32: wgrad_go<32>(x3, grid, st, x, dy, p); break;
+    case 64: wgrad_go<64>(x3, grid, st, x, dy, p); break;
+    default: wgrad_go<128>(x3, grid, st, x, dy, p); break;
   }
-  const int gy = ceil_div(Cin, 32);
-  const int gx = max(1, min(p.tiles_m, sm_count() / (gy * gz)));
-  if (x3) launch(conv_wgrad_tc_kernel<1>, dim3(gx, gy, gz), dim3(192), smem, st, mx, mdy, p);
-  else launch(conv_wgrad_tc_kernel<0>, dim3(gx, gy, gz), dim3(192), smem, st, mx, mdy, p);
-  return check_launch("conv_wgrad_tc_kernel");
+  rc = check_launch("conv_wgrad_tc_kernel");
+  if (rc || !p.ws) return rc;
+  return wgrad_reduce(p.ws, (int)(2 * gx), T, d->Cout, dw, dbias, st);
 }
 
 }  // namespace se

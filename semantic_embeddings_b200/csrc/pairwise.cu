@@ -5,7 +5,7 @@
 // (SURVEY.md section 8d); the contraction must therefore be cheap enough to hide behind the
 // output stream.  Two arithmetic modes share the prep kernel below:
 //   SE_MODE_F32  : fp32 FFMA tiles (this file) -- exact-fp32 parity mode
-//   SE_MODE_TF32 : tcgen05 3xTF32 split (pairwise_tc.cu) -- tensor-pipe fast mode
+//   SE_MODE_TF32 : wgmma split-fp16 x3 (pairwise_tc.cu) -- tensor-pipe fast mode
 #include "common.cuh"
 
 namespace se {

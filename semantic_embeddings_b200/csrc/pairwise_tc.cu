@@ -1,20 +1,19 @@
-// All-pairs distance (evaluate_retrieval.py:56-63) on the 5th-gen tensor cores -- SE_MODE_TF32 path.
+// All-pairs distance (evaluate_retrieval.py:56-63) on the tensor cores -- SE_MODE_TF32 / SE_MODE_TF32X3 path.
 //
 // Arithmetic: "split-fp16 x3".  After a global power-of-two scaling that brings max|f| <= 1, every fp32
 // feature value f is split into h = fp16(f) and l = fp16(f - h) (11 + 11 significand bits, the low part
 // may be subnormal: absolute error <= 2^-25).  The fp32 product sum is recovered from three fp16 tensor-core
-// products accumulated in ONE fp32 TMEM accumulator:  F F^T ~= Fh Fh^T + Fh Fl^T + Fl Fh^T  (missing l*l term
-// <= 2^-24).  kind::f16 moves 2 bytes per element and runs at twice the TF32 rate, which is what keeps the
+// products accumulated in ONE fp32 accumulator:  F F^T ~= Fh Fh^T + Fh Fl^T + Fl Fh^T  (missing l*l term
+// <= 2^-24).  fp16 wgmma moves 2 bytes per element and runs at twice the TF32 rate, which is what keeps the
 // contraction hidden behind the fp32 output stream (4 bytes per pair -- the HBM roofline of this kernel).
 //
-// Structure (one persistent CTA per SM, 256 threads, warp-specialised):
-//   warp 0 : TMA producer -- A row block (128 rows, h and l, all K) stays RESIDENT while the CTA sweeps the
-//            column tiles; B tiles (256 rows) stream through a 2-stage ring, one 64-wide K block per stage
-//   warp 1 : single-thread tcgen05.mma issuer, M=128 N=256 K=16, accumulators double-buffered in TMEM (2 x 256 cols)
-//   warp 2 : TMEM allocator
-//   warps 4-11: epilogue -- warp w owns TMEM lanes 32*(w%4).. and one half of the 256 columns; per 32x32 block:
-//            tcgen05.ld, apply norms / sign, write a private swizzled 4 KB staging buffer, TMA store it
-//            (coalesced 128-byte rows; out-of-range rows/columns clipped by the tensor map).  No cross-warp barriers.
+// Structure (one persistent CTA per SM, 384 threads, warp-specialised):
+//   warpgroup 0 : one thread issues the TMA loads -- the A row block (128 rows, h and l, all K) stays RESIDENT while
+//                 the CTA sweeps the column tiles; B tiles (128 rows) stream through a 2-stage ring, one 64-wide K
+//                 block per stage
+//   warpgroups 1, 2 : each owns 64 rows of the 128 x 128 tile: m64n128k16 wgmma into registers, then the accumulator
+//                 goes through shared memory so that one thread holds one row of 32 columns at a time for the
+//                 epilogue (norms / sign, then a coalesced streaming store, or the ranking passes of the fused top-k)
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -24,27 +23,29 @@ namespace se {
 
 using namespace tc;
 
-constexpr int PW_BM = 128, PW_BN = 256, PW_KB = 64;     // K block = 64 halfs = 128 bytes (SWIZZLE_128B row)
+constexpr int PW_BM = 128, PW_BN = 128, PW_KB = 64;     // K block = 64 halfs = 128 bytes (SWIZZLE_128B row)
 constexpr int PW_MAXKB = 2;                              // resident A: at most 2 K blocks (D <= 128)
 constexpr int PW_STAGES = 2;
 constexpr int PW_A_BYTES = PW_BM * 128;                  // one K block of A (h or l): 16 KB
-constexpr int PW_B_BYTES = PW_BN * 128;                  // one K block of B (h or l): 32 KB
-constexpr int PW_EPI_WARPS = 8;
-constexpr int PW_OUT_BYTES = 32 * 128;                   // per-warp staging: 32 rows x 32 fp32 = 4 KB
-constexpr int PW_SMEM = 2 * PW_MAXKB * PW_A_BYTES + PW_STAGES * 2 * PW_B_BYTES + PW_EPI_WARPS * PW_OUT_BYTES + 1024 /*align*/ + 256;
+constexpr int PW_B_BYTES = PW_BN * 128;                  // one K block of B (h or l): 16 KB
+constexpr int PW_PITCH = PW_BN + 8;                      // accumulator staging row pitch (floats)
+constexpr int PW_THREADS = 384;
+constexpr int PW_SMEM = 2 * PW_MAXKB * PW_A_BYTES + PW_STAGES * 2 * PW_B_BYTES + PW_BM * PW_PITCH * 4 + 1024 /*align*/ + 256;
 
 struct PwParams {
   int N, row0, rows, pmode, tiles_m, tiles_n, kblocks, ksteps_total;
+  long long ldout;
+  float* out;
   const float* sq;       // squared norms of the (normalised) query rows, [N]
   const float* sq_b;     // squared norms of the column items (== sq for the all-pairs matrix; a sample's norms otherwise)
   const float* scal;     // scal[1] = 4^e: undoes the power-of-two input scaling
-  // fused ranking (se_pairwise_topk).  EPI == 2, sample pass: every (row, 128-column half tile) adds the SECOND smallest of
-  // its 128 distances to tau_sum[row] -- the mean of those order statistics (quantile ~2/129 of the row) is the row's
-  // candidate threshold.  EPI == 1, sweep: entries below the threshold become (value, column) candidates in the region
-  // of the writing (row, column half, part of the row block) -- a lane owns its row for the CTA's whole stretch of the
-  // row block, so the fill count lives in a register and no atomics are needed.
+  // fused ranking (se_pairwise_topk).  EPI == 2, sample pass: every (row, 64-column half tile with >= 8 columns) adds the
+  // j-th smallest of its distances to tau_sum[row] -- the mean of those order statistics is the row's candidate threshold.  EPI == 1,
+  // sweep: entries below the threshold become (value, column) candidates in the region of the writing (row, column
+  // half, part of the row block) -- a thread owns its row for the CTA's whole stretch of the row block, so the fill
+  // count lives in a register and no atomics are needed.
   float* tau_sum;        // [rows]   EPI 2: accumulates; EPI 1: threshold = tau_sum[row] * tau_scale
-  float tau_scale;       // 1 / (number of half tiles of the sample pass)
+  float tau_scale;       // 1 / (number of half tiles of the sample pass with >= 8 columns)
   int* cnt;              // [rows, 4] candidates per region (may exceed capr: the finishing kernel reports it)
   float* cand_val;       // [rows, 4, capr]
   int* cand_idx;         // [rows, 4, capr]
@@ -91,241 +92,211 @@ pairwise_split_kernel(const float* __restrict__ F, int ldF, int N, int D, int KW
 
 // ---- main kernel
 // map_h / map_l: split operands of the query rows (A); map_bh / map_bl: of the column items (B; the same arrays for the
-// all-pairs matrix).  EPI 0: distances out through map_out; EPI 1: thresholded candidates (fused ranking).
+// all-pairs matrix).  EPI 0: distances to p.out; EPI 1: thresholded candidates; EPI 2: threshold sample (fused ranking).
 template <int EPI>
-__global__ void __launch_bounds__(128 + 32 * PW_EPI_WARPS, 1)
+__global__ void __launch_bounds__(PW_THREADS, 1)
 pairwise_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l,
-                   const __grid_constant__ CUtensorMap map_bh, const __grid_constant__ CUtensorMap map_bl,
-                   const __grid_constant__ CUtensorMap map_out, PwParams p) {
+                   const __grid_constant__ CUtensorMap map_bh, const __grid_constant__ CUtensorMap map_bl, PwParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sA = smem;                                            // [h|l][kb] x 16 KB
-  uint8_t* sB = sA + 2 * PW_MAXKB * PW_A_BYTES;                  // [stage][h|l] x 32 KB
-  uint8_t* sOut = sB + PW_STAGES * 2 * PW_B_BYTES;               // [PW_EPI_WARPS] x 4 KB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sOut + PW_EPI_WARPS * PW_OUT_BYTES);
+  uint8_t* sB = sA + 2 * PW_MAXKB * PW_A_BYTES;                  // [stage][h|l] x 16 KB
+  float* sAcc = reinterpret_cast<float*>(sB + PW_STAGES * 2 * PW_B_BYTES);   // [128 rows][PW_PITCH]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + PW_BM * PW_PITCH);
   uint64_t* full = bars;                 // [PW_STAGES]
   uint64_t* empty = bars + PW_STAGES;    // [PW_STAGES]
   uint64_t* a_full = bars + 2 * PW_STAGES;
   uint64_t* a_empty = a_full + 1;
-  uint64_t* t_full = a_empty + 1;        // [2]
-  uint64_t* t_empty = t_full + 2;        // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
 
-  const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
+  const int tid = threadIdx.x;
   const int total_tiles = p.tiles_m * p.tiles_n;
   const int per_cta = (total_tiles + gridDim.x - 1) / gridDim.x;
   const int t_begin = blockIdx.x * per_cta;
   const int t_end = min(total_tiles, t_begin + per_cta);
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&map_h); prefetch_tmap(&map_l); prefetch_tmap(&map_bh); prefetch_tmap(&map_bl); prefetch_tmap(&map_out);
-    for (int s = 0; s < PW_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(a_full, 1); mbar_init(a_empty, 1);
-    for (int a = 0; a < 2; ++a) { mbar_init(&t_full[a], 1); mbar_init(&t_empty[a], 32 * PW_EPI_WARPS); }
+  if (tid == 0) {
+    prefetch_tmap(&map_h); prefetch_tmap(&map_l); prefetch_tmap(&map_bh); prefetch_tmap(&map_bl);
+    for (int s = 0; s < PW_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+    mbar_init(a_full, 1); mbar_init(a_empty, 8);
     fence_barrier_init();
-    fence_proxy_async();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);   // provably warp-uniform (see tc.cuh elect_one)
   pdl_wait();                               // nothing above touches global memory (see common.cuh)
 
-  if (warp == 0 && elect_one()) {
+  if (tid < 128) {
     // ===================== TMA producer
-    int stage = 0, phase = 0, cur_tm = -1, a_phase = 0;
-    // the split operands (2 x 11 MB at N = 50 000) are re-read by every CTA for every row block: keep them in L2 while
-    // the 10 GB output streams through (measured without the hint: 856 MB of DRAM reads for the 22 MB operands)
-    const uint64_t keep = l2_policy_evict_last();
-    for (int t = t_begin; t < t_end; ++t) {
-      const int tm = t / p.tiles_n, tn = t % p.tiles_n;
-      if (tm != cur_tm) {
-        if (cur_tm >= 0) { mbar_wait(a_empty, a_phase); a_phase ^= 1; }   // MMAs reading the old A have retired
-        mbar_expect_tx(a_full, 2 * p.kblocks * PW_A_BYTES);
+    if (tid == 0) {
+      int stage = 0, phase = 0, cur_tm = -1, a_phase = 0;
+      // the split operands (2 x 11 MB at N = 50 000) are re-read by every CTA for every row block: keep them in L2 while
+      // the output streams through
+      const uint64_t keep = l2_policy_evict_last();
+      for (int t = t_begin; t < t_end; ++t) {
+        const int tm = t / p.tiles_n, tn = t % p.tiles_n;
+        if (tm != cur_tm) {
+          if (cur_tm >= 0) { mbar_wait(a_empty, a_phase); a_phase ^= 1; }   // MMAs reading the old A have retired
+          mbar_expect_tx(a_full, 2 * p.kblocks * PW_A_BYTES);
+          for (int kb = 0; kb < p.kblocks; ++kb) {
+            tma_load_2d_hint(sA + (0 * PW_MAXKB + kb) * PW_A_BYTES, &map_h, a_full, kb * PW_KB, p.row0 + tm * PW_BM, keep);
+            tma_load_2d_hint(sA + (1 * PW_MAXKB + kb) * PW_A_BYTES, &map_l, a_full, kb * PW_KB, p.row0 + tm * PW_BM, keep);
+          }
+          cur_tm = tm;
+        }
         for (int kb = 0; kb < p.kblocks; ++kb) {
-          tma_load_2d_hint(sA + (0 * PW_MAXKB + kb) * PW_A_BYTES, &map_h, a_full, kb * PW_KB, p.row0 + tm * PW_BM, keep);
-          tma_load_2d_hint(sA + (1 * PW_MAXKB + kb) * PW_A_BYTES, &map_l, a_full, kb * PW_KB, p.row0 + tm * PW_BM, keep);
+          mbar_wait(&empty[stage], phase ^ 1);
+          mbar_expect_tx(&full[stage], 2 * PW_B_BYTES);
+          tma_load_2d_hint(sB + (stage * 2 + 0) * PW_B_BYTES, &map_bh, &full[stage], kb * PW_KB, tn * PW_BN, keep);
+          tma_load_2d_hint(sB + (stage * 2 + 1) * PW_B_BYTES, &map_bl, &full[stage], kb * PW_KB, tn * PW_BN, keep);
+          if (++stage == PW_STAGES) { stage = 0; phase ^= 1; }
         }
-        cur_tm = tm;
-      }
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        mbar_wait(&empty[stage], phase ^ 1);
-        mbar_expect_tx(&full[stage], 2 * PW_B_BYTES);
-        uint8_t* bh = sB + (stage * 2 + 0) * PW_B_BYTES;
-        uint8_t* bl = sB + (stage * 2 + 1) * PW_B_BYTES;
-        tma_load_2d_hint(bh, &map_bh, &full[stage], kb * PW_KB, tn * PW_BN, keep);
-        tma_load_2d_hint(bh + PW_A_BYTES, &map_bh, &full[stage], kb * PW_KB, tn * PW_BN + 128, keep);
-        tma_load_2d_hint(bl, &map_bl, &full[stage], kb * PW_KB, tn * PW_BN, keep);
-        tma_load_2d_hint(bl + PW_A_BYTES, &map_bl, &full[stage], kb * PW_KB, tn * PW_BN + 128, keep);
-        if (++stage == PW_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1 && elect_one()) {
-    // ===================== MMA issuer (one thread)
-    constexpr uint32_t idesc = umma_idesc(0 /*f16*/, PW_BM, PW_BN);
-    int stage = 0, phase = 0, cur_tm = -1, a_phase = 0, acc = 0, acc_phase = 0;
-    for (int t = t_begin; t < t_end; ++t) {
-      const int tm = t / p.tiles_n;
-      if (tm != cur_tm) { mbar_wait(a_full, a_phase); a_phase ^= 1; cur_tm = tm; }
-      mbar_wait(&t_empty[acc], acc_phase ^ 1);          // epilogue has drained this accumulator
-      fence_after_sync();
-      const uint32_t d_tmem = tmem_base + acc * PW_BN;
-      int ks_done = 0;
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        mbar_wait(&full[stage], phase);
-        fence_after_sync();
-        const uint32_t ah = smem_u32(sA + (0 * PW_MAXKB + kb) * PW_A_BYTES);
-        const uint32_t al = smem_u32(sA + (1 * PW_MAXKB + kb) * PW_A_BYTES);
-        const uint32_t bh = smem_u32(sB + (stage * 2 + 0) * PW_B_BYTES);
-        const uint32_t bl = smem_u32(sB + (stage * 2 + 1) * PW_B_BYTES);
-        const int nks = min(PW_KB / 16, p.ksteps_total - ks_done);
-        for (int ks = 0; ks < nks; ++ks) {
-          const uint32_t off = ks * 32;                 // 16 halfs = 32 bytes inside the 128-byte swizzled row
-          const uint64_t dah = umma_desc_kmajor(ah + off, 1024, 128), dal = umma_desc_kmajor(al + off, 1024, 128);
-          const uint64_t dbh = umma_desc_kmajor(bh + off, 1024, 128), dbl = umma_desc_kmajor(bl + off, 1024, 128);
-          // the two products with B_h back to back (consecutive MMAs with the same B operand: the 8 KB B slab is not
-          // staged twice), then the one with B_l
-          mma_f16(d_tmem, dah, dbh, idesc, (ks_done + ks) > 0 ? 1u : 0u);
-          mma_f16(d_tmem, dal, dbh, idesc, 1u);
-          mma_f16(d_tmem, dah, dbl, idesc, 1u);
-        }
-        ks_done += nks;
-        mma_commit(&empty[stage]);                      // frees the B stage once these MMAs retire
-        if (++stage == PW_STAGES) { stage = 0; phase ^= 1; }
-      }
-      mma_commit(&t_full[acc]);                         // accumulator complete -> epilogue
-      const bool last_of_row = (t + 1 == t_end) || ((t + 1) / p.tiles_n != tm);
-      if (last_of_row) mma_commit(a_empty);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue (8 warps)
-    const int q4 = warp & 3;                            // TMEM lane quarter this warp may read
-    const int half = (warp - 4) >> 2;                   // which 128-column half of the tile
-    uint8_t* ob = sOut + (warp - 4) * PW_OUT_BYTES;
-    const float s2 = p.scal[1];
-    const uint64_t stream_out = l2_policy_evict_first();   // the distances are written once and not read by this kernel
-    constexpr int CHUNKS = PW_BN / 2 / 32;              // 4 blocks of 32 columns per warp and tile
-    int acc = 0, acc_phase = 0;
-    int e_tm = -1, e_pos = 0, e_region = 0;              // EPI 1: row block / fill count / region of this lane's candidates
-    for (int t = t_begin; t < t_end; ++t) {
-      const int tm = t / p.tiles_n, tn = t % p.tiles_n;
-      const int r_local = q4 * 32 + lane;               // row inside the tile == TMEM lane
-      const int gi = p.row0 + tm * PW_BM + r_local;
-      const float a_sq = p.sq[gi];                      // (rows past N read workspace padding; clipped at the store)
-      // squared norms of this warp's 128 columns: lane i keeps columns 4i..4i+3, handed out by shuffles below
-      // (issued before the accumulator wait so that the L2 latency is off the critical path)
-      const float4 sqv = __ldg(reinterpret_cast<const float4*>(p.sq_b + tn * PW_BN + half * (PW_BN / 2)) + lane);
-      const int lrow = tm * PW_BM + r_local;             // row inside this call's row range
-      const bool row_ok = lrow < p.rows;
-      float tau = 0.f;
-      if (EPI == 1) {
-        tau = row_ok ? p.tau_sum[lrow] * p.tau_scale : 0.f;
-        if (tm != e_tm) {                                // a new row block: flush the previous block's fill count
-          if (e_tm >= 0 && e_tm * PW_BM + r_local < p.rows) p.cnt[(long long)(e_tm * PW_BM + r_local) * 4 + e_region] = e_pos;
-          e_tm = tm; e_pos = 0;
-          e_region = half * 2 + ((t_begin > tm * p.tiles_n) ? 1 : 0);
-        }
-      }
-      float ms[8];                                         // EPI 2: the eight smallest distances of this half tile, ascending
-#pragma unroll
-      for (int i = 0; i < 8; ++i) ms[i] = 3.0e38f;
-      mbar_wait(&t_full[acc], acc_phase);
-      fence_after_sync();
-      for (int c = 0; c < CHUNKS; ++c) {
-        const int col = half * (PW_BN / 2) + c * 32;
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(q4 * 32) << 16) + acc * PW_BN + col, v);
-        tmem_ld_wait();
-        if (c == CHUNKS - 1) {                          // this warp is done with the accumulator
-          fence_before_sync();
-          mbar_arrive(&t_empty[acc]);
-        }
-        const int j0 = tn * PW_BN + col;
-        float4 o[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const int src = c * 8 + q;
-          const float bx = __shfl_sync(0xffffffffu, sqv.x, src), by = __shfl_sync(0xffffffffu, sqv.y, src);
-          const float bz = __shfl_sync(0xffffffffu, sqv.z, src), bw = __shfl_sync(0xffffffffu, sqv.w, src);
-          float c0 = __uint_as_float(v[4 * q + 0]) * s2, c1 = __uint_as_float(v[4 * q + 1]) * s2;
-          float c2 = __uint_as_float(v[4 * q + 2]) * s2, c3 = __uint_as_float(v[4 * q + 3]) * s2;
-          if (p.pmode == SE_PDIST_NEGDOT) {
-            o[q] = make_float4(-c0, -c1, -c2, -c3);
-          } else {
-            o[q] = make_float4((a_sq + bx) - 2.f * c0, (a_sq + by) - 2.f * c1, (a_sq + bz) - 2.f * c2, (a_sq + bw) - 2.f * c3);
-          }
-        }
-        if (EPI == 1) {
-          // branch-free pass mask (bit i = column j0 + i is a candidate), then the few set bits are handled one by one;
-          // the values are parked in this warp's staging rows so that the rare path can fetch entry i by index
-          unsigned mask = 0;
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            mask |= (o[q].x < tau ? 1u : 0u) << (4 * q) | (o[q].y < tau ? 1u : 0u) << (4 * q + 1) |
-                    (o[q].z < tau ? 1u : 0u) << (4 * q + 2) | (o[q].w < tau ? 1u : 0u) << (4 * q + 3);
-          }
-          const int nvalid = p.ncols - j0;                   // columns of this block inside the matrix
-          if (nvalid < 32) mask &= nvalid > 0 ? ((1u << nvalid) - 1u) : 0u;
-          if (!row_ok) mask = 0;
-          if (__any_sync(0xffffffffu, mask != 0)) {
-            float* rowbuf = reinterpret_cast<float*>(ob + lane * 128);
-#pragma unroll
-            for (int q = 0; q < 8; ++q) *reinterpret_cast<float4*>(rowbuf + 4 * q) = o[q];     // own row only: no sync needed
-            float* cv = p.cand_val + ((long long)lrow * 4 + e_region) * p.capr;
-            int* ci = p.cand_idx + ((long long)lrow * 4 + e_region) * p.capr;
-            while (mask) {
-              const int i = __ffs(mask) - 1;
-              mask &= mask - 1;
-              if (e_pos < p.capr) { cv[e_pos] = rowbuf[i]; ci[e_pos] = j0 + i; }
-              ++e_pos;
-            }
-          }
-          continue;
-        }
-        if (EPI == 2) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float vv[4] = {o[q].x, o[q].y, o[q].z, o[q].w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              float x = (j0 + 4 * q + e < p.ncols) ? vv[e] : 3.0e38f;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) { const float lo = fminf(ms[i], x); x = fmaxf(ms[i], x); ms[i] = lo; }
-            }
-          }
-          if (c == CHUNKS - 1 && row_ok) {
-            float sel = ms[0];
-#pragma unroll
-            for (int i = 1; i < 8; ++i) if (i == p.jsel) sel = ms[i];
-            atomicAdd(&p.tau_sum[lrow], sel);
-          }
-          continue;
-        }
-        if (lane == 0) tma_store_wait_read<0>();        // the previous store of this warp has read the buffer
-        __syncwarp();
-        // SWIZZLE_128B staging: 16-byte chunk q of row r lives at chunk (q ^ (r & 7))
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          *reinterpret_cast<float4*>(ob + lane * 128 + ((q ^ (lane & 7)) << 4)) = o[q];
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d_hint(&map_out, ob, j0, tm * PW_BM + q4 * 32, stream_out);
-          tma_store_commit();
-        }
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-    if (EPI == 1 && e_tm >= 0 && e_tm * PW_BM + (q4 * 32 + lane) < p.rows)
-      p.cnt[(long long)(e_tm * PW_BM + q4 * 32 + lane) * 4 + e_region] = e_pos;
-    if (lane == 0) tma_store_wait_all<0>();
+    return;
   }
 
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
+  // ===================== consumers
+  const int wg = (tid >> 7) - 1, tid_wg = tid & 127, lane = tid & 31, wq = tid_wg >> 5;
+  const int half = wq >> 1;                               // which 64-column half of the tile this warp's epilogue covers
+  const int r_local = wg * 64 + (wq & 1) * 32 + lane;     // the row this thread owns in the epilogue
+  float* myrow = sAcc + r_local * PW_PITCH;
+  const float s2 = p.scal[1];
+  int stage = 0, phase = 0, cur_tm = -1, a_phase = 0;
+  int e_tm = -1, e_pos = 0, e_region = 0;                 // EPI 1: row block / fill count / region of this thread's candidates
+  for (int t = t_begin; t < t_end; ++t) {
+    const int tm = t / p.tiles_n, tn = t % p.tiles_n;
+    if (tm != cur_tm) { mbar_wait(a_full, a_phase); a_phase ^= 1; cur_tm = tm; }
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    int ks_done = 0;
+    for (int kb = 0; kb < p.kblocks; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t ah = smem_u32(sA + (0 * PW_MAXKB + kb) * PW_A_BYTES) + wg * 64 * 128;
+      const uint32_t al = smem_u32(sA + (1 * PW_MAXKB + kb) * PW_A_BYTES) + wg * 64 * 128;
+      const uint32_t bh = smem_u32(sB + (stage * 2 + 0) * PW_B_BYTES);
+      const uint32_t bl = smem_u32(sB + (stage * 2 + 1) * PW_B_BYTES);
+      const int nks = min(PW_KB / 16, p.ksteps_total - ks_done);
+      wgmma_fence();
+      for (int ks = 0; ks < nks; ++ks) {
+        const uint32_t off = ks * 32;                 // 16 halfs = 32 bytes inside the 128-byte swizzled row
+        const uint64_t dah = wgmma_desc(ah + off, 128), dal = wgmma_desc(al + off, 128);
+        const uint64_t dbh = wgmma_desc(bh + off, 128), dbl = wgmma_desc(bl + off, 128);
+        wgmma_f16_n128(acc, dah, dbh, (ks_done + ks) > 0 ? 1 : 0);
+        wgmma_f16_n128(acc, dal, dbh, 1);
+        wgmma_f16_n128(acc, dah, dbl, 1);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      ks_done += nks;
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[stage]);      // frees the B stage
+      if (++stage == PW_STAGES) { stage = 0; phase ^= 1; }
+    }
+    const bool last_of_row = (t + 1 == t_end) || ((t + 1) / p.tiles_n != tm);
+    if (last_of_row && lane == 0) mbar_arrive(a_empty);
+    // accumulator -> shared memory (this warpgroup's 64 rows), then one row per thread
+#pragma unroll
+    for (int i = 0; i < 64; i += 2)
+      *reinterpret_cast<float2*>(sAcc + (wg * 64 + fragment_row(i, tid_wg)) * PW_PITCH + fragment_col(i, tid_wg)) =
+          make_float2(acc[i], acc[i + 1]);
+    named_bar_sync(1 + wg, 128);
+
+    const int gi = p.row0 + tm * PW_BM + r_local;
+    const float a_sq = p.sq[gi];                      // (rows past N read workspace padding; never stored)
+    const int lrow = tm * PW_BM + r_local;            // row inside this call's row range
+    const bool row_ok = lrow < p.rows;
+    float tau = 0.f;
+    if (EPI == 1) {
+      tau = row_ok ? p.tau_sum[lrow] * p.tau_scale : 0.f;
+      if (tm != e_tm) {                                // a new row block: flush the previous block's fill count
+        if (e_tm >= 0 && e_tm * PW_BM + r_local < p.rows) p.cnt[(long long)(e_tm * PW_BM + r_local) * 4 + e_region] = e_pos;
+        e_tm = tm; e_pos = 0;
+        e_region = half * 2 + ((t_begin > tm * p.tiles_n) ? 1 : 0);
+      }
+    }
+    float ms[8];                                       // EPI 2: the eight smallest distances of this half tile, ascending
+#pragma unroll
+    for (int i = 0; i < 8; ++i) ms[i] = 3.0e38f;
+    for (int c = 0; c < 2; ++c) {
+      const int col = half * (PW_BN / 2) + c * 32;
+      const int j0 = tn * PW_BN + col;
+      float4 o[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const float4 v = *reinterpret_cast<const float4*>(myrow + col + 4 * q);
+        const float4 b = __ldg(reinterpret_cast<const float4*>(p.sq_b + j0) + q);
+        const float c0 = v.x * s2, c1 = v.y * s2, c2 = v.z * s2, c3 = v.w * s2;
+        if (p.pmode == SE_PDIST_NEGDOT) o[q] = make_float4(-c0, -c1, -c2, -c3);
+        else o[q] = make_float4((a_sq + b.x) - 2.f * c0, (a_sq + b.y) - 2.f * c1, (a_sq + b.z) - 2.f * c2, (a_sq + b.w) - 2.f * c3);
+      }
+      if (EPI == 1) {
+        // branch-free pass mask (bit i = column j0 + i is a candidate), then the few set bits are handled one by one
+        unsigned mask = 0;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          mask |= (o[q].x < tau ? 1u : 0u) << (4 * q) | (o[q].y < tau ? 1u : 0u) << (4 * q + 1) |
+                  (o[q].z < tau ? 1u : 0u) << (4 * q + 2) | (o[q].w < tau ? 1u : 0u) << (4 * q + 3);
+        }
+        const int nvalid = p.ncols - j0;                   // columns of this block inside the matrix
+        if (nvalid < 32) mask &= nvalid > 0 ? ((1u << nvalid) - 1u) : 0u;
+        if (!row_ok) mask = 0;
+        if (mask) {
+#pragma unroll
+          for (int q = 0; q < 8; ++q) *reinterpret_cast<float4*>(myrow + col + 4 * q) = o[q];     // own row only
+          float* cv = p.cand_val + ((long long)lrow * 4 + e_region) * p.capr;
+          int* ci = p.cand_idx + ((long long)lrow * 4 + e_region) * p.capr;
+          while (mask) {
+            const int i = __ffs(mask) - 1;
+            mask &= mask - 1;
+            if (e_pos < p.capr) { cv[e_pos] = myrow[col + i]; ci[e_pos] = j0 + i; }
+            ++e_pos;
+          }
+        }
+        continue;
+      }
+      if (EPI == 2) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const float vv[4] = {o[q].x, o[q].y, o[q].z, o[q].w};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            float x = (j0 + 4 * q + e < p.ncols) ? vv[e] : 3.0e38f;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) { const float lo = fminf(ms[i], x); x = fmaxf(ms[i], x); ms[i] = lo; }
+          }
+        }
+        if (c == 1 && row_ok && p.ncols - (tn * PW_BN + half * (PW_BN / 2)) >= 8) {   // half tiles with >= 8 columns
+          float sel = ms[0];
+#pragma unroll
+          for (int i = 1; i < 8; ++i) if (i == p.jsel) sel = ms[i];
+          atomicAdd(&p.tau_sum[lrow], sel);
+        }
+        continue;
+      }
+      // EPI 0: back into this thread's row, then the warp stores its 32 rows x 32 columns with coalesced 128-byte rows
+#pragma unroll
+      for (int q = 0; q < 8; ++q) *reinterpret_cast<float4*>(myrow + col + 4 * q) = o[q];
+      __syncwarp();
+      const int rbase = r_local - lane;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int rr = rbase + 4 * i + (lane >> 3), cc = col + 4 * (lane & 7);
+        const int orow = tm * PW_BM + rr, ocol = tn * PW_BN + cc;
+        if (orow >= p.rows || ocol >= p.ncols) continue;
+        const float4 v = *reinterpret_cast<const float4*>(sAcc + rr * PW_PITCH + cc);
+        float* dst = p.out + (long long)orow * p.ldout + ocol;
+        if (ocol + 4 <= p.ncols) {
+          __stcs(reinterpret_cast<float4*>(dst), v);
+        } else {
+          const float e[4] = {v.x, v.y, v.z, v.w};
+          for (int k = 0; k < p.ncols - ocol; ++k) __stcs(dst + k, e[k]);
+        }
+      }
+      __syncwarp();
+    }
+    named_bar_sync(1 + wg, 128);                      // the staging rows are free for the next tile
+  }
+  if (EPI == 1 && e_tm >= 0 && e_tm * PW_BM + r_local < p.rows) p.cnt[(long long)(e_tm * PW_BM + r_local) * 4 + e_region] = e_pos;
 }
 
 // ---- host side
@@ -381,8 +352,8 @@ struct PwEpi { int kind; float* tau_sum; float tau_scale; int* cnt; float* cand_
 // rows [row0, row0+rows) of the N query items against `ncols` column items given by (Bh, Bl, sq_b)
 static int pw_launch(const PwLayout& L, int N, int row0, int rows, const __half* Bh, const __half* Bl, const float* sq_b,
                      int ncols, int pmode, float* out, long long ldout, const PwEpi* e1, cudaStream_t st) {
-  if (!e1 && ((ldout % 4) != 0 || (reinterpret_cast<uintptr_t>(out) & 15) != 0)) return SE_ERR_UNSUPPORTED;  // TMA store alignment
-  CUtensorMap mh, ml, mbh, mbl, mo;
+  if (!e1 && ((ldout % 4) != 0 || (reinterpret_cast<uintptr_t>(out) & 15) != 0)) return SE_ERR_UNSUPPORTED;  // 16-byte stores
+  CUtensorMap mh, ml, mbh, mbl;
   {
     uint64_t dims[2] = {(uint64_t)L.KW, (uint64_t)N};
     uint64_t strides[1] = {(uint64_t)L.KW * 2};
@@ -394,19 +365,12 @@ static int pw_launch(const PwLayout& L, int N, int row0, int rows, const __half*
     if (!make_tmap(&mbh, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(Bh), bdims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B) ||
         !make_tmap(&mbl, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(Bl), bdims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
       return SE_ERR_CUDA;
-    mo = mh;
-    if (!e1) {
-      uint64_t odims[2] = {(uint64_t)ncols, (uint64_t)rows};
-      uint64_t ostrides[1] = {(uint64_t)ldout * 4};
-      uint32_t obox[2] = {32, 32};
-      if (!make_tmap(&mo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, out, odims, ostrides, obox, CU_TENSOR_MAP_SWIZZLE_128B))
-        return SE_ERR_CUDA;
-    }
   }
   PwParams p;
   p.N = N; p.row0 = row0; p.rows = rows; p.pmode = pmode;
   p.tiles_m = ceil_div(rows, PW_BM); p.tiles_n = ceil_div(ncols, PW_BN);
   p.kblocks = L.kblocks; p.ksteps_total = L.KW / 16;
+  p.out = out; p.ldout = ldout;
   p.sq = L.sq; p.sq_b = sq_b; p.scal = L.scal; p.ncols = ncols;
   p.tau_sum = nullptr; p.tau_scale = 0.f; p.cnt = nullptr; p.cand_val = nullptr; p.cand_idx = nullptr; p.capr = 0; p.jsel = 1;
   if (e1) { p.jsel = e1->jsel; p.tau_sum = e1->tau_sum; p.tau_scale = e1->tau_scale; p.cnt = e1->cnt; p.cand_val = e1->cand_val; p.cand_idx = e1->cand_idx; p.capr = e1->capr; }
@@ -415,9 +379,9 @@ static int pw_launch(const PwLayout& L, int N, int row0, int rows, const __half*
   int grid = min(sm_count(), p.tiles_m * p.tiles_n);
   // candidate sweep: a row block may be shared by at most two CTAs (regions are per (row, column half, part))
   if (e1 && e1->kind == 1) grid = max(1, min(grid, p.tiles_m));
-  if (e1 && e1->kind == 1) launch(pairwise_tc_kernel<1>, dim3(grid), dim3(128 + 32 * PW_EPI_WARPS), PW_SMEM, st, mh, ml, mbh, mbl, mo, p);
-  else if (e1) launch(pairwise_tc_kernel<2>, dim3(grid), dim3(128 + 32 * PW_EPI_WARPS), PW_SMEM, st, mh, ml, mbh, mbl, mo, p);
-  else launch(pairwise_tc_kernel<0>, dim3(grid), dim3(128 + 32 * PW_EPI_WARPS), PW_SMEM, st, mh, ml, mbh, mbl, mo, p);
+  if (e1 && e1->kind == 1) launch(pairwise_tc_kernel<1>, dim3(grid), dim3(PW_THREADS), PW_SMEM, st, mh, ml, mbh, mbl, p);
+  else if (e1) launch(pairwise_tc_kernel<2>, dim3(grid), dim3(PW_THREADS), PW_SMEM, st, mh, ml, mbh, mbl, p);
+  else launch(pairwise_tc_kernel<0>, dim3(grid), dim3(PW_THREADS), PW_SMEM, st, mh, ml, mbh, mbl, p);
   return check_launch("pairwise_tc_kernel");
 }
 
@@ -431,9 +395,9 @@ int pairwise_tc(const float* F, int ldF, int N, int D, int row0, int rows, int p
 
 // ---------------------------------------------------------------------------------------- fused distance + top-k
 // SURVEY.md section 8(f) rank 1: the k nearest items of every query WITHOUT the rows x N distance matrix in HBM.
-//   1. sample pass (EPI 2): distances to a strided sample of S <= 4096 column items; every (row, 128-column half tile)
-//      contributes the j-th smallest of its distances (j = 2..8 by k / N), and their mean -- roughly the j/129 quantile of
-//      the row -- is the row's candidate threshold (~3 k of the N entries: j = 2 for k = 251 at N = 50 000);
+//   1. sample pass (EPI 2): distances to a strided sample of S <= 4096 column items; every (row, 64-column half tile)
+//      contributes the j-th smallest of its distances (j = 2..8 by k / N), and their mean -- roughly the j/65 quantile of
+//      the row -- is the row's candidate threshold (~3 k of the N entries);
 //   2. sweep (EPI 1): the tensor-core kernel over all N columns keeps the entries below the threshold as (value, column)
 //      candidates in per-(row, column half, part) regions -- no atomics, nothing else is written;
 //   3. one CTA per row sorts its candidates as (key, column) words and writes the first k.
@@ -553,15 +517,17 @@ int pairwise_tc_topk(const float* F, int ldF, int N, int D, int row0, int rows, 
          w.Sh, w.Sl, w.sq_s);
   rc = check_launch("pairwise_sample_kernel");
   if (rc) return rc;
-  // thresholds: mean over the sample's half tiles (128 distances each) of the j-th smallest distance, j chosen so that
-  // ~3k of the row's N entries are expected below it (j / 129 of the row).  j > 8 is not tracked: such shapes (k large
+  // thresholds: mean over the sample's half tiles (64 distances each) of the j-th smallest distance, j chosen so that
+  // ~3k of the row's N entries are expected below it (j / 65 of the row).  j > 8 is not tracked: such shapes (k large
   // against N) simply find fewer than k candidates, report status != 0 and take the matrix path.
-  int j = (int)((3LL * k * 129 + N / 2) / N);
+  int j = (int)((3LL * k * (PW_BN / 2 + 1) + N / 2) / N);
   j = max(2, min(8, j));
   PwEpi e2 = {2, w.tau_sum, 0.f, nullptr, nullptr, nullptr, 0, j - 1};
   rc = pw_launch(L, N, row0, rows, w.Sh, w.Sl, w.sq_s, S, pmode, nullptr, 0, &e2, st);
   if (rc) return rc;
-  PwEpi e1 = {1, w.tau_sum, 1.f / (2.f * (float)ceil_div(S, PW_BN)), w.cnt, w.cv, w.ci, PT_CAPR, 0};
+  // the mean over the half tiles that fed the thresholds: those with >= 8 sample columns (a ragged last one may have fewer)
+  const int halves = S / (PW_BN / 2) + (S % (PW_BN / 2) >= 8 ? 1 : 0);
+  PwEpi e1 = {1, w.tau_sum, 1.f / (float)halves, w.cnt, w.cv, w.ci, PT_CAPR, 0};
   rc = pw_launch(L, N, row0, rows, L.Fh, L.Fl, L.sq, N, pmode, nullptr, 0, &e1, st);
   if (rc) return rc;
   launch(pairwise_topk_finish_kernel, dim3(rows), dim3(PT_THREADS), 0, st, w.cnt, w.cv, w.ci, k, out_idx, out_val, ldo, status);

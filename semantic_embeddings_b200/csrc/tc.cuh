@@ -1,7 +1,6 @@
-// sm_100a building blocks for the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor), tcgen05
-// (alloc / mma / commit / ld), UMMA shared-memory + instruction descriptors, host-side tensor maps.
-// Inline PTX only (no CUTLASS); bit layouts follow the PTX ISA "tcgen05" chapter (cross-checked against
-// cute/arch/mma_sm100_desc.hpp in the image's vendored CUTLASS headers).
+// sm_90a building blocks for the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma)
+// with shared-memory matrix descriptors, host-side tensor maps.  Inline PTX only; bit layouts follow the PTX ISA
+// "wgmma" chapter.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -115,107 +114,85 @@ __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ------------------------------------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ------------------------------------------------------------------------------------------- wgmma
+// Warpgroup MMA (sm_90a): the 128 threads of a warpgroup issue D[64 x N] (+)= A[64 x K] * B[N x K]^T together, both
+// operands read from shared memory through matrix descriptors, the fp32 accumulator in registers.  Fragment layout of
+// d[i] (thread t of the warpgroup, lane = t & 31, warp = t >> 5):
+//   row = 16 * warp + (lane >> 2) + 8 * ((i >> 1) & 1),   column = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ int fragment_row(int i, int tid_wg) { return 16 * (tid_wg >> 5) + ((tid_wg & 31) >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int fragment_col(int i, int tid_wg) { return 8 * (i >> 2) + 2 * (tid_wg & 3) + (i & 1); }
 
-// D[tmem] (+)= A[smem] * B[smem]; kind::f16 (fp16/bf16 inputs) or kind::tf32 (fp32 inputs read as tf32)
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// K-major operand tile in shared memory written by TMA (or by threads in the same layout): rows of `swizzle_bytes`
+// (64 or 128) bytes, 8-row groups 8 * swizzle_bytes apart.  A K step inside the swizzle row is a start-address offset.
+//   bits [0,14) start address >> 4   [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1)
+//   bits [32,46) stride byte offset >> 4   [62,64) layout: 1 = 128B, 2 = 64B, 3 = 32B swizzle
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t swizzle_bytes) {
+  const uint64_t layout = swizzle_bytes == 128 ? 1ull : (swizzle_bytes == 64 ? 2ull : 3ull);
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(((8 * swizzle_bytes) >> 4) & 0x3FFFu) << 32;
+  d |= layout << 62;
+  return d;
 }
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// byte offset of 16-byte chunk `chunk` of row `row` in a tile of `row_bytes`-byte rows in the matching TMA swizzle
+__device__ __forceinline__ uint32_t swizzle_offset(int row, int chunk, int row_bytes) {
+  return row_bytes == 128 ? row * 128 + ((chunk ^ (row & 7)) << 4) : row * 64 + ((chunk ^ ((row >> 1) & 3)) << 4);
 }
-// same with the accumulate flag fixed at compile time: no runtime predicate (which costs a divergence-safe
-// uniform-predicate sequence per instruction) -- use these in latency-critical issue loops
-template <bool ACC>
-__device__ __forceinline__ void mma_tf32_c(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc) {
-  if (ACC)
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc) : "memory");
-  else
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc) : "memory");
-}
-// One lane of a CONVERGENT warp.  Issue loops are written as "whole warp runs the loop, elect_one() guards the
-// instruction": loop counters, descriptors and addresses then live in uniform registers.  Running the loop inside
-// `if (lane == 0)` instead makes the compiler wrap every tcgen05.mma / TMA in a divergence-safe ELECT + R2UR +
-// BRA.U.ANY waterfall (~200 cycles per instruction, measured).  The elected lane is the same on every call with the
-// same mask, so tcgen05.commit sees the MMAs of "its" thread.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-// warp index the compiler can prove warp-uniform (a shuffle from lane 0), so `if (warp == k)` is a uniform branch
-__device__ __forceinline__ int uniform_warp_idx() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
 
-// shared-memory descriptor split into its constant high word and the low word (start address + LBO field)
-__device__ __forceinline__ uint32_t umma_desc_hi_kmajor(uint32_t sbo_bytes, uint32_t swizzle_bytes) {
-  uint32_t layout = swizzle_bytes == 128 ? 2u : (swizzle_bytes == 64 ? 4u : (swizzle_bytes == 32 ? 6u : 0u));
-  return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | (layout << 29);
-}
-__device__ __forceinline__ uint64_t umma_desc_join(uint32_t hi, uint32_t addr_bytes) {
-  return ((uint64_t)hi << 32) | (uint64_t)(((addr_bytes & 0x3FFFFu) >> 4) | (1u << 16));
-}
-// arrive on an mbarrier when every previously issued tcgen05.mma of this thread has completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (lane = TMEM lane, register j = column j)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
+__device__ __forceinline__ void wgmma_tf32_n16(float (&d)[8], uint64_t da, uint64_t db, int acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(acc)
       : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], uint64_t da, uint64_t db, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(acc)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t da, uint64_t db, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t da, uint64_t db, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t da, uint64_t db, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc)
+      : "memory");
+}
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-
-// ------------------------------------------------------------------------------------------- descriptors
-// K-major operand tile in shared memory, rows of `swizzle_bytes` (32/64/128) written by TMA with the same
-// swizzle mode; 8-row groups are `sbo_bytes` apart (8*swizzle_bytes for a dense tile).
-//   bits [0,14)  start address >> 4      bits [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1)
-//   bits [32,46) stride byte offset >> 4 bits [46,48) descriptor version = 1 (sm_100)
-//   bits [61,64) layout: 0 none, 2 = 128B, 4 = 64B, 6 = 32B swizzle
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t swizzle_bytes) {
-  uint64_t layout = swizzle_bytes == 128 ? 2ull : (swizzle_bytes == 64 ? 4ull : (swizzle_bytes == 32 ? 6ull : 0ull));
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= layout << 61;
-  return d;
-}
-// instruction descriptor: fp32 accumulate, both operands K-major.  fmt: 0 = f16, 1 = bf16, 2 = tf32
-__host__ __device__ constexpr uint32_t umma_idesc(int fmt, int M, int N) {
-  return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+// x - tf32_trunc(x): the part of an fp32 operand that a TF32 tensor-core operand does not carry (exact in fp32)
+__device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
+__device__ __forceinline__ float tf32_lo(float x) { return x - tf32_hi(x); }
 
 // ------------------------------------------------------------------------------------------- host: tensor maps
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,

@@ -56,9 +56,8 @@ class Engine:
         # data-parallel gradient exchange: 'torch' (and 'auto') = one all_reduce of the flat buffer through
         # torch.distributed between the fwd+bwd graph and the optimizer graph; 'native' = the library's own NCCL
         # communicator (se_comm_*), bucketed all-reduces issued by the plan runner on its communication stream while the
-        # backward pass continues, everything captured in ONE step graph.  Measured on 8 B200 (ResNet-110, 128 images per
-        # GPU): native 166.0 k images/s, torch 168.0 k images/s -- the 6.9 MB exchange is latency-bound and the NCCL
-        # kernels take SMs from a backward chain that is latency-bound itself, so overlapping buys nothing here; and the
+        # backward pass continues, everything captured in ONE step graph.  The 6.9 MB exchange of ResNet-110 is
+        # latency-bound and the NCCL kernels take SMs from a backward chain that is latency-bound itself; and the
         # BatchNorm kernels' grid barriers assume that all their CTAs are co-resident, which concurrent NCCL kernels do
         # not guarantee (one 8-rank run at 16 images per GPU hung).  'native' therefore stays opt-in.
         self.comm_native = False
@@ -180,7 +179,7 @@ class Engine:
         self.P = torch.zeros(off, **f32)
         self.G = torch.zeros(off, **f32)
         self.V = torch.zeros(off, **f32)
-        # K-major ([tap][co][ci]) copies of the conv kernels for the tcgen05 forward path, refreshed once per step
+        # K-major ([tap][co][ci]) copies of the conv kernels for the tensor-core forward path, refreshed once per step
         tc = self.mode in (_lib.SE_MODE_TF32, _lib.SE_MODE_TF32X3)
         self.PT = torch.zeros(off, **f32) if tc else None
         # error-compensated mode: low parts (w - tf32_trunc(w)) of the kernels in the HWIO and the transposed order

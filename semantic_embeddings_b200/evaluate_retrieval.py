@@ -36,7 +36,7 @@ def pairwise_distances(features, normalize=False, row0=0, rows=None, mode=None, 
 
     normalize=True : -F^ F^T with F^ = F/||F||        (evaluate_retrieval.py:57-59)
     normalize=False: sq_i + sq_j - 2 F F^T            (evaluate_retrieval.py:61-62)
-    `mode`: _lib.SE_MODE_F32 (exact fp32 FFMA) or SE_MODE_TF32 (tcgen05 3xTF32, default)."""
+    `mode`: _lib.SE_MODE_F32 (exact fp32 FFMA) or SE_MODE_TF32 (tensor-core split-fp16 x3, default)."""
     import torch
     if feat_dev is None:
         f = np.ascontiguousarray(np.asarray(features, dtype=np.float32))

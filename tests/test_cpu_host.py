@@ -374,7 +374,7 @@ def test_finetune_weights_are_loaded_by_name_with_mismatches_skipped(built_lib, 
 
 
 def test_tensor_core_coverage_of_the_baseline_networks(built_lib):
-    """se_conv2d_path (host-side planning, no GPU): which convolutions of the BASELINE architectures run on the tcgen05
+    """se_conv2d_path (host-side planning, no GPU): which convolutions of the BASELINE architectures run on the tensor-core
     kernels in the benchmarked arithmetic, per direction (forward, backward data, weight gradient)."""
     from semantic_embeddings_b200 import utils
     from semantic_embeddings_b200.models import resnet50
