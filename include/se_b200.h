@@ -124,7 +124,8 @@ int se_conv2d_wgrad(const se_conv_desc* d, const float* x, const float* dy, floa
 /* Which kernel family takes this layer in `mode` (pure host-side planning: no device work, callable without a GPU):
  * 1 = a tensor-core kernel, 0 = an fp32 kernel; direction 0 forward, 1 backward data, 2 weight gradient.  (Forward: given the
  * auxiliary kernel copies of se_conv_aux; with BatchNorm statistics wider than 384 channels the sums come from a separate
- * se_bn_stats pass, see se_conv2d_fwd_aux.) */
+ * se_bn_stats pass, see se_conv2d_fwd_aux.)  The plan sees the descriptor only, not the buffers: a weight gradient whose
+ * dw or dbias is not 16-byte aligned runs on the fp32 kernels even where this returns 1. */
 int se_conv2d_path(const se_conv_desc* d, int mode, int direction);
 /* Dense (models/cifar_resnet.py:233, plainnet.py:67,76, wide_residual_network.py:96, utils.py:242,
  * learn_image_embeddings.py:44): y = x W + b as a 1x1 convolution over a (B,1,1,Cin) tensor. */

@@ -373,6 +373,87 @@ def test_finetune_weights_are_loaded_by_name_with_mismatches_skipped(built_lib, 
         np.testing.assert_array_equal(eng._pview(name).numpy(), ws[name])
 
 
+# se_conv2d_path of every test_gpu_ops.CONV_CASES entry: (forward, backward data, weight gradient), 1 = tensor-core kernel,
+# 0 = fp32 kernel -- the same in SE_MODE_TF32 and SE_MODE_TF32X3.  The GPU parity test judges each direction by what
+# the planner says, so this table is what pins the routing itself; the comments name the predicate that decides.
+CONV_PLAN = {
+    (4, 32, 32, 3, 16, 3, 1, 'same'): (0, 0, 0),          # 3-channel stem
+    (4, 32, 32, 16, 16, 3, 1, 'same'): (1, 1, 1),
+    (4, 32, 32, 16, 32, 3, 2, 'same'): (0, 0, 0),         # narrow 3x3 / stride 2
+    (4, 16, 16, 32, 32, 3, 1, 'same'): (1, 1, 1),
+    (3, 8, 8, 64, 64, 3, 1, 'same'): (1, 1, 1),
+    (2, 16, 16, 16, 160, 1, 2, 'same'): (1, 1, 1),
+    (2, 18, 18, 3, 64, 7, 2, (3, 3, 3, 3)): (0, 0, 0),    # 7x7
+    (2, 9, 7, 8, 24, 3, 1, 'same'): (0, 0, 0),            # channels not multiples of 16
+    (5, 1, 1, 64, 100, 1, 1, 'valid'): (0, 0, 0),
+    (3, 1, 1, 20, 555, 1, 1, 'valid'): (0, 0, 0),
+    (2, 12, 12, 32, 64, 3, 1, 'same'): (1, 1, 1),
+    (5, 16, 16, 32, 64, 3, 1, 'same'): (1, 1, 1),
+    (6, 8, 8, 64, 64, 3, 1, 'same'): (1, 1, 1),
+    (3, 8, 8, 64, 160, 3, 1, 'same'): (1, 1, 1),
+    (2, 32, 32, 32, 16, 3, 1, 'same'): (1, 1, 1),
+    (2, 4, 4, 32, 32, 3, 1, 'same'): (1, 1, 1),
+    (1, 32, 32, 64, 320, 3, 1, 'same'): (1, 1, 1),
+    (5, 4, 8, 32, 48, 3, 1, 'same'): (1, 0, 1),           # dgrad K = 48
+    (3, 64, 64, 16, 16, 3, 1, 'same'): (0, 0, 1),         # W = 64: wgrad only
+    (2, 14, 14, 64, 256, 1, 1, 'valid'): (1, 1, 1),
+    (3, 7, 7, 256, 64, 1, 1, 'valid'): (1, 1, 1),
+    (1, 28, 28, 128, 512, 1, 1, 'valid'): (1, 1, 1),
+    (4, 8, 8, 16, 48, 1, 1, 'valid'): (1, 0, 1),
+    (8, 56, 56, 64, 64, 1, 1, 'valid'): (1, 1, 1),
+    (3, 28, 28, 32, 64, 3, 1, 'same'): (1, 1, 1),
+    (5, 14, 14, 64, 32, 3, 1, 'same'): (1, 1, 1),
+    (5, 7, 7, 64, 64, 3, 1, 'same'): (1, 1, 1),
+    (2, 55, 55, 32, 32, 3, 1, 'same'): (1, 1, 1),
+    (2, 16, 12, 16, 16, 3, 1, 'same'): (1, 1, 1),
+    (1, 40, 40, 32, 48, 3, 1, 'same'): (1, 0, 1),
+    (2, 55, 55, 64, 128, 1, 2, 'valid'): (1, 1, 1),
+    (3, 28, 28, 128, 64, 1, 2, 'valid'): (1, 1, 1),
+    (4, 14, 14, 64, 96, 1, 2, 'valid'): (1, 1, 1),
+    (2, 16, 16, 128, 160, 3, 2, 'same'): (0, 1, 1),       # conv3x3s2_tc_ok: backward only
+    (1, 32, 32, 160, 320, 3, 2, 'same'): (0, 1, 1),
+    (2, 6, 56, 32, 32, 3, 1, 'same'): (1, 1, 1),          # geometry_ok: W = 56
+    (2, 6, 57, 32, 32, 3, 1, 'same'): (0, 0, 1),          # geometry_ok: W = 57; conv3x3_wgrad_tc_ok: W <= 64
+    (1, 5, 64, 32, 16, 3, 1, 'same'): (0, 0, 1),          # conv3x3_wgrad_tc_ok: W = 64
+    (1, 5, 65, 32, 16, 3, 1, 'same'): (0, 0, 0),          # conv3x3_wgrad_tc_ok: W = 65
+    (4, 3, 3, 32, 32, 3, 1, 'same'): (0, 0, 0),           # W = 3
+    (3, 5, 4, 16, 32, 3, 1, 'same'): (1, 1, 1),           # W = 4
+    (1, 4, 64, 32, 32, 1, 2, 'valid'): (1, 1, 1),         # tc_shape_ok_1x1_s2: Wo = 32
+    (1, 4, 66, 32, 32, 1, 2, 'valid'): (0, 0, 0),         # Wo = 33
+    (2, 6, 6, 32, 64, 1, 2, 'valid'): (0, 0, 1),          # Wo = 3: geometry_ok; conv1x1_wgrad_tc_ok has no lower limit
+    (2, 8, 8, 32, 64, 1, 2, 'valid'): (1, 1, 1),          # Wo = 4
+    (1, 1, 127, 32, 32, 1, 1, 'valid'): (0, 0, 1),        # tc_shape_ok_1x1: 127 pixels
+    (1, 2, 64, 32, 32, 1, 1, 'valid'): (1, 1, 1),         # 128 pixels
+    (1, 1, 31, 32, 48, 1, 1, 'valid'): (0, 0, 0),         # conv1x1_wgrad_tc_ok: 31 pixels
+    (2, 4, 4, 32, 48, 1, 1, 'valid'): (0, 0, 1),          # 32 pixels
+    (2, 8, 8, 48, 32, 3, 1, 'same'): (0, 1, 1),           # tc_shape_ok: forward K = 48
+    (2, 8, 8, 32, 80, 3, 1, 'same'): (1, 0, 1),           # pick_bn -> 16; dgrad K = 80
+    (2, 8, 8, 32, 192, 3, 1, 'same'): (1, 1, 1),          # pick_bn -> 64
+    (2, 4, 4, 128, 128, 3, 2, 'same'): (0, 0, 1),         # conv3x3s2_tc_ok at Wo = 2; dgrad tiles need Wo >= 4
+    (1, 4, 64, 128, 128, 3, 2, 'same'): (0, 1, 1),        # conv3x3s2_tc_ok at Wo = 32
+    (2, 8, 8, 112, 128, 3, 2, 'same'): (0, 0, 0),         # conv3x3s2_tc_ok: Cin = 112 < 128
+    (1, 8, 8, 32, 384, 3, 1, 'same'): (1, 1, 1),
+    (1, 8, 8, 32, 640, 3, 1, 'same'): (1, 1, 1),          # forward statistics from se_bn_stats: still tensor-core
+}
+
+
+def test_conv_planner_table(built_lib):
+    """se_conv2d_path (host-side planning, no GPU) over the GPU parity test's case list against CONV_PLAN: a predicate of
+    conv_tc.cu / conv_wgrad_tc.cu that moves a boundary changes this table."""
+    if os.path.join(ROOT, 'tests') not in sys.path:
+        sys.path.insert(0, os.path.join(ROOT, 'tests'))
+    from test_gpu_ops import CONV_CASES, conv_desc
+    L = built_lib
+    lib = L.load()
+    assert sorted(map(str, CONV_PLAN)) == sorted(str(c[:8]) for c in CONV_CASES)
+    for case in CONV_CASES:
+        d = conv_desc(L, case)
+        for mode, want in ((L.SE_MODE_F32, (0, 0, 0)), (L.SE_MODE_TF32, CONV_PLAN[case[:8]]),
+                           (L.SE_MODE_TF32X3, CONV_PLAN[case[:8]])):
+            got = tuple(lib.se_conv2d_path(d, mode, k) for k in range(3))
+            assert got == want, (case, L.MODE_NAMES[mode], got, want)
+
+
 def test_tensor_core_coverage_of_the_baseline_networks(built_lib):
     """se_conv2d_path (host-side planning, no GPU): which convolutions of the BASELINE architectures run on the tensor-core
     kernels in the benchmarked arithmetic, per direction (forward, backward data, weight gradient)."""
