@@ -234,6 +234,17 @@ int se_softmax_xent_fwd_bwd(const float* logits, int ld, const int32_t* labels, 
  * (utils.py:49-54, in_top_k) = mean(rank_out < k) */
 int se_softmax_xent_fwd_bwd_ex(const float* logits, int ld, const int32_t* labels, int B, int C, float scale,
                                float* prob, float* loss, float* acc, float* dlogits, float* rank_out, void* stream);
+/* the same with label smoothing (learn_classifier.py:17-22 transform_inputs + Keras categorical_crossentropy): for
+ * 0 < smoothing < 1 the targets are t_hi = float(1 - smoothing) on the label and t_lo = float(smoothing / (C - 1)) on
+ * every other class (C >= 2); any other value means one-hot targets and runs se_softmax_xent_fwd_bwd_ex.
+ *   loss[b]    = -sum_c t_c log clip(p_c, 1e-7, 1 - 1e-7), over all classes
+ *   dlogits    = scale * (p_j T - live_j t_j), live = 1e-7 <= p <= 1 - 1e-7 (tf.clip_by_value's gradient mask),
+ *                T = sum_c live_c t_c
+ *   acc, rank_out: as above against argmax(y_true) -- the label, or the lowest other index when t_lo > t_hi
+ *                (smoothing > (C-1)/C) */
+int se_softmax_xent_smooth_fwd_bwd(const float* logits, int ld, const int32_t* labels, int B, int C, float smoothing,
+                                   float scale, float* prob, float* loss, float* acc, float* dlogits, float* rank_out,
+                                   void* stream);
 
 /* ------------------------------------------------------------------ optimizer
  * keras.optimizers.SGD(lr, momentum, decay, nesterov, clipnorm) + kernel_regularizer=l2(.)

@@ -88,6 +88,7 @@ _SIGS = {
     'se_embed_head_fwd_bwd': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P]),
     'se_softmax_xent_fwd_bwd': (c_int, [_P, c_int, _P, c_int, c_int, c_float, _P, _P, _P, _P, _P]),
     'se_softmax_xent_fwd_bwd_ex': (c_int, [_P, c_int, _P, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P]),
+    'se_softmax_xent_smooth_fwd_bwd': (c_int, [_P, c_int, _P, c_int, c_int, c_float, c_float, _P, _P, _P, _P, _P, _P]),
     'se_embed_head_fwd_bwd_ex': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P]),
     'se_sgd_schedule': (c_int, [_P, _P]),
     'se_pairwise_topk_workspace_bytes': (c_int64, [c_int, c_int, c_int]),

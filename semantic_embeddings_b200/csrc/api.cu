@@ -416,8 +416,13 @@ static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* f
                                       (float*)p[7], (float*)p[8], stream);
         break;
       case SE_OP_XENT:
-        rc = se_softmax_xent_fwd_bwd_ex((const float*)p[0], i[0], (const int32_t*)p[1], i[1], i[2], f[0], (float*)p[2],
-                                        (float*)p[3], (float*)p[4], (float*)p[5], (float*)p[6], stream);
+        // f[1] = label smoothing (learn_classifier.py --label_smoothing); 0 in every embedding-training plan
+        if (f[1] != 0.f)
+          rc = se_softmax_xent_smooth_fwd_bwd((const float*)p[0], i[0], (const int32_t*)p[1], i[1], i[2], f[1], f[0],
+                                              (float*)p[2], (float*)p[3], (float*)p[4], (float*)p[5], (float*)p[6], stream);
+        else
+          rc = se_softmax_xent_fwd_bwd_ex((const float*)p[0], i[0], (const int32_t*)p[1], i[1], i[2], f[0], (float*)p[2],
+                                          (float*)p[3], (float*)p[4], (float*)p[5], (float*)p[6], stream);
         break;
       case SE_OP_MEMSET: {
         if (i[0] & 1) {

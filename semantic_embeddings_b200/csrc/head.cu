@@ -242,10 +242,14 @@ embed_head_kernel(const float* __restrict__ z, int ldz, const int* __restrict__ 
 }
 
 // softmax + Keras categorical_crossentropy(prob) + arg-max accuracy + backward; one warp per row.
+// SMOOTH = false: one-hot targets.  SMOOTH = true: the label-smoothed targets of learn_classifier.py:17-22, t_hi on the
+// label and t_lo on every other class (the float32 values of the reference's float32 target array); every class then
+// contributes to the loss and, through its clip mask, to the gradient.
+template <bool SMOOTH>
 __global__ void __launch_bounds__(HEAD_WARPS * 32)
 softmax_xent_kernel(const float* __restrict__ logits, int ld, const int* __restrict__ labels, int B, int C, float scale,
                     float* __restrict__ prob, float* __restrict__ loss, float* __restrict__ acc,
-                    float* __restrict__ dlogits, float* __restrict__ rank_out) {
+                    float* __restrict__ dlogits, float* __restrict__ rank_out, float t_hi, float t_lo) {
   pdl_grid_sync();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row = blockIdx.x * HEAD_WARPS + warp;
@@ -265,26 +269,55 @@ softmax_xent_kernel(const float* __restrict__ logits, int ld, const int* __restr
   s = warp_sum(s);
   const float invs = 1.f / s;
   const int lab = labels[row];
-  const float py = expf(lr[lab] - m) * invs;
-  // Keras: p /= sum(p); p = clip(p, 1e-7, 1-1e-7); loss = -log p_y.  Gradient is zero where the clip is active.
+  // Keras: p /= sum(p); p = clip(p, 1e-7, 1-1e-7); loss = -sum_c t_c log p_c.  The clip passes the gradient where
+  // lo <= p <= hi (tf.clip_by_value).  (p is exp(z - m) / s: the renormalisation is a no-op up to rounding and does not
+  // change the gradient.)
   const float lo = 1e-7f, hi = 1.f - 1e-7f;
-  const float pyc = fminf(fmaxf(py, lo), hi);
-  if (lane == 0) {
-    if (loss) loss[row] = -logf(pyc);
-    if (acc) acc[row] = (arg == lab) ? 1.f : 0.f;
+  // argmax(y_true), the class Keras' accuracy metrics compare against: the label, unless smoothing gives the label the
+  // smaller target (ls > (C-1)/C) -- then the lowest other index
+  const int tgt = (!SMOOTH || t_hi >= t_lo) ? lab : (lab == 0 ? 1 : 0);
+  float row_loss;
+  bool live = true;   // one-hot: the label's clip mask
+  float tl = 1.f;     // smoothed: T = sum_c live_c t_c
+  if constexpr (!SMOOTH) {
+    const float py = expf(lr[lab] - m) * invs;
+    const float pyc = fminf(fmaxf(py, lo), hi);
+    row_loss = -logf(pyc);
+    live = (py >= lo) && (py <= hi);
+  } else {
+    float l = 0.f, t_live = 0.f;
+    for (int i = lane; i < C; i += 32) {
+      const float p = expf(lr[i] - m) * invs;
+      const float t = (i == lab) ? t_hi : t_lo;
+      l = fmaf(t, logf(fminf(fmaxf(p, lo), hi)), l);
+      if (p >= lo && p <= hi) t_live += t;
+    }
+    row_loss = -warp_sum(l);
+    tl = warp_sum(t_live);
   }
-  if (rank_out) {   // utils.top_k_acc (utils.py:49-54) = in_top_k: classes with a strictly larger probability than the label's
-    const float ll = lr[lab];
+  if (lane == 0) {
+    if (loss) loss[row] = row_loss;
+    if (acc) acc[row] = (arg == tgt) ? 1.f : 0.f;
+  }
+  if (rank_out) {   // utils.top_k_acc (utils.py:49-54) = in_top_k: classes with a strictly larger probability than the target's
+    const float ll = lr[tgt];
     float above = 0.f;
     for (int i = lane; i < C; i += 32) above += (lr[i] > ll) ? 1.f : 0.f;
     above = warp_sum(above);
     if (lane == 0) rank_out[row] = above;
   }
-  const bool live = (py >= lo) && (py <= hi);
   for (int i = lane; i < C; i += 32) {
     float p = expf(lr[i] - m) * invs;
     if (prob) prob[(long long)row * ld + i] = p;
-    if (dlogits) dlogits[(long long)row * ld + i] = live ? scale * (p - (i == lab ? 1.f : 0.f)) : 0.f;
+    if (dlogits) {
+      if constexpr (!SMOOTH) {
+        dlogits[(long long)row * ld + i] = live ? scale * (p - (i == lab ? 1.f : 0.f)) : 0.f;
+      } else {
+        // dz_j = scale * (p_j T - live_j t_j); with one-hot targets this is the branch above
+        const float t = (i == lab) ? t_hi : t_lo;
+        dlogits[(long long)row * ld + i] = scale * (p * tl - ((p >= lo && p <= hi) ? t : 0.f));
+      }
+    }
   }
 }
 
@@ -337,7 +370,22 @@ extern "C" int se_softmax_xent_fwd_bwd(const float* logits, int ld, const int32_
 extern "C" int se_softmax_xent_fwd_bwd_ex(const float* logits, int ld, const int32_t* labels, int B, int C, float scale,
                                           float* prob, float* loss, float* acc, float* dlogits, float* rank_out, void* stream) {
   SE_REQUIRE(logits && labels && B > 0 && C > 0 && ld >= C, "bad arguments");
-  launch(softmax_xent_kernel, dim3(ceil_div(B, HEAD_WARPS)), dim3(HEAD_WARPS * 32), 0, as_stream(stream), logits, ld, labels, B, C, scale,
-         prob, loss, acc, dlogits, rank_out);
+  launch(softmax_xent_kernel<false>, dim3(ceil_div(B, HEAD_WARPS)), dim3(HEAD_WARPS * 32), 0, as_stream(stream), logits, ld, labels, B,
+         C, scale, prob, loss, acc, dlogits, rank_out, 1.f, 0.f);
+  return check_launch("softmax_xent_kernel");
+}
+
+extern "C" int se_softmax_xent_smooth_fwd_bwd(const float* logits, int ld, const int32_t* labels, int B, int C,
+                                              float smoothing, float scale, float* prob, float* loss, float* acc,
+                                              float* dlogits, float* rank_out, void* stream) {
+  // learn_classifier.py:20 smooths only for 0 < ls < 1; any other value keeps the one-hot targets
+  if (!(smoothing > 0.f && smoothing < 1.f))
+    return se_softmax_xent_fwd_bwd_ex(logits, ld, labels, B, C, scale, prob, loss, acc, dlogits, rank_out, stream);
+  SE_REQUIRE(logits && labels && B > 0 && C > 1 && ld >= C, "bad arguments (label smoothing needs C >= 2)");
+  // Y * (1 - ls) + (1 - Y) * (ls / (C - 1)) on a float32 Y: the factors are formed in double and rounded once
+  const float t_hi = (float)(1.0 - (double)smoothing);
+  const float t_lo = (float)((double)smoothing / (double)(C - 1));
+  launch(softmax_xent_kernel<true>, dim3(ceil_div(B, HEAD_WARPS)), dim3(HEAD_WARPS * 32), 0, as_stream(stream), logits, ld, labels, B,
+         C, scale, prob, loss, acc, dlogits, rank_out, t_hi, t_lo);
   return check_launch("softmax_xent_kernel");
 }

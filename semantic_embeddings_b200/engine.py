@@ -30,13 +30,37 @@ def _vp(x):
     return int(x)
 
 
+OBJECTIVES = ('embedding', 'softmax')
+
+
 class Engine:
-    def __init__(self, graph, batch, embedding, loss='inv_corr', cls_weight=0.0, num_classes=None,
+    """objective='embedding' (learn_image_embeddings.py): the graph's output is the embedding, the fused head compares it
+    with the rows of `embedding` under `loss`, optionally with the softmax classifier branch of `cls_weight`.
+
+    objective='softmax' (learn_classifier.py): the graph's output are the logits of the top layer 'prob'; one cross-entropy
+    op (softmax + Keras categorical_crossentropy, optionally on label-smoothed targets) is the whole loss, with weight 1.
+    There is no class-embedding matrix (`embedding` must be None).  The metrics are the classifier's: 'loss', 'acc' and
+    'acc<k>' (utils.top_k_acc)."""
+
+    def __init__(self, graph, batch, embedding=None, loss='inv_corr', cls_weight=0.0, num_classes=None,
                  mode=_lib.SE_MODE_F32, device='cuda:0', momentum=0.9, nesterov=False, clipnorm=10.0,
                  world_size=1, fuse_stats=True, use_cuda_graph=True, seed=0, decay=0.0,
-                 grad_buckets=3, comm='auto', cls_base=None):
+                 grad_buckets=3, comm='auto', cls_base=None, objective='embedding', label_smoothing=0.0):
         if loss not in LOSS_KINDS:
             raise ValueError('unknown loss %r' % loss)
+        if objective not in OBJECTIVES:
+            raise ValueError('unknown objective %r (one of %s)' % (objective, ', '.join(OBJECTIVES)))
+        self.objective = objective
+        self.label_smoothing = float(label_smoothing)
+        if objective == 'softmax':
+            if embedding is not None:
+                raise ValueError("objective='softmax' trains a classifier: it takes no class embedding")
+            if cls_weight:
+                raise ValueError("cls_weight belongs to objective='embedding'")
+        elif embedding is None:
+            raise ValueError("objective='embedding' needs the class-embedding matrix")
+        elif self.label_smoothing != 0.0:
+            raise ValueError("label_smoothing belongs to objective='softmax'")
         self.decay = float(decay)
         self.lib = _lib.load()
         self.dev = torch.device(device)
@@ -65,11 +89,19 @@ class Engine:
             self.comm_native = self._init_native_comm(required=True)
         self.fuse_stats = fuse_stats
         self.use_cuda_graph = use_cuda_graph
-        emb = np.asarray(embedding, dtype=np.float32)
-        self.C, self.D = emb.shape
-        if graph.output.shape != (self.D,):
-            raise ValueError('network output %s does not match the %d-d class embeddings' % (graph.output.shape, self.D))
-        self.E = torch.from_numpy(np.ascontiguousarray(emb)).to(self.dev)
+        if objective == 'softmax':
+            if len(graph.output.shape) != 1:
+                raise ValueError('network output %s is not a vector of class logits' % (graph.output.shape,))
+            self.C = self.D = graph.output.shape[0]
+            if num_classes is not None and int(num_classes) != self.C:
+                raise ValueError('network output %s does not match the %d classes' % (graph.output.shape, int(num_classes)))
+            self.E = None
+        else:
+            emb = np.asarray(embedding, dtype=np.float32)
+            self.C, self.D = emb.shape
+            if graph.output.shape != (self.D,):
+                raise ValueError('network output %s does not match the %d-d class embeddings' % (graph.output.shape, self.D))
+            self.E = torch.from_numpy(np.ascontiguousarray(emb)).to(self.dev)
         self.num_classes = int(num_classes or self.C)
         self._extend_graph()
         self._alloc(seed)
@@ -122,6 +154,18 @@ class Engine:
         self.nodes = list(g.nodes)
         self.pspecs = OrderedDict(g.params)
         z = g.output
+        if self.objective == 'softmax':
+            # learn_classifier.py: Dense(C, softmax, name='prob') + categorical_crossentropy -- the softmax and the loss are
+            # one op on the logits, whose gradient seeds the backward pass
+            prob = T('prob_out', (self.num_classes,))
+            xe = Node('xent', 'xent', [z], prob)
+            prob.producer = xe
+            self.nodes.append(xe)
+            self.head_node = None
+            self.xent_node = xe
+            self.has_cls_branch = False
+            self._index_consumers()
+            return
         x_out = T('head_out', (self.D,))
         head = Node('head', 'head', [z], x_out)
         x_out.producer = head
@@ -152,6 +196,10 @@ class Engine:
             prob.producer = xe
             self.nodes.append(xe)
             self.xent_node = xe
+        self.has_cls_branch = self.xent_node is not None     # the --cls_weight classifier beside the embedding head
+        self._index_consumers()
+
+    def _index_consumers(self):
         self.consumers = {}
         for n in self.nodes:
             for idx, t in enumerate(n.inputs):
@@ -403,6 +451,16 @@ class Engine:
                 inf.append(self._op(_lib.OP_HEAD, ii, [scale], [z, self.labels, self.E, None, out, None, None, None]))
                 self._eval_head = self._op(_lib.OP_HEAD, ii, [scale], [z, self.labels, self.E, None, out, self.loss_buf,
                                                                         self.acc_buf, None, self.rank_buf])
+            elif n.op == 'xent' and self.objective == 'softmax':
+                # the whole loss (weight 1); f[1] = label smoothing
+                lg = n.inputs[0]
+                ii = [self.num_classes, self.B, self.num_classes]
+                ls = self.label_smoothing
+                fwd.append(self._op(_lib.OP_XENT, ii, [scale, ls],
+                                    [A[lg.name], self.labels, out, self.loss_buf, self.acc_buf, Gd[lg.name], self.rank_buf]))
+                inf.append(self._op(_lib.OP_XENT, ii, [0.0, ls], [A[lg.name], self.labels, out, None, None, None]))
+                self._eval_xent = self._op(_lib.OP_XENT, ii, [0.0, ls], [A[lg.name], self.labels, out, self.loss_buf,
+                                                                          self.acc_buf, None, self.rank_buf])
             elif n.op == 'xent':
                 lg = n.inputs[0]
                 fwd.append(self._op(_lib.OP_XENT, [self.num_classes, self.B, self.num_classes],
@@ -431,7 +489,7 @@ class Engine:
         bwd.append(self._op(_lib.OP_MEMSET, p=[self.G, nbytes(self.G)]))
         if self.xent_node is not None:
             written.add(self.xent_node.inputs[0].name)
-        if not self.consumers.get(self.head_node.output.name):
+        if self.head_node is not None and not self.consumers.get(self.head_node.output.name):
             written.add(self.head_node.inputs[0].name)
         for n in reversed(self.nodes):
             if n.op == 'xent':
@@ -725,7 +783,7 @@ class Engine:
     def metrics(self):
         """Host copies of the last step's per-sample loss / accuracy (one small D2H read)."""
         out = {'loss': float(self.loss_buf.cpu().numpy().mean()), 'acc': float(self.acc_buf.cpu().numpy().mean())}
-        if self.xent_node is not None:
+        if self.has_cls_branch:
             out['cls_loss'] = float(self.cls_loss_buf.cpu().numpy().mean())
             out['cls_acc'] = float(self.cls_acc_buf.cpu().numpy().mean())
         return out
@@ -737,7 +795,7 @@ class Engine:
         r = self.rank_buf.cpu().numpy() if ks else None
         for k in ks:
             out['acc%d' % k] = (r < k).astype(np.float32)
-        if self.xent_node is not None:
+        if self.has_cls_branch:
             out['cls_loss'] = self.cls_loss_buf.cpu().numpy()
             out['cls_acc'] = self.cls_acc_buf.cpu().numpy()
             rc = self.cls_rank_buf.cpu().numpy() if ks else None
@@ -750,28 +808,33 @@ class Engine:
         of the true class that the head kernels wrote: {'acc<k>': ..., 'cls_acc<k>': ...}."""
         r = self.rank_buf.cpu().numpy()
         out = {'acc%d' % k: float((r < k).mean()) for k in ks}
-        if self.xent_node is not None:
+        if self.has_cls_branch:
             rc = self.cls_rank_buf.cpu().numpy()
             out.update({'cls_acc%d' % k: float((rc < k).mean()) for k in ks})
         return out
 
-    def metrics_async(self):
+    def metrics_async(self, ks=()):
         """Enqueue the D2H read of the step that was just launched and return a handle; `metrics_result(handle)` waits
         for that copy only.  Lets a training loop read the PREVIOUS step's numbers while the next step runs (the
-        reference's Keras progress bar shows running means, learn_image_embeddings.py:238)."""
+        reference's Keras progress bar shows running means, learn_image_embeddings.py:238).  `ks`: also accuracy@k
+        ('acc<k>') for every k, from the rank of the true class."""
         if not hasattr(self, '_mring'):
-            n = 4 if self.xent_node is not None else 2
+            n = 5 if self.has_cls_branch else 3          # loss, acc[, cls_loss, cls_acc], rank
             self._mring = [torch.empty(n, self.B, dtype=torch.float32).pin_memory() for _ in range(4)]
             self._mev = [torch.cuda.Event() for _ in range(4)]
+            self._mks = [()] * 4
             self._mpos = 0
         k = self._mpos
         self._mpos = (k + 1) % 4
         host = self._mring[k]
         host[0].copy_(self.loss_buf, non_blocking=True)
         host[1].copy_(self.acc_buf, non_blocking=True)
-        if self.xent_node is not None:
+        if self.has_cls_branch:
             host[2].copy_(self.cls_loss_buf, non_blocking=True)
             host[3].copy_(self.cls_acc_buf, non_blocking=True)
+        if ks:
+            host[-1].copy_(self.rank_buf, non_blocking=True)
+        self._mks[k] = tuple(ks)
         self._mev[k].record()
         return k
 
@@ -779,9 +842,11 @@ class Engine:
         self._mev[handle].synchronize()
         host = self._mring[handle]
         out = {'loss': float(host[0].mean()), 'acc': float(host[1].mean())}
-        if self.xent_node is not None:
+        if self.has_cls_branch:
             out['cls_loss'] = float(host[2].mean())
             out['cls_acc'] = float(host[3].mean())
+        for kk in self._mks[handle]:
+            out['acc%d' % kk] = float((host[-1] < kk).float().mean())
         return out
 
     def grad_norm_and_reg(self):
@@ -789,12 +854,14 @@ class Engine:
         return float(np.sqrt(o[0])), float(o[1])
 
     def predict(self, x):
-        """Inference forward (BatchNorm moving statistics), returns the wrapped embeddings (B,D) as numpy."""
+        """Inference forward (BatchNorm moving statistics), returns the wrapped embeddings (B,D) -- or, for
+        objective='softmax', the class probabilities (B,C) -- as numpy."""
         x = torch.as_tensor(x)
         self.x.copy_(x, non_blocking=True)
         self._run('infer')
         torch.cuda.synchronize(self.dev)
-        return self.act[self.head_node.output.name].detach().cpu().numpy().copy()
+        out = self.head_node.output if self.head_node is not None else self.xent_node.output
+        return self.act[out.name].detach().cpu().numpy().copy()
 
     def activation(self, name_prefix):
         """Debug/test helper: host copy of the activation whose tensor name starts with `name_prefix:`."""

@@ -22,8 +22,9 @@ def unit(g, x, filters, n, prefix, stride=1, regularizer=0.0002):
 
 
 def SmallResNet(n=9, filters=(16, 32, 64), include_top=True, input_shape=(32, 32, 3), regularizer=0.0002,
-                classes=100, name=None):
-    """cifar_resnet.py:149-257 with pooling='avg', bn=True, conv_shortcut=False, top_activation=None."""
+                classes=100, name=None, top_name='embedding'):
+    """cifar_resnet.py:149-257 with pooling='avg', bn=True, conv_shortcut=False.  The top layer is named 'embedding'
+    (top_activation=None) or 'prob' (top_activation='softmax': the softmax itself is part of the cross-entropy op)."""
     g = Graph(name or 'cifar-resnet%d' % (2 * len(filters) * n), input_shape)
     x = g.conv(g.input, 'conv0', filters[0], 3, l2=regularizer)
     x = g.bn(x, 'bn0', relu=True)
@@ -32,5 +33,5 @@ def SmallResNet(n=9, filters=(16, 32, 64), include_top=True, input_shape=(32, 32
         x = unit(g, x, [filters[i - 1], filters[i]], n, str(i + 1) + '-', 2, regularizer)
     x = g.gap(x, 'avg_pool')
     if include_top:
-        x = g.dense(x, 'embedding', classes, l2=regularizer)      # :233
+        x = g.dense(x, top_name, classes, l2=regularizer)         # :233
     return g.set_output(x)

@@ -7,7 +7,7 @@ projection shortcut with BN, all convs with bias, BN eps 1e-3)."""
 from ..graph import Graph
 
 
-def ResNet50(num_outputs, input_shape=(224, 224, 3), name=None):
+def ResNet50(num_outputs, input_shape=(224, 224, 3), name=None, top_name='embedding'):
     g = Graph(name or 'resnet50', input_shape)
     x = g.conv(g.input, 'conv1', 64, 7, stride=2, padding=(3, 3, 3, 3))
     x = g.bn(x, 'bn_conv1', relu=True)
@@ -30,5 +30,5 @@ def ResNet50(num_outputs, input_shape=(224, 224, 3), name=None):
             y = g.conv(y, base + '2c', f3, 1, padding='valid')
             x = g.bn(y, bnb + '2c', relu=True, residual=sc)
     x = g.gap(x, 'avg_pool')
-    x = g.dense(x, 'embedding', num_outputs)
+    x = g.dense(x, top_name, num_outputs)
     return g.set_output(x)

@@ -24,7 +24,7 @@ class _Namer:
         return 'add_%d' % self.a
 
 
-def create_wide_residual_network(input_dim, nb_classes=100, N=2, k=1, name=None):
+def create_wide_residual_network(input_dim, nb_classes=100, N=2, k=1, name=None, top_name='embedding'):
     g = Graph(name or 'wrn-%d-%d' % (6 * N + 4, k), input_dim)
     nm = _Namer()
     # initial_conv (:8-16)
@@ -49,5 +49,5 @@ def create_wide_residual_network(input_dim, nb_classes=100, N=2, k=1, name=None)
             nm.add()
         x = g.bn(x, nm.bn(), relu=True, **_BN)                    # :91-92
     x = g.gap(x, 'avg_pool')
-    x = g.dense(x, 'embedding', nb_classes)                        # :96
+    x = g.dense(x, top_name, nb_classes)                           # :96 ('prob' with final_activation='softmax')
     return g.set_output(x)

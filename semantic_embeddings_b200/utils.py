@@ -25,33 +25,36 @@ def build_network(num_outputs, architecture, classification=False, no_softmax=Fa
     """utils.py:130-276.  Returns a graph.Graph whose output is the raw embedding (no l2norm wrapper; the
     wrapper and the loss are the fused head of the engine, learn_image_embeddings.py:127-128).
 
-    `classification=True` (softmax classifier training) belongs to learn_classifier.py, which is outside the
-    hot path: it raises NotImplementedError.  Unknown names raise ValueError like utils.py:276."""
+    `classification=True` (learn_classifier.py:88) builds the softmax classifier: the top layer is the Dense layer
+    'prob' and the graph's output are its logits -- the softmax is part of the engine's cross-entropy op
+    (Engine(objective='softmax')).  With `no_softmax=True` as well the top layer stays 'embedding', as in the
+    reference.  Unknown names raise ValueError like utils.py:276."""
     if architecture.lower().endswith('-selu'):
         raise NotImplementedError('SELU variants (utils.py:152-156) are outside the accelerated hot path')
-    if classification and not no_softmax:
-        raise NotImplementedError('softmax classification heads belong to learn_classifier.py (not on the hot path)')
+    softmax_top = classification and not no_softmax
+    top = 'prob' if softmax_top else 'embedding'
     ic = 3 if input_channels is None else input_channels
     hw = input_size
     if architecture == 'resnet-32':
         return cifar_resnet.SmallResNet(5, [16, 32, 64], include_top=classification, input_shape=(hw or 32, hw or 32, ic),
-                                        classes=num_outputs, name=name)
+                                        classes=num_outputs, name=name, top_name=top)
     elif architecture == 'resnet-110':
-        # utils.py:168-172: include_top=classification -> the 64-d pooled output, num_outputs ignored
+        # utils.py:168-172: include_top=classification -> otherwise the 64-d pooled output, num_outputs ignored
         return cifar_resnet.SmallResNet(18, [16, 32, 64], include_top=classification, input_shape=(hw or 32, hw or 32, ic),
-                                        classes=num_outputs, name=name)
+                                        classes=num_outputs, name=name, top_name=top)
     elif architecture == 'resnet-110-fc':
         return cifar_resnet.SmallResNet(18, [16, 32, 64], include_top=True, input_shape=(hw or 32, hw or 32, ic),
-                                        classes=num_outputs, name=name)
+                                        classes=num_outputs, name=name, top_name=top)
     elif architecture == 'resnet-110-wfc':
         return cifar_resnet.SmallResNet(18, [32, 64, 128], include_top=True, input_shape=(hw or 32, hw or 32, ic),
-                                        classes=num_outputs, name=name)
+                                        classes=num_outputs, name=name, top_name=top)
     elif architecture == 'wrn-28-10':
-        return wrn.create_wide_residual_network((hw or 32, hw or 32, ic), nb_classes=num_outputs, N=4, k=10, name=name)
+        return wrn.create_wide_residual_network((hw or 32, hw or 32, ic), nb_classes=num_outputs, N=4, k=10, name=name,
+                                                top_name=top)
     elif architecture == 'simple':
-        return plainnet.PlainNet(num_outputs, input_shape=(hw or 32, hw or 32, ic), name=name)
+        return plainnet.PlainNet(num_outputs, input_shape=(hw or 32, hw or 32, ic), name=name, top_name=top)
     elif architecture == 'resnet-50':
-        return resnet50.ResNet50(num_outputs, input_shape=(hw or 224, hw or 224, ic), name=name)
+        return resnet50.ResNet50(num_outputs, input_shape=(hw or 224, hw or 224, ic), name=name, top_name=top)
     elif architecture in REFERENCE_ARCHITECTURES:
         raise NotImplementedError('architecture {} exists in the reference but is outside the accelerated hot path '
                                   '(SURVEY.md section 2)'.format(architecture))
@@ -110,6 +113,19 @@ def nn_accuracy(embedding, dot_prod_sim=False, k=1):
 
 
 # ------------------------------------------------------------------------------------------------ LR schedules
+def feature_layer(graph):
+    """The layer whose output learn_classifier.py:179 dumps as features: model.layers[-2], or layers[-3] when [-2] is a
+    BatchNormalization -- the input of the top Dense layer, or the input of the BatchNormalization in front of it
+    (avg_pool for the CIFAR ResNets, WRN and ResNet-50; the post-ReLU fc output for `simple`).  Returns its tensor."""
+    top = graph.output.producer
+    if top is None or top.op != 'dense':
+        raise ValueError('the network has no top Dense layer: its output %s is already the feature vector' % graph.output.name)
+    feat = top.inputs[0]
+    if feat.producer is not None and feat.producer.op == 'bn':
+        feat = feat.producer.inputs[0]
+    return feat
+
+
 def get_lr_schedule(schedule, num_samples, batch_size, schedule_args={}):
     """utils.py:288-399.  Returns ([schedule objects], suggested number of epochs).  Only the SGDR branch
     (utils.py:357-368, the default of learn_image_embeddings.py:67) is on the hot path."""
