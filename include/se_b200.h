@@ -50,6 +50,7 @@ extern "C" {
 #define SE_LOSS_UNNORM_CORR 1  /* no wrapper     + 1 - <t,z>      */
 #define SE_LOSS_MSE 2          /* no wrapper     + sum (z-t)^2    */
 #define SE_LOSS_SOFTMAX_CORR 3 /* softmax wrapper + 1 - <t,x>     (learn_image_embeddings.py:129-130) */
+#define SE_LOSS_DEVISE_RANK 4  /* no wrapper     + sum_c relu(m - <t,z> + <z,E_c>) - m   (learn_devise.py; se_devise_rank_fwd_bwd) */
 
 /* pairwise modes: evaluate_retrieval.py:57-62 */
 #define SE_PDIST_SQEUCLID 0    /* A + B - 2 F F^T                 */
@@ -226,6 +227,15 @@ int se_embed_head_fwd_bwd(const float* z, int ldz, const int32_t* labels, const 
 int se_embed_head_fwd_bwd_ex(const float* z, int ldz, const int32_t* labels, const float* E, int ldE, int B,
                              int D, int C, int loss_kind, float loss_scale, const float* extra_dx,
                              float* x_out, float* loss, float* acc, float* dz, float* rank_out, void* stream);
+/* the DeViSE hinge ranking loss (utils.devise_ranking_loss, learn_devise.py) with the same arguments plus the margin m;
+ * loss_kind must be SE_LOSS_DEVISE_RANK (se_embed_head_fwd_bwd_ex rejects it).  No output wrapper: x_out = z.
+ *   loss[b] = sum_c relu(m - <t,z> + <z,E_c>) - m             (t = E[label])
+ *   dz      = loss_scale * (sum_{c in A} E_c - |A| t) + extra_dx,  A = {c : m - <t,z> + <z,E_c> > 0} (strict)
+ *   acc, rank_out: those of SE_LOSS_UNNORM_CORR (max_sim_acc), bit for bit
+ * The gradient sums the active rows in class order: reruns give the same bits. */
+int se_devise_rank_fwd_bwd(const float* z, int ldz, const int32_t* labels, const float* E, int ldE, int B, int D, int C,
+                           int loss_kind, float loss_scale, const float* extra_dx, float* x_out, float* loss, float* acc,
+                           float* dz, float* rank_out, float margin, void* stream);
 /* softmax + Keras categorical_crossentropy (clip 1e-7) + argmax accuracy + backward
  * (learn_image_embeddings.py:44,230-231): dlogits = scale * dCE/dlogits. */
 int se_softmax_xent_fwd_bwd(const float* logits, int ld, const int32_t* labels, int B, int C, float scale,
@@ -274,6 +284,12 @@ int se_sgd_schedule(float* lr_state, void* stream);
  * that a CUDA-graph-captured step follows the SGDR schedule (sgdr_callback.py:75-87) without re-capture */
 int se_sgd_apply_devlr(float* p, const float* g, float* v, int64_t n, const float* lr_dev, float momentum,
                        int nesterov, float clipnorm, const double* out, void* stream);
+/* keras.optimizers.Adagrad(lr, epsilon, decay) (learn_devise.py:87,114), the update pass after se_sgd_prepare: with
+ * s = clipnorm/norm when clipnorm > 0 and norm = sqrt(out[0]) >= clipnorm, else 1, per element
+ *   a += (s g)^2 ;  p -= lr_t s g / (sqrt(a) + epsilon)
+ * a [n] is the accumulator (zero at the start of a training phase); lr_dev is the lr_t of se_sgd_schedule (lr_state + 3). */
+int se_adagrad_apply_devlr(float* p, const float* g, float* a, int64_t n, const float* lr_dev, float epsilon, float clipnorm,
+                           const double* out, void* stream);
 
 /* ------------------------------------------------------------------ data-parallel gradient exchange
  * keras.utils.multi_gpu_model (learn_image_embeddings.py:133,148) -> one process per GPU + NCCL.  The communicator lives

@@ -13,14 +13,14 @@ LIB_PATH = os.path.join(_HERE, 'libse_b200.so')
 
 SE_MODE_F32, SE_MODE_TF32, SE_MODE_TF32X3 = 0, 1, 2
 MODE_NAMES = {0: 'f32', 1: 'tf32', 2: 'tf32x3'}
-SE_LOSS_INV_CORR, SE_LOSS_UNNORM_CORR, SE_LOSS_MSE, SE_LOSS_SOFTMAX_CORR = 0, 1, 2, 3
+SE_LOSS_INV_CORR, SE_LOSS_UNNORM_CORR, SE_LOSS_MSE, SE_LOSS_SOFTMAX_CORR, SE_LOSS_DEVISE_RANK = 0, 1, 2, 3, 4
 SE_PDIST_SQEUCLID, SE_PDIST_NEGDOT = 0, 1
 
 # opcodes of se_run_ops (csrc/opcodes.h)
 OP_CONV_FWD, OP_CONV_DGRAD, OP_CONV_WGRAD, OP_BN_STATS, OP_BN_FWD_TRAIN, OP_BN_FWD_INFER, OP_BN_BWD, \
     OP_SHORTCUT_BWD, OP_AVGPOOL_FWD, OP_AVGPOOL_BWD, OP_MAXPOOL_FWD, OP_MAXPOOL_BWD, OP_GAP_FWD, OP_GAP_BWD, \
     OP_ADD_FWD, OP_ADD_BWD, OP_HEAD, OP_XENT, OP_MEMSET, OP_SGD_PREPARE, OP_SGD_APPLY, OP_TRANSPOSE_FILTERS, \
-    OP_CONV_BN_FWD, OP_ALLREDUCE = range(1, 25)
+    OP_CONV_BN_FWD, OP_ALLREDUCE, OP_ADAGRAD_APPLY = range(1, 26)
 
 
 class SeError(RuntimeError):
@@ -90,6 +90,8 @@ _SIGS = {
     'se_softmax_xent_fwd_bwd_ex': (c_int, [_P, c_int, _P, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P]),
     'se_softmax_xent_smooth_fwd_bwd': (c_int, [_P, c_int, _P, c_int, c_int, c_float, c_float, _P, _P, _P, _P, _P, _P]),
     'se_embed_head_fwd_bwd_ex': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P]),
+    'se_devise_rank_fwd_bwd': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P,
+                                       c_float, _P]),
     'se_sgd_schedule': (c_int, [_P, _P]),
     'se_pairwise_topk_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'se_pairwise_topk': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, _P]),
@@ -106,6 +108,7 @@ _SIGS = {
     'se_sgd_prepare': (c_int, [_P, _P, c_int64, POINTER(L2Segment), c_int, _P, _P]),
     'se_sgd_apply': (c_int, [_P, _P, _P, c_int64, c_float, c_float, c_int, c_float, _P, _P]),
     'se_sgd_apply_devlr': (c_int, [_P, _P, _P, c_int64, _P, c_float, c_int, c_float, _P, _P]),
+    'se_adagrad_apply_devlr': (c_int, [_P, _P, _P, c_int64, _P, c_float, c_float, _P, _P]),
     'se_pairwise_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'se_pairwise_dist': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, c_int, _P]),
     'se_run_ops': (c_int, [POINTER(Op), c_int, c_int, _P]),

@@ -411,7 +411,13 @@ static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* f
         rc = se_add_bwd((const float*)p[0], (const float*)p[1], i[0], (float*)p[2], f[0], (float*)p[3], f[1], i[1], stream);
         break;
       case SE_OP_HEAD:
-        rc = se_embed_head_fwd_bwd_ex((const float*)p[0], i[0], (const int32_t*)p[1], (const float*)p[2], i[1], i[2], i[3],
+        // i[5] = SE_LOSS_DEVISE_RANK: the ranking loss with the margin in f[1] (0 in every other head op)
+        if (i[5] == SE_LOSS_DEVISE_RANK)
+          rc = se_devise_rank_fwd_bwd((const float*)p[0], i[0], (const int32_t*)p[1], (const float*)p[2], i[1], i[2], i[3],
+                                      i[4], i[5], f[0], (const float*)p[3], (float*)p[4], (float*)p[5], (float*)p[6],
+                                      (float*)p[7], (float*)p[8], f[1], stream);
+        else
+          rc = se_embed_head_fwd_bwd_ex((const float*)p[0], i[0], (const int32_t*)p[1], (const float*)p[2], i[1], i[2], i[3],
                                       i[4], i[5], f[0], (const float*)p[3], (float*)p[4], (float*)p[5], (float*)p[6],
                                       (float*)p[7], (float*)p[8], stream);
         break;
@@ -498,6 +504,18 @@ static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* f
         if (rc == SE_OK)
           rc = se_sgd_apply_devlr((float*)p[0], (const float*)p[1], (float*)p[5], (int64_t)(uintptr_t)p[2],
                                   (const float*)p[3] + 3, f[0], i[0], f[1], (const double*)p[4], stream);
+        break;
+      case SE_OP_ADAGRAD_APPLY:
+        // the Adagrad update in place of SGD_APPLY: same p[0..5] (p[5] = accumulators), f[0] = epsilon, f[1] = clipnorm
+        if (*forked) {
+          cudaEventRecord(g_ev_join, g_side);
+          cudaStreamWaitEvent(as_stream(stream), g_ev_join, 0);
+          *forked = false;
+        }
+        rc = se_sgd_schedule((float*)p[3], stream);
+        if (rc == SE_OK)
+          rc = se_adagrad_apply_devlr((float*)p[0], (const float*)p[1], (float*)p[5], (int64_t)(uintptr_t)p[2],
+                                      (const float*)p[3] + 3, f[0], f[1], (const double*)p[4], stream);
         break;
       default:
         set_error("se_run_ops: unknown opcode %d at index %d", o.opcode, k);

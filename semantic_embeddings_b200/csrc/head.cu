@@ -10,7 +10,8 @@
 //   utils.nn_accuracy         utils.py:57-100       |max_c <x,E_c> - <x,t>| < 1e-6  (k<=1)
 //   + TF autodiff of the above (learn_image_embeddings.py:238)
 // and Activation('softmax') + categorical_crossentropy of the classifier branch
-// (learn_image_embeddings.py:44,230-231).
+// (learn_image_embeddings.py:44,230-231), and the DeViSE hinge ranking loss
+//   utils.devise_ranking_loss utils.py:103-122   sum_c relu(m - <t,z> + <z,E_c>) - m   (learn_devise.py)
 #include <float.h>
 
 #include "common.cuh"
@@ -41,12 +42,13 @@ __global__ void __launch_bounds__(HEAD_WARPS_SPLIT * 32)
 embed_head_kernel(const float* __restrict__ z, int ldz, const int* __restrict__ labels, const float* __restrict__ E,
                   int ldE, int B, int D, int C, int loss_kind, float loss_scale, const float* __restrict__ extra_dx,
                   float* __restrict__ x_out, float* __restrict__ loss, float* __restrict__ acc, float* __restrict__ dz,
-                  float* __restrict__ rank_out, int es_classes, int split) {
+                  float* __restrict__ rank_out, int es_classes, int split, float margin) {
   // split == 0: one row per warp.  split == 1 (large class matrices read from global memory): one row per CTA -- every
   // warp holds the row, the warps share the class loop of the accuracy metric, warp 0 writes the row's outputs.
   pdl_grid_sync();
   extern __shared__ __align__(16) float smem[];
   __shared__ float s_red[HEAD_WARPS_SPLIT][4];
+  __shared__ float s_hinge[HEAD_WARPS_SPLIT];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nw = blockDim.x >> 5;
   const int Dp = (D + 3) & ~3;
@@ -55,7 +57,9 @@ embed_head_kernel(const float* __restrict__ z, int ldz, const int* __restrict__ 
   // es_classes == 0 -> the matrix does not fit, the accuracy loop reads it from global memory
   float* Es = smem + HEAD_WARPS * Dp;
   const bool want_acc = acc || rank_out;
-  if (es_classes > 0 && want_acc) {
+  // the ranking loss' pass over the classes (its loss and its gradient both need it)
+  const bool want_rank = loss_kind == SE_LOSS_DEVISE_RANK && (loss || dz);
+  if (es_classes > 0 && (want_acc || want_rank)) {
     for (int c = warp; c < C; c += HEAD_WARPS)
       for (int i = lane; i < D; i += 32) Es[c * (D + 1) + i] = E[(long long)c * ldE + i];
     __syncthreads();
@@ -123,7 +127,7 @@ embed_head_kernel(const float* __restrict__ z, int ldz, const int* __restrict__ 
   } else {
     l = 1.f - true_sim;
   }
-  if (loss && lane == 0 && lead) loss[row] = l;
+  if (loss && lane == 0 && lead && loss_kind != SE_LOSS_DEVISE_RANK) loss[row] = l;
 
   // ---- accuracy: nearest class over the whole class matrix (utils.py:73-93)
   if (loss_kind == SE_LOSS_SOFTMAX_CORR) {
@@ -204,8 +208,66 @@ embed_head_kernel(const float* __restrict__ z, int ldz, const int* __restrict__ 
     }
   }
 
+  // ---- DeViSE hinge ranking loss (utils.py:116-120): h_c = (m - <t,z>) + <z,E_c>; loss = sum_c relu(h_c) - m;
+  // dL/dz = scale * sum_{h_c > 0} (E_c - t) = scale * (sum_{c in A} E_c - |A| t).  One class per lane and step (the
+  // scores come from the same expression as the accuracy loop's); the active set A goes to a shared-memory bit mask
+  // (bit c%32 of word c/32), and the gradient sums the active rows in class order -- a fixed order per row.
+  if (want_rank) {
+    const float* Eb = es_classes > 0 ? Es : E;
+    const long long ep = es_classes > 0 ? (long long)(D + 1) : (long long)ldE;
+    const int mw = (C + 31) >> 5;
+    unsigned* act = reinterpret_cast<unsigned*>(smem + nw * Dp + es_classes * (D + 1)) + (split ? 0 : warp * mw);
+    const float base = margin - true_sim;
+    float hsum = 0.f;
+    for (int cb = c_first - lane; cb < C; cb += c_step) {    // uniform over the warp: one 32-class word per step
+      const int c = cb + lane;
+      bool on = false;
+      if (c < C) {
+        const float* e = Eb + c * ep;
+        float sim = 0.f;
+#pragma unroll 8
+        for (int i = 0; i < D; ++i) sim = fmaf(xs[i], e[i], sim);
+        const float h = base + sim;
+        on = h > 0.f;                     // relu'(0) = 0: a hinge of exactly zero is not active
+        if (on) hsum += h;
+      }
+      const unsigned bits = __ballot_sync(0xffffffffu, on);
+      if (lane == 0) act[cb >> 5] = bits;
+    }
+    hsum = warp_sum(hsum);
+    if (split) {
+      if (lane == 0) s_hinge[warp] = hsum;
+      __syncthreads();                    // (also publishes every warp's words of the mask)
+      hsum = 0.f;
+      for (int w2 = 0; w2 < nw; ++w2) hsum += s_hinge[w2];
+    } else {
+      __syncwarp();
+    }
+    if (loss && lane == 0 && lead) loss[row] = hsum - margin;
+    if (dz) {
+      int na = 0;
+      for (int w = 0; w < mw; ++w) na += __popc(act[w]);
+      const float fa = (float)na;
+      float* dzr = dz + (long long)row * ldz;
+      const float* ex = extra_dx ? extra_dx + (long long)row * ldz : nullptr;
+      // split: the warps share the dimensions of the row
+      for (int i = split ? warp * 32 + lane : lane; i < D; i += split ? 32 * nw : 32) {
+        float s = 0.f;
+        for (int w = 0; w < mw; ++w) {
+          unsigned bits = act[w];
+          while (bits) {
+            const int b = __ffs(bits) - 1;
+            bits &= bits - 1;
+            s += Eb[(long long)(w * 32 + b) * ep + i];
+          }
+        }
+        dzr[i] = loss_scale * (s - fa * t[i]) + (ex ? ex[i] : 0.f);
+      }
+    }
+  }
+
   // ---- backward
-  if (dz && lead) {
+  if (dz && lead && loss_kind != SE_LOSS_DEVISE_RANK) {
     float* dzr = dz + (long long)row * ldz;
     const float* ex = extra_dx ? extra_dx + (long long)row * ldz : nullptr;
     if (loss_kind == SE_LOSS_INV_CORR) {
@@ -332,12 +394,11 @@ extern "C" int se_embed_head_fwd_bwd(const float* z, int ldz, const int32_t* lab
                                   nullptr, stream);
 }
 
-extern "C" int se_embed_head_fwd_bwd_ex(const float* z, int ldz, const int32_t* labels, const float* E, int ldE, int B,
-                                        int D, int C, int loss_kind, float loss_scale, const float* extra_dx, float* x_out,
-                                        float* loss, float* acc, float* dz, float* rank_out, void* stream) {
+static int embed_head(const float* z, int ldz, const int32_t* labels, const float* E, int ldE, int B, int D, int C,
+                      int loss_kind, float loss_scale, const float* extra_dx, float* x_out, float* loss, float* acc,
+                      float* dz, float* rank_out, float margin, void* stream) {
   SE_REQUIRE(z && labels && E && B > 0 && D > 0 && C > 0, "bad arguments");
   SE_REQUIRE(ldz >= D && ldE >= D, "leading dimension smaller than D");
-  SE_REQUIRE(loss_kind >= 0 && loss_kind <= 3, "unknown loss kind");
   SE_REQUIRE(loss_kind != SE_LOSS_SOFTMAX_CORR || C >= 1, "bad arguments");
   const int Dp = (D + 3) & ~3;
   size_t smem = (size_t)HEAD_WARPS * Dp * sizeof(float);
@@ -348,18 +409,42 @@ extern "C" int se_embed_head_fwd_bwd_ex(const float* z, int ldz, const int32_t* 
   int grid = ceil_div(B, HEAD_WARPS);
   int es_classes = 0;
   const size_t es_bytes = (size_t)C * (D + 1) * sizeof(float);
-  if ((acc || rank_out) && loss_kind != SE_LOSS_SOFTMAX_CORR && smem + es_bytes <= 48 * 1024) { es_classes = C; smem += es_bytes; }
-  else if ((acc || rank_out) && loss_kind != SE_LOSS_SOFTMAX_CORR && (size_t)HEAD_WARPS_SPLIT * Dp * sizeof(float) <= 48 * 1024) {
+  // the ranking loss reads the class matrix for its hinge terms and keeps a bit mask of the active classes per row
+  const bool rank = loss_kind == SE_LOSS_DEVISE_RANK && (loss || dz);
+  const size_t mask_row = rank ? (size_t)((C + 31) / 32) * sizeof(unsigned) : 0;
+  const bool need_E = (acc || rank_out || rank) && loss_kind != SE_LOSS_SOFTMAX_CORR;
+  if (need_E && smem + es_bytes + HEAD_WARPS * mask_row <= 48 * 1024) {
+    es_classes = C; smem += es_bytes + HEAD_WARPS * mask_row;
+  } else if (need_E && (size_t)HEAD_WARPS_SPLIT * Dp * sizeof(float) + mask_row <= 48 * 1024) {
     // the class matrix stays in global memory: the loop over it is latency-bound per warp, so a row gets a whole CTA
-    split = 1; nwarps = HEAD_WARPS_SPLIT; grid = B; smem = (size_t)HEAD_WARPS_SPLIT * Dp * sizeof(float);
+    split = 1; nwarps = HEAD_WARPS_SPLIT; grid = B; smem = (size_t)HEAD_WARPS_SPLIT * Dp * sizeof(float) + mask_row;
+  } else {
+    smem += HEAD_WARPS * mask_row;
   }
+  SE_REQUIRE(smem <= 48 * 1024, "too many classes for the ranking loss' active-set mask");
   if (vec)
     launch(embed_head_kernel<true>, dim3(grid), dim3(nwarps * 32), smem, as_stream(stream), z, ldz, labels, E, ldE, B, D, C, loss_kind,
-           loss_scale, extra_dx, x_out, loss, acc, dz, rank_out, es_classes, split);
+           loss_scale, extra_dx, x_out, loss, acc, dz, rank_out, es_classes, split, margin);
   else
     launch(embed_head_kernel<false>, dim3(grid), dim3(nwarps * 32), smem, as_stream(stream), z, ldz, labels, E, ldE, B, D, C, loss_kind,
-           loss_scale, extra_dx, x_out, loss, acc, dz, rank_out, es_classes, split);
+           loss_scale, extra_dx, x_out, loss, acc, dz, rank_out, es_classes, split, margin);
   return check_launch("embed_head_kernel");
+}
+
+extern "C" int se_embed_head_fwd_bwd_ex(const float* z, int ldz, const int32_t* labels, const float* E, int ldE, int B,
+                                        int D, int C, int loss_kind, float loss_scale, const float* extra_dx, float* x_out,
+                                        float* loss, float* acc, float* dz, float* rank_out, void* stream) {
+  SE_REQUIRE(loss_kind >= 0 && loss_kind <= 3, "unknown loss kind");
+  return embed_head(z, ldz, labels, E, ldE, B, D, C, loss_kind, loss_scale, extra_dx, x_out, loss, acc, dz, rank_out, 0.f,
+                    stream);
+}
+
+extern "C" int se_devise_rank_fwd_bwd(const float* z, int ldz, const int32_t* labels, const float* E, int ldE, int B, int D,
+                                      int C, int loss_kind, float loss_scale, const float* extra_dx, float* x_out, float* loss,
+                                      float* acc, float* dz, float* rank_out, float margin, void* stream) {
+  SE_REQUIRE(loss_kind == SE_LOSS_DEVISE_RANK, "se_devise_rank_fwd_bwd computes SE_LOSS_DEVISE_RANK only");
+  return embed_head(z, ldz, labels, E, ldE, B, D, C, SE_LOSS_DEVISE_RANK, loss_scale, extra_dx, x_out, loss, acc, dz,
+                    rank_out, margin, stream);
 }
 
 extern "C" int se_softmax_xent_fwd_bwd(const float* logits, int ld, const int32_t* labels, int B, int C, float scale,

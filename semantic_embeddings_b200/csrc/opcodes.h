@@ -26,4 +26,5 @@ enum {
   SE_OP_TRANSPOSE_FILTERS = 22,
   SE_OP_CONV_BN_FWD = 23,
   SE_OP_ALLREDUCE = 24,
+  SE_OP_ADAGRAD_APPLY = 25,
 };

@@ -102,6 +102,43 @@ sgd_apply_kernel(float* __restrict__ p, const float* __restrict__ g, float* __re
   }
 }
 
+// keras.optimizers.Adagrad (Keras 2.2): a += g^2; p -= lr_t g / (sqrt(a) + eps), no momentum; g is the gradient after
+// sgd_prepare_kernel (L2 terms added, global norm in out[0]) and the optional clip.  Reads p, g, a and writes p, a.
+__global__ void __launch_bounds__(256)
+adagrad_apply_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ a, long long n,
+                     const float* lr_dev, float eps, float clipnorm, const double* __restrict__ out) {
+  pdl_grid_sync();
+  // lr_dev is written by the schedule kernel just before: no __restrict__, so that the load is not hoisted above the
+  // grid dependency wait as a read-only one
+  const float lr = *lr_dev;
+  float scale = 1.f;
+  if (clipnorm > 0.f) {
+    float norm = (float)sqrt(out[0]);
+    if (norm >= clipnorm) scale = clipnorm / norm;
+  }
+  const long long n4 = n >> 2;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    float4 gv = *reinterpret_cast<const float4*>(g + 4 * i);
+    float4 av = *reinterpret_cast<const float4*>(a + 4 * i);
+    float4 pv = *reinterpret_cast<const float4*>(p + 4 * i);
+    float gg[4] = {gv.x, gv.y, gv.z, gv.w}, ac[4] = {av.x, av.y, av.z, av.w}, pp[4] = {pv.x, pv.y, pv.z, pv.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float gs = scale * gg[j];
+      ac[j] = fmaf(gs, gs, ac[j]);
+      pp[j] -= lr * gs / (sqrtf(ac[j]) + eps);
+    }
+    *reinterpret_cast<float4*>(a + 4 * i) = make_float4(ac[0], ac[1], ac[2], ac[3]);
+    *reinterpret_cast<float4*>(p + 4 * i) = make_float4(pp[0], pp[1], pp[2], pp[3]);
+  }
+  for (long long i = (n4 << 2) + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float gs = scale * g[i];
+    const float na = fmaf(gs, gs, a[i]);
+    a[i] = na;
+    p[i] -= lr * gs / (sqrtf(na) + eps);
+  }
+}
+
 static int flat_grid(long long n) {
   long long g = ceil_div<long long>(ceil_div<long long>(n, 4), 256);
   return (int)max(1LL, min(g, (long long)sm_count() * 4));
@@ -161,4 +198,11 @@ extern "C" int se_sgd_step(float* p, float* g, float* v, int64_t n, const se_l2_
   int rc = se_sgd_prepare(p, g, n, segs, nsegs, out, stream);
   if (rc) return rc;
   return se_sgd_apply(p, g, v, n, lr, momentum, nesterov, clipnorm, out, stream);
+}
+
+extern "C" int se_adagrad_apply_devlr(float* p, const float* g, float* a, int64_t n, const float* lr_dev, float epsilon,
+                                      float clipnorm, const double* out, void* stream) {
+  SE_REQUIRE(p && g && a && out && lr_dev && n > 0, "bad arguments");
+  launch(adagrad_apply_kernel, dim3(flat_grid(n)), dim3(256), 0, as_stream(stream), p, g, a, n, lr_dev, epsilon, clipnorm, out);
+  return check_launch("adagrad_apply_kernel");
 }

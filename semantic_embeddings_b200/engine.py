@@ -18,7 +18,8 @@ from ._lib import Op
 from .graph import Graph, Node, T
 
 LOSS_KINDS = {'inv_corr': _lib.SE_LOSS_INV_CORR, 'unnorm_corr': _lib.SE_LOSS_UNNORM_CORR, 'mse': _lib.SE_LOSS_MSE,
-              'softmax_corr': _lib.SE_LOSS_SOFTMAX_CORR}
+              'softmax_corr': _lib.SE_LOSS_SOFTMAX_CORR, 'devise_rank': _lib.SE_LOSS_DEVISE_RANK}
+OPTIMIZERS = ('sgd', 'adagrad')
 
 
 def _vp(x):
@@ -40,14 +41,32 @@ class Engine:
     objective='softmax' (learn_classifier.py): the graph's output are the logits of the top layer 'prob'; one cross-entropy
     op (softmax + Keras categorical_crossentropy, optionally on label-smoothed targets) is the whole loss, with weight 1.
     There is no class-embedding matrix (`embedding` must be None).  The metrics are the classifier's: 'loss', 'acc' and
-    'acc<k>' (utils.top_k_acc)."""
+    'acc<k>' (utils.top_k_acc).
+
+    loss='devise_rank' (learn_devise.py): the DeViSE hinge ranking loss on the raw output with margin `margin` (0.1 by
+    default); its metric is max_sim_acc, as for 'unnorm_corr'.
+
+    optimizer='sgd': Keras SGD(lr, momentum (0.9 by default), decay, nesterov, clipnorm).  optimizer='adagrad': Keras
+    Adagrad(lr, epsilon, decay) with the same optional clipnorm; its accumulators live where SGD keeps its velocity
+    (get_velocity / set_velocity), and it takes no momentum."""
 
     def __init__(self, graph, batch, embedding=None, loss='inv_corr', cls_weight=0.0, num_classes=None,
-                 mode=_lib.SE_MODE_F32, device='cuda:0', momentum=0.9, nesterov=False, clipnorm=10.0,
+                 mode=_lib.SE_MODE_F32, device='cuda:0', momentum=None, nesterov=False, clipnorm=10.0,
                  world_size=1, fuse_stats=True, use_cuda_graph=True, seed=0, decay=0.0,
-                 grad_buckets=3, comm='auto', cls_base=None, objective='embedding', label_smoothing=0.0):
+                 grad_buckets=3, comm='auto', cls_base=None, objective='embedding', label_smoothing=0.0,
+                 margin=None, optimizer='sgd', epsilon=1e-7):
         if loss not in LOSS_KINDS:
             raise ValueError('unknown loss %r' % loss)
+        if margin is not None and loss != 'devise_rank':
+            raise ValueError("margin belongs to loss='devise_rank'")
+        self.margin = float(0.1 if margin is None else margin) if loss == 'devise_rank' else 0.0
+        if optimizer not in OPTIMIZERS:
+            raise ValueError('unknown optimizer %r (one of %s)' % (optimizer, ', '.join(OPTIMIZERS)))
+        if optimizer == 'adagrad' and ((momentum is not None and float(momentum) != 0.0) or nesterov):
+            raise ValueError('Adagrad has no momentum: momentum / nesterov belong to optimizer=\'sgd\'')
+        self.optimizer = optimizer
+        self.epsilon = float(epsilon)
+        momentum = (0.9 if optimizer == 'sgd' else 0.0) if momentum is None else momentum
         if objective not in OBJECTIVES:
             raise ValueError('unknown objective %r (one of %s)' % (objective, ', '.join(OBJECTIVES)))
         self.objective = objective
@@ -315,7 +334,7 @@ class Engine:
         return OrderedDict((n, self._pview(n, self.G).detach().cpu().numpy().copy()) for n in self.offsets)
 
     def set_velocity(self, vel):
-        """Optimizer momentum buffers by weight name (resuming a snapshot; tests)."""
+        """Optimizer state by weight name: SGD's momentum buffers or Adagrad's accumulators (resuming a snapshot; tests)."""
         for name, a in vel.items():
             v = self._pview(name, self.V)
             v.copy_(torch.from_numpy(np.ascontiguousarray(np.asarray(a, dtype=np.float32))))
@@ -445,12 +464,13 @@ class Engine:
                 z = A[n.inputs[0].name]
                 has_cls = bool(self.consumers.get(n.output.name))
                 ii = [self.D, self.D, self.B, self.D, self.C, LOSS_KINDS[self.loss]]
+                ff = self._head_f(scale)
                 dz = None if has_cls else Gd[n.inputs[0].name]
-                fwd.append(self._op(_lib.OP_HEAD, ii, [scale],
+                fwd.append(self._op(_lib.OP_HEAD, ii, ff,
                                     [z, self.labels, self.E, None, out, self.loss_buf, self.acc_buf, dz, self.rank_buf]))
-                inf.append(self._op(_lib.OP_HEAD, ii, [scale], [z, self.labels, self.E, None, out, None, None, None]))
-                self._eval_head = self._op(_lib.OP_HEAD, ii, [scale], [z, self.labels, self.E, None, out, self.loss_buf,
-                                                                        self.acc_buf, None, self.rank_buf])
+                inf.append(self._op(_lib.OP_HEAD, ii, ff, [z, self.labels, self.E, None, out, None, None, None]))
+                self._eval_head = self._op(_lib.OP_HEAD, ii, ff, [z, self.labels, self.E, None, out, self.loss_buf,
+                                                                   self.acc_buf, None, self.rank_buf])
             elif n.op == 'xent' and self.objective == 'softmax':
                 # the whole loss (weight 1); f[1] = label smoothing
                 lg = n.inputs[0]
@@ -500,7 +520,7 @@ class Engine:
                     z = n.inputs[0]
                     ii = [self.D, self.D, self.B, self.D, self.C, LOSS_KINDS[self.loss]]
                     written.add(z.name)
-                    bwd.append(self._op(_lib.OP_HEAD, ii, [scale],
+                    bwd.append(self._op(_lib.OP_HEAD, ii, self._head_f(scale),
                                         [A[z.name], self.labels, self.E, dY, None, None, None, Gd[z.name]]))
                 continue
             assert n.output.name in written, 'no gradient reaches %s' % n.output.name
@@ -601,15 +621,23 @@ class Engine:
             self._parts['bwd_dp'] = self._with_allreduce(bwd, final)
             self.plans['step_dp'] = self._pack(fwd + self._parts['bwd_dp'] + opt)
 
+    def _head_f(self, scale):
+        """Float slots of a head op: the loss scale, and the margin for the ranking loss (f[1])."""
+        return [scale, self.margin] if self.loss == 'devise_rank' else [scale]
+
     def _opt_ops(self):
-        """Optimizer ops of a step: [zero the gradients of frozen parameters], global norm + L2 terms, clip + SGD update."""
+        """Optimizer ops of a step: [zero the gradients of frozen parameters], global norm + L2 terms, clip + SGD (or
+        Adagrad) update."""
         nbytes = lambda t: t.numel() * t.element_size()
         # i[0] = 1: the runner joins the weight-gradient side stream (and pending all-reduces) before this memset
         freeze = [self._op(_lib.OP_MEMSET, [1], p=[self.G[o:o + n], nbytes(self.G[o:o + n])]) for o, n in self.frozen_runs]
-        return freeze + [
-            self._op(_lib.OP_MEMSET, p=[self.sgd_out, 16]),
-            self._op(_lib.OP_SGD_PREPARE, [self.n_active_segs],
-                     p=[self.P, self.G, self.nparams, ctypes.addressof(self.seg_array), self.sgd_out]),
+        prep = [self._op(_lib.OP_MEMSET, p=[self.sgd_out, 16]),
+                self._op(_lib.OP_SGD_PREPARE, [self.n_active_segs],
+                         p=[self.P, self.G, self.nparams, ctypes.addressof(self.seg_array), self.sgd_out])]
+        if self.optimizer == 'adagrad':
+            return freeze + prep + [self._op(_lib.OP_ADAGRAD_APPLY, [], [self.epsilon, self.clipnorm],
+                                             [self.P, self.G, self.nparams, self.lr_dev, self.sgd_out, self.V])]
+        return freeze + prep + [
             self._op(_lib.OP_SGD_APPLY, [1 if self.nesterov else 0], [self.momentum, self.clipnorm],
                      [self.P, self.G, self.nparams, self.lr_dev, self.sgd_out, self.V])]
 
@@ -647,7 +675,7 @@ class Engine:
             self.seg_array[k].begin, self.seg_array[k].end, self.seg_array[k].l2 = b, e, l
         self.n_active_segs = len(segs)
         self.frozen_runs = [tuple(r) for r in runs]
-        for off, sz in self.frozen_runs:          # no momentum carried into (or out of) the frozen phase
+        for off, sz in self.frozen_runs:          # no momentum (or Adagrad accumulator) carried into or out of the frozen phase
             self.V[off:off + sz].zero_()
         opt = self._opt_ops()
         self.plans['opt'] = self._pack(opt)

@@ -1,6 +1,7 @@
-"""Training-script machinery shared by learn_image_embeddings.py and learn_classifier.py: what Keras' `fit_generator`,
-`evaluate_generator`, `ModelCheckpoint` and `load_weights(by_name=True)` do for the reference scripts, on top of
-engine.Engine.  The scripts only differ in the network's top, the engine objective and what they print at the end."""
+"""Training-script machinery shared by learn_image_embeddings.py, learn_classifier.py and learn_devise.py: what Keras'
+`fit_generator`, `evaluate_generator`, `ModelCheckpoint` and `load_weights(by_name=True)` do for the reference scripts,
+on top of engine.Engine.  The scripts only differ in the network's top, the engine objective and what they print at the
+end."""
 import os
 import pickle
 from collections import OrderedDict
@@ -170,6 +171,25 @@ def pretrain_new_layers(eng, data, args, new_layers, rng, rank, world, ks, say, 
     eng.V.zero_()
     eng.set_iterations(0)
     eng.lr_dev[1:2].fill_(dec)
+
+
+def fresh_optimizer(eng, decay=0.0):
+    """What a new Keras `compile` does to the optimizer state (learn_devise.py:87,114): momentum buffers / Adagrad
+    accumulators and the iteration count start at 0, with the given learning-rate decay."""
+    eng.V.zero_()
+    eng.set_iterations(0)
+    eng.lr_dev[1:2].fill_(float(decay))
+
+
+def fit_constant_lr(eng, data, batch_size, lr, epochs, rng, ks, say, rank=0, world=1):
+    """fit_generator without a schedule callback (learn_devise.py:91-96,118-123): the optimizer's own learning rate (and
+    decay) for every epoch; a training pass and a validation pass per epoch, logged like the other trainers."""
+    eng.set_lr(lr)
+    for epoch in range(epochs):
+        logs = train_epoch(eng, data, batch_size, rng, rank, world)
+        val, _ = run_validation(eng, data, ks, None)
+        logs.update({'val_' + k: v for k, v in val.items()})
+        say('Epoch {}/{} - '.format(epoch + 1, epochs) + format_logs(logs))
 
 
 def fit(eng, data, args, sched, epochs, rng, rank, world, ks, say, train_ks=()):

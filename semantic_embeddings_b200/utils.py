@@ -2,7 +2,7 @@
 meaning and error behaviour (reference file:line cited per function), returning layer-list graphs
 (graph.Graph) instead of Keras models and plain schedule objects instead of Keras callbacks.
 
-The tensor functions (l2norm, inv_correlation, squared_distance, nn_accuracy) are the stand-alone
+The tensor functions (l2norm, inv_correlation, squared_distance, devise_ranking_loss, nn_accuracy) are the stand-alone
 forms of what the fused head kernel computes inside a training step; they run the same CUDA kernel
 (se_embed_head_fwd_bwd) on device tensors -- there is no CPU implementation in the product."""
 import numpy as np
@@ -62,8 +62,24 @@ def build_network(num_outputs, architecture, classification=False, no_softmax=Fa
         raise ValueError('Unknown network architecture: {}'.format(architecture))
 
 
+def build_devise_network(embed_dim, architecture, num_classes, input_channels=None, input_size=None):
+    """The network learn_devise.py:68-72 trains from --init_weights: the classifier of build_network(num_classes,
+    architecture, classification=True) with its top Dense layer 'prob' replaced by a linear Dense(embed_dim,
+    name='embedding') on the tensor 'prob' read (glorot_uniform kernel, zero bias, no regulariser).  Every other layer,
+    and so every other weight name, is the classifier's."""
+    g = build_network(num_classes, architecture, classification=True, input_channels=input_channels,
+                      input_size=input_size)
+    top = g.output.producer
+    if top is None or top.op != 'dense' or top.name != 'prob':
+        raise ValueError('the classifier of {} has no top Dense layer \'prob\''.format(architecture))
+    g.nodes.remove(top)
+    for name in top.params:
+        del g.params[name]
+    return g.set_output(g.dense(top.inputs[0], 'embedding', embed_dim))
+
+
 # ------------------------------------------------------------------------------------------------ head functions
-def _head(z, labels, embedding, loss_kind, want):
+def _head(z, labels, embedding, loss_kind, want, margin=None):
     import torch
     z = z.contiguous().float()
     B, D = z.shape
@@ -74,8 +90,12 @@ def _head(z, labels, embedding, loss_kind, want):
     x = torch.empty_like(z)
     loss = torch.empty(B, device=z.device)
     acc = torch.empty(B, device=z.device)
-    _lib.call('se_embed_head_fwd_bwd', z.data_ptr(), D, lab.data_ptr(), E.data_ptr(), D, B, D, C, loss_kind, 1.0, None,
-              x.data_ptr(), loss.data_ptr(), acc.data_ptr(), None, _lib.stream_ptr())
+    if loss_kind == _lib.SE_LOSS_DEVISE_RANK:
+        _lib.call('se_devise_rank_fwd_bwd', z.data_ptr(), D, lab.data_ptr(), E.data_ptr(), D, B, D, C, loss_kind, 1.0, None,
+                  x.data_ptr(), loss.data_ptr(), acc.data_ptr(), None, None, float(margin), _lib.stream_ptr())
+    else:
+        _lib.call('se_embed_head_fwd_bwd', z.data_ptr(), D, lab.data_ptr(), E.data_ptr(), D, B, D, C, loss_kind, 1.0, None,
+                  x.data_ptr(), loss.data_ptr(), acc.data_ptr(), None, _lib.stream_ptr())
     return {'x': x, 'loss': loss, 'acc': acc}[want]
 
 
@@ -95,6 +115,16 @@ def inv_correlation(embedding, labels, y_pred):
 def squared_distance(embedding, labels, y_pred):
     """utils.py:34-36."""
     return _head(y_pred, labels, embedding, _lib.SE_LOSS_MSE, 'loss')
+
+
+def devise_ranking_loss(embedding, margin=0.1):
+    """utils.py:103-122: returns loss(labels, y_pred) -> per-sample sum_c relu(margin - <t,y> + <y,E_c>) - margin with
+    t = embedding[labels] (the target gather of learn_devise.transform_inputs folded in), on the raw output y."""
+
+    def _loss(labels, y_pred):
+        return _head(y_pred, labels, embedding, _lib.SE_LOSS_DEVISE_RANK, 'loss', margin)
+
+    return _loss
 
 
 def nn_accuracy(embedding, dot_prod_sim=False, k=1):
