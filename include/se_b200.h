@@ -183,6 +183,24 @@ int se_bn_bwd(const float* x, const float* y, const float* dout, int64_t rows, i
               const float* save_mean, const float* save_invstd, int relu, int relu_in, float* dx,
               float beta_dx, float* dres, float beta_res, float* dgamma, float* dbeta, double* scratch,
               void* stream);
+/* Which implementation se_bn_bwd runs for (rows, C) on a device with `sms` SMs (sms <= 0: the current device; a positive
+ * sms is pure host-side planning, callable without a GPU).  se_bn_bwd decides by the same function, and SE_BN_NO_FUSE /
+ * SE_BN_NO_REG in the environment move both alike.  Bits 0-1 name the path, bit 2 its float4 / fixed-quad variant:
+ *   SE_BN_BWD_SCALAR       bn_bwd_reduce_kernel + bn_bwd_apply_kernel, scalar branch (C % 4 != 0)          2 launches
+ *   SE_BN_BWD_VEC          the same two kernels, float4 branch                                             2 launches
+ *   SE_BN_BWD_SLAB_ATOMIC  bn_bwd_fused_kernel (slab in shared memory, grid barrier), per-element shared
+ *                          atomics: 512 threads do not divide into channel quads (512 % (C/4) != 0)        1 launch
+ *   SE_BN_BWD_SLAB_QUAD    bn_bwd_fused_kernel, every thread keeps one channel quad                         1 launch
+ *   SE_BN_BWD_SLAB_REG     bn_bwd_reg_kernel (slab in registers, grid barrier): C <= 128, 512 % (C/4) == 0,
+ *                          at most 8 float4 of the slab per thread                                          1 launch
+ * The slab paths hold rows/sms rows per CTA (rounded up to a multiple of 4) and need them to fit; every
+ * other C % 4 == 0 layer is SE_BN_BWD_VEC.  Returns < 0 (SE_ERR_ARG) for rows <= 0 or C <= 0. */
+#define SE_BN_BWD_SCALAR 0
+#define SE_BN_BWD_SLAB_ATOMIC 1
+#define SE_BN_BWD_SLAB_REG 2
+#define SE_BN_BWD_VEC 4
+#define SE_BN_BWD_SLAB_QUAD 5
+int se_bn_bwd_path(int64_t rows, int C, int sms);
 /* gradient of the pooled / channel-padded shortcut (cifar_resnet.py:117-121):
  * dsrc[n,2h+i,2w+j,c] = beta*dsrc + 0.25 * g[n,h,w,c+pad_lo], g = dout*(y>0) if relu. */
 int se_shortcut_bwd(const float* dout, const float* y, int relu, int N, int H, int W, int C,

@@ -15,6 +15,8 @@ SE_MODE_F32, SE_MODE_TF32, SE_MODE_TF32X3 = 0, 1, 2
 MODE_NAMES = {0: 'f32', 1: 'tf32', 2: 'tf32x3'}
 SE_LOSS_INV_CORR, SE_LOSS_UNNORM_CORR, SE_LOSS_MSE, SE_LOSS_SOFTMAX_CORR, SE_LOSS_DEVISE_RANK = 0, 1, 2, 3, 4
 SE_PDIST_SQEUCLID, SE_PDIST_NEGDOT = 0, 1
+# se_bn_bwd_path: bits 0-1 = path (0 reduce + apply, 1 shared-memory slab, 2 register slab), bit 2 = float4 / fixed quad
+SE_BN_BWD_SCALAR, SE_BN_BWD_SLAB_ATOMIC, SE_BN_BWD_SLAB_REG, SE_BN_BWD_VEC, SE_BN_BWD_SLAB_QUAD = 0, 1, 2, 4, 5
 
 # opcodes of se_run_ops (csrc/opcodes.h)
 OP_CONV_FWD, OP_CONV_DGRAD, OP_CONV_WGRAD, OP_BN_STATS, OP_BN_FWD_TRAIN, OP_BN_FWD_INFER, OP_BN_BWD, \
@@ -74,6 +76,7 @@ _SIGS = {
     'se_bn_fwd_train': (c_int, [_P, c_int64, c_int, _P, _P, _P, c_float, c_float, _P, _P, _P, _P, POINTER(Residual), c_int, _P, _P]),
     'se_bn_fwd_infer': (c_int, [_P, c_int64, c_int, _P, _P, _P, _P, c_float, POINTER(Residual), c_int, _P, _P]),
     'se_bn_bwd': (c_int, [_P, _P, _P, c_int64, c_int, _P, _P, _P, c_int, c_int, _P, c_float, _P, c_float, _P, _P, _P, _P]),
+    'se_bn_bwd_path': (c_int, [c_int64, c_int, c_int]),
     'se_shortcut_bwd': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, POINTER(Residual), _P, c_float, _P]),
     'se_avgpool2_fwd': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     'se_avgpool2_bwd': (c_int, [_P, _P, c_float, c_int, c_int, c_int, c_int, _P]),

@@ -750,6 +750,30 @@ static int red_rows_per_cta(long long rows, int* grid) {
   return (int)per;
 }
 
+// The backward implementation of (rows, C) on a device with `sms` SMs (SE_BN_BWD_* in se_b200.h): the one decision that
+// bn_bwd launches and se_bn_bwd_path reports.  Host arithmetic only.  The slab paths also get their rows per CTA, grid
+// and dynamic shared memory.
+static constexpr size_t BNF_MAX_SMEM = 200 * 1024;   // shared-memory slab: dynamic shared memory limit per CTA
+static int bn_bwd_plan(long long rows, int C, int sms, long long* per_cta, int* grid, size_t* smem) {
+  if ((C & 3) != 0) return SE_BN_BWD_SCALAR;
+  // one slab of rows per CTA, a multiple of 4 rows, at most one CTA per SM (the grid barrier needs them co-resident)
+  long long per_l = ceil_div<long long>(rows, sms);
+  per_l = (per_l + 3) / 4 * 4;
+  const int gridf = (int)ceil_div<long long>(rows, per_l);
+  const size_t bytes = (size_t)per_l * C * 8 + 2 * C * sizeof(double) + 4 * C * sizeof(float) + 16;
+  if (per_cta) *per_cta = per_l;
+  if (grid) *grid = gridf;
+  if (smem) *smem = bytes;
+  static const bool no_fuse = getenv("SE_BN_NO_FUSE") != nullptr;
+  static const bool no_reg = getenv("SE_BN_NO_REG") != nullptr;
+  const int C4 = C >> 2;
+  if (!no_fuse && !no_reg && gridf <= sms && C <= BNR_MAXC && (512 % C4) == 0 && per_l * C4 <= (long long)BNR * 512)
+    return SE_BN_BWD_SLAB_REG;
+  if (!no_fuse && bytes <= BNF_MAX_SMEM && gridf <= sms)
+    return (512 % C4) == 0 ? SE_BN_BWD_SLAB_QUAD : SE_BN_BWD_SLAB_ATOMIC;   // bn_bwd_fused_kernel's fixed_quad (512 threads)
+  return SE_BN_BWD_VEC;
+}
+
 }  // namespace se
 
 using namespace se;
@@ -801,38 +825,32 @@ int se::bn_bwd(const float* x, const float* y, const float* dout, int64_t rows, 
                float beta_res, float* dgamma, float* dbeta, double* scratch, int early, void* stream) {
   SE_REQUIRE(x && dout && dx && gamma && save_mean && save_invstd && scratch && rows > 0 && C > 0, "bad arguments");
   SE_REQUIRE(!relu || y, "relu backward needs y");
-  if ((C & 3) == 0) {
-    // fused single-launch path when every CTA's slab of x and g fits in shared memory (one CTA per SM)
-    const int sms = sm_count();
-    long long per_l = ceil_div<long long>(rows, sms);
-    per_l = (per_l + 3) / 4 * 4;
-    const int gridf = (int)ceil_div<long long>(rows, per_l);
-    const size_t smem = (size_t)per_l * C * 8 + 2 * C * sizeof(double) + 4 * C * sizeof(float) + 16;
-    static const bool no_fuse = getenv("SE_BN_NO_FUSE") != nullptr;
-    static const bool no_reg = getenv("SE_BN_NO_REG") != nullptr;
-    static const char* bn_trace_env = getenv("SE_BN_TRACE_PTR");
-    long long* bn_trace = bn_trace_env ? reinterpret_cast<long long*>(strtoull(bn_trace_env, nullptr, 0)) : nullptr;
-    const int C4 = C >> 2;
-    if (!no_fuse && !no_reg && gridf <= sms && C <= BNR_MAXC && (512 % C4) == 0 && per_l * C4 <= (long long)BNR * 512) {
-      launch_grid_barrier(bn_bwd_reg_kernel, dim3(gridf), dim3(512), 0, as_stream(stream), x, y ? y : x, dout, rows, C, gamma, save_mean, save_invstd,
-             relu, relu_in, dx, beta_dx, dres, beta_res, dgamma, dbeta, scratch, (int)per_l, early && pdl_enabled() ? 1 : 0, bn_trace);
-      return check_launch("bn_bwd_reg_kernel");
-    }
-    if (!no_fuse && smem <= 200 * 1024 && gridf <= sms) {
-      static bool configured = false;
-      if (!configured) {
-        if (cudaFuncSetAttribute(bn_bwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) {
-          set_error("bn_bwd_fused: cannot raise the shared-memory limit");
-          return SE_ERR_CUDA;
-        }
-        configured = true;
+  long long per_l = 0;
+  int gridf = 0;
+  size_t smem = 0;
+  const int path = bn_bwd_plan(rows, C, sm_count(), &per_l, &gridf, &smem);
+  static const char* bn_trace_env = getenv("SE_BN_TRACE_PTR");
+  long long* bn_trace = bn_trace_env ? reinterpret_cast<long long*>(strtoull(bn_trace_env, nullptr, 0)) : nullptr;
+  if (path == SE_BN_BWD_SLAB_REG) {
+    launch_grid_barrier(bn_bwd_reg_kernel, dim3(gridf), dim3(512), 0, as_stream(stream), x, y ? y : x, dout, rows, C, gamma, save_mean, save_invstd,
+           relu, relu_in, dx, beta_dx, dres, beta_res, dgamma, dbeta, scratch, (int)per_l, early && pdl_enabled() ? 1 : 0, bn_trace);
+    return check_launch("bn_bwd_reg_kernel");
+  }
+  if (path == SE_BN_BWD_SLAB_QUAD || path == SE_BN_BWD_SLAB_ATOMIC) {
+    // fused single-launch path: every CTA's slab of x and g fits in shared memory (one CTA per SM)
+    static bool configured = false;
+    if (!configured) {
+      if (cudaFuncSetAttribute(bn_bwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BNF_MAX_SMEM) != cudaSuccess) {
+        set_error("bn_bwd_fused: cannot raise the shared-memory limit");
+        return SE_ERR_CUDA;
       }
-      // at least 116 KB per CTA would be needed to force one CTA per SM; co-residency only needs grid <= #SMs
-      launch_grid_barrier(bn_bwd_fused_kernel, dim3(gridf), dim3(512), smem, as_stream(stream), x, y, dout, rows, C, gamma, save_mean, save_invstd, relu,
-                                                                    relu_in, dx, beta_dx, dres, beta_res, dgamma, dbeta,
-                                                                    scratch, (int)per_l);
-      return check_launch("bn_bwd_fused_kernel");
+      configured = true;
     }
+    // at least 116 KB per CTA would be needed to force one CTA per SM; co-residency only needs grid <= #SMs
+    launch_grid_barrier(bn_bwd_fused_kernel, dim3(gridf), dim3(512), smem, as_stream(stream), x, y, dout, rows, C, gamma, save_mean, save_invstd, relu,
+                                                                  relu_in, dx, beta_dx, dres, beta_res, dgamma, dbeta,
+                                                                  scratch, (int)per_l);
+    return check_launch("bn_bwd_fused_kernel");
   }
   int grid;
   int per = red_rows_per_cta(rows, &grid);
@@ -845,6 +863,11 @@ int se::bn_bwd(const float* x, const float* y, const float* dout, int64_t rows, 
       x, y, dout, rows, C, gamma, save_mean, save_invstd, relu, relu_in, dx, beta_dx, dres, beta_res, dgamma, dbeta,
       scratch);
   return check_launch("bn_bwd_apply_kernel");
+}
+
+extern "C" int se_bn_bwd_path(int64_t rows, int C, int sms) {
+  SE_REQUIRE(rows > 0 && C > 0, "bad arguments");
+  return bn_bwd_plan(rows, C, sms > 0 ? sms : sm_count(), nullptr, nullptr, nullptr);
 }
 
 extern "C" int se_shortcut_bwd(const float* dout, const float* y, int relu, int N, int H, int W, int C,
