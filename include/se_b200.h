@@ -273,6 +273,28 @@ int se_softmax_xent_fwd_bwd_ex(const float* logits, int ld, const int32_t* label
 int se_softmax_xent_smooth_fwd_bwd(const float* logits, int ld, const int32_t* labels, int B, int C, float smoothing,
                                    float scale, float* prob, float* loss, float* acc, float* dlogits, float* rank_out,
                                    void* stream);
+/* the loss of the label embedding network (Sun et al.; learn_labelembedding.py:21-37) and its gradients.  out1, out2
+ * [B, ld] are the logits of 'prob' and 'out2', emb [C, ldE] the label-embedding table, tar = emb[y].  With
+ * p1 = softmax(out1), p2 = softmax(out2), q2 = softmax(out2 / tau), s = softmax(tar) and Keras' sparse cross-entropy on
+ * probabilities, sCE(p, y) = -log c_y + log sum_j c_j with c = clip(p, 1e-7, 1 - 1e-7) (gradient only where the clip is
+ * inactive):
+ *   mask_i   = argmax(out2_i) == y_i (first maximum)        F = B_eff / (sum_i mask_i + 1e-8)   (float32)
+ *   loss[i]  = beta sCE(p1, y) - (1-beta) sum_j s_j log_softmax(out1)_j + sCE(p2, y)
+ *              - sum_j q2_j log_softmax(tar)_j * mask_i * F + relu(p2_y - alpha)
+ *   acc[i]   = argmax(out1_i) == y_i (first maximum)
+ *   d_out1   = scale * (beta dsCE(p1, y)/dout1 + (1-beta) (p1 sum_j s_j - s))
+ *   d_out2   = scale * (dsCE(p2, y)/dout2 + [p2_y > alpha] p2_y (e_y - p2))      (q2, s and mask carry no gradient)
+ *   d_emb[c] = scale * F * sum_{i: y_i = c, mask_i} (s_i sum_j q2_ij - q2_i)   summed in increasing i; every row of
+ *              d_emb [C, ldE] is written (zeros for classes without such a sample)
+ * Rows with a label outside [0, C) (label < 0: padding) count neither in B_eff nor in sum mask; their loss, accuracy
+ * and gradients are 0.  B_eff is the number of the other rows.  loss, acc, d_out1, d_out2 and d_emb may be NULL.
+ * work: se_labelembed_workspace_bytes(B, C) bytes, 16-byte aligned; it starts with [B] float4
+ * {mask, CE(q2, softmax(tar)), beta sCE(p1) + (1-beta) CE(s, p1) + sCE(p2), relu term}.  1 <= B <= 8192, C >= 2,
+ * tau > 0; else SE_ERR_ARG.  Two launches, no float atomics: reruns give the same bits. */
+int64_t se_labelembed_workspace_bytes(int B, int C);
+int se_labelembed_fwd_bwd(const float* out1, const float* out2, int ld, const int32_t* labels, const float* emb, int ldE,
+                          int B, int C, float tau, float alpha, float beta, float scale, float* loss, float* acc,
+                          float* d_out1, float* d_out2, float* d_emb, void* work, void* stream);
 
 /* ------------------------------------------------------------------ optimizer
  * keras.optimizers.SGD(lr, momentum, decay, nesterov, clipnorm) + kernel_regularizer=l2(.)

@@ -1,0 +1,172 @@
+#!/usr/bin/env python
+"""Drop-in for the reference's learn_labelembedding.py (same flags, same feature pickles) on the H100-native engine: the
+label embedding network of Sun et al., a classifier that learns a soft target distribution per class alongside.
+Reference: learn_labelembedding.py:17-208.
+
+What each part of the reference script maps to:
+  build_network(embed_dim, arch) (:123)           -> semantic_embeddings_b200.utils.build_network (resnet-110: the 64-d
+                                                     pool, embed_dim ignored)
+  labelembed_model (:40-56), labelembed_loss (:21-37)
+                                                  -> engine.Engine(objective='labelembed', tau, alpha, beta): relu ->
+                                                     'embedding_bn' -> 'prob' / stop-gradient 'out2', the identity-initialised
+                                                     table 'labelembeddings/embeddings'; the five-term loss, its mask
+                                                     normalisation and every gradient are one op (se_labelembed_fwd_bwd)
+  SGD(sgd_lr, decay, momentum 0.9, nesterov, clipnorm) under SGDR (:158-178)
+                                                  -> the engine's SGD; the table's gradient is part of the clip norm
+  --finetune / --finetune_init (:137-155)         -> Engine.set_trainable: only embedding, embedding_bn, prob, out2,
+                                                     labelembeddings and the base network's last layer train
+  multi_gpu_model (:122-130)                      -> one process per GPU; every replica normalises the mask over its own
+                                                     slice of the batch, as the towers do
+  evaluate_generator (:181)                       -> the same list: [loss, prob_loss (= 0), labelembed_loss_loss, prob_acc]
+  weight / model dumps (:193-202)                 -> pickles of {'architecture', 'weights': {Keras weight name: array}}
+  feature dump (:205-208)                         -> identical pickle: {'feat': {test index: (d,) float32}} of the raw
+                                                     output of the base network
+Deviations, all stated at run time when they apply:
+  * the reference's 'Accuracy' / 'Average Accuracy' lines (:182-190) feed the two-input model only the images, which
+    raises inside a bare `except`, so the reference never prints them; this script prints both, computed from
+    argmax(out1) as the code intends;
+  * --finetune reads this package's own dumps (pickle / .npz of Keras-named arrays), not Keras HDF5; --log_dir is
+    accepted and ignored with a message; validation runs with --batch_size (its last batch is padded with rows that
+    take no part in the loss's normalisation);
+  * --gpus N > 1: launch with `python -m torch.distributed.run --nproc-per-node N learn_labelembedding.py ...`;
+  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles) and 'synthetic[:n]'; LR schedule: SGDR;
+  * --arith selects the arithmetic of the convolutions (see learn_image_embeddings.py).
+"""
+import argparse
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+from semantic_embeddings_b200 import trainer, utils  # noqa: E402
+from semantic_embeddings_b200.datasets import get_data_generator  # noqa: E402  (re-exported like the reference's import)
+from semantic_embeddings_b200.trainer import load_weights_by_name, read_class_list  # noqa: E402,F401
+
+# the layers --finetune_init trains first (learn_labelembedding.py:143), besides the base network's last layer (:144)
+NEW_LAYERS = ('embedding', 'embedding_bn', 'prob', 'out2', 'labelembeddings')
+
+
+def build_parser():
+    """learn_labelembedding.py:68-99 -- same flags, types and defaults, plus --arith."""
+    parser = argparse.ArgumentParser(description='Trains a label embedding network (Sun et al.).',
+                                     formatter_class=argparse.ArgumentDefaultsHelpFormatter)
+    g = parser.add_argument_group('Data parameters')
+    g.add_argument('--dataset', type=str, required=True, help='Training dataset.')
+    g.add_argument('--data_root', type=str, required=True, help='Root directory of the dataset.')
+    g.add_argument('--class_list', type=str, default=None,
+                   help='Path to a file containing the IDs of the subset of classes to be used (as first words per line).')
+    g = parser.add_argument_group('Label embedding parameters')
+    g.add_argument('--embed_dim', type=int, default=100, help='Embedding dimensionality.')
+    g.add_argument('--tau', type=float, default=2., help='Softmax temperature.')
+    g.add_argument('--alpha', type=float, default=0.9)
+    g.add_argument('--beta', type=float, default=0.5)
+    g = parser.add_argument_group('Training parameters')
+    g.add_argument('--architecture', type=str, default='simple', choices=utils.REFERENCE_ARCHITECTURES,
+                   help='Type of network architecture.')
+    g.add_argument('--lr_schedule', type=str, default='SGDR', choices=utils.LR_SCHEDULES, help='Type of learning rate schedule.')
+    g.add_argument('--clipgrad', type=float, default=10.0, help='Gradient norm clipping.')
+    g.add_argument('--max_decay', type=float, default=0.0, help='Learning Rate decay at the end of training.')
+    g.add_argument('--nesterov', action='store_true', default=False, help='Use Nesterov momentum instead of standard momentum.')
+    g.add_argument('--epochs', type=int, default=None, help='Number of training epochs.')
+    g.add_argument('--batch_size', type=int, default=100, help='Batch size.')
+    g.add_argument('--val_batch_size', type=int, default=None, help='Validation batch size.')
+    g.add_argument('--finetune', type=str, default=None,
+                   help='Path to pre-trained weights to be fine-tuned (will be loaded by layer name).')
+    g.add_argument('--finetune_init', type=int, default=3,
+                   help='Number of initial epochs for training just the new layers before fine-tuning.')
+    g.add_argument('--gpus', type=int, default=1, help='Number of GPUs to be used.')
+    g.add_argument('--read_workers', type=int, default=8, help='Number of parallel data pre-processing processes.')
+    g.add_argument('--queue_size', type=int, default=100, help='Maximum size of data queue.')
+    g.add_argument('--gpu_merge', action='store_true', default=False, help='Merge weights on the GPU.')
+    g = parser.add_argument_group('Output parameters')
+    g.add_argument('--model_dump', type=str, default=None,
+                   help='Filename where the learned model definition and weights should be written to.')
+    g.add_argument('--weight_dump', type=str, default=None,
+                   help='Filename where the learned model weights should be written to (without model definition).')
+    g.add_argument('--feature_dump', type=str, default=None,
+                   help='Filename where learned embeddings for test images should be written to.')
+    g.add_argument('--log_dir', type=str, default=None, help='Tensorboard log directory.')
+    g.add_argument('--no_progress', action='store_true', default=False,
+                   help='Do not display training progress, but just the final performance.')
+    g.add_argument('--arith', type=str, default='tf32x3', choices=['tf32x3', 'f32', 'tf32'],
+                   help='(new) arithmetic of the convolution kernels, see learn_image_embeddings.py')
+    utils.add_lr_schedule_arguments(parser)
+    return parser
+
+
+def finetune_layers(graph):
+    """The layer names --finetune_init trains: NEW_LAYERS and the base network's last layer."""
+    top = graph.output.producer
+    return set(NEW_LAYERS) | ({top.name} if top is not None else set())
+
+
+def l2_term(eng):
+    """The regularisation losses Keras adds to the total loss: sum of l2 * ||w||^2 over the regularised weights."""
+    w = eng.get_weights()
+    return float(sum(spec.l2 * float(np.sum(np.square(w[n], dtype=np.float64)))
+                     for n, spec in eng.pspecs.items() if spec.l2 > 0))
+
+
+def main(argv=None):
+    args = build_parser().parse_args(argv)
+    if args.val_batch_size is None:
+        args.val_batch_size = args.batch_size
+    # snapshot flags the shared epoch loop reads; the reference's script has none of them
+    args.snapshot, args.snapshot_best, args.initial_epoch = None, None, 0
+
+    from semantic_embeddings_b200.engine import Engine
+    from semantic_embeddings_b200.parallel import broadcast_parameters
+
+    local, rank, world, say = trainer.init_distributed(args)
+
+    # Load dataset (learn_labelembedding.py:110-119)
+    class_list = read_class_list(args.class_list) if args.class_list is not None else None
+    data = get_data_generator(args.dataset, args.data_root, classes=class_list, device='cuda:%d' % local)
+
+    graph = utils.build_network(args.embed_dim, args.architecture, input_channels=data.num_channels)
+    mode = trainer.arith_mode(args, say)
+    callbacks, epochs, decay = trainer.schedule(args, data)        # learn_labelembedding.py:158,165-168
+    pb = args.batch_size // world
+    eng = Engine(graph, pb, objective='labelembed', num_classes=data.num_classes, tau=args.tau, alpha=args.alpha,
+                 beta=args.beta, mode=mode, device='cuda:%d' % local, nesterov=args.nesterov, clipnorm=args.clipgrad,
+                 world_size=world, decay=decay)
+    broadcast_parameters([eng.P, eng.S, eng.V, eng.lr_dev])
+    if not args.no_progress:
+        say('{}: {} layers, {} trainable parameters'.format(args.architecture, len(eng.nodes),
+                                                            sum(int(np.prod(s)) for _, s in eng.offsets.values())))
+
+    ks = ()
+    rng = np.random.RandomState(1234)          # identical stream on every rank: the permutation is shared, slices differ
+
+    # Load pre-trained weights and train the new layers for a few epochs (learn_labelembedding.py:137-155)
+    if args.finetune:
+        say('Loading pre-trained weights from {}'.format(args.finetune))
+        loaded, skipped = load_weights_by_name(eng, args.finetune)
+        say('  {} tensors loaded, {} skipped (unknown name or shape mismatch)'.format(len(loaded), len(skipped)))
+        broadcast_parameters([eng.P, eng.S])
+        if args.finetune_init > 0:
+            say('Pre-training new layers')
+            trainer.pretrain_new_layers(eng, data, args, finetune_layers(graph), rng, rank, world, ks, say)
+            say('Full model training')
+
+    trainer.fit(eng, data, args, callbacks[0], epochs, rng, rank, world, ks, say)
+
+    # Evaluate final performance (learn_labelembedding.py:181-190)
+    val, pred = trainer.run_validation(eng, data, ks, None)
+    if rank == 0:
+        say([val['loss'] + l2_term(eng), 0.0, val['loss'], val['acc']])
+        labels = np.asarray(data.labels_test)
+        say('Accuracy: {:.4f}'.format(np.mean(pred == labels)))
+        say('Average Accuracy: {:.4f}'.format(trainer.average_accuracy(pred, labels)))
+        trainer.dump_weights(eng, args)
+        if args.feature_dump:                                  # learn_labelembedding.py:205-208
+            trainer.dump_features(eng, data, graph.output.name, args.feature_dump)
+    return 0
+
+
+if __name__ == '__main__':
+    sys.exit(main())

@@ -430,6 +430,13 @@ static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* f
           rc = se_softmax_xent_fwd_bwd_ex((const float*)p[0], i[0], (const int32_t*)p[1], i[1], i[2], f[0], (float*)p[2],
                                           (float*)p[3], (float*)p[4], (float*)p[5], (float*)p[6], stream);
         break;
+      case SE_OP_LABELEMBED:
+        // i: ld, ldE, B, C;  f: scale, tau, alpha, beta;
+        // p: 0 out1, 1 out2, 2 labels, 3 table, 4 loss, 5 acc, 6 d_out1, 7 d_out2, 8 d_table, 9 workspace
+        rc = se_labelembed_fwd_bwd((const float*)p[0], (const float*)p[1], i[0], (const int32_t*)p[2], (const float*)p[3],
+                                   i[1], i[2], i[3], f[1], f[2], f[3], f[0], (float*)p[4], (float*)p[5], (float*)p[6],
+                                   (float*)p[7], (float*)p[8], p[9], stream);
+        break;
       case SE_OP_MEMSET: {
         if (i[0] & 1) {
           // a memset of GRADIENT memory (frozen parameters, Engine.set_trainable): the weight-gradient kernels of the side

@@ -27,4 +27,5 @@ enum {
   SE_OP_CONV_BN_FWD = 23,
   SE_OP_ALLREDUCE = 24,
   SE_OP_ADAGRAD_APPLY = 25,
+  SE_OP_LABELEMBED = 26,
 };

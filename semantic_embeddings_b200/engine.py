@@ -8,6 +8,7 @@ per-GPU batch, and pre-builds three `se_op` arrays (training forward, backward, 
 PyTorch is used only for device memory, streams, CUDA-graph capture and `torch.distributed`.
 """
 import ctypes
+import math
 from collections import OrderedDict
 
 import numpy as np
@@ -15,7 +16,7 @@ import torch
 
 from . import _lib
 from ._lib import Op
-from .graph import Graph, Node, T
+from .graph import Graph, Node, ParamSpec, T
 
 LOSS_KINDS = {'inv_corr': _lib.SE_LOSS_INV_CORR, 'unnorm_corr': _lib.SE_LOSS_UNNORM_CORR, 'mse': _lib.SE_LOSS_MSE,
               'softmax_corr': _lib.SE_LOSS_SOFTMAX_CORR, 'devise_rank': _lib.SE_LOSS_DEVISE_RANK}
@@ -31,7 +32,8 @@ def _vp(x):
     return int(x)
 
 
-OBJECTIVES = ('embedding', 'softmax')
+OBJECTIVES = ('embedding', 'softmax', 'labelembed')
+LABELEMBED_TABLE = 'labelembeddings/embeddings'
 
 
 class Engine:
@@ -46,6 +48,13 @@ class Engine:
     loss='devise_rank' (learn_devise.py): the DeViSE hinge ranking loss on the raw output with margin `margin` (0.1 by
     default); its metric is max_sim_acc, as for 'unnorm_corr'.
 
+    objective='labelembed' (learn_labelembedding.py, Sun et al.): the graph's output z is the raw embedding; on top of
+    it the engine builds relu -> BatchNormalization 'embedding_bn' -> Dense(C) 'prob' (out1) and, on the same input
+    behind a stop-gradient, Dense(C) 'out2', plus the trainable C x C table 'labelembeddings/embeddings' (identity
+    init, no L2).  One op in the forward plan (se_labelembed_fwd_bwd, temperature `tau`, `alpha`, `beta`) computes the
+    per-sample loss, argmax(out1) accuracy and the gradients of out1, out2 and the table; the table's gradient goes
+    straight into the flat gradient buffer.  The metrics are 'loss' and 'acc'.  The infer plan ends at the logits.
+
     optimizer='sgd': Keras SGD(lr, momentum (0.9 by default), decay, nesterov, clipnorm).  optimizer='adagrad': Keras
     Adagrad(lr, epsilon, decay) with the same optional clipnorm; its accumulators live where SGD keeps its velocity
     (get_velocity / set_velocity), and it takes no momentum."""
@@ -54,7 +63,7 @@ class Engine:
                  mode=_lib.SE_MODE_F32, device='cuda:0', momentum=None, nesterov=False, clipnorm=10.0,
                  world_size=1, fuse_stats=True, use_cuda_graph=True, seed=0, decay=0.0,
                  grad_buckets=3, comm='auto', cls_base=None, objective='embedding', label_smoothing=0.0,
-                 margin=None, optimizer='sgd', epsilon=1e-7):
+                 margin=None, optimizer='sgd', epsilon=1e-7, tau=None, alpha=None, beta=None):
         if loss not in LOSS_KINDS:
             raise ValueError('unknown loss %r' % loss)
         if margin is not None and loss != 'devise_rank':
@@ -71,7 +80,21 @@ class Engine:
             raise ValueError('unknown objective %r (one of %s)' % (objective, ', '.join(OBJECTIVES)))
         self.objective = objective
         self.label_smoothing = float(label_smoothing)
-        if objective == 'softmax':
+        if objective != 'labelembed' and (tau is not None or alpha is not None or beta is not None):
+            raise ValueError("tau, alpha and beta belong to objective='labelembed'")
+        self.tau = float(2.0 if tau is None else tau)
+        self.alpha = float(0.9 if alpha is None else alpha)
+        self.beta = float(0.5 if beta is None else beta)
+        if objective == 'labelembed':
+            if embedding is not None:
+                raise ValueError("objective='labelembed' learns its own label embedding: it takes no class embedding")
+            if cls_weight or self.label_smoothing != 0.0 or margin is not None:
+                raise ValueError("cls_weight, label_smoothing and margin do not apply to objective='labelembed'")
+            if num_classes is None:
+                raise ValueError("objective='labelembed' needs num_classes")
+            if not (self.tau > 0.0 and math.isfinite(self.tau)):
+                raise ValueError('the temperature tau must be positive and finite')
+        elif objective == 'softmax':
             if embedding is not None:
                 raise ValueError("objective='softmax' trains a classifier: it takes no class embedding")
             if cls_weight:
@@ -114,6 +137,12 @@ class Engine:
             self.C = self.D = graph.output.shape[0]
             if num_classes is not None and int(num_classes) != self.C:
                 raise ValueError('network output %s does not match the %d classes' % (graph.output.shape, int(num_classes)))
+            self.E = None
+        elif objective == 'labelembed':
+            if len(graph.output.shape) != 1:
+                raise ValueError('network output %s is not a feature vector' % (graph.output.shape,))
+            self.D = graph.output.shape[0]
+            self.C = int(num_classes)
             self.E = None
         else:
             emb = np.asarray(embedding, dtype=np.float32)
@@ -182,9 +211,29 @@ class Engine:
             self.nodes.append(xe)
             self.head_node = None
             self.xent_node = xe
+            self.le_node = None
             self.has_cls_branch = False
             self._index_consumers()
             return
+        if self.objective == 'labelembed':
+            # labelembed_model (learn_labelembedding.py:40-56): relu -> BatchNormalization('embedding_bn') -> Dense(C, 'prob')
+            # = out1, Dense(C, 'out2') on stop_gradient of the same tensor, and the label-indexed C x C table
+            sub, b, out1 = self._relu_bn_dense(z, 'labelembed_relu', 'embedding_bn', 'prob', l2=0.0)
+            out2 = sub.dense(b, 'out2', self.num_classes, stop_gradient=True)
+            self.nodes += sub.nodes
+            self.pspecs.update(sub.params)
+            self.pspecs[LABELEMBED_TABLE] = ParamSpec(LABELEMBED_TABLE, (self.num_classes, self.num_classes), 'identity')
+            lo = T('labelembed_loss', (1,))
+            le = Node('labelembed', 'labelembed_loss', [out1, out2], lo, params=[LABELEMBED_TABLE])
+            lo.producer = le
+            self.nodes.append(le)
+            self.head_node = None
+            self.xent_node = None
+            self.le_node = le
+            self.has_cls_branch = False
+            self._index_consumers()
+            return
+        self.le_node = None
         x_out = T('head_out', (self.D,))
         head = Node('head', 'head', [z], x_out)
         x_out.producer = head
@@ -203,11 +252,7 @@ class Engine:
                 if len(base.shape) != 1:
                     raise ValueError('cls_base %r has a %d-d output %s: the classifier needs a feature vector (e.g. avg_pool)'
                                      % (self.cls_base, len(base.shape), tuple(base.shape)))
-            sub = Graph('cls', tuple(base.shape))
-            sub.input = base
-            r = sub.relu(base, 'cls_relu')
-            b = sub.bn(r, 'cls_bn')
-            logits = sub.dense(b, 'prob', self.num_classes, l2=5e-4)
+            sub, _, logits = self._relu_bn_dense(base, 'cls_relu', 'cls_bn', 'prob', l2=5e-4)
             self.nodes += sub.nodes
             self.pspecs.update(sub.params)
             prob = T('prob_out', (self.num_classes,))
@@ -217,6 +262,15 @@ class Engine:
             self.xent_node = xe
         self.has_cls_branch = self.xent_node is not None     # the --cls_weight classifier beside the embedding head
         self._index_consumers()
+
+    def _relu_bn_dense(self, base, relu_name, bn_name, dense_name, l2):
+        """relu -> BatchNormalization() -> Dense(num_classes) on tensor `base`, as a sub-graph: (graph, BN output, logits).
+        The classifier branch of cls_model and the label embedding branch share it."""
+        sub = Graph('cls', tuple(base.shape))
+        sub.input = base
+        r = sub.relu(base, relu_name)
+        b = sub.bn(r, bn_name)
+        return sub, b, sub.dense(b, dense_name, self.num_classes, l2=l2)
 
     def _index_consumers(self):
         self.consumers = {}
@@ -286,6 +340,12 @@ class Engine:
         self.cls_acc_buf = torch.zeros(B, **f32)
         self.rank_buf = torch.zeros(B, **f32)          # top-k metrics: rank of the true class (se_embed_head_fwd_bwd_ex)
         self.cls_rank_buf = torch.zeros(B, **f32)
+        self.le_work = None                            # se_labelembed_fwd_bwd's workspace (per-row terms, table-gradient rows)
+        if self.le_node is not None:
+            nb = int(self.lib.se_labelembed_workspace_bytes(B, self.num_classes))
+            if nb < 0:
+                raise ValueError('se_labelembed_workspace_bytes(%d, %d) failed' % (B, self.num_classes))
+            self.le_work = torch.zeros((nb + 15) // 16 * 4, **f32)
         # BatchNorm scratch: per BN [fwd sums 2C | bwd sums 2C] float64, saved mean / invstd
         self.bn_slot, tot = {}, 0
         for n in self.nodes:
@@ -492,6 +552,19 @@ class Engine:
                 self._eval_xent = self._op(_lib.OP_XENT, [self.num_classes, self.B, self.num_classes], [0.0],
                                            [A[lg.name], self.labels, out, self.cls_loss_buf, self.cls_acc_buf, None,
                                             self.cls_rank_buf])
+            elif n.op == 'labelembed':
+                # the whole loss (weight 1), in the forward plan like the softmax objective's cross-entropy; it writes the
+                # gradients of both logit heads and the table's gradient (into G, which the backward memset spares)
+                o1, o2 = n.inputs
+                C = self.num_classes
+                ii = [C, C, self.B, C]
+                table = self._pview(LABELEMBED_TABLE)
+                fwd.append(self._op(_lib.OP_LABELEMBED, ii, [scale, self.tau, self.alpha, self.beta],
+                                    [A[o1.name], A[o2.name], self.labels, table, self.loss_buf, self.acc_buf, Gd[o1.name],
+                                     Gd[o2.name], self._pview(LABELEMBED_TABLE, self.G), self.le_work]))
+                self._eval_le = self._op(_lib.OP_LABELEMBED, ii, [0.0, self.tau, self.alpha, self.beta],
+                                         [A[o1.name], A[o2.name], self.labels, table, self.loss_buf, self.acc_buf, None,
+                                          None, None, self.le_work])
             else:
                 raise ValueError(n.op)
         # ---------------- backward
@@ -506,13 +579,22 @@ class Engine:
             written.add(t.name)
             return Gd[t.name], beta
 
-        bwd.append(self._op(_lib.OP_MEMSET, p=[self.G, nbytes(self.G)]))
+        if self.le_node is not None:
+            # the forward plan has already written the table's gradient; the table is the last tensor of the flat buffer
+            # (L2 0, added last), so the memset clears everything before it
+            t_off, t_shape = self.offsets[LABELEMBED_TABLE]
+            assert t_off + (int(np.prod(t_shape)) + 3) // 4 * 4 == self.nparams, 'the label table must end the gradient buffer'
+            bwd.append(self._op(_lib.OP_MEMSET, p=[self.G, 4 * t_off]))
+            final[LABELEMBED_TABLE] = 0
+            written.update(t.name for t in self.le_node.inputs)
+        else:
+            bwd.append(self._op(_lib.OP_MEMSET, p=[self.G, nbytes(self.G)]))
         if self.xent_node is not None:
             written.add(self.xent_node.inputs[0].name)
         if self.head_node is not None and not self.consumers.get(self.head_node.output.name):
             written.add(self.head_node.inputs[0].name)
         for n in reversed(self.nodes):
-            if n.op == 'xent':
+            if n.op in ('xent', 'labelembed'):
                 continue
             dY = Gd[n.output.name]
             if n.op == 'head':
@@ -534,7 +616,7 @@ class Engine:
                 final[n.name + '/kernel'] = len(bwd)
                 if n.attrs['use_bias']:
                     final[n.name + '/bias'] = len(bwd)
-                dx, beta = gb(x)
+                dx, beta = gb(x) if not n.attrs.get('stop_gradient') else (None, 0.0)
                 if dx is not None:
                     Wl = self._pview(n.name + '/kernel', self.PL) if (self.PL is not None and n.op == 'conv') else None
                     bwd.append(self._op(_lib.OP_CONV_DGRAD, d, [beta], [dY, W, dx, Wl]))
@@ -612,6 +694,8 @@ class Engine:
                 ev.append(self._eval_xent)
             else:
                 ev.append(o)
+        if self.le_node is not None:
+            ev.append(self._eval_le)
         self.plans = {'fwd': self._pack(fwd), 'bwd': self._pack(bwd), 'opt': self._pack(opt), 'infer': self._pack(inf),
                       'eval': self._pack(ev),
                       'fwdbwd': self._pack(fwd + bwd), 'step': self._pack(fwd + bwd + opt)}
@@ -883,12 +967,16 @@ class Engine:
 
     def predict(self, x):
         """Inference forward (BatchNorm moving statistics), returns the wrapped embeddings (B,D) -- or, for
-        objective='softmax', the class probabilities (B,C) -- as numpy."""
+        objective='softmax', the class probabilities (B,C), for objective='labelembed' the logits of 'prob' (B,C) -- as
+        numpy."""
         x = torch.as_tensor(x)
         self.x.copy_(x, non_blocking=True)
         self._run('infer')
         torch.cuda.synchronize(self.dev)
-        out = self.head_node.output if self.head_node is not None else self.xent_node.output
+        if self.le_node is not None:
+            out = self.le_node.inputs[0]
+        else:
+            out = self.head_node.output if self.head_node is not None else self.xent_node.output
         return self.act[out.name].detach().cpu().numpy().copy()
 
     def activation(self, name_prefix):

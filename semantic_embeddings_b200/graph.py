@@ -97,13 +97,18 @@ class Graph:
                               dict(k=k, stride=stride, pad_t=pt, pad_l=pl, use_bias=use_bias, relu=relu,
                                    residual=residual is not None), params))
 
-    def dense(self, x, name, units, use_bias=True, relu=False, l2=0.0):
+    def dense(self, x, name, units, use_bias=True, relu=False, l2=0.0, stop_gradient=False):
+        """Dense (+ optional fused ReLU).  stop_gradient=True: Dense(...)(Lambda(K.stop_gradient)(x)) -- the layer's
+        weights train, but no gradient flows back into x through it."""
         (cin,) = x.shape
         params = [self._param(name + '/kernel', (cin, units), 'glorot_uniform', l2)]
         if use_bias:
             params.append(self._param(name + '/bias', (units,), 'zeros'))
         out = self._tensor(name, (units,))
-        return self._add(Node('dense', name, [x], out, dict(use_bias=use_bias, relu=relu), params))
+        attrs = dict(use_bias=use_bias, relu=relu)
+        if stop_gradient:
+            attrs['stop_gradient'] = True
+        return self._add(Node('dense', name, [x], out, attrs, params))
 
     def bn(self, x, name, momentum=0.99, eps=1e-3, relu=False, residual=None, res_pool=1, res_pad_lo=0,
            gamma_init='ones'):
@@ -175,6 +180,8 @@ class Graph:
                 a = np.zeros(p.shape, np.float32)
             elif p.init == 'ones':
                 a = np.ones(p.shape, np.float32)
+            elif p.init == 'identity':           # Keras Identity(gain=1) of a square matrix; draws nothing
+                a = np.eye(p.shape[0], p.shape[1], dtype=np.float32)
             elif p.init == 'uniform':            # Keras RandomUniform(-0.05, 0.05), wide_residual_network.py:14
                 a = rng.uniform(-0.05, 0.05, p.shape).astype(np.float32)
             elif p.init == 'glorot_uniform':
