@@ -295,6 +295,19 @@ int64_t se_labelembed_workspace_bytes(int B, int C);
 int se_labelembed_fwd_bwd(const float* out1, const float* out2, int ld, const int32_t* labels, const float* emb, int ldE,
                           int B, int C, float tau, float alpha, float beta, float scale, float* loss, float* acc,
                           float* d_out1, float* d_out2, float* d_emb, void* work, void* stream);
+/* the center loss of Wen et al. (learn_center_loss.py:17-41) and its gradients.  z [B, ldz] is the raw embedding,
+ * cent [C, ldc] the class centroids (the 'cls_centroids' Embedding), labels [B] the classes.  For every row b with
+ * 0 <= y_b < C, d_b = z_b - cent[y_b]:
+ *   loss[b]    = 1/2 sum_j d_bj^2                                  (the unweighted per-sample center loss)
+ *   d_z[b]     = scale * d_b                                       (overwritten, not accumulated)
+ *   d_cent[k]  = -scale * sum_{b: y_b = k} (z_b - cent[k])         summed in increasing b; every row k of d_cent [C, ldc]
+ *                is written (zeros for a class without a sample)
+ * scale is the loss weight over the global batch (w / (B * world) for Keras' mean).  Rows with a label outside [0, C)
+ * (padding) get loss 0 and d_z 0 and take no part in d_cent.  Only the first D columns of every row are read or
+ * written.  loss, d_z and d_cent may each be NULL (skipped).  B, C, D >= 1, ldz >= D, ldc >= D, z, labels and cent not
+ * NULL; else SE_ERR_ARG.  One launch, no float atomics: reruns give the same bits. */
+int se_center_loss_fwd_bwd(const float* z, int ldz, const int32_t* labels, const float* cent, int ldc, int B, int C, int D,
+                           float scale, float* loss, float* d_z, float* d_cent, void* stream);
 
 /* ------------------------------------------------------------------ optimizer
  * keras.optimizers.SGD(lr, momentum, decay, nesterov, clipnorm) + kernel_regularizer=l2(.)

@@ -104,13 +104,6 @@ def finetune_layers(graph):
     return set(NEW_LAYERS) | ({top.name} if top is not None else set())
 
 
-def l2_term(eng):
-    """The regularisation losses Keras adds to the total loss: sum of l2 * ||w||^2 over the regularised weights."""
-    w = eng.get_weights()
-    return float(sum(spec.l2 * float(np.sum(np.square(w[n], dtype=np.float64)))
-                     for n, spec in eng.pspecs.items() if spec.l2 > 0))
-
-
 def main(argv=None):
     args = build_parser().parse_args(argv)
     if args.val_batch_size is None:
@@ -158,7 +151,7 @@ def main(argv=None):
     # Evaluate final performance (learn_labelembedding.py:181-190)
     val, pred = trainer.run_validation(eng, data, ks, None)
     if rank == 0:
-        say([val['loss'] + l2_term(eng), 0.0, val['loss'], val['acc']])
+        say([val['loss'] + trainer.l2_term(eng), 0.0, val['loss'], val['acc']])
         labels = np.asarray(data.labels_test)
         say('Accuracy: {:.4f}'.format(np.mean(pred == labels)))
         say('Average Accuracy: {:.4f}'.format(trainer.average_accuracy(pred, labels)))

@@ -22,7 +22,7 @@ SE_BN_BWD_SCALAR, SE_BN_BWD_SLAB_ATOMIC, SE_BN_BWD_SLAB_REG, SE_BN_BWD_VEC, SE_B
 OP_CONV_FWD, OP_CONV_DGRAD, OP_CONV_WGRAD, OP_BN_STATS, OP_BN_FWD_TRAIN, OP_BN_FWD_INFER, OP_BN_BWD, \
     OP_SHORTCUT_BWD, OP_AVGPOOL_FWD, OP_AVGPOOL_BWD, OP_MAXPOOL_FWD, OP_MAXPOOL_BWD, OP_GAP_FWD, OP_GAP_BWD, \
     OP_ADD_FWD, OP_ADD_BWD, OP_HEAD, OP_XENT, OP_MEMSET, OP_SGD_PREPARE, OP_SGD_APPLY, OP_TRANSPOSE_FILTERS, \
-    OP_CONV_BN_FWD, OP_ALLREDUCE, OP_ADAGRAD_APPLY, OP_LABELEMBED = range(1, 27)
+    OP_CONV_BN_FWD, OP_ALLREDUCE, OP_ADAGRAD_APPLY, OP_LABELEMBED, OP_CENTER_LOSS = range(1, 28)
 
 
 class SeError(RuntimeError):
@@ -98,6 +98,7 @@ _SIGS = {
     'se_labelembed_workspace_bytes': (c_int64, [c_int, c_int]),
     'se_labelembed_fwd_bwd': (c_int, [_P, _P, c_int, _P, _P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, _P, _P,
                                       _P, _P, _P, _P, _P]),
+    'se_center_loss_fwd_bwd': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_float, _P, _P, _P, _P]),
     'se_sgd_schedule': (c_int, [_P, _P]),
     'se_pairwise_topk_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'se_pairwise_topk': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, _P]),

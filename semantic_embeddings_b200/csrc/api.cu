@@ -437,6 +437,12 @@ static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* f
                                    i[1], i[2], i[3], f[1], f[2], f[3], f[0], (float*)p[4], (float*)p[5], (float*)p[6],
                                    (float*)p[7], (float*)p[8], p[9], stream);
         break;
+      case SE_OP_CENTER_LOSS:
+        // i: ldz, ldc, B, C, D;  f: scale (the loss weight over the global batch);
+        // p: 0 z, 1 labels, 2 centroids, 3 loss, 4 d_z, 5 d_centroids
+        rc = se_center_loss_fwd_bwd((const float*)p[0], i[0], (const int32_t*)p[1], (const float*)p[2], i[1], i[2], i[3],
+                                    i[4], f[0], (float*)p[3], (float*)p[4], (float*)p[5], stream);
+        break;
       case SE_OP_MEMSET: {
         if (i[0] & 1) {
           // a memset of GRADIENT memory (frozen parameters, Engine.set_trainable): the weight-gradient kernels of the side

@@ -28,4 +28,5 @@ enum {
   SE_OP_ALLREDUCE = 24,
   SE_OP_ADAGRAD_APPLY = 25,
   SE_OP_LABELEMBED = 26,
+  SE_OP_CENTER_LOSS = 27,
 };

@@ -32,8 +32,9 @@ def _vp(x):
     return int(x)
 
 
-OBJECTIVES = ('embedding', 'softmax', 'labelembed')
+OBJECTIVES = ('embedding', 'softmax', 'labelembed', 'center_loss')
 LABELEMBED_TABLE = 'labelembeddings/embeddings'
+CENTROIDS = 'cls_centroids/embeddings'
 
 
 class Engine:
@@ -55,6 +56,15 @@ class Engine:
     per-sample loss, argmax(out1) accuracy and the gradients of out1, out2 and the table; the table's gradient goes
     straight into the flat gradient buffer.  The metrics are 'loss' and 'acc'.  The infer plan ends at the logits.
 
+    objective='center_loss' (learn_center_loss.py, Wen et al.): the graph's output z is the raw embedding; on top of it
+    the engine builds relu -> BatchNormalization 'embedding_bn' -> Dense(C) 'prob' (no L2) with the one-hot
+    cross-entropy (weight 1), plus the C x D centroids 'cls_centroids/embeddings' (Keras 'uniform' init, no L2).  The
+    center loss w * mean_b 1/2 ||z_b - c_{y_b}||^2 (w = `center_loss_weight`, 0.1 by default) is one op at the head of
+    the backward plan (se_center_loss_fwd_bwd): it writes the gradient of z first and the centroids' gradient into the
+    flat gradient buffer.  `centroids` (a C x D array) fixes the centroids: they are set from it and frozen with
+    set_trainable, which set_trainable(None) undoes.  The metrics are 'loss' (prob cross-entropy + w * center loss),
+    'prob_loss', 'center_loss' (unweighted) and 'acc'.  The infer plan ends at the class probabilities.
+
     optimizer='sgd': Keras SGD(lr, momentum (0.9 by default), decay, nesterov, clipnorm).  optimizer='adagrad': Keras
     Adagrad(lr, epsilon, decay) with the same optional clipnorm; its accumulators live where SGD keeps its velocity
     (get_velocity / set_velocity), and it takes no momentum."""
@@ -63,7 +73,8 @@ class Engine:
                  mode=_lib.SE_MODE_F32, device='cuda:0', momentum=None, nesterov=False, clipnorm=10.0,
                  world_size=1, fuse_stats=True, use_cuda_graph=True, seed=0, decay=0.0,
                  grad_buckets=3, comm='auto', cls_base=None, objective='embedding', label_smoothing=0.0,
-                 margin=None, optimizer='sgd', epsilon=1e-7, tau=None, alpha=None, beta=None):
+                 margin=None, optimizer='sgd', epsilon=1e-7, tau=None, alpha=None, beta=None, center_loss_weight=None,
+                 centroids=None):
         if loss not in LOSS_KINDS:
             raise ValueError('unknown loss %r' % loss)
         if margin is not None and loss != 'devise_rank':
@@ -85,7 +96,23 @@ class Engine:
         self.tau = float(2.0 if tau is None else tau)
         self.alpha = float(0.9 if alpha is None else alpha)
         self.beta = float(0.5 if beta is None else beta)
-        if objective == 'labelembed':
+        if objective != 'center_loss' and (center_loss_weight is not None or centroids is not None):
+            raise ValueError("center_loss_weight and centroids belong to objective='center_loss'")
+        self.center_loss_weight = float(0.1 if center_loss_weight is None else center_loss_weight)
+        if objective == 'center_loss':
+            if embedding is not None:
+                raise ValueError("objective='center_loss' learns its own class centroids: it takes no class embedding")
+            if cls_weight or self.label_smoothing != 0.0 or margin is not None:
+                raise ValueError("cls_weight, label_smoothing and margin do not apply to objective='center_loss'")
+            if num_classes is None:
+                raise ValueError("objective='center_loss' needs num_classes")
+            if not math.isfinite(self.center_loss_weight):
+                raise ValueError('the center loss weight must be finite')
+            if centroids is not None:
+                centroids = np.asarray(centroids, dtype=np.float64)
+                if not np.isfinite(centroids).all():
+                    raise ValueError('the fixed centroids must be finite')
+        elif objective == 'labelembed':
             if embedding is not None:
                 raise ValueError("objective='labelembed' learns its own label embedding: it takes no class embedding")
             if cls_weight or self.label_smoothing != 0.0 or margin is not None:
@@ -138,12 +165,15 @@ class Engine:
             if num_classes is not None and int(num_classes) != self.C:
                 raise ValueError('network output %s does not match the %d classes' % (graph.output.shape, int(num_classes)))
             self.E = None
-        elif objective == 'labelembed':
+        elif objective in ('labelembed', 'center_loss'):
             if len(graph.output.shape) != 1:
                 raise ValueError('network output %s is not a feature vector' % (graph.output.shape,))
             self.D = graph.output.shape[0]
             self.C = int(num_classes)
             self.E = None
+            if centroids is not None and centroids.shape != (self.C, self.D):
+                raise ValueError('the fixed centroids are %s, but the %d classes and the %d-d network output need (%d, %d)'
+                                 % (centroids.shape, self.C, self.D, self.C, self.D))
         else:
             emb = np.asarray(embedding, dtype=np.float32)
             self.C, self.D = emb.shape
@@ -156,6 +186,10 @@ class Engine:
         self._build_plans()
         self._graphs = {}
         self.iterations = 0
+        if centroids is not None:
+            # learn_center_loss.py:31-33: set_weights([centroids]) and trainable = False
+            self.set_weights({CENTROIDS: centroids})
+            self.set_trainable(lambda n: n != CENTROIDS)
 
     def _init_native_comm(self, required):
         """se_comm_init over the ranks of the default torch.distributed group (which only carries the 128-byte NCCL id)."""
@@ -202,6 +236,30 @@ class Engine:
         self.nodes = list(g.nodes)
         self.pspecs = OrderedDict(g.params)
         z = g.output
+        self.center_node = None
+        if self.objective == 'center_loss':
+            # center_loss_model (learn_center_loss.py:17-41): relu -> BatchNormalization('embedding_bn') -> Dense(C,
+            # softmax, 'prob') with the one-hot cross-entropy, and the label-indexed C x D centroids compared with z itself;
+            # the centroids come after the branch's weights, so the initial values of those do not change
+            sub, _, logits = self._relu_bn_dense(z, 'center_loss_relu', 'embedding_bn', 'prob', l2=0.0)
+            self.nodes += sub.nodes
+            self.pspecs.update(sub.params)
+            prob = T('prob_out', (self.num_classes,))
+            xe = Node('xent', 'xent', [logits], prob)
+            prob.producer = xe
+            self.nodes.append(xe)
+            self.pspecs[CENTROIDS] = ParamSpec(CENTROIDS, (self.num_classes, self.D), 'uniform')
+            cl = T('center_loss', (1,))
+            cn = Node('center_loss', 'center_loss', [z], cl, params=[CENTROIDS])
+            cl.producer = cn
+            self.nodes.append(cn)
+            self.head_node = None
+            self.xent_node = xe
+            self.le_node = None
+            self.center_node = cn
+            self.has_cls_branch = False
+            self._index_consumers()
+            return
         if self.objective == 'softmax':
             # learn_classifier.py: Dense(C, softmax, name='prob') + categorical_crossentropy -- the softmax and the loss are
             # one op on the logits, whose gradient seeds the backward pass
@@ -340,6 +398,7 @@ class Engine:
         self.cls_acc_buf = torch.zeros(B, **f32)
         self.rank_buf = torch.zeros(B, **f32)          # top-k metrics: rank of the true class (se_embed_head_fwd_bwd_ex)
         self.cls_rank_buf = torch.zeros(B, **f32)
+        self.center_buf = torch.zeros(B, **f32)        # objective='center_loss': per-sample 1/2 ||z - c_y||^2
         self.le_work = None                            # se_labelembed_fwd_bwd's workspace (per-row terms, table-gradient rows)
         if self.le_node is not None:
             nb = int(self.lib.se_labelembed_workspace_bytes(B, self.num_classes))
@@ -531,8 +590,8 @@ class Engine:
                 inf.append(self._op(_lib.OP_HEAD, ii, ff, [z, self.labels, self.E, None, out, None, None, None]))
                 self._eval_head = self._op(_lib.OP_HEAD, ii, ff, [z, self.labels, self.E, None, out, self.loss_buf,
                                                                    self.acc_buf, None, self.rank_buf])
-            elif n.op == 'xent' and self.objective == 'softmax':
-                # the whole loss (weight 1); f[1] = label smoothing
+            elif n.op == 'xent' and self.objective in ('softmax', 'center_loss'):
+                # the whole loss of the classifier (center_loss: the 'prob' term), weight 1; f[1] = label smoothing
                 lg = n.inputs[0]
                 ii = [self.num_classes, self.B, self.num_classes]
                 ls = self.label_smoothing
@@ -565,6 +624,11 @@ class Engine:
                 self._eval_le = self._op(_lib.OP_LABELEMBED, ii, [0.0, self.tau, self.alpha, self.beta],
                                          [A[o1.name], A[o2.name], self.labels, table, self.loss_buf, self.acc_buf, None,
                                           None, None, self.le_work])
+            elif n.op == 'center_loss':
+                # training: emitted by the backward plan; here only the loss-only form of the validation pass
+                self._eval_center = self._op(_lib.OP_CENTER_LOSS, self._center_i(), [0.0],
+                                             [A[n.inputs[0].name], self.labels, self._pview(CENTROIDS), self.center_buf,
+                                              None, None])
             else:
                 raise ValueError(n.op)
         # ---------------- backward
@@ -595,6 +659,17 @@ class Engine:
             written.add(self.head_node.inputs[0].name)
         for n in reversed(self.nodes):
             if n.op in ('xent', 'labelembed'):
+                continue
+            if n.op == 'center_loss':
+                # the last node, so the first op after the memset: it writes the gradient of z (beta 0; the relu of the
+                # classifier branch adds onto it) and the centroids' gradient, weighted by center_loss_weight
+                z = n.inputs[0]
+                dz, beta = gb(z)
+                assert beta == 0.0, 'the center loss must be the first writer of the gradient of %s' % z.name
+                bwd.append(self._op(_lib.OP_CENTER_LOSS, self._center_i(), [self.center_loss_weight * scale],
+                                    [A[z.name], self.labels, self._pview(CENTROIDS), self.center_buf, dz,
+                                     self._pview(CENTROIDS, self.G)]))
+                final[CENTROIDS] = len(bwd)
                 continue
             dY = Gd[n.output.name]
             if n.op == 'head':
@@ -696,6 +771,8 @@ class Engine:
                 ev.append(o)
         if self.le_node is not None:
             ev.append(self._eval_le)
+        if self.center_node is not None:
+            ev.append(self._eval_center)
         self.plans = {'fwd': self._pack(fwd), 'bwd': self._pack(bwd), 'opt': self._pack(opt), 'infer': self._pack(inf),
                       'eval': self._pack(ev),
                       'fwdbwd': self._pack(fwd + bwd), 'step': self._pack(fwd + bwd + opt)}
@@ -704,6 +781,10 @@ class Engine:
             # data parallel: the same step with bucketed all-reduces inside the backward pass (one graph, no host in between)
             self._parts['bwd_dp'] = self._with_allreduce(bwd, final)
             self.plans['step_dp'] = self._pack(fwd + self._parts['bwd_dp'] + opt)
+
+    def _center_i(self):
+        """Int slots of a center-loss op: ldz, ldc, B, C, D (z and the centroids are dense rows of D)."""
+        return [self.D, self.D, self.B, self.num_classes, self.D]
 
     def _head_f(self, scale):
         """Float slots of a head op: the loss scale, and the margin for the ranking loss (f[1])."""
@@ -895,6 +976,8 @@ class Engine:
     def metrics(self):
         """Host copies of the last step's per-sample loss / accuracy (one small D2H read)."""
         out = {'loss': float(self.loss_buf.cpu().numpy().mean()), 'acc': float(self.acc_buf.cpu().numpy().mean())}
+        if self.center_node is not None:
+            out.update(self._center_terms(out['loss'], float(self.center_buf.cpu().numpy().mean())))
         if self.has_cls_branch:
             out['cls_loss'] = float(self.cls_loss_buf.cpu().numpy().mean())
             out['cls_acc'] = float(self.cls_acc_buf.cpu().numpy().mean())
@@ -904,6 +987,8 @@ class Engine:
         """Per-sample loss / accuracy arrays of the last batch (and accuracy@k for k in ks): what a validation loop sums
         when its last batch is only partly filled."""
         out = {'loss': self.loss_buf.cpu().numpy(), 'acc': self.acc_buf.cpu().numpy()}
+        if self.center_node is not None:
+            out.update(self._center_terms(out['loss'].astype(np.float64), self.center_buf.cpu().numpy().astype(np.float64)))
         r = self.rank_buf.cpu().numpy() if ks else None
         for k in ks:
             out['acc%d' % k] = (r < k).astype(np.float32)
@@ -931,7 +1016,8 @@ class Engine:
         reference's Keras progress bar shows running means, learn_image_embeddings.py:238).  `ks`: also accuracy@k
         ('acc<k>') for every k, from the rank of the true class."""
         if not hasattr(self, '_mring'):
-            n = 5 if self.has_cls_branch else 3          # loss, acc[, cls_loss, cls_acc], rank
+            # loss, acc[, cls_loss, cls_acc | center_loss], rank
+            n = 5 if self.has_cls_branch else 4 if self.center_node is not None else 3
             self._mring = [torch.empty(n, self.B, dtype=torch.float32).pin_memory() for _ in range(4)]
             self._mev = [torch.cuda.Event() for _ in range(4)]
             self._mks = [()] * 4
@@ -944,6 +1030,8 @@ class Engine:
         if self.has_cls_branch:
             host[2].copy_(self.cls_loss_buf, non_blocking=True)
             host[3].copy_(self.cls_acc_buf, non_blocking=True)
+        if self.center_node is not None:
+            host[2].copy_(self.center_buf, non_blocking=True)
         if ks:
             host[-1].copy_(self.rank_buf, non_blocking=True)
         self._mks[k] = tuple(ks)
@@ -954,6 +1042,8 @@ class Engine:
         self._mev[handle].synchronize()
         host = self._mring[handle]
         out = {'loss': float(host[0].mean()), 'acc': float(host[1].mean())}
+        if self.center_node is not None:
+            out.update(self._center_terms(out['loss'], float(host[2].mean())))
         if self.has_cls_branch:
             out['cls_loss'] = float(host[2].mean())
             out['cls_acc'] = float(host[3].mean())
@@ -961,14 +1051,19 @@ class Engine:
             out['acc%d' % kk] = float((host[-1] < kk).float().mean())
         return out
 
+    def _center_terms(self, prob_loss, center_loss):
+        """objective='center_loss': Keras' output losses and their weighted sum (without the L2 terms)."""
+        return {'loss': prob_loss + self.center_loss_weight * center_loss, 'prob_loss': prob_loss,
+                'center_loss': center_loss}
+
     def grad_norm_and_reg(self):
         o = self.sgd_out.cpu().numpy()
         return float(np.sqrt(o[0])), float(o[1])
 
     def predict(self, x):
         """Inference forward (BatchNorm moving statistics), returns the wrapped embeddings (B,D) -- or, for
-        objective='softmax', the class probabilities (B,C), for objective='labelembed' the logits of 'prob' (B,C) -- as
-        numpy."""
+        objective='softmax' and 'center_loss', the class probabilities (B,C), for objective='labelembed' the logits of
+        'prob' (B,C) -- as numpy."""
         x = torch.as_tensor(x)
         self.x.copy_(x, non_blocking=True)
         self._run('infer')

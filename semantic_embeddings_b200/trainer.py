@@ -1,4 +1,5 @@
-"""Training-script machinery shared by learn_image_embeddings.py, learn_classifier.py and learn_devise.py: what Keras'
+"""Training-script machinery shared by learn_image_embeddings.py, learn_classifier.py, learn_devise.py,
+learn_labelembedding.py and learn_center_loss.py: what Keras'
 `fit_generator`, `evaluate_generator`, `ModelCheckpoint` and `load_weights(by_name=True)` do for the reference scripts,
 on top of engine.Engine.  The scripts only differ in the network's top, the engine objective and what they print at the
 end."""
@@ -228,6 +229,13 @@ def average_accuracy(pred, labels):
     labels = np.asarray(labels)
     class_freq = np.bincount(labels)
     return ((pred == labels).astype(np.float64) / class_freq[labels]).sum() / len(class_freq)
+
+
+def l2_term(eng):
+    """The regularisation losses Keras adds to the total loss: sum of l2 * ||w||^2 over the regularised weights."""
+    w = eng.get_weights()
+    return float(sum(spec.l2 * float(np.sum(np.square(w[n], dtype=np.float64)))
+                     for n, spec in eng.pspecs.items() if spec.l2 > 0))
 
 
 def dump_weights(eng, args):
