@@ -32,6 +32,55 @@ def hinges(E, T, Y, margin):
     return margin - (T * Y).sum(-1, keepdims=True) + Y @ E.T
 
 
+def _f32_fma(s, a, b):
+    """float32 fmaf(a, b, s), rounded once as the hardware does.  The product of two float32 values is exact in float64;
+    the float64 sum hi = s + a b and its exact error lo (two-sum) give s + a b = hi + lo.  Rounding hi to float32 is then
+    correct unless hi lies exactly halfway between two float32 values while lo pushes the true sum past that midpoint:
+    those elements round to the other neighbour (a plain float64 sum would round twice there)."""
+    s64 = s.astype(np.float64)
+    p = a.astype(np.float64) * b.astype(np.float64)
+    hi = s64 + p
+    bb = hi - s64
+    lo = (s64 - (hi - bb)) + (p - bb)
+    r = hi.astype(np.float32)
+    d = hi - r.astype(np.float64)
+    with np.errstate(over='ignore', invalid='ignore'):
+        nb = np.nextafter(r, np.where(d > 0, np.float32(np.inf), np.float32(-np.inf)).astype(np.float32))
+        fix = (d != 0) & (2.0 * d == nb.astype(np.float64) - r.astype(np.float64)) & (lo != 0) & \
+            (np.sign(lo) == np.sign(d))
+    return np.where(fix, nb, r).astype(np.float32)
+
+
+def kernel_similarities(E, Z):
+    """The head kernels' fp32 scores <z,E_c>: one sequential fmaf chain over the dimensions (float32 numpy (B, C))."""
+    E, Z = np.asarray(E, np.float32), np.asarray(Z, np.float32)
+    sim = np.zeros((Z.shape[0], E.shape[0]), np.float32)
+    for i in range(Z.shape[1]):
+        sim = _f32_fma(sim, Z[:, i:i + 1], E[None, :, i])
+    return sim
+
+
+def kernel_hinges(E, T, Z, margin):
+    """se_devise_rank_fwd_bwd's fp32 hinge arguments: (m - <t,z>) + <z,E_c> with <t,z> summed as warp_dot does
+    (lane-strided float4 or scalar chains, then the xor-shuffle tree) and <z,E_c> as kernel_similarities."""
+    E, T, Z = (np.asarray(a, np.float32) for a in (E, T, Z))
+    B, D = Z.shape
+    vec = D % 4 == 0
+    lanes = np.zeros((B, 32), np.float32)
+    for lane in range(32):
+        if vec:
+            for g in range(lane, D // 4, 32):
+                for j in range(4):
+                    lanes[:, lane] = _f32_fma(lanes[:, lane], Z[:, 4 * g + j], T[:, 4 * g + j])
+        else:
+            for i in range(lane, D, 32):
+                lanes[:, lane] = _f32_fma(lanes[:, lane], Z[:, i], T[:, i])
+    for o in (16, 8, 4, 2, 1):
+        lanes = (lanes + lanes[:, np.arange(32) ^ o]).astype(np.float32)
+    base = (np.float32(margin) - lanes[:, 0]).astype(np.float32)
+    return (base[:, None] + kernel_similarities(E, Z)).astype(np.float32)
+
+
 def gradient_from_active(E, T, active, scale):
     """scale * (sum_{c in A} E_c - |A| t) per row, for a boolean (B, C) active set."""
     a = np.asarray(active, dtype=np.float64)

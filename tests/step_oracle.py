@@ -11,10 +11,16 @@ the layer sizes of the benchmarked networks.  They work on CPU or CUDA tensors; 
                                    gradients, given the upstream gradient dy of its output
   backward_walk(eng, ...)          the nodes in reverse order: the gradient of a tensor is the sum of its consumers'
                                    contributions (Engine._build_plans: gb() and beta)
-  sgd(...)                         the optimizer over the flat buffers (oracle.train.sgd_step with the L2 terms)
+  sgd(...), adagrad(...)           the optimizer over the flat buffers (oracle.train.sgd_step / devise_oracle.adagrad_step
+                                   with the L2 terms and the frozen runs of set_trainable)
+  metrics(ctx, node, out)          the per-sample accuracy and rank a loss op writes, decided on the engine's fp32 values
   *_ops(eng, node)                 the se_run_ops opcodes whose results a node's check covers (plan coverage)
+  build_engine(...)                the Engine of a test configuration, built the way its trainer builds it
 
-test_cpu_step_oracle.py checks the composition against torch.autograd and oracle.train.train_step."""
+The loss nodes call the per-op references of each objective, which are pinned to the reference's fixtures:
+classifier_oracle.smoothed_targets (label smoothing), devise_oracle (the ranking loss), labelembed_oracle.op_reference
+and center_loss_oracle.op_reference.  test_cpu_step_oracle.py checks the composition against torch.autograd and each
+objective's own train_step."""
 import collections
 import types
 
@@ -23,18 +29,40 @@ import torch
 import torch.nn.functional as F
 
 import bn_oracle
+import center_loss_oracle
+import classifier_oracle
+import devise_oracle
+import labelembed_oracle
 from oracle import nn as onn
 from oracle import train as otrain
 
+LOSS_OPS = ('xent', 'labelembed', 'center_loss')       # nodes whose output takes no gradient
+TABLE = labelembed_oracle.TABLE
+CENTROIDS = center_loss_oracle.CENTROIDS
 
-def loss_spec(eng, labels, E=None):
-    """What the loss nodes of the embedding objective need: loss kind, class matrix (float64), labels (int64), the
-    1/global-batch scale and the classifier weight."""
-    if eng.objective != 'embedding' or eng.optimizer != 'sgd' or eng.loss == 'devise_rank':
-        raise NotImplementedError('step_oracle restates the embedding objective with SGD')
-    E = eng.E.double() if E is None else E
-    return types.SimpleNamespace(kind=eng.loss, E=E, labels=labels.long().to(E.device), scale=1.0 / (eng.B * eng.world),
-                                 cls_weight=eng.cls_weight, num_classes=eng.num_classes)
+
+def context(eng, labels, E=None):
+    """What the loss nodes and the optimizer need, for every objective of Engine: the objective, the loss kind of the
+    head, the class matrix (float64; embedding and DeViSE), the labels (int64), scale = 1/(B world), the weight of the
+    cross-entropy (cls_weight for the embedding objective's classifier branch, else 1), label smoothing, the ranking
+    margin, tau / alpha / beta, the center loss weight and the optimizer."""
+    if E is None and eng.E is not None:
+        E = eng.E.double()
+    return types.SimpleNamespace(
+        objective=eng.objective, kind=eng.loss, E=E, labels=labels.long(), scale=1.0 / (eng.B * eng.world),
+        cls_weight=eng.cls_weight, xent_weight=eng.cls_weight if eng.objective == 'embedding' else 1.0,
+        label_smoothing=eng.label_smoothing, margin=eng.margin, tau=eng.tau, alpha=eng.alpha, beta=eng.beta,
+        center_loss_weight=eng.center_loss_weight, optimizer=eng.optimizer, num_classes=eng.num_classes)
+
+
+def targets(ctx, like):
+    """The cross-entropy's targets: one-hot, or learn_classifier.transform_inputs' smoothed ones (float32 values)."""
+    t = classifier_oracle.smoothed_targets(ctx.labels.cpu().numpy(), like.shape[-1], ctx.label_smoothing)
+    return torch.as_tensor(t).to(like)
+
+
+def _np(t):
+    return t.detach().cpu().numpy()
 
 
 def pads(node):
@@ -61,11 +89,12 @@ def _conv(node, x, W):
 def forward(node, ins, p, training=True, ctx=None):
     """ins: float64 inputs of the node (batch first); p: name -> float64 parameter or moving statistic.
     Returns {'y': output} plus, for 'bn' in training: mean, var, invstd, xhat, moving_mean, moving_variance (updated);
-    for 'head' and 'xent': loss (per sample; training only)."""
+    for the loss nodes: loss (per sample), and for 'labelembed' / 'center_loss' the op's other outputs (y is None)."""
     op, a, nm = node.op, node.attrs, node.name
     if op in ('conv', 'dense'):
         W, b = p[nm + '/kernel'], p.get(nm + '/bias') if a['use_bias'] else None
-        y = _conv(node, ins[0], W) if op == 'conv' else ins[0] @ W
+        x = ins[0].detach() if a.get('stop_gradient') else ins[0]
+        y = _conv(node, x, W) if op == 'conv' else x @ W
         if b is not None:
             y = y + b
         if a.get('residual'):
@@ -99,17 +128,26 @@ def forward(node, ins, p, training=True, ctx=None):
     if op == 'relu':
         return {'y': torch.relu(ins[0])}
     if op == 'head':
+        if ctx.kind == 'devise_rank':
+            # no output wrapper: the output is z itself
+            return {'y': ins[0], 'loss': devise_oracle.ranking_loss(ctx.E, ctx.E[ctx.labels], ins[0], ctx.margin)}
         out = otrain.head_forward(ins[0], ctx.kind)
-        r = {'y': out}
-        if training:
-            r['loss'] = otrain.per_sample_loss(ctx.E[ctx.labels], out, ctx.kind)
-        return r
+        return {'y': out, 'loss': otrain.per_sample_loss(ctx.E[ctx.labels], out, ctx.kind)}
     if op == 'xent':
         prob = torch.softmax(ins[0], dim=-1)
-        r = {'y': prob}
-        if training:
-            r['loss'] = onn.categorical_crossentropy(F.one_hot(ctx.labels, prob.shape[-1]).to(prob.dtype), prob)
-        return r
+        return {'y': prob, 'loss': onn.categorical_crossentropy(targets(ctx, prob), prob)}
+    if op == 'labelembed':
+        # se_labelembed_fwd_bwd: the mask argmax(out2) == y is taken on the out2 it is given; rows with label < 0 are padding
+        r = labelembed_oracle.op_reference(_np(ins[0]), _np(ins[1]), _np(p[TABLE]), _np(ctx.labels), ctx.tau, ctx.alpha,
+                                           ctx.beta, ctx.scale)
+        r = [torch.as_tensor(v).to(ins[0]) for v in r]
+        return dict(zip(('loss', 'acc', 'mask', 'd_out1', 'd_out2', 'd_table'), r), y=None)
+    if op == 'center_loss':
+        # se_center_loss_fwd_bwd at the weighted scale: the per-sample loss is unweighted, both gradients weighted
+        r = center_loss_oracle.op_reference(_np(ins[0]), _np(p[CENTROIDS]), _np(ctx.labels),
+                                            ctx.center_loss_weight * ctx.scale)
+        r = [torch.as_tensor(v).to(ins[0]) for v in r]
+        return dict(zip(('loss', 'dz', 'dc'), r), y=None)
     raise NotImplementedError(op)
 
 
@@ -190,6 +228,21 @@ def backward(node, ins, y, dy, p, ctx=None, need=None, fwd=None):
         g = dy * (y > 0) if (op == 'relu' or a['relu']) else dy
         out['dx'] = [g if need[k] else None for k in range(len(ins))]
         return out
+    if op == 'head' and ctx.kind == 'devise_rank':
+        # scale * (sum of the active classes' E_c - |A| t) per row.  A hinge within 1e-5 of zero is decided by the fp32
+        # hinges the kernel computes (devise_oracle.kernel_hinges; the true class' own hinge adds E_t - t = 0 either way)
+        assert dy is None, 'nothing reads the output of the ranking loss head'
+        E, z, y = _np(ctx.E), _np(ins[0]), _np(ctx.labels)
+        T = E[y]
+        h = devise_oracle.hinges(E, T, z, ctx.margin)
+        active = h > 0
+        off = np.ones_like(active)
+        off[np.arange(len(y)), y] = False
+        near = ((np.abs(h) < 1e-5) & off).any(-1)
+        if near.any():
+            active[near] = devise_oracle.kernel_hinges(E, T[near], z[near], ctx.margin) > 0
+        out['dx'][0] = torch.as_tensor(devise_oracle.gradient_from_active(E, T, active, ctx.scale)).to(ins[0])
+        return out
     if op == 'head':
         # d(scale * sum_b loss_b)/dz + J^T dy, dy = the gradient of the wrapped output from the classifier branch
         z = ins[0].detach().requires_grad_(True)
@@ -200,11 +253,20 @@ def backward(node, ins, y, dy, p, ctx=None, need=None, fwd=None):
         out['dx'][0] = torch.autograd.grad(f, [z])[0]
         return out
     if op == 'xent':
-        # the classifier's cross-entropy, weighted by cls_weight (oracle.train.train_objective)
+        # the cross-entropy on (smoothed) targets, weighted by cls_weight (oracle.train.train_objective) or 1
         lg = ins[0].detach().requires_grad_(True)
         prob = torch.softmax(lg, dim=-1)
-        ce = onn.categorical_crossentropy(F.one_hot(ctx.labels, prob.shape[-1]).to(prob.dtype), prob)
-        out['dx'][0] = torch.autograd.grad(ctx.cls_weight * ctx.scale * ce.sum(), [lg])[0]
+        ce = onn.categorical_crossentropy(targets(ctx, prob), prob)
+        out['dx'][0] = torch.autograd.grad(ctx.xent_weight * ctx.scale * ce.sum(), [lg])[0]
+        return out
+    if op in ('labelembed', 'center_loss'):
+        f = forward(node, ins, p, True, ctx) if fwd is None or 'loss' not in fwd else fwd
+        if op == 'labelembed':
+            out['dx'] = [f['d_out1'] if need[0] else None, f['d_out2'] if need[1] else None]
+            out[TABLE] = f['d_table']
+        else:
+            out['dx'][0] = f['dz'] if need[0] else None
+            out[CENTROIDS] = f['dc']
         return out
     raise NotImplementedError(op)
 
@@ -212,14 +274,15 @@ def backward(node, ins, y, dy, p, ctx=None, need=None, fwd=None):
 def has_gradient(eng, t):
     """Whether the backward pass computes a gradient for tensor t: not the network input, not a loss output, and not
     the wrapped embedding when nothing reads it."""
-    if t.name == eng.g.input.name or (t.producer is not None and t.producer.op == 'xent'):
+    if t.name == eng.g.input.name or (t.producer is not None and t.producer.op in LOSS_OPS):
         return False
     return bool(eng.consumers.get(t.name))
 
 
 def grad_class(ops):
     """Which kernel family dominates a gradient tensor: the first of these among the ops that contributed to it."""
-    for op in ('conv', 'dense', 'bn', 'head', 'xent', 'maxpool', 'avgpool2', 'gap', 'add', 'relu'):
+    for op in ('conv', 'dense', 'bn', 'head', 'xent', 'labelembed', 'center_loss', 'maxpool', 'avgpool2', 'gap', 'add',
+               'relu'):
         if op in ops:
             return op
     raise ValueError(ops)
@@ -241,7 +304,7 @@ def backward_walk(eng, act, upstream, p, ctx):
             dy = total if upstream is None else upstream(t.name)
             del total
         else:
-            assert not has_gradient(eng, t) or n.op == 'xent', 'no gradient reaches %s' % t.name
+            assert not has_gradient(eng, t), 'no gradient reaches %s' % t.name
             dy = None
         if n.op == 'head' and not eng.consumers.get(t.name):
             dy = None
@@ -285,11 +348,23 @@ def l2_per_element(eng, device=None):
     return lam
 
 
-def sgd(P, G, V, lam, lr_state, momentum, nesterov, clipnorm):
-    """se_sgd_prepare + se_sgd_schedule + se_sgd_apply over flat float64 buffers: g = G + 2 lam P (regularizers.l2),
-    global-norm clip, lr / (1 + decay * iterations), (Nesterov) momentum -- oracle.train.sgd_step on one flat tensor.
-    lr_state = (lr, decay, iterations).  Returns dict P, V, G (= g), sumsq, reg, lr_t."""
+def _unfrozen(G, lam, frozen_runs):
+    """set_trainable: the gradient of a frozen run is zeroed before the norm is taken, and it takes no L2 term."""
+    if not frozen_runs:
+        return G, lam
+    G, lam = G.clone(), lam.clone()
+    for off, n in frozen_runs:
+        G[off:off + n] = 0.0
+        lam[off:off + n] = 0.0
+    return G, lam
+
+
+def sgd(P, G, V, lam, lr_state, momentum, nesterov, clipnorm, frozen_runs=()):
+    """[frozen-run memsets] + se_sgd_prepare + se_sgd_schedule + se_sgd_apply over flat float64 buffers: g = G + 2 lam P
+    (regularizers.l2), global-norm clip, lr / (1 + decay * iterations), (Nesterov) momentum -- oracle.train.sgd_step on
+    one flat tensor.  lr_state = (lr, decay, iterations).  Returns dict P, V, G (= g), sumsq, reg, lr_t."""
     lr, decay, it = (float(v) for v in lr_state[:3])
+    G, lam = _unfrozen(G, lam, frozen_runs)
     g = G + 2.0 * lam * P
     params, vel = {'flat': P.clone()}, {'flat': V.clone()}
     otrain.sgd_step(params, {'flat': g}, vel, lr, momentum, nesterov, clipnorm, decay, it)
@@ -297,9 +372,61 @@ def sgd(P, G, V, lam, lr_state, momentum, nesterov, clipnorm):
                 lr_t=lr / (1.0 + decay * it))
 
 
+def adagrad(P, G, A, lam, lr_state, epsilon, clipnorm, frozen_runs=()):
+    """The same with se_adagrad_apply: Keras Adagrad (devise_oracle.adagrad_step) with its accumulators A.  Returns dict
+    P, V (= the accumulators), G (= g), sumsq, reg, lr_t."""
+    lr, decay, it = (float(v) for v in lr_state[:3])
+    G, lam = _unfrozen(G, lam, frozen_runs)
+    g = G + 2.0 * lam * P
+    params, acc = {'flat': P.clone()}, {'flat': A.clone()}
+    devise_oracle.adagrad_step(params, {'flat': g}, acc, lr, decay, it, epsilon, clipnorm)
+    return dict(P=params['flat'], V=acc['flat'], G=g, sumsq=float((g * g).sum()), reg=float((lam * P * P).sum()),
+                lr_t=lr / (1.0 + decay * it))
+
+
+def optimizer(eng, P, G, V, lam, lr_state):
+    """The engine's optimizer step (sgd or adagrad with its settings and frozen runs) on float64 flat buffers."""
+    if eng.optimizer == 'adagrad':
+        return adagrad(P, G, V, lam, lr_state, eng.epsilon, eng.clipnorm, eng.frozen_runs)
+    return sgd(P, G, V, lam, lr_state, eng.momentum, eng.nesterov, eng.clipnorm, eng.frozen_runs)
+
+
+# ----------------------------------------------------------------------------------------------------------- metrics
+def metrics(ctx, node, out):
+    """(acc, rank) per sample as the loss op decides them, from the engine's fp32 tensor `out` (float64 numpy; rank is
+    None where the op writes none):
+      xent        the logits: acc = argmax (first maximum) == argmax(targets), rank = number of logits strictly above
+                  the target's (utils.top_k_acc)
+      labelembed  out1: acc = argmax == label, 0 on padding rows
+      head        the wrapped output: fp32 scores <x,E_c> (devise_oracle.kernel_similarities); acc = the best score within
+                  1e-6 of the true class' (utils.nn_accuracy), rank = classes better by >= 1e-6, or C when none is within"""
+    o = out.detach().float().cpu().numpy()
+    y = ctx.labels.cpu().numpy()
+    rows = np.arange(len(y))
+    if node.op == 'xent':
+        tgt = classifier_oracle.smoothed_targets(np.maximum(y, 0), o.shape[-1], ctx.label_smoothing).argmax(-1)
+        own = o[rows, tgt]
+        return (o.argmax(-1) == tgt).astype(np.float64), (o > own[:, None]).sum(-1).astype(np.float64)
+    if node.op == 'labelembed':
+        return ((o.argmax(-1) == y) & (y >= 0)).astype(np.float64), None
+    if node.op == 'head':
+        if ctx.kind not in ('inv_corr', 'unnorm_corr', 'devise_rank'):
+            raise NotImplementedError('metrics of the %s head' % ctx.kind)
+        sim = devise_oracle.kernel_similarities(_np(ctx.E), o)
+        mine = sim[rows, y]
+        acc = np.abs(sim.max(-1) - mine) < np.float32(1e-6)
+        within = np.abs(sim - mine[:, None]) < np.float32(1e-6)
+        better = ~within & (sim > mine[:, None])
+        rank = np.where(within.any(-1), better.sum(-1), sim.shape[1])
+        return acc.astype(np.float64), rank.astype(np.float64)
+    raise ValueError(node.op)
+
+
 # --------------------------------------------------------------------------------------------------- plan coverage
 def fwd_ops(eng, node, training=True):
-    """Opcodes of the forward (training=True) or inference plan that a check of this node's forward outputs covers."""
+    """Opcodes of the forward (training=True) or inference plan that a check of this node's forward outputs covers.
+    The label embedding loss is in the forward plan (it writes the gradients of both logit heads and of the table), the
+    center loss in the backward plan; neither is in the inference plan."""
     from semantic_embeddings_b200 import _lib as L
     op = node.op
     if op in ('conv', 'dense'):
@@ -310,13 +437,23 @@ def fwd_ops(eng, node, training=True):
         prod = node.inputs[0].producer
         fused = eng.fuse_stats and prod is not None and prod.op in ('conv', 'dense')
         return ([] if fused else [L.OP_BN_STATS]) + [L.OP_BN_FWD_TRAIN]
+    if op == 'labelembed':
+        return [L.OP_LABELEMBED] if training else []
     return {'avgpool2': [L.OP_AVGPOOL_FWD], 'maxpool': [L.OP_MAXPOOL_FWD], 'gap': [L.OP_GAP_FWD], 'add': [L.OP_ADD_FWD],
-            'relu': [L.OP_ADD_FWD], 'head': [L.OP_HEAD], 'xent': [L.OP_XENT]}[op]
+            'relu': [L.OP_ADD_FWD], 'head': [L.OP_HEAD], 'xent': [L.OP_XENT], 'center_loss': []}[op]
+
+
+def eval_ops(eng, node):
+    """Opcodes of the validation plan: the inference plan with the loss ops in their metric-writing form, plus the
+    loss-only label embedding and center loss ops."""
+    from semantic_embeddings_b200 import _lib as L
+    return fwd_ops(eng, node, False) + {'labelembed': [L.OP_LABELEMBED], 'center_loss': [L.OP_CENTER_LOSS]}.get(node.op, [])
 
 
 def bwd_ops(eng, node):
     """Opcodes of the backward plan that a check of this node's local gradients covers.  The loss nodes' gradients are
-    computed by their forward ops (the head also by a backward op when the classifier branch reads its output)."""
+    computed by their forward ops (the embedding head also by a backward op when the classifier branch reads its output;
+    the center loss only by its backward op)."""
     from semantic_embeddings_b200 import _lib as L
     op, a = node.op, node.attrs
     if op in ('conv', 'dense'):
@@ -328,17 +465,22 @@ def bwd_ops(eng, node):
     if op == 'head':
         return [L.OP_HEAD] if eng.consumers.get(node.output.name) else []
     return {'avgpool2': [L.OP_AVGPOOL_BWD], 'maxpool': [L.OP_MAXPOOL_BWD], 'gap': [L.OP_GAP_BWD], 'add': [L.OP_ADD_BWD],
-            'relu': [L.OP_ADD_BWD], 'xent': []}[op]
+            'relu': [L.OP_ADD_BWD], 'xent': [], 'labelembed': [], 'center_loss': [L.OP_CENTER_LOSS]}[op]
 
 
 def buffer_ops(eng):
     """Opcodes covered by the checks of whole buffers: the statistics memset (the statistics sums), the filter copies
-    (PT / PL / PTL against P), the gradient memset (every gradient, and zeros between the tensors) and the optimizer
-    (the updated P, V, G and its norm / L2 outputs)."""
+    (PT / PL / PTL against P), the gradient memset (every gradient, and zeros between the tensors; for the label
+    embedding objective it spares the table's gradient, which the check then finds intact) and the optimizer (the
+    frozen-run memsets, and the updated P, V, G and its norm / L2 outputs)."""
     from semantic_embeddings_b200 import _lib as L
     tr = [L.OP_TRANSPOSE_FILTERS] if eng.PT is not None and eng.n_tr else []
-    return {'fwd': [L.OP_MEMSET] + tr, 'bwd': [L.OP_MEMSET], 'infer': list(tr),
-            'opt': [L.OP_MEMSET] * (1 + len(eng.frozen_runs)) + [L.OP_SGD_PREPARE, L.OP_SGD_APPLY]}
+    apply = L.OP_ADAGRAD_APPLY if eng.optimizer == 'adagrad' else L.OP_SGD_APPLY
+    return {'fwd': [L.OP_MEMSET] + tr, 'bwd': [L.OP_MEMSET], 'infer': list(tr), 'eval': list(tr),
+            'opt': [L.OP_MEMSET] * (1 + len(eng.frozen_runs)) + [L.OP_SGD_PREPARE, apply]}
+
+
+PLANS = ('fwd', 'bwd', 'opt', 'infer', 'eval')
 
 
 def covered_ops(eng):
@@ -347,10 +489,80 @@ def covered_ops(eng):
     for n in eng.nodes:
         cov['fwd'].update(fwd_ops(eng, n, True))
         cov['infer'].update(fwd_ops(eng, n, False))
+        cov['eval'].update(eval_ops(eng, n))
         cov['bwd'].update(bwd_ops(eng, n))
     return cov
 
 
 def plan_ops(eng):
     """plan -> Counter of the opcodes it holds."""
-    return {k: collections.Counter(int(o.opcode) for o in eng.plans[k]) for k in ('fwd', 'bwd', 'opt', 'infer')}
+    return {k: collections.Counter(int(o.opcode) for o in eng.plans[k]) for k in PLANS}
+
+
+# ---------------------------------------------------------------------------------------------- test configurations
+# the configurations of test_gpu_step_layers.py (and of the plan coverage test of test_cpu_step_oracle.py):
+# arch, batch, mode, options (build_engine)
+CONFIGS = [
+    ('resnet-110-fc', 128, 'tf32x3', {}),                                  # what bench.py times
+    ('resnet-110-fc', 128, 'f32', {}),                                     # the fp32 kernels at the same sizes
+    ('wrn-28-10', 64, 'tf32x3', dict(cls_weight=0.1, decay=1e-3)),         # per-GPU shard of the WRN configuration
+    ('simple', 128, 'tf32x3', dict(nesterov=True, decay=1e-3)),            # fc512: tensor-core dense backward
+    ('resnet-50', 32, 'tf32x3', {}),                                       # per-GPU shard of the ResNet-50 configuration
+    # learn_classifier.py: the cosine-loss recipe's CIFAR-100 classifier, and 1000 classes one-hot
+    ('resnet-110-wfc', 100, 'tf32x3', dict(tag='softmax', objective='softmax', num_classes=100, label_smoothing=0.1,
+                                           clipnorm=10.0)),
+    ('simple', 100, 'f32', dict(tag='softmax', objective='softmax', num_classes=1000, nesterov=True)),
+    # learn_devise.py --init_weights: the fine-tuning phase, and phase 1 with only 'embedding' trained
+    ('resnet-110-wfc', 100, 'tf32x3', dict(tag='devise', loss='devise_rank', margin=0.1, optimizer='adagrad',
+                                           clipnorm=0.0, decay=1e-3, devise_classes=100)),
+    ('resnet-110-wfc', 100, 'tf32x3', dict(tag='devise-phase1', loss='devise_rank', margin=0.1, optimizer='adagrad',
+                                           clipnorm=1.0, devise_classes=100, train=('embedding',))),
+    # learn_labelembedding.py and learn_center_loss.py on the CIFAR-100 recipes' network
+    ('resnet-110-wfc', 100, 'tf32x3', dict(tag='labelembed', objective='labelembed', num_classes=100, embed_dim=100,
+                                           tau=2.0, alpha=0.9, beta=0.5)),
+    ('resnet-110-wfc', 100, 'tf32x3', dict(tag='center_loss', objective='center_loss', num_classes=100, embed_dim=100,
+                                           center_loss_weight=0.1)),
+    ('simple', 100, 'f32', dict(tag='center_loss-fixed', objective='center_loss', num_classes=100, embed_dim=100,
+                                center_loss_weight=0.1, fixed_centroids=True)),
+]
+
+
+def config_id(cfg):
+    arch, B, mode, opts = cfg
+    return ('%s-' % opts['tag'] if 'tag' in opts else '') + '%s-b%d-%s' % (arch, B, mode)
+
+
+def build_engine(cfg, device='cuda:0', use_cuda_graph=True):
+    """The Engine of a configuration (arch, batch, mode, options), built the way its trainer builds it.  Options are
+    Engine's, plus: 'tag' (the name of the case), 'devise_classes' (learn_devise.py --init_weights: the network of
+    utils.build_devise_network with that many classes before), 'embed_dim' (learn_labelembedding.py /
+    learn_center_loss.py), 'fixed_centroids' (--centroids: a seeded C x D array, which the engine freezes) and 'train'
+    (the layers that train, as set_trainable(lambda name: name.split('/')[0] in train))."""
+    import os
+    from semantic_embeddings_b200 import _lib as L, utils
+    from semantic_embeddings_b200.engine import Engine
+    arch, B, mode, opts = cfg
+    opts = dict(opts)
+    opts.pop('tag', None)
+    devise_classes, embed_dim = opts.pop('devise_classes', None), opts.pop('embed_dim', None)
+    fixed, train = opts.pop('fixed_centroids', False), opts.pop('train', None)
+    objective = opts.get('objective', 'embedding')
+    if objective == 'embedding':
+        key = 'nab' if arch == 'resnet-50' else 'cifar100'
+        emb = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'class_matrices.npz'))[key + '_embedding']
+        D = emb.shape[1]
+        graph = utils.build_devise_network(D, arch, devise_classes, input_channels=3) if devise_classes else \
+            utils.build_network(D, arch, input_channels=3)
+        opts.update(embedding=emb, num_classes=emb.shape[0])
+    elif objective == 'softmax':
+        graph = utils.build_network(opts['num_classes'], arch, classification=True, input_channels=3)
+    else:
+        graph = utils.build_network(embed_dim, arch, input_channels=3)
+        if fixed:
+            C, D = opts['num_classes'], graph.output.shape[0]
+            opts['centroids'] = np.random.RandomState(C + D).uniform(-0.05, 0.05, (C, D))
+    eng = Engine(graph, B, device=device, use_cuda_graph=use_cuda_graph,
+                 mode={'f32': L.SE_MODE_F32, 'tf32x3': L.SE_MODE_TF32X3}[mode], **opts)
+    if train is not None:
+        eng.set_trainable(lambda name: name.split('/')[0] in train)
+    return eng

@@ -22,36 +22,7 @@ import devise_oracle as do  # noqa: E402
 from test_gpu_models import rel_max, report  # noqa: E402
 
 
-# ------------------------------------------------------------------------------------------ fp32 scores of the kernel
-def _f32_fma(s, a, b):
-    """float32 fmaf(a, b, s): the product of two float32 values is exact in float64."""
-    return (s.astype(np.float64) + a.astype(np.float64) * b.astype(np.float64)).astype(np.float32)
-
-
-def _kernel_hinges(E, T, Z, margin):
-    """The kernel's fp32 hinge arguments: (m - <t,z>) + <z,E_c> with <t,z> summed as warp_dot does (lane-strided float4
-    or scalar chains, then the xor-shuffle tree) and <z,E_c> as one sequential fmaf chain over the dimensions."""
-    B, D = Z.shape
-    vec = D % 4 == 0
-    lanes = np.zeros((B, 32), np.float32)
-    for lane in range(32):
-        if vec:
-            for g in range(lane, D // 4, 32):
-                for j in range(4):
-                    lanes[:, lane] = _f32_fma(lanes[:, lane], Z[:, 4 * g + j], T[:, 4 * g + j])
-        else:
-            for i in range(lane, D, 32):
-                lanes[:, lane] = _f32_fma(lanes[:, lane], Z[:, i], T[:, i])
-    for o in (16, 8, 4, 2, 1):
-        lanes = (lanes + lanes[:, np.arange(32) ^ o]).astype(np.float32)
-    true_sim = lanes[:, 0]
-    sim = np.zeros((B, E.shape[0]), np.float32)
-    for i in range(D):
-        sim = _f32_fma(sim, Z[:, i:i + 1], E[None, :, i])
-    base = (np.float32(margin) - true_sim).astype(np.float32)
-    return (base[:, None] + sim).astype(np.float32)
-
-
+# ------------------------------------------------------------------------------------------ ranking-loss head kernel
 def _inputs(C, D, margin, seed):
     g = np.random.RandomState(seed)
     E = g.randn(C, D)
@@ -114,7 +85,7 @@ def test_devise_rank_kernel_matches_oracle(C, D, margin):
     e_far = float(row_err[~near].max()) if (~near).any() else 0.0
     e_near = 0.0
     if near.any():
-        h32 = _kernel_hinges(E, T64.astype(np.float32), Z, margin)
+        h32 = do.kernel_hinges(E, T64.astype(np.float32), Z, margin)
         g32 = do.gradient_from_active(E64, T64, h32 > 0, scale)
         e_near = float((np.linalg.norm(dz - g32, axis=-1) / np.maximum(np.linalg.norm(g32, axis=-1), scale))[near].max())
     report('devise_rank_head', C=C, D=D, margin=margin, loss=e_loss, grad_far=e_far, grad_near=e_near,

@@ -12,11 +12,26 @@ float64 optimizer on the engine's own gradient, and `infer` op by op with BatchN
 - every conv / dense weight and bias gradient equals, bit for bit, a standalone se_conv2d_wgrad on the same x and dY
   into zeroed buffers: the side stream of the graph reduced its split-K slices in slice order (workspace mode), not
   with float atomics (DESIGN.md section 5.1);
-- the ops checked, counted by opcode, are exactly the ops of the plans.
+- the ops checked, counted by opcode, are exactly the ops of the plans;
+- the per-sample accuracy and rank the loss ops write equal, bit for bit, the decisions taken on the engine's own fp32
+  logits / outputs (step_oracle.metrics);
+- the label embedding op's outputs -- the gradients of both logit heads and the table's gradient, which the forward
+  plan writes into G and the backward memset spares -- equal a standalone run of the op bit for bit after the whole
+  backward plan; its mask (argmax(out2) == y) equals the one taken on the engine's out2;
+- after `opt`, frozen parameters (set_trainable) are bit-unchanged with zero gradient and zero optimizer state;
+- the `eval` plan (the validation pass) writes the `infer` plan's activations bit for bit, and its loss / metric
+  buffers match float64 on those activations; for the label embedding objective the last 28 rows are padding (label -1,
+  as trainer.run_validation pads the last batch) and write 0.
 
-Errors are max-norm relative.  Bounds (TOL) are about 3x the largest value measured on an H100 80GB HBM3 (132 SMs,
-400 W power limit) over the configurations, never above the 2e-5 per-op contract of DESIGN.md section 2; the measured
-value stands beside each.  The whole file runs in about 20 s there."""
+The configurations cover every objective and optimizer of Engine at the trainers' batch of 100 and the recipes'
+networks (resnet-110-wfc: 32/64/128 channels): the label-smoothed classifier, DeViSE with Adagrad (both phases), the
+label embedding network and the center loss with learned and fixed centroids.
+
+Errors are max-norm relative.  Bounds (TOL) are about 3x the largest value measured on an H100 80GB HBM3 (132 SMs) over
+the configurations, never above the 2e-5 per-op contract of DESIGN.md section 2; the measured value stands beside each.
+The classes up to 'add_infer_y' were measured over the first five configurations at a 400 W power limit (the new
+configurations stay within them); the classes after it, over all configurations at a 700 W power limit.  The whole file
+runs in about 25 s there."""
 import collections
 import os
 
@@ -25,6 +40,7 @@ import pytest
 import torch
 
 import step_oracle as so
+from oracle import nn as onn
 from test_gpu_ops import _lib, report
 
 pytestmark = pytest.mark.gpu
@@ -81,6 +97,46 @@ TOL = {
     'avgpool2_infer_y': 3e-7,  # 9.9e-8
     'gap_infer_y': 1e-6,      # 2.9e-7
     'add_infer_y': 1.2e-7, 'relu_infer_y': 0.0, 'maxpool_infer_y': 0.0,
+    # the moving statistics against the update with the decay the kernel applies, 1.f - momentum in fp32
+    # (0.0099999905 for momentum 0.99; Keras applies float32(1 - 0.99) = 0.01): what is left is the fp32 rounding
+    'bn_moving_mean_f32decay': 3.5e-7,     # 1.1e-7
+    'bn_moving_variance_f32decay': 4.5e-7,  # 1.6e-7
+    # ... and against Keras' update where Adagrad (lr 0.01) has moved every weight twice (DeViSE): a channel's batch
+    # variance then dwarfs its moving variance, and the decay's 9.5e-7 relative difference shows in full (the
+    # f32decay class above holds the same layers to 8e-8)
+    'bn_moving_variance_adagrad': 3e-6,    # 9.5e-7
+    # 'embedding_bn', the BatchNorm behind relu(z) in the label embedding and center loss branches (100 rows): 2.3e-6
+    # in its output and 2.0e-6 in dgamma.  Every other BatchNorm, the 2-D ones included (<= 2e-7), keeps bn_y / bn_dgamma
+    'embedding_bn_y': 7e-6,       # 2.3e-6
+    'embedding_bn_dgamma': 6e-6,  # 2.0e-6
+    # label-smoothed cross-entropy (learn_classifier.py)
+    'xent_ls_y': 2e-7,        # 6.9e-8
+    'xent_ls_loss': 2e-7,     # 6.9e-8
+    'xent_ls_dx': 2.5e-7,     # 8.6e-8
+    'xent_ls_infer_y': 4.5e-7,  # 0 (the kernel of xent_infer_y)
+    # DeViSE ranking loss: the head's output is z itself
+    'devise_y': 0.0, 'devise_infer_y': 0.0,
+    'devise_loss': 3.5e-7,    # 1.2e-7
+    'devise_dx': 2.5e-7,      # 7.7e-8
+    # label embedding loss: per-sample loss and the gradients of out1, out2 and the table
+    'labelembed_loss': 4.5e-7,    # 1.5e-7
+    'labelembed_dout1': 4.5e-7,   # 1.5e-7
+    'labelembed_dout2': 2.5e-7,   # 7.6e-8
+    'labelembed_dtable': 5e-7,    # 1.7e-7
+    # center loss: per-sample loss, the gradient of z (center loss + the branch's relu) and of the centroids
+    'center_loss_loss': 3e-7,     # 9.8e-8
+    'center_loss_dx': 2.5e-7,     # 7.7e-8
+    'center_loss_dc': 3e-7,       # 1.0e-7
+    # the validation plan's loss buffers (the label embedding one over the 72 real rows of a padded batch)
+    'head_eval_loss': 3e-7,       # 9.9e-8
+    'devise_eval_loss': 2.5e-7,   # 7.8e-8
+    'xent_eval_loss': 2e-7,       # 6.4e-8
+    'xent_ls_eval_loss': 4e-7,    # 1.3e-7
+    'labelembed_eval_loss': 6e-7,  # 2.0e-7
+    'center_loss_eval_loss': 3.5e-7,  # 1.2e-7
+    # Adagrad: accumulators and parameter update
+    'adagrad_a': 1.5e-7,      # 4.9e-8
+    'adagrad_dp': 2e-5,       # 6.1e-6 (as opt_dp: the fp32 rounding of p + dp counts in full)
     # optimizer: the gradient with its L2 terms (element-wise, against |g| + |2 lam p|), squared norm and L2 sum,
     # velocity, parameter update (against the size of the update: the fp32 rounding of p + dp counts in full)
     'opt_g': 3e-7,            # 1.0e-7
@@ -92,16 +148,12 @@ TOL = {
     'opt_iterations': 0.0,
     # bit-for-bit checks (1.0 = differs)
     'wgrad_bits': 0.0, 'grad_padding': 0.0, 'filter_copies': 0.0,
+    'acc_bits': 0.0, 'rank_bits': 0.0, 'labelembed_mask': 0.0, 'labelembed_bits': 0.0, 'labelembed_padding': 0.0,
+    'frozen_bits': 0.0, 'eval_bits': 0.0,
 }
 
-# arch, batch, mode, engine options
-CONFIGS = [
-    ('resnet-110-fc', 128, 'tf32x3', {}),                                  # what bench.py times
-    ('resnet-110-fc', 128, 'f32', {}),                                     # the fp32 kernels at the same sizes
-    ('wrn-28-10', 64, 'tf32x3', dict(cls_weight=0.1, decay=1e-3)),         # per-GPU shard of the WRN configuration
-    ('simple', 128, 'tf32x3', dict(nesterov=True, decay=1e-3)),            # fc512: tensor-core dense backward
-    ('resnet-50', 32, 'tf32x3', {}),                                       # per-GPU shard of the ResNet-50 configuration
-]
+CONFIGS = so.CONFIGS
+PAD = 28            # padding rows of the label embedding validation batch
 
 
 def derr(got, ref):
@@ -127,24 +179,55 @@ class Errors:
         return {k: v for k, v in self.worst.items() if not v[0] <= TOL[k]}
 
 
-def _engine(arch, B, mode, opts):
-    from semantic_embeddings_b200 import _lib as L, utils
-    from semantic_embeddings_b200.engine import Engine
+def _engine(cfg):
     from oracle import models as omodels
-    emb = np.load(os.path.join(G, 'class_matrices.npz'))[('nab' if arch == 'resnet-50' else 'cifar100') + '_embedding']
-    graph = utils.build_network(emb.shape[1], arch, input_channels=3)
-    eng = Engine(graph, B, emb, num_classes=emb.shape[0], use_cuda_graph=True,
-                 mode={'f32': L.SE_MODE_F32, 'tf32x3': L.SE_MODE_TF32X3}[mode], **opts)
+    arch, B = cfg[:2]
+    eng = so.build_engine(cfg)
     # Keras initial weights, with seeded non-trivial biases, BatchNorm parameters and moving statistics
     w = {k: torch.as_tensor(v).double() for k, v in eng.get_weights().items()}
     omodels.randomize(w, seed=len(eng.nodes))
     eng.set_weights({k: v.numpy() for k, v in w.items()})
     g = torch.Generator().manual_seed(B + len(eng.nodes))
-    x = torch.randn((B,) + tuple(graph.input.shape), generator=g)
-    y = torch.randint(0, emb.shape[0], (B,), generator=g)
+    x = torch.randn((B,) + tuple(eng.g.input.shape), generator=g)
+    y = torch.randint(0, eng.num_classes, (B,), generator=g)
     eng.load_batch(x.cuda(), y.cuda())
-    eng.set_lr(0.1)
+    # Adagrad moves every weight by about lr per step: learn_devise.py's --init_lr 0.01 keeps the network finite
+    eng.set_lr(0.1 if eng.optimizer == 'sgd' else 0.01)
     return eng
+
+
+def _name(eng, op):
+    """The class prefix of a loss op's checks: the smoothed cross-entropy and the ranking loss have their own."""
+    if op == 'xent' and 0.0 < eng.label_smoothing < 1.0:
+        return 'xent_ls'
+    if op == 'head' and eng.loss == 'devise_rank':
+        return 'devise'
+    return op
+
+
+def _bits(a, b):
+    return 0.0 if np.array_equal(np.asarray(a), np.asarray(b)) else 1.0
+
+
+def _metric_bufs(eng, n):
+    """(loss, acc, rank) buffers a loss node writes: the classifier branch of the embedding objective has its own."""
+    if n.op == 'xent' and eng.objective == 'embedding':
+        return eng.cls_loss_buf, eng.cls_acc_buf, eng.cls_rank_buf
+    if n.op == 'center_loss':
+        return eng.center_buf, None, None
+    return eng.loss_buf, eng.acc_buf, None if n.op == 'labelembed' else eng.rank_buf
+
+
+def _check_metrics(eng, errs, ctx, n, rows):
+    """The accuracy and rank a loss op wrote against step_oracle.metrics on the engine's own fp32 values."""
+    _, acc, rank = _metric_bufs(eng, n)
+    if acc is None:
+        return
+    src = eng.act[n.output.name] if n.op == 'head' else eng.act[n.inputs[0].name]
+    ra, rr = so.metrics(ctx, n, src)
+    errs.add('acc_bits', _bits(acc.cpu().numpy()[rows], ra[rows]), n.name)
+    if rank is not None:
+        errs.add('rank_bits', _bits(rank.cpu().numpy()[rows], rr[rows]), n.name)
 
 
 def _params(eng, P, S):
@@ -181,32 +264,97 @@ def _check_forward(eng, errs, p, ctx, training):
     """Every node of the forward (training) or inference plan against step_oracle.forward on the engine's inputs."""
     A = eng.act
     plan = 'fwd' if training else 'infer'
+    rows = np.arange(eng.B)
     for n in eng.nodes:
+        errs.covered(plan, so.fwd_ops(eng, n, training))
+        if not training and n.op in ('labelembed', 'center_loss'):
+            continue                                  # not in the inference plan
         ins = [A[t.name].double() for t in n.inputs]
         ref = so.forward(n, ins, p, training, ctx)
-        got = A[n.output.name]
-        cls = n.op + ('_y' if training else '_infer_y')
-        if n.op == 'maxpool':
-            errs.add(cls, 0.0 if torch.equal(got.double(), ref['y']) else 1.0, n.name)
-        else:
-            errs.add(cls, derr(got, ref['y']), n.name)
+        cls = _name(eng, n.op) + ('_y' if training else '_infer_y')
+        if training and cls == 'bn_y' and n.name == 'embedding_bn':
+            cls = 'embedding_bn_y'
+        if n.op in ('maxpool',) or cls.startswith('devise'):
+            errs.add(cls, _bits(A[n.output.name].cpu(), ref['y'].float().cpu()), n.name)
+        elif ref['y'] is not None:
+            errs.add(cls, derr(A[n.output.name], ref['y']), n.name)
         if training and n.op == 'bn':
             off, c = eng.bn_slot[n.name]
             errs.add('bn_mean', derr(eng.saved[off // 2:off // 2 + c], ref['mean']), n.name)
             errs.add('bn_invstd', derr(eng.saved[off // 2 + c:off // 2 + 2 * c], ref['invstd']), n.name)
+            m32 = np.float32(n.attrs['momentum'])
+            batch = {'moving_mean': ref['mean'],
+                     'moving_variance': onn.unbiased_var(ref['var'], ins[0].numel() // c, n.attrs['eps'])}
             for s in ('moving_mean', 'moving_variance'):
-                errs.add('bn_' + s, derr(eng._pview(n.name + '/' + s), ref[s]), n.name)
+                got = eng._pview(n.name + '/' + s)
+                key = 'bn_moving_variance_adagrad' if s == 'moving_variance' and eng.optimizer == 'adagrad' else 'bn_' + s
+                errs.add(key, derr(got, ref[s]), n.name)
+                f32 = p[n.name + '/' + s] * float(m32) + batch[s] * float(np.float32(1.0) - m32)
+                errs.add('bn_%s_f32decay' % s, derr(got, f32), n.name)
             # the statistics slot: float64 sums of the BatchNorm input as it was stored
             xs = ins[0].reshape(-1, c)
             st = eng.stats[off:off + 2 * c]
             errs.add('stats_sum', derr(st[:c], xs.sum(0)), n.name)
             errs.add('stats_sumsq', derr(st[c:], (xs * xs).sum(0)), n.name)
-        if training and n.op == 'head':
-            errs.add('head_loss', derr(eng.loss_buf, ref['loss']), n.name)
-        if training and n.op == 'xent':
-            errs.add('xent_loss', derr(eng.cls_loss_buf, ref['loss']), n.name)
-        errs.covered(plan, so.fwd_ops(eng, n, training))
+        if training and n.op in so.LOSS_OPS + ('head',):
+            # the per-sample loss (the center loss op runs in the backward plan, which has run by now)
+            errs.add(_name(eng, n.op) + '_loss', derr(_metric_bufs(eng, n)[0], ref['loss']), n.name)
+            _check_metrics(eng, errs, ctx, n, rows)
+        if training and n.op == 'labelembed':
+            # the mask, argmax(out2) == y on the engine's out2: the first float of each row's workspace terms
+            mask = eng.le_work[:4 * eng.B].view(eng.B, 4)[:, 0]
+            errs.add('labelembed_mask', _bits(mask.double().cpu(), ref['mask'].cpu()), n.name)
         del ins, ref
+
+
+def _check_eval(eng, errs, p):
+    """The validation plan after `infer`: every activation as `infer` wrote it, bit for bit, and the loss / metric
+    buffers against float64 on them.  The label embedding objective's batch ends with PAD padding rows (label -1)."""
+    A = eng.act
+    infer = {k: v.cpu() for k, v in A.items()}       # on the host: the activations of ResNet-50 at 224 px take 2.4 GB
+    rows = np.arange(eng.B)
+    if eng.le_node is not None:
+        eng.labels[eng.B - PAD:] = -1
+        rows = rows[:eng.B - PAD]
+    for b in (eng.loss_buf, eng.acc_buf, eng.rank_buf, eng.cls_loss_buf, eng.cls_acc_buf, eng.cls_rank_buf,
+              eng.center_buf):
+        b.fill_(7.0)
+    eng._run('eval')
+    torch.cuda.synchronize()
+    errs.add('eval_bits', 0.0 if all(torch.equal(A[k].cpu(), v) for k, v in infer.items()) else 1.0, 'act')
+    del infer
+    ctx = so.context(eng, eng.labels)
+    for n in eng.nodes:
+        errs.covered('eval', so.eval_ops(eng, n))
+        if n.op not in so.LOSS_OPS + ('head',):
+            continue
+        ref = so.forward(n, [A[t.name].double() for t in n.inputs], p, False, ctx)
+        loss = _metric_bufs(eng, n)[0]
+        r = torch.as_tensor(rows, device=loss.device)
+        errs.add(_name(eng, n.op) + '_eval_loss', derr(loss[r], ref['loss'][r]), n.name)
+        _check_metrics(eng, errs, ctx, n, rows)
+        if n.op == 'labelembed':
+            pad = torch.cat([eng.loss_buf[eng.B - PAD:], eng.acc_buf[eng.B - PAD:]])
+            errs.add('labelembed_padding', float(pad.abs().max()), n.name)
+    errs.covered('eval', so.buffer_ops(eng)['eval'])
+
+
+def _labelembed_bits(eng, errs, ctx):
+    """A standalone run of the forward plan's label embedding op into zeroed buffers: after the backward plan, the
+    gradients of out1 and out2 and the table's gradient in G must still equal its outputs bit for bit."""
+    from semantic_embeddings_b200 import _lib as L
+    A, Gd = eng.act, eng.grad
+    o1, o2 = eng.le_node.inputs
+    C = eng.num_classes
+    outs = [torch.zeros_like(t) for t in (eng.loss_buf, eng.acc_buf, Gd[o1.name], Gd[o2.name],
+                                          eng._pview(so.TABLE, eng.G), eng.le_work)]
+    op = eng._op(L.OP_LABELEMBED, [C, C, eng.B, C], [ctx.scale, eng.tau, eng.alpha, eng.beta],
+                 [A[o1.name], A[o2.name], eng.labels, eng._pview(so.TABLE)] + outs)
+    L.check(eng.lib.se_run_ops(eng._pack([op]), 1, eng.mode, L.stream_ptr()), 'se_run_ops(labelembed)')
+    torch.cuda.synchronize()
+    same = all(torch.equal(a, b) for a, b in zip(outs[:5], (eng.loss_buf, eng.acc_buf, Gd[o1.name], Gd[o2.name],
+                                                           eng._pview(so.TABLE, eng.G))))
+    errs.add('labelembed_bits', 0.0 if same else 1.0, eng.le_node.name)
 
 
 def _check_backward(eng, errs, p, ctx):
@@ -219,7 +367,10 @@ def _check_backward(eng, errs, p, ctx):
     for ev in walk:
         if ev[0] == 'grad':
             _, name, ref, ops = ev
-            errs.add(so.grad_class(ops) + '_dx', derr(Gd[name], ref), name)
+            cls = _name(eng, so.grad_class(ops)) + '_dx'
+            if ops == {'labelembed'}:
+                cls = 'labelembed_dout%d' % (1 if name == eng.le_node.inputs[0].name else 2)
+            errs.add(cls, derr(Gd[name], ref), name)
             continue
         _, n, local = ev
         errs.covered('bwd', so.bwd_ops(eng, n))
@@ -229,7 +380,8 @@ def _check_backward(eng, errs, p, ctx):
             off, shape = eng.offsets[pname]
             covered[off:off + int(np.prod(shape))] = True
             kind = 'dw' if pname.endswith('/kernel') else 'db' if pname.endswith('/bias') else \
-                'dgamma' if pname.endswith('/gamma') else 'dbeta'
+                'dgamma' if pname.endswith('/gamma') else 'dbeta' if pname.endswith('/beta') else \
+                {so.TABLE: 'dtable', so.CENTROIDS: 'dc'}[pname]
             got = eng._pview(pname, eng.G)
             if kind == 'db':
                 # a bias in front of a BatchNorm has a gradient that is zero in exact arithmetic (BatchNorm's dx sums to
@@ -238,7 +390,8 @@ def _check_backward(eng, errs, p, ctx):
                 mag = dy.double().abs().reshape(-1, dy.shape[-1]).sum(0).max()
                 errs.add('%s_db' % n.op, float((got.double() - ref).abs().max() / mag.clamp_min(1e-30)), pname)
             else:
-                errs.add('%s_%s' % (n.op, kind), derr(got, ref), pname)
+                key = 'embedding_bn_dgamma' if pname == 'embedding_bn/gamma' else '%s_%s' % (n.op, kind)
+                errs.add(key, derr(got, ref), pname)
         if n.op in ('conv', 'dense'):
             d = L.ConvDesc(*eng._conv_desc(n))
             dw = torch.zeros_like(eng._pview(n.name + '/kernel', eng.G))
@@ -251,12 +404,13 @@ def _check_backward(eng, errs, p, ctx):
         del local
     # the gradient memset: nothing but zeros between the tensors
     errs.add('grad_padding', float(eng.G[~covered].abs().max()) if bool((~covered).any()) else 0.0, 'G')
+    if eng.le_node is not None:
+        _labelembed_bits(eng, errs, ctx)
 
 
 def _check_optimizer(eng, errs, P0, G0, V0, lr0):
     lam = so.l2_per_element(eng, device='cuda')
-    ref = so.sgd(P0.double(), G0.double(), V0.double(), lam, lr0.double().tolist(), eng.momentum, eng.nesterov,
-                 eng.clipnorm)
+    ref = so.optimizer(eng, P0.double(), G0.double(), V0.double(), lam, lr0.double().tolist())
     # g = fma(2 lam, p, g) per element: its error against the magnitudes of the two terms, element by element
     mag = G0.double().abs() + 2.0 * lam * P0.double().abs()
     errs.add('opt_g', float(((eng.G.double() - ref['G']).abs() / mag.clamp_min(1e-30)).max()), 'G')
@@ -264,23 +418,27 @@ def _check_optimizer(eng, errs, P0, G0, V0, lr0):
     out = eng.sgd_out.cpu()
     errs.add('opt_sumsq', abs(float(out[0]) - ref['sumsq']) / ref['sumsq'], 'sgd_out[0]')
     errs.add('opt_reg', abs(float(out[1]) - ref['reg']) / max(ref['reg'], 1e-30) if ref['reg'] else float(out[1]), 'sgd_out[1]')
-    errs.add('opt_v', derr(eng.V, ref['V']), 'V')
-    errs.add('opt_dp', derr(eng.P.double() - P0.double(), ref['P'] - P0.double()), 'P')
+    v, dp = ('adagrad_a', 'adagrad_dp') if eng.optimizer == 'adagrad' else ('opt_v', 'opt_dp')
+    errs.add(v, derr(eng.V, ref['V']), 'V')
+    errs.add(dp, derr(eng.P.double() - P0.double(), ref['P'] - P0.double()), 'P')
     lr = eng.lr_dev.cpu()
     errs.add('opt_lr_t', abs(float(lr[3]) - ref['lr_t']) / ref['lr_t'], 'lr_dev[3]')
     errs.add('opt_iterations', 0.0 if float(lr[2]) == float(lr0[2]) + 1 else 1.0, 'lr_dev[2]')
+    # set_trainable: no gradient, no update and no optimizer state in the frozen runs
+    for off, n in eng.frozen_runs:
+        fz = slice(off, off + n)
+        ok = bool((eng.G[fz] == 0).all()) and torch.equal(eng.P[fz], P0[fz]) and bool((eng.V[fz] == 0).all())
+        errs.add('frozen_bits', 0.0 if ok else 1.0, 'frozen run at %d' % off)
     errs.covered('opt', so.buffer_ops(eng)['opt'])
 
 
-@pytest.mark.parametrize('cfg', CONFIGS, ids=lambda c: '%s-b%d-%s' % c[:3])
+@pytest.mark.parametrize('cfg', CONFIGS, ids=so.config_id)
 def test_every_op_of_the_captured_step_against_float64(cfg):
     import time
     t0 = time.time()
-    arch, B, mode, opts = cfg
     _lib()
-    eng = _engine(arch, B, mode, opts)
+    eng = _engine(cfg)
     errs = Errors()
-    ctx = so.loss_spec(eng, eng.labels)
     # 1-2: two steps through the captured step graph; the second made its filter copies from the first one's parameters
     eng._run('step')
     torch.cuda.synchronize()
@@ -289,6 +447,13 @@ def test_every_op_of_the_captured_step_against_float64(cfg):
     torch.cuda.synchronize()
     errs.add('filter_copies', 0.0 if _check_filter_copies(eng, P1) else 1.0, 'after step')
     del P1
+    if eng.le_node is not None:
+        # half of the labels at argmax(out2) of this forward pass (which the next one repeats): the mask and its
+        # normalisation take part
+        eng._run('fwd')
+        half = torch.arange(eng.B, device='cuda') < eng.B // 2
+        eng.labels.copy_(torch.where(half, eng.act[eng.le_node.inputs[1].name].argmax(-1).int(), eng.labels))
+    ctx = so.context(eng, eng.labels)
     # 3: snapshot
     P0, V0, S0, lr0 = eng.P.clone(), eng.V.clone(), eng.S.clone(), eng.lr_dev.cpu().clone()
     # 4: one forward + backward from its captured graph, every op checked on its own inputs
@@ -308,19 +473,20 @@ def test_every_op_of_the_captured_step_against_float64(cfg):
     torch.cuda.synchronize()
     _check_optimizer(eng, errs, P0, G0, V0, lr0)
     del P0, G0, V0, S0
-    # 6: the inference plan with the updated parameters and moving statistics
+    # 6: the inference plan with the updated parameters and moving statistics, then the validation plan
     eng._run('infer')
     torch.cuda.synchronize()
     errs.add('filter_copies', 0.0 if _check_filter_copies(eng, eng.P) else 1.0, 'after infer')
     p = _params(eng, eng.P.double(), eng.S.double())
     _check_forward(eng, errs, p, ctx, training=False)
     errs.covered('infer', so.buffer_ops(eng)['infer'])
+    _check_eval(eng, errs, p)
     del p
     plans = so.plan_ops(eng)
     from semantic_embeddings_b200 import _lib as L
     names = {v: k for k, v in vars(L).items() if k.startswith('OP_')}
     counts = {k: {names[o]: c for o, c in sorted(errs.ops[k].items())} for k in plans}
-    report('step_layers', case='%s B=%d %s' % (arch, B, mode), seconds=round(time.time() - t0, 1), ops=counts,
+    report('step_layers', case=so.config_id(cfg), seconds=round(time.time() - t0, 1), ops=counts,
            **{k: v[0] for k, v in sorted(errs.worst.items())}, worst_at={k: v[1] for k, v in errs.worst.items()})
     for k in plans:
         assert errs.ops[k] == plans[k], (k, counts[k], {names[o]: c for o, c in sorted(plans[k].items())})
