@@ -426,6 +426,38 @@ int64_t se_row_argsort_workspace_bytes(int rows, int n);
 int se_row_argsort(const float* dist, int64_t ld, int rows, int n, int32_t* out_idx, int64_t ldo, void* workspace,
                    void* stream);
 
+/* ------------------------------------------------------------------ classification (evaluate_classification_accuracy.py)
+ * One-vs-rest linear SVM of the reference's train_and_predict (:20-48, sklearn LinearSVC(C): squared hinge loss, L2
+ * penalty, intercept as a constant feature 1 that is regularised like the weights).  For class c, y_i = +1 where
+ * labels[i] == c and -1 elsewhere, x~ = [x, 1], w~ = [W[:, c], b[c]]:
+ *   f_c(w~) = 1/2 |w~|^2 + penalty * sum_i max(0, 1 - y_i w~.x~_i)^2
+ * solved for all classes at once by the trust-region Newton method with conjugate-gradient steps (liblinear's primal
+ * solver for L2R_L2LOSS_SVC); class c stops when |grad f_c| <= tol * max(min(pos_c, neg_c), 1) / N * |grad f_c(0)|
+ * (sklearn's defaults: tol 1e-4, max_iter 1000).  The row sums are se_dense_fwd / se_dense_bwd in SE_MODE_TF32X3 with D
+ * padded to a multiple of 4 and C to a multiple of 16 (zero columns); the weight gradient must add its split-K slices in
+ * a fixed order, so (D+1) x C is limited by the library's workspace (about 4M elements: 2048 x 2048 fits) and
+ * SE_ERR_UNSUPPORTED names the shape otherwise.  No float atomics: reruns give the same bits.
+ * X [N, ldx] float32 features; labels [N] int32 in [0, C) (else SE_ERR_ARG); outputs W [D, C] (Dense layout), b [C],
+ * iters [C] int32 accepted Newton steps, gnorm [C] float32 = final |grad f_c| / |grad f_c(0)| (b, iters, gnorm may be
+ * NULL).  workspace: se_linear_svm_workspace_bytes(N, D, C) bytes of device memory, 256-byte aligned.
+ * The call BLOCKS: the host reads the classes' convergence flags after every CG step, so it synchronises with `stream`
+ * and cannot be captured into a CUDA graph (SE_ERR_ARG inside a capture). */
+int64_t se_linear_svm_workspace_bytes(int N, int D, int C);
+int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, const int32_t* labels, int C, float penalty, float tol,
+                      int max_iter, float* W, float* b, int32_t* iters, float* gnorm, void* workspace, void* stream);
+/* Feature scaling of train_and_predict (:33-38) with numpy's float32 results bit for bit, and score negation:
+ *   SE_SCALE_ROW_L2      y = x / ||x||_2 per row (float32 squares summed in numpy's pairwise order, true division)
+ *   SE_SCALE_COL_MAXABS  colmax[j] = max_i |x_ij|          (y is not written)
+ *   SE_SCALE_COL_DIV     y = x / max(1e-8, colmax[j])      (true division)
+ *   SE_SCALE_MUL         y = scale * x                     (scale = -1 turns se_row_topk's ascending order descending)
+ * x [rows, ldx], y [rows, ldy]; y may be x. */
+#define SE_SCALE_ROW_L2 0
+#define SE_SCALE_COL_MAXABS 1
+#define SE_SCALE_COL_DIV 2
+#define SE_SCALE_MUL 3
+int se_scale_features(const float* x, int64_t ldx, int rows, int D, int op, float* colmax, float scale, float* y, int64_t ldy,
+                      void* stream);
+
 /* ------------------------------------------------------------------ plan runner
  * Runs a host-built array of ops (one training step is ~900 launches) in one call so that
  * neither Python nor ctypes sits between launches.  Each op is an opcode plus the argument

@@ -15,6 +15,7 @@ SE_MODE_F32, SE_MODE_TF32, SE_MODE_TF32X3 = 0, 1, 2
 MODE_NAMES = {0: 'f32', 1: 'tf32', 2: 'tf32x3'}
 SE_LOSS_INV_CORR, SE_LOSS_UNNORM_CORR, SE_LOSS_MSE, SE_LOSS_SOFTMAX_CORR, SE_LOSS_DEVISE_RANK = 0, 1, 2, 3, 4
 SE_PDIST_SQEUCLID, SE_PDIST_NEGDOT = 0, 1
+SE_SCALE_ROW_L2, SE_SCALE_COL_MAXABS, SE_SCALE_COL_DIV, SE_SCALE_MUL = 0, 1, 2, 3
 # se_bn_bwd_path: bits 0-1 = path (0 reduce + apply, 1 shared-memory slab, 2 register slab), bit 2 = float4 / fixed quad
 SE_BN_BWD_SCALAR, SE_BN_BWD_SLAB_ATOMIC, SE_BN_BWD_SLAB_REG, SE_BN_BWD_VEC, SE_BN_BWD_SLAB_QUAD = 0, 1, 2, 4, 5
 
@@ -99,6 +100,9 @@ _SIGS = {
     'se_labelembed_fwd_bwd': (c_int, [_P, _P, c_int, _P, _P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, _P, _P,
                                       _P, _P, _P, _P, _P]),
     'se_center_loss_fwd_bwd': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_float, _P, _P, _P, _P]),
+    'se_linear_svm_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
+    'se_linear_svm_fit': (c_int, [_P, c_int64, c_int, c_int, _P, c_int, c_float, c_float, c_int, _P, _P, _P, _P, _P, _P]),
+    'se_scale_features': (c_int, [_P, c_int64, c_int, c_int, c_int, _P, c_float, _P, c_int64, _P]),
     'se_sgd_schedule': (c_int, [_P, _P]),
     'se_pairwise_topk_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'se_pairwise_topk': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, _P]),

@@ -297,6 +297,15 @@ bool conv_wgrad_tc_would_run(const se_conv_desc* d, int x3) {
   return conv1x1_wgrad_tc_ok(d) || conv3x3s2_tc_ok(d) || conv3x3_wgrad_tc_ok(d);
 }
 
+// se_linear_svm_fit: does the tensor-core kernel take this shape on stream `st` and add its split-K slices in a fixed
+// order, i.e. does at least one pair of slices fit a workspace that exists or can be allocated now?
+bool conv_wgrad_tc_fixed_order(const se_conv_desc* d, cudaStream_t st) {
+  if (!conv_wgrad_tc_would_run(d, 1)) return false;
+  const long long T = (long long)d->kh * d->kw * d->Cin * d->Cout;
+  float* ws = nullptr;
+  return wgrad_workspace(2 * (T + d->Cout), st, &ws) == SE_OK && ws != nullptr;
+}
+
 template <int BN>
 static void wgrad_go(int x3, dim3 grid, cudaStream_t st, const float* x, const float* dy, const WgTcParams& p) {
   const size_t smem = 1024 + 2 * (size_t)(WG_MT * 128 + BN * 128) * (x3 ? 2 : 1);
