@@ -78,6 +78,25 @@ def test_svm_oracle_matches_sklearn(C):
         assert np.linalg.norm(w - w_ref) <= 1e-6 * np.linalg.norm(w_ref), c
 
 
+@pytest.mark.parametrize('N', [1, 20, 31, 32, 33, 64, 65, 2999, 50000])
+@pytest.mark.parametrize('D', [1, 5, 63, 64, 130, 640])
+@pytest.mark.parametrize('C', [3, 16, 17, 33, 100])
+def test_svm_workspace_layout_matches_the_library(N, D, C):
+    """svm_oracle.svm_layout (the region views the solver's step tests read) ends where se_linear_svm_workspace_bytes
+    says, over the padding edges of N (< 32 rows, 64-row blocks), D (multiples of 4) and C (multiples of 16)."""
+    from semantic_embeddings_b200 import _lib
+    if not os.path.exists(_lib.LIB_PATH):
+        import __graft_entry__ as ge
+        ge.build()
+    dims, regions, total = svm_oracle.svm_layout(N, D, C)
+    assert int(_lib.load().se_linear_svm_workspace_bytes(N, D, C)) == total
+    assert all(off % 256 == 0 for _, off, _, _ in regions)
+    assert [r[0] for r in regions] == ['xp', 's_cur', 's_trial', 'R'] + list(svm_oracle.SVM_VECTORS) + \
+        ['partial', 'state', 'counts', 'ctr']
+    assert dims['Np'] >= 32 and dims['Dp'] % 4 == 0 and dims['Cp'] % 16 == 0 and dims['nrb'] * 64 >= dims['Np']
+    assert svm_oracle.svm_state_dtype().itemsize == 128
+
+
 def test_svm_path_rejects_two_classes_and_empty_classes():
     from semantic_embeddings_b200.classification import check_training_labels, svm_predict
     X = np.zeros((6, 4), np.float32)

@@ -17,12 +17,7 @@ def _cls():
 
 
 def _scaled(N, D, K, seed, normalize):
-    X, y = svm_oracle.clustered_features(N, D, K, seed)
-    if normalize:
-        X = X / np.linalg.norm(X, axis=-1, keepdims=True)
-    else:
-        X = X / np.maximum(1e-8, np.abs(X).max(axis=0, keepdims=True))
-    return X, y
+    return svm_oracle.scaled_features(N, D, K, seed, normalize)
 
 
 @pytest.mark.parametrize('D', [3, 7, 64, 100, 129, 640, 2049])
@@ -45,7 +40,10 @@ def test_scaling_equals_numpy_float32_bit_for_bit(D):
 
 
 CASES = [(N, D, K, C) for N, D, K in ((3000, 64, 10), (2999, 100, 17), (50000, 64, 100)) for C in (0.1, 1.0)] + \
-    [(50000, 640, 100, 0.1)]
+    [(50000, 640, 100, 0.1)] + \
+    [(20, 5, 3, 1.0),            # N < 32 padding rows, D % 4 != 0, a single 16-column class tile
+     (33, 63, 16, 0.1),          # one row past the padding, Dp = 64, C = Cp = 16
+     (4000, 130, 33, 1.0)]       # Cp = 48: two 32-class blocks of the per-class kernels, the second mostly padding
 
 
 @pytest.mark.parametrize('N,D,K,C', CASES)
@@ -62,7 +60,9 @@ def test_svm_wide_features_at_c1_measured_level(normalize):
     """640-d features at C = 1 stop short of the 1e-5 objective gap at sklearn's tol = 1e-4: measured on an H100,
     column scaling 1.06e-3 with |w~ - w~*| up to 3.0e-2 relative after 20-37 Newton steps, L2 rows 5.8e-5 and 6.3e-3
     after 11-12.  The stopping rule |grad| <= tol min(pos, neg) / N |grad(0)| is met there before that gap (liblinear's
-    rule, not the fp32 arithmetic: at tol = 1e-6 the same fit reaches 4.4e-7, test below).  This pins the level."""
+    rule, not the fp32 arithmetic: at tol = 1e-6 the same fit reaches 4.4e-7, test below; test_svm_steps_gpu.py finds
+    the float64 gradient at the returned point within 0.999 of the threshold and the fp32 gradient within 3% of the
+    threshold of it at every iterate).  This pins the level."""
     _check_svm(50000, 640, 100, 1.0, normalize, 2e-3, 5e-2, min_safe=0.0)
 
 
@@ -115,6 +115,76 @@ def test_svm_rejects_bad_labels():
     X = np.random.RandomState(0).randn(100, 8).astype(np.float32)
     with pytest.raises(_lib.SeError, match='outside'):
         cls.linear_svm_fit(X, np.r_[np.arange(99) % 3, 3], 3)
+
+
+def _fit_raw(x, ldx, N, D, lab, K, C, max_iter=1000, tol=1e-4):
+    import torch
+    from semantic_embeddings_b200 import _lib
+    ws = torch.empty(int(_lib.load().se_linear_svm_workspace_bytes(N, D, K)), dtype=torch.uint8, device='cuda')
+    W, b = torch.empty(D, K, device='cuda'), torch.empty(K, device='cuda')
+    it = torch.empty(K, dtype=torch.int32, device='cuda')
+    _lib.call('se_linear_svm_fit', x.data_ptr(), ldx, N, D, lab.data_ptr(), K, float(C), float(tol), int(max_iter),
+              W.data_ptr(), b.data_ptr(), it.data_ptr(), None, ws.data_ptr(), _lib.stream_ptr())
+    return W, b, it
+
+
+def test_svm_on_a_strided_feature_matrix():
+    """ldx = D + 3 (rows of a wider buffer, the padding filled with NaN): the same bits as the contiguous copy."""
+    import torch
+    N, D, K = 3001, 61, 7
+    X, y = _scaled(N, D, K, seed=4, normalize=False)
+    buf = torch.full((N, D + 3), float('nan'), device='cuda')
+    buf[:, :D] = torch.from_numpy(X).cuda()
+    lab = torch.from_numpy(y).cuda()
+    W, b, it = _fit_raw(buf, D + 3, N, D, lab, K, 1.0)
+    W2, b2, it2 = _fit_raw(torch.from_numpy(X).cuda(), D, N, D, lab, K, 1.0)
+    assert torch.isfinite(W).all()
+    assert torch.equal(W, W2) and torch.equal(b, b2) and torch.equal(it, it2)
+
+
+def test_scaling_strided_and_in_place_equals_numpy():
+    """se_scale_features with ldx, ldy > D (columns past D untouched) and in place (y == x) for the row norms."""
+    import torch
+    from semantic_embeddings_b200 import _lib
+    cls = _cls()
+    rng = np.random.RandomState(12)
+    N, D = 777, 133
+    X = (rng.randn(N, D) * rng.rand(1, D) * 5).astype(np.float32)
+    xb = torch.full((N, D + 5), 7.0, device='cuda')
+    xb[:, :D] = torch.from_numpy(X).cuda()
+    yb = torch.full((N, D + 9), -3.0, device='cuda')
+    row = X / np.linalg.norm(X, axis=-1, keepdims=True)
+    _lib.call('se_scale_features', xb.data_ptr(), D + 5, N, D, _lib.SE_SCALE_ROW_L2, None, 1.0, yb.data_ptr(), D + 9,
+              _lib.stream_ptr())
+    assert np.array_equal(yb[:, :D].cpu().numpy(), row) and bool((yb[:, D:] == -3.0).all())
+    colmax = torch.empty(D, device='cuda')
+    _lib.call('se_scale_features', xb.data_ptr(), D + 5, N, D, _lib.SE_SCALE_COL_MAXABS, colmax.data_ptr(), 1.0, None, 0,
+              _lib.stream_ptr())
+    m = np.abs(X).max(axis=0)
+    assert np.array_equal(colmax.cpu().numpy(), m)
+    _lib.call('se_scale_features', xb.data_ptr(), D + 5, N, D, _lib.SE_SCALE_COL_DIV, colmax.data_ptr(), 1.0, yb.data_ptr(),
+              D + 9, _lib.stream_ptr())
+    assert np.array_equal(yb[:, :D].cpu().numpy(), X / np.maximum(1e-8, m)) and bool((yb[:, D:] == -3.0).all())
+    cls._scale(xb[:, :D], _lib.SE_SCALE_ROW_L2)                # in place, stride D + 5
+    assert np.array_equal(xb[:, :D].cpu().numpy(), row) and bool((xb[:, D:] == 7.0).all())
+
+
+def test_svm_fixed_order_refusal_boundary():
+    """(D+1) x C must fit the fixed-order weight-gradient workspace (two slices of Dp Cp + Cp floats in 8 M): (Dp, Cp) =
+    (4 092, 1 024) is the last D that fits at C = 1 024 and reruns to the same bits; D = 4 096 is refused with its shape."""
+    import torch
+    from semantic_embeddings_b200 import _lib
+    N, K = 64, 1024
+    lab = torch.from_numpy((np.arange(N) * 17 % K).astype(np.int32)).cuda()
+    for D in (4092, 4096):
+        x = torch.from_numpy(np.random.RandomState(D).randn(N, D).astype(np.float32) / 64).cuda()
+        if D == 4092:
+            runs = [_fit_raw(x, D, N, D, lab, K, 1.0, max_iter=1) for _ in range(2)]
+            assert all(torch.equal(a, b) for a, b in zip(*runs))
+            assert bool((runs[0][2] == 1).all()) and bool(torch.isfinite(runs[0][0]).all())
+        else:
+            with pytest.raises(_lib.SeError, match=r'rc=-3.*4096 x 1024 does not fit the fixed-order'):
+                _fit_raw(x, D, N, D, lab, K, 1.0, max_iter=1)
 
 
 def test_nearest_centroid_ranking_equals_the_float64_cdist_argsort():
