@@ -15,15 +15,23 @@
 //   1x1 / stride 1 layers are the same GEMM over the flat pixel list (tiles of 128 consecutive pixels), 1x1 / stride 2
 //   layers address the input (forward) or the output (backward data) through the sub-sampled view x[:, ::2, ::2, :].
 //
-// Warp-specialised (384 threads): warp 0 issues the TMA loads of a ring of (tap, channel block) stages, the two
-// consumer warpgroups (threads 128..383) each own 64 rows of the tile and issue m64nBNk8 wgmma on them; the epilogue
-// (bias / residual / ReLU / BatchNorm sums, or the accumulate of the data gradient) runs on the accumulator registers.
+// Warp-specialised (384 threads): warp 0 issues the TMA loads of a ring of stages, the two consumer warpgroups
+// (threads 128..383) each own 64 rows of the tile and issue m64nBNk8 wgmma on them; the epilogue (bias / residual /
+// ReLU / BatchNorm sums, or the accumulate of the data gradient) runs on the accumulator registers.
+//
+// Stages.  A stage is one (filter tap, channel block) pair, in that order (tap-major).  3x3 layers whose channels fit
+// ("resident box", ConvTcParams::res): TMA loads the (Wb + 2) x (Hb + 2) x Nb pixels around the tile -- every channel
+// block, once per tile -- and the stages carry only B; tap (r, s) reads the box r * (Wb + 2) + s rows further on, so
+// every input pixel is loaded once per tile instead of 9 times.  Other layers (1x1, wide 3x3) load A with each stage,
+// as the box shifted by the tap.  Both read A into registers per thread (wgmma with A from registers), so a tap's rows
+// need not be whole swizzle groups, and both issue the same MMAs in the same order.
 //
 // X3 = error-compensated arithmetic ("3xTF32"): every fp32 operand is the sum of hi = its mantissa truncated to 10
 // bits and lo = x - hi, and the product is accumulated as A_hi*B_hi + A_hi*B_lo + A_lo*B_hi in the same fp32
 // accumulator (the dropped A_lo*B_lo and the truncation of lo are ~2^-21 relative: fp32-level results from
-// tensor-core tiles).  Weights: lo is a second B tile written once per step by se_split_filters.  Activations: the
-// consumer threads split each stage in shared memory (A -> hi in place, lo into a second A tile) before its MMAs.
+// tensor-core tiles).  Weights: lo is a second B tile written once per step by se_split_filters.  Activations: each
+// consumer thread splits its A fragments in registers and feeds both halves to wgmma from registers; nothing in shared
+// memory is rewritten.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -36,7 +44,7 @@ using namespace tc;
 constexpr int CT_BM = 128;
 constexpr int CT_THREADS = 384;        // warpgroup 0: TMA producer (one thread), warpgroups 1 and 2: MMA + epilogue
 constexpr int CT_MAX_STAGES = 6;
-constexpr int CT_SMEM_BUDGET = 200 * 1024;
+constexpr int CT_SMEM_LIMIT = 227 * 1024;
 
 struct ConvTcParams {
   int N, H, W;              // extent of the grid the pixel tiles cover (images, rows, pixels)
@@ -45,7 +53,10 @@ struct ConvTcParams {
   int tw, th;               // tiles along a row / along the rows of an image
   int cblk, kblocks;        // channels per pipeline stage (16 or 32), Kc / cblk
   int taps, pad, flip;      // filter size (3 or 1), 'same' padding rows (1 or 0), 1: dgrad (tap order reversed for B)
-  int stages, stage_bytes, a_bytes, b_bytes;
+  int res;                  // 1: resident box (A loaded once per tile, stages hold B only), 0: per-tap stages
+  int ring_off;             // bytes of shared memory before the stage ring (the resident box)
+  int stages, stage_bytes, b_bytes;   // stage = [A of one tap (per-tap only)] B [B_lo (X3)]
+  int a_bytes, a_tx;        // one A tile (per-tap stage / channel block of the resident box): slot size, TMA bytes
   long long o_sn, o_sh, o_sw;   // output (and residual) element strides of an image, a row, a pixel
   int ovh, ovw;             // rows / pixels of the output view that exist (a strided view may be one short)
   int relu;
@@ -64,27 +75,55 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a, uint6
   else wgmma_tf32_n128(d, a, b, acc);
 }
 
-// in place: x -> tf32_hi(x), and lo = x - hi into a second tile (X3 only)
-__device__ __forceinline__ void split_tile(uint8_t* hi, uint8_t* lo, int bytes, int tid, int nthreads) {
-  float4* h = reinterpret_cast<float4*>(hi);
-  float4* l = reinterpret_cast<float4*>(lo);
-  for (int i = tid; i < (bytes >> 4); i += nthreads) {
-    const float4 v = h[i];
-    if (lo) l[i] = make_float4(tf32_lo(v.x), tf32_lo(v.y), tf32_lo(v.z), tf32_lo(v.w));
-    h[i] = make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w));
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t b, int acc) {
+  if constexpr (BN == 16) wgmma_tf32_rs_n16(d, a, b, acc);
+  else if constexpr (BN == 32) wgmma_tf32_rs_n32(d, a, b, acc);
+  else if constexpr (BN == 64) wgmma_tf32_rs_n64(d, a, b, acc);
+  else wgmma_tf32_rs_n128(d, a, b, acc);
+}
+
+// The A words of k-steps 0..nks-1 for this thread's two rows: a[ks] = (row0, 8ks + t), (row1, 8ks + t),
+// (row0, 8ks + 4 + t), (row1, 8ks + 4 + t) -- the register fragment of wgmma_tf32_rs_n*.  Rows are numbered in the
+// tile `base` (a stage, or one channel block of the resident box); channel 8ks + 4c + t of a row lies in its 16-byte
+// chunk 2ks + c, which the TMA swizzle moves to chunk (2ks + c) ^ (row & 7) for 128-byte rows and
+// (2ks + c) ^ ((row >> 1) & 3) for 64-byte rows (tile bases are 1024-byte aligned).
+//   Bank conflicts: one load instruction of a warp reads word t of one logical chunk from the rows of 8 consecutive
+//   output pixels g = 0..7.  Where these are 8 consecutive rows of the tile (every tile of the per-tap staging; the
+//   resident box when Wb >= 8), the load is conflict-free for both widths: 128-byte rows each span all 32 banks and
+//   their XOR terms row & 7 are 8 different values -> 8 chunks x 4 words = 32 banks; 64-byte rows alternate between
+//   the two bank halves, and the four rows of a half have four different XOR terms (row >> 1) & 3 -> 32 banks.  Only
+//   4-pixel-wide boxes (two image rows per 8 pixels) can meet 2-way conflicts.
+__device__ __forceinline__ void load_a(uint32_t (&a)[4][4], const uint8_t* base, int row0, int row1, int nks, int row_bytes,
+                                       int t) {
+  const uint8_t* p0 = base + row0 * row_bytes + 4 * t;
+  const uint8_t* p1 = base + row1 * row_bytes + 4 * t;
+  const int sw0 = row_bytes == 128 ? row0 & 7 : (row0 >> 1) & 3;
+  const int sw1 = row_bytes == 128 ? row1 & 7 : (row1 >> 1) & 3;
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    if (ks < nks) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int c = 2 * ks + (i >> 1);
+        a[ks][i] = *reinterpret_cast<const uint32_t*>((i & 1) ? p1 + ((c ^ sw1) << 4) : p0 + ((c ^ sw0) << 4));
+      }
+    }
   }
 }
 
 template <int BN, int X3>
-__global__ void __launch_bounds__(CT_THREADS, 1)
+__global__ void __launch_bounds__(CT_THREADS, (X3 && BN == 16) ? 2 : 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                const __grid_constant__ CUtensorMap map_bl, ConvTcParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * p.stage_bytes);
+  uint8_t* ring = smem + p.ring_off;
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + (size_t)p.stages * p.stage_bytes);
   uint64_t* empty = full + CT_MAX_STAGES;
-  float* s_stats = reinterpret_cast<float*>(empty + CT_MAX_STAGES);     // [8 consumer warps][2][BN]
+  uint64_t* abar = empty + CT_MAX_STAGES;                                // resident box loaded
+  float* s_stats = reinterpret_cast<float*>(abar + 1);                   // [8 consumer warps][2][BN]
 
   const int tid = threadIdx.x;
   const int tm = blockIdx.x, tn = blockIdx.y;
@@ -97,6 +136,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     prefetch_tmap(&map_a); prefetch_tmap(&map_b);
     if (X3) prefetch_tmap(&map_bl);
     for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+    mbar_init(abar, 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -105,17 +145,25 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (tid < 128) {
     // ===================== TMA producer
     if (tid == 0) {
+      if (p.res) {
+        // the resident box: every channel block of the (Wb + 2) x (Hb + 2) x Nb pixels around the tile, once
+        mbar_expect_tx(abar, p.kblocks * p.a_tx);
+        for (int kb = 0; kb < p.kblocks; ++kb)
+          tma_load_4d(smem + (size_t)kb * p.a_bytes, &map_a, abar, kb * p.cblk, w0 - 1, h0 - 1, n0);
+      }
       int stage = 0, phase = 0;
-      const uint32_t tx = (p.a_bytes + p.b_bytes) * (X3 ? 2 : 1) - (X3 ? p.a_bytes : 0);
+      const uint32_t tx = (p.res ? 0 : p.a_tx) + p.b_bytes * (X3 ? 2 : 1);
       for (int it = 0; it < nk; ++it) {
         const int tap = it / p.kblocks, kb = it - tap * p.kblocks;
         const int r = tap / p.taps, s = tap - r * p.taps;
         const int btap = p.flip ? p.taps * p.taps - 1 - tap : tap;
         mbar_wait(&empty[stage], phase ^ 1);
         mbar_expect_tx(&full[stage], tx);
-        uint8_t* sa = smem + (size_t)stage * p.stage_bytes;
-        uint8_t* sb = sa + p.a_bytes;
-        tma_load_4d(sa, &map_a, &full[stage], kb * p.cblk, w0 + s - p.pad, h0 + r - p.pad, n0);
+        uint8_t* sb = ring + (size_t)stage * p.stage_bytes;
+        if (!p.res) {
+          tma_load_4d(sb, &map_a, &full[stage], kb * p.cblk, w0 + s - p.pad, h0 + r - p.pad, n0);
+          sb += p.a_bytes;
+        }
         tma_load_2d(sb, &map_b, &full[stage], kb * p.cblk, btap * p.Nc + tn * BN);
         if (X3) tma_load_2d(sb + p.b_bytes, &map_bl, &full[stage], kb * p.cblk, btap * p.Nc + tn * BN);
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
@@ -126,43 +174,69 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 
   // ===================== consumers: warpgroup wg owns rows 64*wg .. 64*wg+63 of the tile
   const int wg = (tid >> 7) - 1, tid_wg = tid & 127, lane = tid & 31;
+  const int nks = p.cblk / 8;
+  // the tile rows of this thread's two A rows (output pixels m and m + 8): in a per-tap stage the pixel index itself,
+  // in the resident box the pixel's row for filter tap (0, 0); tap (r, s) is r * (Wb + 2) + s rows further on
+  int arow[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = wg * 64 + fragment_row(2 * h, tid_wg);
+    const int wb = m % p.Wb, hb = (m / p.Wb) % p.Hb, nb = m / (p.Wb * p.Hb);
+    arow[h] = p.res ? (nb * (p.Hb + 2) + hb) * (p.Wb + 2) + wb : m;
+  }
   // X3: each stage's MMAs start a fresh register tile `part` that is then added into `acc` -- the tensor core's own
   // accumulation loses low bits with every instruction, which over the 3 x 9 x Kc / 8 MMAs of a wide layer exceeds the
   // fp32-level error budget of this mode
   float acc[BN / 2], part[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  if (p.res) mbar_wait(abar, 0);
   int stage = 0, phase = 0;
   for (int it = 0; it < nk; ++it) {
+    const int tap = it / p.kblocks, kb = it - tap * p.kblocks;
+    const int r = tap / p.taps, s = tap - r * p.taps;
     mbar_wait(&full[stage], phase);
-    uint8_t* sa = smem + (size_t)stage * p.stage_bytes;
-    uint8_t* sb = sa + p.a_bytes;
-    uint8_t* sbl = sb + p.b_bytes;
-    uint8_t* sal = sbl + p.b_bytes;
+    const uint8_t* sst = ring + (size_t)stage * p.stage_bytes;
+    const uint8_t* abase = p.res ? smem + (size_t)kb * p.a_bytes : sst;
+    const int aoff = p.res ? r * (p.Wb + 2) + s : 0;
+    const uint32_t b0 = smem_u32(p.res ? sst : sst + p.a_bytes), bl0 = b0 + p.b_bytes;
+    uint32_t a[4][4];
+    load_a(a, abase, arow[0] + aoff, arow[1] + aoff, nks, row_bytes, lane & 3);
     if (X3) {
-      split_tile(sa, sal, p.a_bytes, tid - 128, 256);
-      split_tile(sb, nullptr, p.b_bytes, tid - 128, 256);
-      fence_proxy_async();                   // generic-proxy writes -> visible to the tensor core
-      named_bar_sync(1, 256);
-    }
-    const uint32_t a0 = smem_u32(sa) + wg * 64 * row_bytes, b0 = smem_u32(sb);
-    wgmma_fence();
-#pragma unroll 1
-    for (int ks = 0; ks < p.cblk / 8; ++ks) {
-      const uint64_t da = wgmma_desc(a0 + ks * 32, row_bytes), db = wgmma_desc(b0 + ks * 32, row_bytes);
-      if (X3) {
-        wgmma_tf32<BN>(part, da, db, ks != 0);
-        wgmma_tf32<BN>(part, da, wgmma_desc(smem_u32(sbl) + ks * 32, row_bytes), 1);
-        wgmma_tf32<BN>(part, wgmma_desc(smem_u32(sal) + wg * 64 * row_bytes + ks * 32, row_bytes), db, 1);
-      } else {
-        wgmma_tf32<BN>(acc, da, db, (it | ks) != 0);
+      // A is split here: hi = the TF32 truncation, lo = x - hi (exact in fp32).  B is fed as TMA delivered it: the
+      // tensor core reads the TF32 truncation of each fp32 word (test_tf32_operands_are_truncated_by_the_tensor_core),
+      // i.e. B_hi of w, and of the low parts w - trunc(w) that se_split_filters wrote
+      uint32_t lo[4][4];
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          if (ks >= nks) break;
+          const uint32_t hi = a[ks][i] & 0xFFFFE000u;
+          lo[ks][i] = __float_as_uint(__uint_as_float(a[ks][i]) - __uint_as_float(hi));
+          a[ks][i] = hi;
+        }
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        if (ks < nks) {
+          const uint64_t db = wgmma_desc(b0 + ks * 32, row_bytes);
+          wgmma_tf32_rs<BN>(part, a[ks], db, ks != 0);
+          wgmma_tf32_rs<BN>(part, a[ks], wgmma_desc(bl0 + ks * 32, row_bytes), 1);
+          wgmma_tf32_rs<BN>(part, lo[ks], db, 1);
+        }
       }
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    if (X3) {
+      wgmma_commit();
+      wgmma_wait<0>();
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+    } else {
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks)
+        if (ks < nks) wgmma_tf32_rs<BN>(acc, a[ks], wgmma_desc(b0 + ks * 32, row_bytes), (it | ks) != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[stage]);
@@ -309,8 +383,9 @@ static int pick_bn(int Nc, int x3) {
 template <int BN>
 static void conv_tc_go(int x3, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& ma, const CUtensorMap& mb,
                        const CUtensorMap& mbl, const ConvTcParams& p) {
-  if (x3) launch(conv_tc_kernel<BN, 1>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
-  else launch(conv_tc_kernel<BN, 0>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
+  if constexpr (BN <= 64)       // pick_bn: <= 64 channels per tile in the error-compensated mode
+    if (x3) return launch(conv_tc_kernel<BN, 1>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
+  launch(conv_tc_kernel<BN, 0>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
 }
 
 static int conv_tc_launch(const se_conv_desc* d, const float* a_tensor, int Kc, const float* bmat, int Nc, int flip,
@@ -346,17 +421,34 @@ static int conv_tc_launch(const se_conv_desc* d, const float* a_tensor, int Kc, 
   if (p.BN == 0 || tiles_m > 0x7fffffffLL || Nc / p.BN > 65535) return SE_ERR_UNSUPPORTED;
   p.cblk = Kc >= 32 ? 32 : 16;
   p.kblocks = Kc / p.cblk;
-  p.a_bytes = CT_BM * p.cblk * 4;
+  // The order in which the products reach the accumulator -- filter tap, then channel block, then k-step -- is the
+  // same for both stagings; only where A comes from differs.  The resident box (every channel block of the
+  // (Wb + 2) x (Hb + 2) x Nb pixels around the tile, loaded once) is taken whenever it leaves room for a two-stage ring
+  // of B tiles; wider 3x3 layers, and the 1x1 layers, stage A once per (tap, channel block).
   p.b_bytes = p.BN * p.cblk * 4;
-  p.stage_bytes = (p.a_bytes + p.b_bytes) * (1 + x3);
-  p.stages = min(CT_MAX_STAGES, CT_SMEM_BUDGET / p.stage_bytes);
+  const int smem_fixed = 1024 + (2 * CT_MAX_STAGES + 1) * 8 + 16 * p.BN * 4;   // alignment slack, barriers, statistics
+  p.res = 0;
+  if (taps == 3) {
+    p.a_tx = (p.Wb + 2) * (p.Hb + 2) * p.Nb * p.cblk * 4;
+    p.a_bytes = (p.a_tx + 1023) & ~1023;                    // 1024-byte aligned: the swizzle pattern starts over
+    p.stage_bytes = p.b_bytes * (1 + x3);
+    p.res = (CT_SMEM_LIMIT - smem_fixed - p.kblocks * p.a_bytes) / p.stage_bytes >= 2;
+  }
+  if (!p.res) {
+    p.a_tx = p.a_bytes = CT_BM * p.cblk * 4;
+    p.stage_bytes = p.a_bytes + p.b_bytes * (1 + x3);
+  }
+  p.ring_off = p.res ? p.kblocks * p.a_bytes : 0;
+  p.stages = min(CT_MAX_STAGES, (CT_SMEM_LIMIT - smem_fixed - p.ring_off) / p.stage_bytes);
   if (p.stages < 2) return SE_ERR_UNSUPPORTED;
+  // a CTA runs one tile: a ring longer than the tile's stages would only hold shared memory that other CTAs can use
+  p.stages = min(p.stages, taps * taps * p.kblocks);
   p.relu = relu; p.beta = beta;
   p.bias = bias; p.residual = residual; p.out = out; p.stats = stats;
   if (stats && (size_t)16 * Nc * sizeof(float) > 24 * 1024) return SE_ERR_UNSUPPORTED;   // wide layers: separate statistics pass
   if (beta != 0.f && (beta != 1.f || residual || relu)) return SE_ERR_UNSUPPORTED;
-  const size_t smem = 1024 + (size_t)p.stages * p.stage_bytes + 2 * CT_MAX_STAGES * 8 + 16 * p.BN * 4;
-  if (smem > 227 * 1024) return SE_ERR_UNSUPPORTED;
+  const size_t smem = (size_t)p.ring_off + (size_t)p.stages * p.stage_bytes + smem_fixed;
+  if (smem > CT_SMEM_LIMIT) return SE_ERR_UNSUPPORTED;
   if (x3_plan >= 0) return SE_OK;
   // output (and residual) addressing: NHWC over the tile grid, or the strided view dx[:, ::2, ::2, :] (s2 backward data)
   p.o_sw = Nc; p.o_sh = (long long)p.W * Nc; p.o_sn = (long long)p.H * p.W * Nc;
@@ -373,7 +465,7 @@ static int conv_tc_launch(const se_conv_desc* d, const float* a_tensor, int Kc, 
     if (s2 && !flip) {      // forward: x[:, ::2, ::2, :]
       strides[0] = (uint64_t)2 * Kc * 4; strides[1] = (uint64_t)2 * d->W * Kc * 4; strides[2] = (uint64_t)d->H * d->W * Kc * 4;
     }
-    uint32_t box[4] = {(uint32_t)p.cblk, (uint32_t)p.Wb, (uint32_t)p.Hb, (uint32_t)p.Nb};
+    uint32_t box[4] = {(uint32_t)p.cblk, (uint32_t)(p.Wb + 2 * p.res), (uint32_t)(p.Hb + 2 * p.res), (uint32_t)p.Nb};
     CUtensorMapSwizzle sw = p.cblk == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
     if (!make_tmap(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(a_tensor), dims, strides, box, sw)) return SE_ERR_CUDA;
     uint64_t bdims[2] = {(uint64_t)Kc, (uint64_t)taps * taps * Nc};
@@ -401,8 +493,10 @@ static int conv_tc_launch(const se_conv_desc* d, const float* a_tensor, int Kc, 
 
 template <int BN>
 static bool set_smem_limit() {
-  return cudaFuncSetAttribute(conv_tc_kernel<BN, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess &&
-         cudaFuncSetAttribute(conv_tc_kernel<BN, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess;
+  if constexpr (BN <= 64)
+    if (cudaFuncSetAttribute(conv_tc_kernel<BN, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM_LIMIT) != cudaSuccess)
+      return false;
+  return cudaFuncSetAttribute(conv_tc_kernel<BN, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM_LIMIT) == cudaSuccess;
 }
 
 int init_conv_tc() {
