@@ -458,6 +458,48 @@ int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, const int32_t* 
 int se_scale_features(const float* x, int64_t ldx, int rows, int D, int op, float* colmax, float scale, float* y, int64_t ldy,
                       void* stream);
 
+/* ------------------------------------------------------------------ class embeddings (compute_class_embedding.py)
+ * float64 throughout (csrc/class_embed.cu).  D [C, ldd] is the LCS-height distance table, S = 1 - D. */
+#define SE_ERR_NOT_CONVERGED (-4)
+/* D_ij = heights[first common entry of the lists of i and j] / max_height, D_ii = 0.  Class c's list is
+ * ancestors[offsets[c] .. offsets[c+1]), its ancestors and itself as node ranks in the order (-depth, node index),
+ * ascending; heights is indexed by rank.  max_len = the longest list (SE_ERR_UNSUPPORTED above 64).  A pair without a
+ * common ancestor gets NaN. */
+int se_lcs_height_table(const int32_t* offsets, const int32_t* ancestors, const int32_t* heights, int max_height, int C,
+                        int max_len, double* D, int64_t ldd, void* stream);
+/* In place: A [n, lda] symmetric (its lower triangle is read) -> its lower Cholesky factor L, upper triangle zeroed.
+ * status (device int): -1, or the first row whose pivot is <= 0 or NaN; that row's diagonal then holds the pivot and
+ * the rows after it are meaningless. */
+int se_cholesky_f64(double* A, int64_t lda, int n, int32_t* status, void* stream);
+/* SE_GRAM_SIM: out [C, C] = 1 - D.  SE_GRAM_SPHERES: out [C-1, C-1] = (D_0,i+1^2 + D_0,j+1^2 - D_i+1,j+1^2) / 2, the Gram
+ * matrix of the classes placed relative to class 0. */
+#define SE_GRAM_SIM 0
+#define SE_GRAM_SPHERES 1
+int se_class_gram_f64(const double* D, int64_t ldd, int C, int op, double* out, int64_t ldo, void* stream);
+/* X [m, ldx]: SE_COL_SQNORM out[j] = sum_i X_ij^2;  SE_COL_CENTER X_ij -= mean_i X_ij (out unused). */
+#define SE_COL_SQNORM 0
+#define SE_COL_CENTER 1
+int se_column_op_f64(double* X, int64_t ldx, int m, int n, int op, double* out, void* stream);
+/* Y[:, c] = X[:, cols[c]] for c < k (cols on the device) */
+int se_gather_columns_f64(const double* X, int64_t ldx, int m, const int32_t* cols, int k, double* Y, int64_t ldy, void* stream);
+/* X_i /= ||X_i||_2 for every row */
+int se_row_normalize_f64(double* X, int64_t ldx, int m, int n, void* stream);
+/* One-sided block Jacobi, in place: right-multiplies X [m, ldx] by plane rotations until every pair of its n columns
+ * satisfies |a.b| <= n eps |a| |b| (pairs with a zero column excepted) over a whole sweep.  Blocks of 16 columns meet in
+ * a fixed round-robin order, so reruns give the same bits.  *sweeps (host) = the sweeps run, the last one included;
+ * SE_ERR_NOT_CONVERGED after max_sweeps.  workspace: se_jacobi_columns_workspace_bytes(m, n) bytes of device memory.
+ * The call BLOCKS (it reads the convergence flag after every sweep) and cannot be captured into a CUDA graph. */
+int64_t se_jacobi_columns_workspace_bytes(int m, int n);
+int se_jacobi_columns_f64(double* X, int64_t ldx, int m, int n, int max_sweeps, int32_t* sweeps, void* workspace, void* stream);
+/* The self-check of compute_class_embedding.py over all C^2 pairs (diagonal included): out (device) [2] = max and mean of
+ * SE_DEV_SIM |E_i.E_j - (1 - D_ij)| or SE_DEV_DIST | ||E_i - E_j|| - D_ij |, E [C, lde] with dim columns.  Tiles are
+ * combined in a fixed order.  workspace: se_embedding_deviation_workspace_bytes(C) bytes of device memory. */
+#define SE_DEV_SIM 0
+#define SE_DEV_DIST 1
+int64_t se_embedding_deviation_workspace_bytes(int C);
+int se_embedding_deviation_f64(const double* E, int64_t lde, int C, int dim, const double* D, int64_t ldd, int mode, double* out,
+                               void* workspace, void* stream);
+
 /* ------------------------------------------------------------------ plan runner
  * Runs a host-built array of ops (one training step is ~900 launches) in one call so that
  * neither Python nor ctypes sits between launches.  Each op is an opcode plus the argument

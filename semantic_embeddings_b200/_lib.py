@@ -16,6 +16,10 @@ MODE_NAMES = {0: 'f32', 1: 'tf32', 2: 'tf32x3'}
 SE_LOSS_INV_CORR, SE_LOSS_UNNORM_CORR, SE_LOSS_MSE, SE_LOSS_SOFTMAX_CORR, SE_LOSS_DEVISE_RANK = 0, 1, 2, 3, 4
 SE_PDIST_SQEUCLID, SE_PDIST_NEGDOT = 0, 1
 SE_SCALE_ROW_L2, SE_SCALE_COL_MAXABS, SE_SCALE_COL_DIV, SE_SCALE_MUL = 0, 1, 2, 3
+SE_ERR_NOT_CONVERGED = -4
+SE_GRAM_SIM, SE_GRAM_SPHERES = 0, 1
+SE_COL_SQNORM, SE_COL_CENTER = 0, 1
+SE_DEV_SIM, SE_DEV_DIST = 0, 1
 # se_bn_bwd_path: bits 0-1 = path (0 reduce + apply, 1 shared-memory slab, 2 register slab), bit 2 = float4 / fixed quad
 SE_BN_BWD_SCALAR, SE_BN_BWD_SLAB_ATOMIC, SE_BN_BWD_SLAB_REG, SE_BN_BWD_VEC, SE_BN_BWD_SLAB_QUAD = 0, 1, 2, 4, 5
 
@@ -27,7 +31,9 @@ OP_CONV_FWD, OP_CONV_DGRAD, OP_CONV_WGRAD, OP_BN_STATS, OP_BN_FWD_TRAIN, OP_BN_F
 
 
 class SeError(RuntimeError):
-    pass
+    def __init__(self, msg, rc=None):
+        RuntimeError.__init__(self, msg)
+        self.rc = rc
 
 
 class ConvDesc(ctypes.Structure):
@@ -122,6 +128,16 @@ _SIGS = {
     'se_adagrad_apply_devlr': (c_int, [_P, _P, _P, c_int64, _P, c_float, c_float, _P, _P]),
     'se_pairwise_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'se_pairwise_dist': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, c_int, _P]),
+    'se_lcs_height_table': (c_int, [_P, _P, _P, c_int, c_int, c_int, _P, c_int64, _P]),
+    'se_cholesky_f64': (c_int, [_P, c_int64, c_int, _P, _P]),
+    'se_class_gram_f64': (c_int, [_P, c_int64, c_int, c_int, _P, c_int64, _P]),
+    'se_column_op_f64': (c_int, [_P, c_int64, c_int, c_int, c_int, _P, _P]),
+    'se_gather_columns_f64': (c_int, [_P, c_int64, c_int, _P, c_int, _P, c_int64, _P]),
+    'se_row_normalize_f64': (c_int, [_P, c_int64, c_int, c_int, _P]),
+    'se_jacobi_columns_workspace_bytes': (c_int64, [c_int, c_int]),
+    'se_jacobi_columns_f64': (c_int, [_P, c_int64, c_int, c_int, c_int, POINTER(c_int32), _P, _P]),
+    'se_embedding_deviation_workspace_bytes': (c_int64, [c_int]),
+    'se_embedding_deviation_f64': (c_int, [_P, c_int64, c_int, c_int, _P, c_int64, c_int, _P, _P, _P]),
     'se_run_ops': (c_int, [POINTER(Op), c_int, c_int, _P]),
     'se_run_ops_timed': (c_int, [POINTER(Op), c_int, c_int, _P, POINTER(c_float)]),
 }
@@ -153,7 +169,7 @@ def load():
 def check(rc, what=''):
     if rc != 0:
         msg = load().se_last_error().decode('utf-8', 'replace')
-        raise SeError('%s failed (rc=%d): %s' % (what or 'se_b200 call', rc, msg))
+        raise SeError('%s failed (rc=%d): %s' % (what or 'se_b200 call', rc, msg), rc)
 
 
 def ptr(t):

@@ -109,6 +109,21 @@ class ClassHierarchy(object):
                     wup[i, j], lcsh[i, j] = self.wup_similarity(a, b), self.lcs_height(a, b)
         return wup, lcsh
 
+    def ancestor_table(self, labels):
+        """Inputs of se_lcs_height_table for the classes `labels`: (offsets int32 [C+1], ancestors int32, heights int32,
+        max_height).  Nodes are numbered by rank in the order (-depth, node index), the tie rule of _lcs_ix, so the first
+        common entry of two classes' ascending ancestor lists (themselves included) is their lowest common subsumer.
+        heights[rank] is that node's height."""
+        order = sorted(range(len(self._ids)), key=lambda h: (-self._depth[h], h))
+        rank = np.empty(len(order), dtype=np.int32)
+        rank[order] = np.arange(len(order), dtype=np.int32)
+        lists = [np.sort(rank[list(self._hyp[self._ix[c]])]) for c in labels]
+        offsets = np.zeros(len(lists) + 1, dtype=np.int32)
+        offsets[1:] = np.cumsum([len(a) for a in lists])
+        ancestors = np.concatenate(lists).astype(np.int32) if lists else np.zeros(0, dtype=np.int32)
+        heights = np.asarray(self._height, dtype=np.int32)[order]
+        return offsets, ancestors, heights, self.max_height
+
     # ------------------------------------------------------------------------------------------- metrics (GPU)
     def hierarchical_precision(self, retrieved, labels, ks=[1, 10, 50, 100], compute_ahp=False, compute_ap=False,
                                ignore_qids=True, all_ids=None, device='cuda'):
