@@ -110,7 +110,8 @@ def main(argv=None):
     perf = OrderedDict()
     for e in entries:
         sys.stderr.write('-- {} --\n'.format(e['name']))
-        eng, kind = load_model(e['model'], data.num_classes, data.num_channels, args.architecture, args.batch_size, mode=mode)
+        eng, kind = load_model(e['model'], data.num_classes, data.num_channels, args.architecture, args.batch_size, mode=mode,
+                               input_size=getattr(data, 'input_size', None))
         sys.stderr.write('model: {} graph of {}\n'.format(kind, e['model']))
         if e['prob_features']:
             pred = extract_predictions(data, eng, e['layer'])

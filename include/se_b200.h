@@ -370,6 +370,40 @@ int se_augment_batch(const void* src, int src_is_u8, const int32_t* index, const
                      const unsigned char* flip, const float* mean, const float* inv_std, float* out, int B, int H, int W,
                      int C, void* stream);
 
+/* File datasets (NABirds / CUB): FileDatasetGenerator.compose_batch (datasets/common.py:380-432) after the decode, for a
+ * batch of B images decoded on the host to uint8 RGB (HWC) and packed into one device buffer `src`.  Per image, one
+ * descriptor (desc_host for the checks and the launch plan, desc_dev the same array in device memory for the kernel):
+ *   src_offset    byte offset of the image in src; src_h x src_w its size (each side <= SE_RESAMPLE_MAX_SIDE)
+ *   rh x rw       the size PIL resize(BILINEAR) gives it (>= the crop, <= SE_RESAMPLE_MAX_RESIZED; source / resized
+ *                 <= 31 on each axis) -- resampled bit-exactly like Pillow's libImaging/Resample.c, see file_augment.cu
+ *   flip          1: the resized image is mirrored left-right before the erase and the crop
+ *   ey, ex, eh, ew  erase rectangle in the (flipped) resized image, eh = 0: none
+ *   cy, cx        crop offset in the (flipped) resized image; the crop is crop_h x crop_w (<= SE_RESAMPLE_MAX_CROP)
+ *   noise_id      the image's number in the erase noise (its position in the global batch; 0 <= noise_id < 2^20)
+ * out [B, crop_h, crop_w, 3] float32 = (x - mean[c]) / std[c] (float32 subtraction, IEEE division, no epsilon), with the
+ * channels reversed when bgr = 1 (normalised in RGB order first, datasets/common.py:514-520).  An erased pixel holds
+ * (float)((u - (double)mean[c]) / (double)std[c]) with mean / std in RGB order even when bgr = 1 (as :538-540) and
+ *   u = se_erase_noise(seed, b, y, x, c), b = noise_id, (y, x) the pixel in the flipped resized image, c the output channel:
+ *     z = seed + (((((b << 20) | y) << 20 | x) << 2 | c) + 1) * 0x9E3779B97F4A7C15     (uint64, wrapping)
+ *     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;  z = (z ^ (z >> 27)) * 0x94D049BB133111EB;  z ^= z >> 31
+ *     u = (double)(z >> 11) * 2^-53 * 255.0                                         (in [0, 255))
+ * mean / std are host arrays of 3.  SE_ERR_ARG for any descriptor outside these limits (there is no reflect padding),
+ * and when a crop row's tables, 4 * crop_w * (3 * 8 + taps + 2) bytes, leave no room for a band row in 200 KB of shared
+ * memory (taps = 2 * ceil(source / resized) + 1 on the horizontal axis).
+ * One launch, no atomics: reruns give the same bits. */
+#define SE_RESAMPLE_MAX_SIDE 4096
+#define SE_RESAMPLE_MAX_RESIZED 65535
+#define SE_RESAMPLE_MAX_CROP 1024
+typedef struct {
+  int64_t src_offset;
+  int32_t src_h, src_w, rh, rw;
+  int32_t flip, ey, ex, eh, ew;
+  int32_t cy, cx, noise_id;
+} se_resample_desc;
+int se_resample_crop_batch(const unsigned char* src, const se_resample_desc* desc_host, const se_resample_desc* desc_dev,
+                           int B, int crop_h, int crop_w, const float* mean, const float* std, int bgr, uint64_t seed,
+                           float* out, void* stream);
+
 /* ------------------------------------------------------------------ retrieval
  * evaluate_retrieval.py:56-63: rows [row0,row0+rows) of the N x N distance matrix of F [N,ldF]
  * (fp32, D columns) against all N columns; out [rows, ldout].  normalize=1 applies line 58

@@ -138,9 +138,11 @@ def main(argv=None):
         embed_dim = centroids.shape[1]
     elif args.class_list is not None:
         class_list = read_class_list(args.class_list)
-    data = get_data_generator(args.dataset, args.data_root, classes=class_list, device='cuda:%d' % local)
+    data = get_data_generator(args.dataset, args.data_root, classes=class_list, device='cuda:%d' % local,
+                              read_workers=args.read_workers)
 
-    graph = utils.build_network(embed_dim, args.architecture, input_channels=data.num_channels)
+    graph = utils.build_network(embed_dim, args.architecture, input_channels=data.num_channels,
+                                input_size=getattr(data, 'input_size', None))
     mode = trainer.arith_mode(args, say)
     callbacks, epochs, decay = trainer.schedule(args, data)        # learn_center_loss.py:151,158-161
     pb = args.batch_size // world

@@ -128,7 +128,8 @@ def main(argv=None):
 
     # Load and L2-normalize class embeddings (learn_devise.py:57-62), load dataset (:65)
     embed_labels, embedding = load_class_embedding(args.embedding)
-    data = get_data_generator(args.dataset, args.data_root, classes=embed_labels, device='cuda:0')
+    data = get_data_generator(args.dataset, args.data_root, classes=embed_labels, device='cuda:0',
+                              read_workers=args.read_workers)
     D = embedding.shape[1]
 
     # Construct model (learn_devise.py:67-74)
@@ -141,9 +142,10 @@ def main(argv=None):
             args.architecture = arch
         say('  {} classifier over {} classes; its top layer \'prob\' becomes a {}-d linear layer \'embedding\''
             .format(args.architecture, num_cls, D))
-        graph = utils.build_devise_network(D, args.architecture, num_cls, input_channels=data.num_channels)
+        graph = utils.build_devise_network(D, args.architecture, num_cls, input_channels=data.num_channels,
+                                             input_size=getattr(data, 'input_size', None))
     else:
-        graph = utils.build_network(D, args.architecture, input_channels=data.num_channels)
+        graph = utils.build_network(D, args.architecture, input_channels=data.num_channels, input_size=getattr(data, 'input_size', None))
     mode = trainer.arith_mode(args, say)
     # Keras Adagrad as the reference compiles it: no clipnorm
     eng = Engine(graph, args.batch_size, embedding, loss='devise_rank', margin=args.margin, optimizer='adagrad',

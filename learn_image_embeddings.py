@@ -16,7 +16,8 @@ Deviations, all stated at run time when they apply:
     with a message;
   * --gpus N > 1: launch with `python -m torch.distributed.run --nproc-per-node N learn_image_embeddings.py ...`
     (one process per GPU, NCCL all-reduce; the reference's in-graph towers have the same arithmetic);
-  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles, datasets/cifar.py) and 'synthetic[:n]';
+  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles, datasets/cifar.py), 'NAB' / 'NAB-large' / 'CUB' (+ '-ilsvrcmean'
+    / '-caffe'; image files decoded on --read_workers threads, the network built for the crop size) and 'synthetic[:n]';
   * --arith selects the arithmetic of the convolutions: tf32x3 (default: tensor-core tiles with error compensation, fp32-level
     results), f32 (fp32 FFMA kernels), tf32 (single-pass TF32, ~1e-3 relative deviation: NOT the reference's arithmetic).
 """
@@ -98,11 +99,14 @@ def main(argv=None):
 
     local, rank, world, say = trainer.init_distributed(args)
 
-    data = get_data_generator(args.dataset, args.data_root, classes=embed_labels, device='cuda:%d' % local)
+    data = get_data_generator(args.dataset, args.data_root, classes=embed_labels, device='cuda:%d' % local,
+                              read_workers=args.read_workers)
     if embedding is None:
         embedding = np.eye(data.num_classes)
 
-    graph = utils.build_network(embedding.shape[1], args.architecture, input_channels=data.num_channels)
+    graph = utils.build_network(embedding.shape[1], args.architecture, input_channels=data.num_channels,
+                                # file datasets (NAB, CUB) crop to their own size; CIFAR / synthetic: the default
+                                input_size=getattr(data, 'input_size', None))
     mode = trainer.arith_mode(args, say)
     callbacks, epochs, decay = trainer.schedule(args, data)        # learn_image_embeddings.py:224-227
     pb = args.batch_size // world

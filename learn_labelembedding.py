@@ -118,9 +118,11 @@ def main(argv=None):
 
     # Load dataset (learn_labelembedding.py:110-119)
     class_list = read_class_list(args.class_list) if args.class_list is not None else None
-    data = get_data_generator(args.dataset, args.data_root, classes=class_list, device='cuda:%d' % local)
+    data = get_data_generator(args.dataset, args.data_root, classes=class_list, device='cuda:%d' % local,
+                              read_workers=args.read_workers)
 
-    graph = utils.build_network(args.embed_dim, args.architecture, input_channels=data.num_channels)
+    graph = utils.build_network(args.embed_dim, args.architecture, input_channels=data.num_channels,
+                                input_size=getattr(data, 'input_size', None))
     mode = trainer.arith_mode(args, say)
     callbacks, epochs, decay = trainer.schedule(args, data)        # learn_labelembedding.py:158,165-168
     pb = args.batch_size // world

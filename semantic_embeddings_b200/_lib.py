@@ -17,6 +17,8 @@ SE_LOSS_INV_CORR, SE_LOSS_UNNORM_CORR, SE_LOSS_MSE, SE_LOSS_SOFTMAX_CORR, SE_LOS
 SE_PDIST_SQEUCLID, SE_PDIST_NEGDOT = 0, 1
 SE_SCALE_ROW_L2, SE_SCALE_COL_MAXABS, SE_SCALE_COL_DIV, SE_SCALE_MUL = 0, 1, 2, 3
 SE_ERR_NOT_CONVERGED = -4
+SE_ERR_ARG = -1
+SE_RESAMPLE_MAX_SIDE, SE_RESAMPLE_MAX_CROP = 4096, 1024
 SE_GRAM_SIM, SE_GRAM_SPHERES = 0, 1
 SE_COL_SQNORM, SE_COL_CENTER = 0, 1
 SE_DEV_SIM, SE_DEV_DIST = 0, 1
@@ -50,6 +52,12 @@ class ConvAux(ctypes.Structure):
 
 class L2Segment(ctypes.Structure):
     _fields_ = [('begin', c_int64), ('end', c_int64), ('l2', c_float)]
+
+
+class ResampleDesc(ctypes.Structure):
+    """se_resample_desc: one image of se_resample_crop_batch."""
+    _fields_ = [('src_offset', c_int64)] + [(n, c_int32) for n in ('src_h', 'src_w', 'rh', 'rw', 'flip', 'ey', 'ex', 'eh',
+                                                                     'ew', 'cy', 'cx', 'noise_id')]
 
 
 class Op(ctypes.Structure):
@@ -121,6 +129,8 @@ _SIGS = {
     'se_row_argsort_workspace_bytes': (c_int64, [c_int, c_int]),
     'se_row_argsort': (c_int, [_P, c_int64, c_int, c_int, _P, c_int64, _P, _P]),
     'se_augment_batch': (c_int, [_P, c_int, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
+    'se_resample_crop_batch': (c_int, [_P, _P, _P, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_int,
+                                       ctypes.c_uint64, _P, _P]),
     'se_sgd_step': (c_int, [_P, _P, _P, c_int64, POINTER(L2Segment), c_int, c_float, c_float, c_int, c_float, _P, _P]),
     'se_sgd_prepare': (c_int, [_P, _P, c_int64, POINTER(L2Segment), c_int, _P, _P]),
     'se_sgd_apply': (c_int, [_P, _P, _P, c_int64, c_float, c_float, c_int, c_float, _P, _P]),

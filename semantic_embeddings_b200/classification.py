@@ -207,20 +207,20 @@ def read_dump(path):
     return None, dict(blob)
 
 
-def _candidates(arch, shapes, num_classes, input_channels):
+def _candidates(arch, shapes, num_classes, input_channels, input_size=None):
     """(name, graph builder, Engine keyword arguments) of every trainer's graph that could have written these tensors."""
     C = num_classes
     D = shapes['embedding/kernel'][1] if 'embedding/kernel' in shapes else \
         (shapes['cls_centroids/embeddings'][1] if 'cls_centroids/embeddings' in shapes else None)
-    ic = input_channels
-    out = [('classifier', lambda: utils.build_network(C, arch, classification=True, input_channels=ic),
+    ic, hw = input_channels, input_size
+    out = [('classifier', lambda: utils.build_network(C, arch, classification=True, input_channels=ic, input_size=hw),
             dict(objective='softmax', num_classes=C))]
     if D is not None:
         emb = np.zeros((C, D), np.float32)            # inference never reads the class matrix
-        net = lambda: utils.build_network(D, arch, input_channels=ic)
+        net = lambda: utils.build_network(D, arch, input_channels=ic, input_size=hw)
         out += [('embedding', net, dict(embedding=emb, num_classes=C)),
                 ('embedding+cls', net, dict(embedding=emb, cls_weight=1.0, num_classes=C)),
-                ('devise', lambda: utils.build_devise_network(D, arch, C, input_channels=ic),
+                ('devise', lambda: utils.build_devise_network(D, arch, C, input_channels=ic, input_size=hw),
                  dict(embedding=emb, loss='devise_rank', num_classes=C)),
                 ('labelembed', net, dict(objective='labelembed', num_classes=C)),
                 ('center_loss', net, dict(objective='center_loss', num_classes=C))]
@@ -231,7 +231,8 @@ def _graph_signature(eng):
     return tuple((n.name, n.op, tuple(n.output.shape)) for n in eng.nodes)
 
 
-def load_model(path, num_classes, input_channels=3, architecture=None, batch_size=1, device=None, mode=None):
+def load_model(path, num_classes, input_channels=3, architecture=None, batch_size=1, device=None, mode=None,
+               input_size=None):
     """Rebuilds the engine a trainer's dump came from: every candidate graph (classifier, embedding net with and without
     the cls_bn branch, DeViSE, label embedding net, center loss net) is built, and the one whose parameter names and
     shapes the dump covers exactly is taken.  Candidates that build the same graph count as one; none or several
@@ -245,7 +246,7 @@ def load_model(path, num_classes, input_channels=3, architecture=None, batch_siz
     if 'prob/kernel' in shapes and shapes['prob/kernel'][-1] != num_classes:
         raise ValueError('{}: prob/kernel has {} classes, the dataset {}'.format(path, shapes['prob/kernel'][-1], num_classes))
     matches, misses = OrderedDict(), []
-    for name, build, kw in _candidates(arch, shapes, num_classes, input_channels):
+    for name, build, kw in _candidates(arch, shapes, num_classes, input_channels, input_size):
         try:
             eng = Engine(build(), 1, device='cpu', use_cuda_graph=False, **kw)
         except (ValueError, KeyError) as e:
