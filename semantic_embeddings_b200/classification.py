@@ -278,16 +278,14 @@ def resolve_layer(eng, layer):
     net), 'l2norm' head_out, 'embedding' the top Dense layer's output, any other node name that node's output (a
     vector).  Integer indices are rejected."""
     if layer is None:
-        layer = 'prob' if eng.xent_node is not None or eng.le_node is not None else 'l2norm'
+        layer = 'prob' if eng.class_scores is not None else 'l2norm'
     layer = str(layer)
     if layer.lstrip('-').isdigit():
         raise ValueError(LAYER_INDEX_ERROR)
     if layer == 'prob':
-        if eng.le_node is not None:
-            return eng.le_node.inputs[0].name
-        if eng.xent_node is None:
+        if eng.class_scores is None:
             raise ValueError("layer 'prob': this model has no classifier")
-        return eng.xent_node.output.name
+        return eng.class_scores.name
     if layer == 'l2norm':
         if eng.head_node is None:
             raise ValueError("layer 'l2norm': this model has no embedding head")

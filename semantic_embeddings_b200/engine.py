@@ -16,7 +16,7 @@ import torch
 
 from . import _lib
 from ._lib import Op
-from .graph import Graph, Node, ParamSpec, T
+from .graph import Graph, Node, T
 
 LOSS_KINDS = {'inv_corr': _lib.SE_LOSS_INV_CORR, 'unnorm_corr': _lib.SE_LOSS_UNNORM_CORR, 'mse': _lib.SE_LOSS_MSE,
               'softmax_corr': _lib.SE_LOSS_SOFTMAX_CORR, 'devise_rank': _lib.SE_LOSS_DEVISE_RANK}
@@ -32,7 +32,17 @@ def _vp(x):
     return int(x)
 
 
-OBJECTIVES = ('embedding', 'softmax', 'labelembed', 'center_loss')
+def _aligned(shape):
+    """Floats a tensor of `shape` takes in a flat buffer: every tensor starts 16-byte aligned."""
+    return (int(np.prod(shape)) + 3) // 4 * 4
+
+
+# The objectives and the options that belong to each: the other objectives reject them when they are set (cls_weight and
+# label_smoothing when non-zero, the others when not None).  Only 'embedding' takes the class-embedding matrix;
+# 'labelembed' and 'center_loss' learn their class parameters and need num_classes.  'softmax' ignores `loss`, and with
+# it the margin of loss='devise_rank'.
+OBJECTIVES = {'embedding': ('cls_weight', 'margin'), 'softmax': ('label_smoothing', 'margin'),
+              'labelembed': ('tau', 'alpha', 'beta'), 'center_loss': ('center_loss_weight', 'centroids')}
 LABELEMBED_TABLE = 'labelembeddings/embeddings'
 CENTROIDS = 'cls_centroids/embeddings'
 
@@ -67,7 +77,15 @@ class Engine:
 
     optimizer='sgd': Keras SGD(lr, momentum (0.9 by default), decay, nesterov, clipnorm).  optimizer='adagrad': Keras
     Adagrad(lr, epsilon, decay) with the same optional clipnorm; its accumulators live where SGD keeps its velocity
-    (get_velocity / set_velocity), and it takes no momentum."""
+    (get_velocity / set_velocity), and it takes no momentum.
+
+    The objective is decided once.  OBJECTIVES says which options belong to which objective; _extend_graph appends the
+    objective's nodes, and everything else follows from them: head_node, xent_node, le_node and center_node (None where
+    absent), has_cls_branch (an embedding head and a cross-entropy), class_scores (the tensor of class scores that
+    predict, the validation loop and the classification evaluator read; None for the pure embedding head), pad_label and
+    metric_bufs (the per-sample metric buffers the loss ops write: 'loss', 'acc', 'rank', then 'cls_loss', 'cls_acc',
+    'cls_rank' or 'center_loss').  Each loss op emits its training, inference and validation forms in one place of
+    _build_plans, and the metrics readers turn host copies of metric_bufs into their dicts with one function."""
 
     def __init__(self, graph, batch, embedding=None, loss='inv_corr', cls_weight=0.0, num_classes=None,
                  mode=_lib.SE_MODE_F32, device='cuda:0', momentum=None, nesterov=False, clipnorm=10.0,
@@ -90,52 +108,35 @@ class Engine:
         if objective not in OBJECTIVES:
             raise ValueError('unknown objective %r (one of %s)' % (objective, ', '.join(OBJECTIVES)))
         self.objective = objective
+        given = dict(cls_weight=cls_weight or None, label_smoothing=label_smoothing or None, margin=margin, tau=tau,
+                     alpha=alpha, beta=beta, center_loss_weight=center_loss_weight, centroids=centroids)
+        foreign = [k for k, v in given.items() if v is not None and k not in OBJECTIVES[objective]]
+        if foreign:
+            raise ValueError('%s: not an option of objective=%r (its options: %s)'
+                             % (', '.join(foreign), objective, ', '.join(OBJECTIVES[objective])))
+        if (embedding is None) == (objective == 'embedding'):
+            raise ValueError("objective='embedding' needs the class-embedding matrix" if embedding is None else
+                             'objective=%r learns its own class parameters: it takes no class embedding' % objective)
+        if num_classes is None and objective in ('labelembed', 'center_loss'):
+            raise ValueError('objective=%r needs num_classes' % objective)
         self.label_smoothing = float(label_smoothing)
-        if objective != 'labelembed' and (tau is not None or alpha is not None or beta is not None):
-            raise ValueError("tau, alpha and beta belong to objective='labelembed'")
         self.tau = float(2.0 if tau is None else tau)
         self.alpha = float(0.9 if alpha is None else alpha)
         self.beta = float(0.5 if beta is None else beta)
-        if objective != 'center_loss' and (center_loss_weight is not None or centroids is not None):
-            raise ValueError("center_loss_weight and centroids belong to objective='center_loss'")
         self.center_loss_weight = float(0.1 if center_loss_weight is None else center_loss_weight)
-        if objective == 'center_loss':
-            if embedding is not None:
-                raise ValueError("objective='center_loss' learns its own class centroids: it takes no class embedding")
-            if cls_weight or self.label_smoothing != 0.0 or margin is not None:
-                raise ValueError("cls_weight, label_smoothing and margin do not apply to objective='center_loss'")
-            if num_classes is None:
-                raise ValueError("objective='center_loss' needs num_classes")
-            if not math.isfinite(self.center_loss_weight):
-                raise ValueError('the center loss weight must be finite')
-            if centroids is not None:
-                centroids = np.asarray(centroids, dtype=np.float64)
-                if not np.isfinite(centroids).all():
-                    raise ValueError('the fixed centroids must be finite')
-        elif objective == 'labelembed':
-            if embedding is not None:
-                raise ValueError("objective='labelembed' learns its own label embedding: it takes no class embedding")
-            if cls_weight or self.label_smoothing != 0.0 or margin is not None:
-                raise ValueError("cls_weight, label_smoothing and margin do not apply to objective='labelembed'")
-            if num_classes is None:
-                raise ValueError("objective='labelembed' needs num_classes")
-            if not (self.tau > 0.0 and math.isfinite(self.tau)):
-                raise ValueError('the temperature tau must be positive and finite')
-        elif objective == 'softmax':
-            if embedding is not None:
-                raise ValueError("objective='softmax' trains a classifier: it takes no class embedding")
-            if cls_weight:
-                raise ValueError("cls_weight belongs to objective='embedding'")
-        elif embedding is None:
-            raise ValueError("objective='embedding' needs the class-embedding matrix")
-        elif self.label_smoothing != 0.0:
-            raise ValueError("label_smoothing belongs to objective='softmax'")
+        if not (self.tau > 0.0 and math.isfinite(self.tau)):
+            raise ValueError('the temperature tau must be positive and finite')
+        if not math.isfinite(self.center_loss_weight):
+            raise ValueError('the center loss weight must be finite')
+        if centroids is not None:
+            centroids = np.asarray(centroids, dtype=np.float64)
+            if not np.isfinite(centroids).all():
+                raise ValueError('the fixed centroids must be finite')
         self.decay = float(decay)
         self.lib = _lib.load()
         self.dev = torch.device(device)
         if self.dev.type == 'cuda':
             torch.cuda.set_device(self.dev)     # (device='cpu' only builds the plans: used by the CPU-side tests)
-        if self.dev.type == 'cuda':
             _lib.check(self.lib.se_init(), 'se_init')
         self.g = graph
         self.B = int(batch)
@@ -230,105 +231,74 @@ class Engine:
             raise _lib.SeError('se_allreduce_sum returned %r instead of the world size %d' % (float(probe[0].item()), self.world))
         return True
 
-    # ------------------------------------------------------------------ graph extension: head (+ classifier)
+    # ------------------------------------------------------------------ graph extension: the objective's loss nodes
     def _extend_graph(self):
-        g = self.g
-        self.nodes = list(g.nodes)
-        self.pspecs = OrderedDict(g.params)
-        z = g.output
-        self.center_node = None
-        if self.objective == 'center_loss':
-            # center_loss_model (learn_center_loss.py:17-41): relu -> BatchNormalization('embedding_bn') -> Dense(C,
-            # softmax, 'prob') with the one-hot cross-entropy, and the label-indexed C x D centroids compared with z itself;
-            # the centroids come after the branch's weights, so the initial values of those do not change
-            sub, _, logits = self._relu_bn_dense(z, 'center_loss_relu', 'embedding_bn', 'prob', l2=0.0)
-            self.nodes += sub.nodes
-            self.pspecs.update(sub.params)
-            prob = T('prob_out', (self.num_classes,))
-            xe = Node('xent', 'xent', [logits], prob)
-            prob.producer = xe
-            self.nodes.append(xe)
-            self.pspecs[CENTROIDS] = ParamSpec(CENTROIDS, (self.num_classes, self.D), 'uniform')
-            cl = T('center_loss', (1,))
-            cn = Node('center_loss', 'center_loss', [z], cl, params=[CENTROIDS])
-            cl.producer = cn
-            self.nodes.append(cn)
-            self.head_node = None
-            self.xent_node = xe
-            self.le_node = None
-            self.center_node = cn
-            self.has_cls_branch = False
-            self._index_consumers()
-            return
-        if self.objective == 'softmax':
+        """Appends the objective's layers and loss nodes to the network's nodes and parameters (in this order: the
+        parameter order fixes the flat-buffer layout and the seeded initial weights), then derives from the appended
+        loss nodes head_node, xent_node, le_node and center_node (None where absent), has_cls_branch, class_scores (the
+        tensor of class scores, None for the pure embedding head) and pad_label."""
+        g, z, C = self.g, self.g.output, self.num_classes
+        self.nodes, self.pspecs = list(g.nodes), OrderedDict(g.params)
+        ext = Graph('cls', ())                   # a builder that appends to the engine's nodes and parameters
+        ext.nodes, ext.params = self.nodes, self.pspecs
+        if self.objective == 'embedding':
+            head = ext._add(Node('head', 'head', [z], T('head_out', (self.D,))))
+            if self.cls_weight > 0:
+                # cls_model (learn_image_embeddings.py:16-45): relu -> BatchNormalization() -> Dense(C, softmax, l2 5e-4)
+                # on the embedding output, or (--cls_base, :34-40) on the output of a named inner layer
+                self._xent(ext, self._relu_bn_dense(ext, self._cls_base_tensor(head), 'cls_relu', 'cls_bn', 5e-4)[1])
+        elif self.objective == 'softmax':
             # learn_classifier.py: Dense(C, softmax, name='prob') + categorical_crossentropy -- the softmax and the loss are
             # one op on the logits, whose gradient seeds the backward pass
-            prob = T('prob_out', (self.num_classes,))
-            xe = Node('xent', 'xent', [z], prob)
-            prob.producer = xe
-            self.nodes.append(xe)
-            self.head_node = None
-            self.xent_node = xe
-            self.le_node = None
-            self.has_cls_branch = False
-            self._index_consumers()
-            return
-        if self.objective == 'labelembed':
-            # labelembed_model (learn_labelembedding.py:40-56): relu -> BatchNormalization('embedding_bn') -> Dense(C, 'prob')
-            # = out1, Dense(C, 'out2') on stop_gradient of the same tensor, and the label-indexed C x C table
-            sub, b, out1 = self._relu_bn_dense(z, 'labelembed_relu', 'embedding_bn', 'prob', l2=0.0)
-            out2 = sub.dense(b, 'out2', self.num_classes, stop_gradient=True)
-            self.nodes += sub.nodes
-            self.pspecs.update(sub.params)
-            self.pspecs[LABELEMBED_TABLE] = ParamSpec(LABELEMBED_TABLE, (self.num_classes, self.num_classes), 'identity')
-            lo = T('labelembed_loss', (1,))
-            le = Node('labelembed', 'labelembed_loss', [out1, out2], lo, params=[LABELEMBED_TABLE])
-            lo.producer = le
-            self.nodes.append(le)
-            self.head_node = None
-            self.xent_node = None
-            self.le_node = le
-            self.has_cls_branch = False
-            self._index_consumers()
-            return
-        self.le_node = None
-        x_out = T('head_out', (self.D,))
-        head = Node('head', 'head', [z], x_out)
-        x_out.producer = head
-        self.nodes.append(head)
-        self.head_node = head
-        self.xent_node = None
-        if self.cls_weight > 0:
-            # cls_model (learn_image_embeddings.py:16-45): relu -> BatchNormalization() -> Dense(C, softmax, l2 5e-4) on the
-            # embedding output, or (--cls_base, :34-40) on the output of a named inner layer
-            base = x_out
-            if self.cls_base is not None:
-                cand = [n for n in g.nodes if n.name == str(self.cls_base)]
-                if not cand:
-                    raise ValueError('cls_base: no layer named %r (layers: %s)' % (self.cls_base, ', '.join(n.name for n in g.nodes)))
-                base = cand[0].output
-                if len(base.shape) != 1:
-                    raise ValueError('cls_base %r has a %d-d output %s: the classifier needs a feature vector (e.g. avg_pool)'
-                                     % (self.cls_base, len(base.shape), tuple(base.shape)))
-            sub, _, logits = self._relu_bn_dense(base, 'cls_relu', 'cls_bn', 'prob', l2=5e-4)
-            self.nodes += sub.nodes
-            self.pspecs.update(sub.params)
-            prob = T('prob_out', (self.num_classes,))
-            xe = Node('xent', 'xent', [logits], prob)
-            prob.producer = xe
-            self.nodes.append(xe)
-            self.xent_node = xe
-        self.has_cls_branch = self.xent_node is not None     # the --cls_weight classifier beside the embedding head
+            self._xent(ext, z)
+        elif self.objective == 'labelembed':
+            # labelembed_model (learn_labelembedding.py:40-56): relu -> BatchNormalization('embedding_bn') -> Dense(C,
+            # 'prob') = out1, Dense(C, 'out2') on stop_gradient of the same tensor, and the label-indexed C x C table
+            b, out1 = self._relu_bn_dense(ext, z, 'labelembed_relu', 'embedding_bn', 0.0)
+            out2 = ext.dense(b, 'out2', C, stop_gradient=True)
+            ext._param(LABELEMBED_TABLE, (C, C), 'identity')
+            ext._add(Node('labelembed', 'labelembed_loss', [out1, out2], T('labelembed_loss', (1,)),
+                          params=[LABELEMBED_TABLE]))
+        else:
+            # center_loss_model (learn_center_loss.py:17-41): relu -> BatchNormalization('embedding_bn') -> Dense(C,
+            # softmax, 'prob') with the one-hot cross-entropy, and the label-indexed C x D centroids compared with z
+            # itself; the centroids come after the branch's weights, so the initial values of those do not change
+            self._xent(ext, self._relu_bn_dense(ext, z, 'center_loss_relu', 'embedding_bn', 0.0)[1])
+            ext._param(CENTROIDS, (C, self.D), 'uniform')
+            ext._add(Node('center_loss', 'center_loss', [z], T('center_loss', (1,)), params=[CENTROIDS]))
+        added = {n.op: n for n in self.nodes[len(g.nodes):]}
+        self.head_node, self.xent_node, self.le_node, self.center_node = (
+            added.get(op) for op in ('head', 'xent', 'labelembed', 'center_loss'))
+        self.has_cls_branch = self.head_node is not None and self.xent_node is not None   # the --cls_weight classifier
+        self.class_scores = (self.le_node.inputs[0] if self.le_node is not None else
+                             self.xent_node.output if self.xent_node is not None else None)
+        # the label of the padding rows of a short last batch (None: repeat the last row's label); the label embedding
+        # loss normalises over the batch, so its padding rows carry -1 and take no part
+        self.pad_label = -1 if self.le_node is not None else None
         self._index_consumers()
 
-    def _relu_bn_dense(self, base, relu_name, bn_name, dense_name, l2):
-        """relu -> BatchNormalization() -> Dense(num_classes) on tensor `base`, as a sub-graph: (graph, BN output, logits).
-        The classifier branch of cls_model and the label embedding branch share it."""
-        sub = Graph('cls', tuple(base.shape))
-        sub.input = base
-        r = sub.relu(base, relu_name)
-        b = sub.bn(r, bn_name)
-        return sub, b, sub.dense(b, dense_name, self.num_classes, l2=l2)
+    def _cls_base_tensor(self, head):
+        """The tensor the --cls_weight classifier reads: the wrapped embedding `head`, or the output of layer cls_base."""
+        if self.cls_base is None:
+            return head
+        cand = [n for n in self.g.nodes if n.name == str(self.cls_base)]
+        if not cand:
+            raise ValueError('cls_base: no layer named %r (layers: %s)' % (self.cls_base, ', '.join(n.name for n in self.g.nodes)))
+        base = cand[0].output
+        if len(base.shape) != 1:
+            raise ValueError('cls_base %r has a %d-d output %s: the classifier needs a feature vector (e.g. avg_pool)'
+                             % (self.cls_base, len(base.shape), tuple(base.shape)))
+        return base
+
+    def _relu_bn_dense(self, ext, base, relu_name, bn_name, l2):
+        """relu -> BatchNormalization() -> Dense(num_classes, name='prob') on tensor `base`: (BN output, logits).  The
+        classifier branch of cls_model, the label embedding and the center loss models share it."""
+        b = ext.bn(ext.relu(base, relu_name), bn_name)
+        return b, ext.dense(b, 'prob', self.num_classes, l2=l2)
+
+    def _xent(self, ext, logits):
+        """The softmax + cross-entropy node on `logits`; its output 'prob_out' holds the class probabilities."""
+        return ext._add(Node('xent', 'xent', [logits], T('prob_out', (self.num_classes,))))
 
     def _index_consumers(self):
         self.consumers = {}
@@ -351,7 +321,7 @@ class Engine:
             for p in order:
                 if p.l2 == l:
                     self.offsets[p.name] = (off, p.shape)
-                    off += (int(np.prod(p.shape)) + 3) // 4 * 4      # keep every tensor 16-byte aligned
+                    off += _aligned(p.shape)
             if l > 0:
                 self.segments.append((beg, off, l))
         self.nparams = off
@@ -374,7 +344,7 @@ class Engine:
         self.soffsets, soff = OrderedDict(), 0
         for p in state:
             self.soffsets[p.name] = (soff, p.shape)
-            soff += (int(np.prod(p.shape)) + 3) // 4 * 4
+            soff += _aligned(p.shape)
         self.S = torch.zeros(max(soff, 4), **f32)
         self.seg_array = (_lib.L2Segment * max(1, len(self.segments)))()
         for k, (b, e, l) in enumerate(self.segments):
@@ -399,7 +369,13 @@ class Engine:
         self.rank_buf = torch.zeros(B, **f32)          # top-k metrics: rank of the true class (se_embed_head_fwd_bwd_ex)
         self.cls_rank_buf = torch.zeros(B, **f32)
         self.center_buf = torch.zeros(B, **f32)        # objective='center_loss': per-sample 1/2 ||z - c_y||^2
-        self.le_work = None                            # se_labelembed_fwd_bwd's workspace (per-row terms, table-gradient rows)
+        # the per-sample metric buffers this engine's loss ops write, by metric name, in the order the readers report them
+        self.metric_bufs = OrderedDict([('loss', self.loss_buf), ('acc', self.acc_buf), ('rank', self.rank_buf)])
+        if self.has_cls_branch:
+            self.metric_bufs.update(cls_loss=self.cls_loss_buf, cls_acc=self.cls_acc_buf, cls_rank=self.cls_rank_buf)
+        if self.center_node is not None:
+            self.metric_bufs['center_loss'] = self.center_buf
+        self.le_work = None                           # se_labelembed_fwd_bwd's workspace (per-row terms, table-gradient rows)
         if self.le_node is not None:
             nb = int(self.lib.se_labelembed_workspace_bytes(B, self.num_classes))
             if nb < 0:
@@ -497,15 +473,22 @@ class Engine:
         return None
 
     def _build_plans(self):
-        fwd, inf, bwd = [], [], []
+        fwd, inf, ev, bwd = [], [], [], []
         A, Gd = self.act, self.grad
         nbytes = lambda t: t.numel() * t.element_size()
+
+        def emit(train, infer, val=None):
+            """A node's op in the training forward, inference and validation plans (None: none there).  The validation
+            pass is the inference forward that also writes the metrics: it runs `infer` unless a loss op gives `val`."""
+            for plan, o in ((fwd, train), (inf, infer), (ev, infer if val is None else val)):
+                if o is not None:
+                    plan.append(o)
+
         fwd.append(self._op(_lib.OP_MEMSET, p=[self.stats, nbytes(self.stats)]))
         if self.PT is not None and self.n_tr:
             tr = self._op(_lib.OP_TRANSPOSE_FILTERS, [self.n_tr],
                           p=[self.P, self.PT, ctypes.addressof(self.tr_table), self.PL, self.PTL])
-            fwd.append(tr)
-            inf.append(tr)
+            emit(tr, tr)
         scale = 1.0 / (self.B * self.world)
         stats_by_conv = {}
         for n in self.nodes:
@@ -532,8 +515,8 @@ class Engine:
                     st = self.stats[off:off + 2 * c]
                 Wt = self._pview(n.name + '/kernel', self.PT) if (self.PT is not None and n.op == 'conv') else None
                 Wtl = self._pview(n.name + '/kernel', self.PTL) if (self.PTL is not None and n.op == 'conv') else None
-                fwd.append(self._op(_lib.OP_CONV_FWD, d + [relu], p=[A[n.inputs[0].name], W, b, res, out, st, Wt, Wtl]))
-                inf.append(self._op(_lib.OP_CONV_FWD, d + [relu], p=[A[n.inputs[0].name], W, b, res, out, None, Wt, Wtl]))
+                emit(self._op(_lib.OP_CONV_FWD, d + [relu], p=[A[n.inputs[0].name], W, b, res, out, st, Wt, Wtl]),
+                     self._op(_lib.OP_CONV_FWD, d + [relu], p=[A[n.inputs[0].name], W, b, res, out, None, Wt, Wtl]))
             elif n.op == 'bn':
                 x = n.inputs[0]
                 c = x.shape[-1]
@@ -556,79 +539,70 @@ class Engine:
                 pp = [A[x.name], st, self._pview(n.name + '/gamma'), self._pview(n.name + '/beta'),
                       self._pview(n.name + '/moving_mean'), self._pview(n.name + '/moving_variance'), sm, si, rp, out]
                 fwd_pos[n.name] = len(fwd)
-                fwd.append(self._op(_lib.OP_BN_FWD_TRAIN, ii, [a['eps'], a['momentum']], pp))
-                inf.append(self._op(_lib.OP_BN_FWD_INFER, ii, [a['eps'], a['momentum']], pp))
+                emit(self._op(_lib.OP_BN_FWD_TRAIN, ii, [a['eps'], a['momentum']], pp),
+                     self._op(_lib.OP_BN_FWD_INFER, ii, [a['eps'], a['momentum']], pp))
             elif n.op == 'avgpool2':
                 h, w, c = n.inputs[0].shape
                 o = self._op(_lib.OP_AVGPOOL_FWD, [self.B, h, w, c], p=[A[n.inputs[0].name], out])
-                fwd.append(o); inf.append(o)
+                emit(o, o)
             elif n.op == 'maxpool':
                 h, w, c = n.inputs[0].shape
                 a = n.attrs
                 o = self._op(_lib.OP_MAXPOOL_FWD, [self.B, h, w, c, a['k'], a['stride'], a['pad_t'], a['pad_l'],
                                                    n.output.shape[0], n.output.shape[1]], p=[A[n.inputs[0].name], out])
-                fwd.append(o); inf.append(o)
+                emit(o, o)
             elif n.op == 'gap':
                 h, w, c = n.inputs[0].shape
                 o = self._op(_lib.OP_GAP_FWD, [self.B, h * w, c], p=[A[n.inputs[0].name], out])
-                fwd.append(o); inf.append(o)
+                emit(o, o)
             elif n.op == 'add':
                 o = self._op(_lib.OP_ADD_FWD, [1 if n.attrs['relu'] else 0, out.numel()],
                              p=[A[n.inputs[0].name], A[n.inputs[1].name], out])
-                fwd.append(o); inf.append(o)
+                emit(o, o)
             elif n.op == 'relu':
                 o = self._op(_lib.OP_ADD_FWD, [1, out.numel()], p=[A[n.inputs[0].name], None, out])
-                fwd.append(o); inf.append(o)
+                emit(o, o)
             elif n.op == 'head':
                 z = A[n.inputs[0].name]
-                has_cls = bool(self.consumers.get(n.output.name))
                 ii = [self.D, self.D, self.B, self.D, self.C, LOSS_KINDS[self.loss]]
                 ff = self._head_f(scale)
-                dz = None if has_cls else Gd[n.inputs[0].name]
-                fwd.append(self._op(_lib.OP_HEAD, ii, ff,
-                                    [z, self.labels, self.E, None, out, self.loss_buf, self.acc_buf, dz, self.rank_buf]))
-                inf.append(self._op(_lib.OP_HEAD, ii, ff, [z, self.labels, self.E, None, out, None, None, None]))
-                self._eval_head = self._op(_lib.OP_HEAD, ii, ff, [z, self.labels, self.E, None, out, self.loss_buf,
-                                                                   self.acc_buf, None, self.rank_buf])
-            elif n.op == 'xent' and self.objective in ('softmax', 'center_loss'):
-                # the whole loss of the classifier (center_loss: the 'prob' term), weight 1; f[1] = label smoothing
+                dz = None if self.consumers.get(n.output.name) else Gd[n.inputs[0].name]
+                emit(self._op(_lib.OP_HEAD, ii, ff, [z, self.labels, self.E, None, out, self.loss_buf, self.acc_buf, dz,
+                                                     self.rank_buf]),
+                     self._op(_lib.OP_HEAD, ii, ff, [z, self.labels, self.E, None, out, None, None, None]),
+                     self._op(_lib.OP_HEAD, ii, ff, [z, self.labels, self.E, None, out, self.loss_buf, self.acc_buf, None,
+                                                     self.rank_buf]))
+            elif n.op == 'xent':
+                # the objective's whole loss (softmax; center_loss: the 'prob' term) with weight 1, or the --cls_weight
+                # classifier beside the embedding head, which writes the cls_* metrics; f[1] = label smoothing
                 lg = n.inputs[0]
                 ii = [self.num_classes, self.B, self.num_classes]
+                w, pre = (self.cls_weight, 'cls_') if self.has_cls_branch else (1.0, '')
+                lb, ab, rb = (self.metric_bufs[pre + m] for m in ('loss', 'acc', 'rank'))
                 ls = self.label_smoothing
-                fwd.append(self._op(_lib.OP_XENT, ii, [scale, ls],
-                                    [A[lg.name], self.labels, out, self.loss_buf, self.acc_buf, Gd[lg.name], self.rank_buf]))
-                inf.append(self._op(_lib.OP_XENT, ii, [0.0, ls], [A[lg.name], self.labels, out, None, None, None]))
-                self._eval_xent = self._op(_lib.OP_XENT, ii, [0.0, ls], [A[lg.name], self.labels, out, self.loss_buf,
-                                                                          self.acc_buf, None, self.rank_buf])
-            elif n.op == 'xent':
-                lg = n.inputs[0]
-                fwd.append(self._op(_lib.OP_XENT, [self.num_classes, self.B, self.num_classes],
-                                    [self.cls_weight * scale],
-                                    [A[lg.name], self.labels, out, self.cls_loss_buf, self.cls_acc_buf, Gd[lg.name],
-                                     self.cls_rank_buf]))
-                inf.append(self._op(_lib.OP_XENT, [self.num_classes, self.B, self.num_classes], [0.0],
-                                    [A[lg.name], self.labels, out, None, None, None]))
-                self._eval_xent = self._op(_lib.OP_XENT, [self.num_classes, self.B, self.num_classes], [0.0],
-                                           [A[lg.name], self.labels, out, self.cls_loss_buf, self.cls_acc_buf, None,
-                                            self.cls_rank_buf])
+                emit(self._op(_lib.OP_XENT, ii, [w * scale, ls], [A[lg.name], self.labels, out, lb, ab, Gd[lg.name], rb]),
+                     self._op(_lib.OP_XENT, ii, [0.0, ls], [A[lg.name], self.labels, out, None, None, None]),
+                     self._op(_lib.OP_XENT, ii, [0.0, ls], [A[lg.name], self.labels, out, lb, ab, None, rb]))
             elif n.op == 'labelembed':
                 # the whole loss (weight 1), in the forward plan like the softmax objective's cross-entropy; it writes the
-                # gradients of both logit heads and the table's gradient (into G, which the backward memset spares)
+                # gradients of both logit heads and the table's gradient (into G, which the backward memset spares); the
+                # inference plan ends at the logits
                 o1, o2 = n.inputs
                 C = self.num_classes
                 ii = [C, C, self.B, C]
                 table = self._pview(LABELEMBED_TABLE)
-                fwd.append(self._op(_lib.OP_LABELEMBED, ii, [scale, self.tau, self.alpha, self.beta],
-                                    [A[o1.name], A[o2.name], self.labels, table, self.loss_buf, self.acc_buf, Gd[o1.name],
-                                     Gd[o2.name], self._pview(LABELEMBED_TABLE, self.G), self.le_work]))
-                self._eval_le = self._op(_lib.OP_LABELEMBED, ii, [0.0, self.tau, self.alpha, self.beta],
-                                         [A[o1.name], A[o2.name], self.labels, table, self.loss_buf, self.acc_buf, None,
-                                          None, None, self.le_work])
+                emit(self._op(_lib.OP_LABELEMBED, ii, [scale, self.tau, self.alpha, self.beta],
+                              [A[o1.name], A[o2.name], self.labels, table, self.loss_buf, self.acc_buf, Gd[o1.name],
+                               Gd[o2.name], self._pview(LABELEMBED_TABLE, self.G), self.le_work]),
+                     None,
+                     self._op(_lib.OP_LABELEMBED, ii, [0.0, self.tau, self.alpha, self.beta],
+                              [A[o1.name], A[o2.name], self.labels, table, self.loss_buf, self.acc_buf, None, None, None,
+                               self.le_work]))
             elif n.op == 'center_loss':
                 # training: emitted by the backward plan; here only the loss-only form of the validation pass
-                self._eval_center = self._op(_lib.OP_CENTER_LOSS, self._center_i(), [0.0],
-                                             [A[n.inputs[0].name], self.labels, self._pview(CENTROIDS), self.center_buf,
-                                              None, None])
+                emit(None, None, self._op(_lib.OP_CENTER_LOSS, self._center_i(), [0.0],
+                                          [A[n.inputs[0].name], self.labels, self._pview(CENTROIDS), self.center_buf,
+                                           None, None]))
             else:
                 raise ValueError(n.op)
         # ---------------- backward
@@ -647,7 +621,7 @@ class Engine:
             # the forward plan has already written the table's gradient; the table is the last tensor of the flat buffer
             # (L2 0, added last), so the memset clears everything before it
             t_off, t_shape = self.offsets[LABELEMBED_TABLE]
-            assert t_off + (int(np.prod(t_shape)) + 3) // 4 * 4 == self.nparams, 'the label table must end the gradient buffer'
+            assert t_off + _aligned(t_shape) == self.nparams, 'the label table must end the gradient buffer'
             bwd.append(self._op(_lib.OP_MEMSET, p=[self.G, 4 * t_off]))
             final[LABELEMBED_TABLE] = 0
             written.update(t.name for t in self.le_node.inputs)
@@ -761,18 +735,6 @@ class Engine:
                 bwd.append(self._op(_lib.OP_ADD_BWD, [1, dY.numel()], [ba, 0.0], [dY, A[n.output.name], da, None]))
         # ---------------- optimizer
         opt = self._opt_ops()
-        ev = []
-        for o in inf:                               # validation pass: inference-mode forward that also writes the metrics
-            if o.opcode == _lib.OP_HEAD:
-                ev.append(self._eval_head)
-            elif o.opcode == _lib.OP_XENT:
-                ev.append(self._eval_xent)
-            else:
-                ev.append(o)
-        if self.le_node is not None:
-            ev.append(self._eval_le)
-        if self.center_node is not None:
-            ev.append(self._eval_center)
         self.plans = {'fwd': self._pack(fwd), 'bwd': self._pack(bwd), 'opt': self._pack(opt), 'infer': self._pack(inf),
                       'eval': self._pack(ev),
                       'fwdbwd': self._pack(fwd + bwd), 'step': self._pack(fwd + bwd + opt)}
@@ -813,14 +775,8 @@ class Engine:
         the global clipping norm is taken and its L2 term is left out (Keras differentiates the total loss with respect to
         the trainable weights only); forward, backward and the BatchNorm moving statistics run as before (Keras 2.2
         semantics).  Returns the names that are now frozen."""
-        size = lambda n: (int(np.prod(self.offsets[n][1])) + 3) // 4 * 4
         frozen = [n for n in self.offsets if trainable is not None and not trainable(n)]
-        runs = []
-        for off, sz in sorted((self.offsets[n][0], size(n)) for n in frozen):
-            if runs and runs[-1][0] + runs[-1][1] == off:
-                runs[-1][1] += sz
-            else:
-                runs.append([off, sz])
+        runs = self._runs(frozen)
         segs = []
         for b, e, l in self.segments:            # L2 segments minus the frozen runs
             cur = b
@@ -851,6 +807,16 @@ class Engine:
             self._graphs.pop(k, None)
         return frozen
 
+    def _runs(self, names):
+        """The flat-buffer ranges of the parameters `names`, merged into sorted [offset, length] runs."""
+        runs = []
+        for off, sz in sorted((self.offsets[n][0], _aligned(self.offsets[n][1])) for n in names):
+            if runs and runs[-1][0] + runs[-1][1] == off:
+                runs[-1][1] += sz
+            else:
+                runs.append([off, sz])
+        return runs
+
     def _with_allreduce(self, bwd, final):
         """Backward plan with SE_OP_ALLREDUCE ops: the flat gradient buffer is cut into `grad_buckets` buckets in the order
         the backward pass completes it (last layers first); a bucket's exchange is issued right after the op that writes
@@ -859,7 +825,6 @@ class Engine:
         per segment)."""
         missing = [n for n in self.offsets if n not in final]
         assert not missing, 'no backward op writes the gradient of %s' % missing
-        size = lambda n: (int(np.prod(self.offsets[n][1])) + 3) // 4 * 4
         order = sorted(self.offsets, key=lambda n: (final[n], self.offsets[n][0]))
         # cuts at equal shares of the backward pass's OPS (a proxy for time), not of the bytes: what is still to be
         # exchanged when the last gradient lands is then only the last stretch's share (for ResNet-110 the 16-channel
@@ -871,12 +836,7 @@ class Engine:
             out += list(bwd[start:cut])
             names = [n for n in order if final[n] <= cut and n not in done]
             done.update(names)
-            runs = []
-            for off, sz in sorted((self.offsets[n][0], size(n)) for n in names):
-                if runs and runs[-1][0] + runs[-1][1] == off:
-                    runs[-1][1] += sz
-                else:
-                    runs.append([off, sz])
+            runs = self._runs(names)
             for g0 in range(0, len(runs), 7):             # an op carries up to 7 ranges
                 grp = runs[g0:g0 + 7]
                 pp = [self.G]
@@ -939,20 +899,6 @@ class Engine:
         self.lr_dev[2:3].fill_(float(n))
         self.iterations = int(n)
 
-    def evaluate(self, x, labels):
-        """Inference-mode forward (BatchNorm moving statistics) + losses / metrics of one batch: what Keras' validation
-        pass and evaluate_generator compute (learn_image_embeddings.py:238-246).  Returns the metrics dict."""
-        self.load_batch(x, labels)
-        self._run('eval')
-        return self.metrics()
-
-    def forward_backward(self):
-        self._run('fwdbwd')
-
-    def apply_gradients(self):
-        self._run('opt')
-        self.iterations += 1
-
     def train_step(self, x=None, labels=None, lr=None, allreduce=None):
         """One reference training step (learn_image_embeddings.py:238): forward, backward, [all-reduce], clip + SGD."""
         if x is not None:
@@ -974,110 +920,71 @@ class Engine:
         allreduce_gradients(flat)                         # loss is already scaled by 1/global_batch
 
     def metrics(self):
-        """Host copies of the last step's per-sample loss / accuracy (one small D2H read)."""
-        out = {'loss': float(self.loss_buf.cpu().numpy().mean()), 'acc': float(self.acc_buf.cpu().numpy().mean())}
-        if self.center_node is not None:
-            out.update(self._center_terms(out['loss'], float(self.center_buf.cpu().numpy().mean())))
-        if self.has_cls_branch:
-            out['cls_loss'] = float(self.cls_loss_buf.cpu().numpy().mean())
-            out['cls_acc'] = float(self.cls_acc_buf.cpu().numpy().mean())
-        return out
+        """Means of the last step's per-sample losses / accuracies (one small D2H read per buffer)."""
+        return self._metrics_of({m: b.cpu().numpy() for m, b in self.metric_bufs.items() if not m.endswith('rank')})
 
     def per_sample_metrics(self, ks=()):
-        """Per-sample loss / accuracy arrays of the last batch (and accuracy@k for k in ks): what a validation loop sums
-        when its last batch is only partly filled."""
-        out = {'loss': self.loss_buf.cpu().numpy(), 'acc': self.acc_buf.cpu().numpy()}
-        if self.center_node is not None:
-            out.update(self._center_terms(out['loss'].astype(np.float64), self.center_buf.cpu().numpy().astype(np.float64)))
-        r = self.rank_buf.cpu().numpy() if ks else None
-        for k in ks:
-            out['acc%d' % k] = (r < k).astype(np.float32)
-        if self.has_cls_branch:
-            out['cls_loss'] = self.cls_loss_buf.cpu().numpy()
-            out['cls_acc'] = self.cls_acc_buf.cpu().numpy()
-            rc = self.cls_rank_buf.cpu().numpy() if ks else None
-            for k in ks:
-                out['cls_acc%d' % k] = (rc < k).astype(np.float32)
-        return out
-
-    def top_k_accuracy(self, ks):
-        """--top_k_acc (learn_image_embeddings.py:167-180): accuracy@k of the last batch for every k in `ks`, from the rank
-        of the true class that the head kernels wrote: {'acc<k>': ..., 'cls_acc<k>': ...}."""
-        r = self.rank_buf.cpu().numpy()
-        out = {'acc%d' % k: float((r < k).mean()) for k in ks}
-        if self.has_cls_branch:
-            rc = self.cls_rank_buf.cpu().numpy()
-            out.update({'cls_acc%d' % k: float((rc < k).mean()) for k in ks})
-        return out
+        """Per-sample loss / accuracy arrays of the last batch (and accuracy@k, also of the classifier branch, for k in
+        ks): what a validation loop sums when its last batch is only partly filled."""
+        return self._metrics_of({m: b.cpu().numpy() for m, b in self.metric_bufs.items() if ks or not m.endswith('rank')},
+                                ks, per_sample=True)
 
     def metrics_async(self, ks=()):
         """Enqueue the D2H read of the step that was just launched and return a handle; `metrics_result(handle)` waits
         for that copy only.  Lets a training loop read the PREVIOUS step's numbers while the next step runs (the
         reference's Keras progress bar shows running means, learn_image_embeddings.py:238).  `ks`: also accuracy@k
-        ('acc<k>') for every k, from the rank of the true class."""
+        ('acc<k>', not of the classifier branch) for every k, from the rank of the true class."""
         if not hasattr(self, '_mring'):
-            # loss, acc[, cls_loss, cls_acc | center_loss], rank
-            n = 5 if self.has_cls_branch else 4 if self.center_node is not None else 3
-            self._mring = [torch.empty(n, self.B, dtype=torch.float32).pin_memory() for _ in range(4)]
+            self._mnames = [m for m in self.metric_bufs if m != 'cls_rank']     # one row each
+            self._mring = [torch.empty(len(self._mnames), self.B, dtype=torch.float32).pin_memory() for _ in range(4)]
             self._mev = [torch.cuda.Event() for _ in range(4)]
             self._mks = [()] * 4
             self._mpos = 0
         k = self._mpos
         self._mpos = (k + 1) % 4
-        host = self._mring[k]
-        host[0].copy_(self.loss_buf, non_blocking=True)
-        host[1].copy_(self.acc_buf, non_blocking=True)
-        if self.has_cls_branch:
-            host[2].copy_(self.cls_loss_buf, non_blocking=True)
-            host[3].copy_(self.cls_acc_buf, non_blocking=True)
-        if self.center_node is not None:
-            host[2].copy_(self.center_buf, non_blocking=True)
-        if ks:
-            host[-1].copy_(self.rank_buf, non_blocking=True)
+        for m, row in zip(self._mnames, self._mring[k]):
+            if ks or m != 'rank':
+                row.copy_(self.metric_bufs[m], non_blocking=True)
         self._mks[k] = tuple(ks)
         self._mev[k].record()
         return k
 
     def metrics_result(self, handle):
         self._mev[handle].synchronize()
-        host = self._mring[handle]
-        out = {'loss': float(host[0].mean()), 'acc': float(host[1].mean())}
-        if self.center_node is not None:
-            out.update(self._center_terms(out['loss'], float(host[2].mean())))
-        if self.has_cls_branch:
-            out['cls_loss'] = float(host[2].mean())
-            out['cls_acc'] = float(host[3].mean())
-        for kk in self._mks[handle]:
-            out['acc%d' % kk] = float((host[-1] < kk).float().mean())
-        return out
+        ks = self._mks[handle]
+        return self._metrics_of({m: row for m, row in zip(self._mnames, self._mring[handle]) if ks or m != 'rank'}, ks)
 
-    def _center_terms(self, prob_loss, center_loss):
-        """objective='center_loss': Keras' output losses and their weighted sum (without the L2 terms)."""
-        return {'loss': prob_loss + self.center_loss_weight * center_loss, 'prob_loss': prob_loss,
-                'center_loss': center_loss}
+    def _metrics_of(self, rows, ks=(), per_sample=False):
+        """The metrics dict of host rows (metric name -> per-sample numpy array or torch tensor): each row's mean, or
+        with per_sample=True the rows themselves; from each rank row ('rank', 'cls_rank') the accuracy@k for every k in
+        ks ('acc<k>', 'cls_acc<k>').  With a center loss row, 'loss' is Keras' weighted sum of the output losses (without
+        the L2 terms), 'prob_loss' the cross-entropy and 'center_loss' the unweighted center loss (per sample in
+        float64)."""
+        reduce = (lambda a: a) if per_sample else (lambda a: float(a.mean()))
+        out = {}
+        for m, row in rows.items():
+            if m.endswith('rank'):
+                for k in ks:
+                    out[m[:-4] + 'acc%d' % k] = reduce((np.asarray(row) < k).astype(np.float32))
+            else:
+                out[m] = reduce(row)
+        if 'center_loss' in rows:
+            prob, center = out['loss'], out['center_loss']
+            if per_sample:
+                prob, center = prob.astype(np.float64), center.astype(np.float64)
+            out.update(loss=prob + self.center_loss_weight * center, prob_loss=prob, center_loss=center)
+        return out
 
     def grad_norm_and_reg(self):
         o = self.sgd_out.cpu().numpy()
         return float(np.sqrt(o[0])), float(o[1])
 
     def predict(self, x):
-        """Inference forward (BatchNorm moving statistics), returns the wrapped embeddings (B,D) -- or, for
-        objective='softmax' and 'center_loss', the class probabilities (B,C), for objective='labelembed' the logits of
-        'prob' (B,C) -- as numpy."""
+        """Inference forward (BatchNorm moving statistics), returns the wrapped embeddings (B,D) of the embedding head, or
+        else the class scores (B,C) (class_scores), as numpy."""
         x = torch.as_tensor(x)
         self.x.copy_(x, non_blocking=True)
         self._run('infer')
         torch.cuda.synchronize(self.dev)
-        if self.le_node is not None:
-            out = self.le_node.inputs[0]
-        else:
-            out = self.head_node.output if self.head_node is not None else self.xent_node.output
+        out = self.head_node.output if self.head_node is not None else self.class_scores
         return self.act[out.name].detach().cpu().numpy().copy()
-
-    def activation(self, name_prefix):
-        """Debug/test helper: host copy of the activation whose tensor name starts with `name_prefix:`."""
-        for k, v in self.act.items():
-            if k == name_prefix or k.startswith(name_prefix + ':'):
-                torch.cuda.synchronize(self.dev)
-                return v.detach().cpu().numpy().copy()
-        raise KeyError(name_prefix)

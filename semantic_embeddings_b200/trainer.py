@@ -128,25 +128,22 @@ def run_validation(eng, data, ks, embed_dst):
     B = eng.B
     sums, count = {}, 0
     cls_pred = []
-    le = getattr(eng, 'le_node', None)
+    scores = eng.class_scores
+    if scores is None and embed_dst is not None:
+        scores = eng.head_node.output
     for idx, y in data.test_batches(B):
         n = len(idx)
         if n < B:                                   # fixed-size launch plans: pad the last batch, count only its head
             idx = np.concatenate([idx, np.repeat(idx[-1:], B - n)])
-            # the label embedding loss normalises over the batch: its padding rows carry label -1 and take no part
-            y = np.concatenate([y, np.full(B - n, -1) if le is not None else np.repeat(y[-1:], B - n)])
+            y = np.concatenate([y, np.repeat(y[-1:], B - n) if eng.pad_label is None else np.full(B - n, eng.pad_label)])
         data.compose_batch(idx, False, eng.x)
         eng.labels.copy_(torch.from_numpy(np.asarray(y, dtype=np.int32)), non_blocking=True)
         eng._run('eval')
         m = eng.per_sample_metrics(ks)
         for k, v in m.items():
             sums[k] = sums.get(k, 0.0) + float(v[:n].sum())
-        if le is not None:
-            cls_pred.append(eng.act[le.inputs[0].name][:n].argmax(dim=-1).cpu().numpy())
-        elif eng.xent_node is not None:
-            cls_pred.append(eng.act['prob_out'][:n].argmax(dim=-1).cpu().numpy())
-        elif embed_dst is not None:
-            cls_pred.append(eng.act['head_out'][:n].argmax(dim=-1).cpu().numpy())
+        if scores is not None:
+            cls_pred.append(eng.act[scores.name][:n].argmax(dim=-1).cpu().numpy())
         count += n
     out = {k: v / max(count, 1) for k, v in sums.items()}
     if eng.has_cls_branch:                          # Keras' total loss: weighted sum of the output losses (+ regulariser)
