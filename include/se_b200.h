@@ -404,6 +404,89 @@ int se_resample_crop_batch(const unsigned char* src, const se_resample_desc* des
                            int B, int crop_h, int crop_w, const float* mean, const float* std, int bgr, uint64_t seed,
                            float* out, void* stream);
 
+/* JPEG decoding for the file datasets, bit-identical to what Pillow (libjpeg-turbo, default settings: integer IDCT,
+ * fancy upsampling) returns after convert('RGB'); see jpeg_parse.cu and jpeg_decode.cu.
+ *
+ * se_jpeg_parse (host, no device needed) walks the markers of one file of n bytes -- never reading past n -- and fills
+ * *out.  It returns out->status: SE_JPEG_OK when the device can decode the file, else the reason it cannot (the file
+ * then takes the host decoder).  Supported: 8-bit baseline / extended sequential Huffman (SOF0 / SOF1) in one scan, 1
+ * component, or 3 components that libjpeg reads as YCbCr (its jdapimin.c rule: JFIF marker, else the Adobe transform
+ * flag, else the component ids) with luma sampling h, v in {1, 2} and chroma 1x1, sides <= SE_RESAMPLE_MAX_SIDE, and a
+ * well-formed restart marker sequence.  SE_ERR_ARG for null pointers or n < 0.
+ * se_jpeg_pack (host) writes the scan of a supported file into `out` (cap >= out->packed_bytes) without byte stuffing
+ * and restart markers:  uint32 int_start[n_intervals + 1] (byte offset of each restart interval in the data, then its
+ * size), uint32 sub_first[n_intervals + 1] (first subsequence of each interval), zero padding to 16 bytes, the data,
+ * 16 zero bytes.  An interval of L bytes is cut into max(1, ceil(L / SE_JPEG_SUBSEQ_BYTES)) subsequences.  Returns the
+ * bytes written, or < 0.
+ * se_jpeg_workspace_bytes (host) sets job[i].ws_offset for a batch of B supported images and returns the device
+ * workspace the batch needs (< 0 on bad arguments).
+ * se_jpeg_decode_batch decodes the batch into `out`: image i, described by info_host[i] (host) and the same bytes at
+ * in + job[i].info_offset (device), with its se_jpeg_pack output at in + job[i].packed_offset, becomes H x W x 3 uint8
+ * RGB at out + job[i].out_offset.  job_host / job_dev: the same jobs in host and device memory.  status[i] (device) is
+ * set to SE_JPEG_OK, or to SE_JPEG_DEV_CORRUPT when the entropy-coded data ends, or holds a code no table matches,
+ * before the image's last block, or a dequantised coefficient falls outside int16 (where libjpeg-turbo's SIMD and C
+ * paths differ); the pixels of such an image are undefined.  Quantisation values above 32767 are SE_JPEG_MALFORMED.
+ * Three plain launches (not programmatic dependent ones) and a memset of the workspace; no
+ * atomics on data: reruns give the same bits. */
+#define SE_JPEG_OK 0
+#define SE_JPEG_NOT_JPEG 1        /* no SOI marker */
+#define SE_JPEG_TRUNCATED 2       /* the file ends inside a segment or the scan, or before EOI */
+#define SE_JPEG_MALFORMED 3       /* a segment or table libjpeg would reject or warn about */
+#define SE_JPEG_PROGRESSIVE 4     /* SOF2 / SOF6 */
+#define SE_JPEG_ARITHMETIC 5      /* SOF9 - SOF15 arithmetic coding, DAC */
+#define SE_JPEG_OTHER_PROCESS 6   /* lossless or hierarchical (SOF3, SOF5 - SOF7) */
+#define SE_JPEG_PRECISION 7       /* not 8-bit samples */
+#define SE_JPEG_COMPONENTS 8      /* neither 1 nor 3 components (CMYK, YCCK, ...) */
+#define SE_JPEG_COLORSPACE 9      /* 3 components libjpeg does not read as YCbCr (RGB) */
+#define SE_JPEG_SAMPLING 10       /* sampling other than 4:4:4, 4:2:2, 4:2:0, 4:4:0 */
+#define SE_JPEG_MULTISCAN 11      /* more than one scan, or a scan without every component */
+#define SE_JPEG_SIZE 12           /* a side of 0 (DNL) or above SE_RESAMPLE_MAX_SIDE */
+#define SE_JPEG_RESTART 13        /* restart markers out of sequence, or not the interval count */
+#define SE_JPEG_NUM_REASONS 14
+#define SE_JPEG_DEV_CORRUPT 1     /* device status word */
+#define SE_JPEG_SUBSEQ_BYTES 128
+typedef struct {
+  uint16_t lookup[512];   /* next 9 bits of the stream -> (code length << 8) | symbol; 0: the code is longer */
+  int32_t maxcode[18];    /* largest code of length l (index l = 1..16), -1 when there is none */
+  int32_t valoffset[18];  /* huffval index of a code of length l = code + valoffset[l] */
+  uint8_t huffval[256];
+} se_jpeg_huff;
+typedef struct {
+  int32_t status;                         /* SE_JPEG_OK or the reason the device does not decode the file */
+  int32_t width, height;
+  int32_t ncomp;                          /* 1 or 3 */
+  int32_t comp_id[3], h[3], v[3], tq[3];  /* per component: id, sampling factors, quantisation table */
+  int32_t td[3], ta[3];                   /* per component: DC / AC Huffman table of the scan */
+  int32_t hmax, vmax;
+  int32_t mcus_x, mcus_y;                 /* MCUs per row / column (blocks, for a 1-component scan) */
+  int32_t restart_interval;               /* MCUs per restart interval, 0: none */
+  int32_t n_intervals, n_subseq;
+  int32_t saw_jfif, saw_adobe, adobe_transform;
+  int32_t qt_mask;                        /* bit t: quantisation table t was defined */
+  int32_t reserved;
+  int64_t scan_begin, scan_end;           /* the entropy-coded segment, RST markers included: bytes [begin, end) */
+  int64_t data_bytes;                     /* its size without byte stuffing and markers */
+  int64_t packed_bytes;                   /* size of the se_jpeg_pack output */
+  uint16_t qt[4][64];                     /* quantisation tables in natural (row-major) order */
+  se_jpeg_huff dc[4], ac[4];
+} se_jpeg_info;
+typedef struct {
+  int64_t info_offset;    /* se_jpeg_info of the image in `in` (8-byte aligned) */
+  int64_t packed_offset;  /* its se_jpeg_pack output in `in` (16-byte aligned) */
+  int64_t out_offset;     /* its RGB output in `out` */
+  int64_t ws_offset;      /* its part of the workspace (set by se_jpeg_workspace_bytes) */
+} se_jpeg_job;
+int se_jpeg_parse(const uint8_t* data, int64_t n, se_jpeg_info* out);
+int64_t se_jpeg_pack(const uint8_t* data, int64_t n, const se_jpeg_info* info, uint8_t* out, int64_t cap);
+int64_t se_jpeg_workspace_bytes(const se_jpeg_info* info, se_jpeg_job* job, int B);
+int se_jpeg_decode_batch(const unsigned char* in, const se_jpeg_info* info_host, const se_jpeg_job* job_host,
+                         const se_jpeg_job* job_dev, int B, unsigned char* out, int32_t* status, void* workspace,
+                         int64_t workspace_bytes, void* stream);
+/* sizeof(se_jpeg_info), sizeof(se_jpeg_huff), sizeof(se_jpeg_job), then the offset of every field of se_jpeg_info,
+ * se_jpeg_huff and se_jpeg_job in declaration order (for bindings to check their mirrors); returns the count written
+ * (at most cap), or the count needed when out is NULL. */
+int se_jpeg_layout(int64_t* out, int cap);
+
 /* ------------------------------------------------------------------ retrieval
  * evaluate_retrieval.py:56-63: rows [row0,row0+rows) of the N x N distance matrix of F [N,ldF]
  * (fp32, D columns) against all N columns; out [rows, ldout].  normalize=1 applies line 58

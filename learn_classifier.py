@@ -68,6 +68,8 @@ def build_parser():
                    help='Number of initial epochs for training just the new layers before fine-tuning.')
     g.add_argument('--gpus', type=int, default=1, help='Number of GPUs to be used.')
     g.add_argument('--read_workers', type=int, default=8, help='Number of parallel data pre-processing processes.')
+    g.add_argument('--decoder', choices=('pil', 'gpu'), default='pil',
+                   help='JPEG decoding of the file datasets: PIL on the read threads, or the GPU (bit-identical).')
     g.add_argument('--queue_size', type=int, default=100, help='Maximum size of data queue.')
     g.add_argument('--gpu_merge', action='store_true', default=False, help='Merge weights on the GPU.')
     g = parser.add_argument_group('Output parameters')
@@ -101,7 +103,7 @@ def main(argv=None):
     # Load dataset (learn_classifier.py:71-80)
     class_list = read_class_list(args.class_list) if args.class_list is not None else None
     data = get_data_generator(args.dataset, args.data_root, classes=class_list, device='cuda:%d' % local,
-                              read_workers=args.read_workers)
+                              read_workers=args.read_workers, decoder=args.decoder)
 
     graph = utils.build_network(data.num_classes, args.architecture, classification=True, input_channels=data.num_channels,
                                 input_size=getattr(data, 'input_size', None))

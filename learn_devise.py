@@ -71,6 +71,8 @@ def build_parser():
     g.add_argument('--max_decay', type=float, default=0.0, help='Learning Rate decay at the end of training.')
     g.add_argument('--margin', type=float, default=0.1, help='Margin of the hinge ranking loss.')
     g.add_argument('--read_workers', type=int, default=8, help='Number of parallel data pre-processing processes.')
+    g.add_argument('--decoder', choices=('pil', 'gpu'), default='pil',
+                   help='JPEG decoding of the file datasets: PIL on the read threads, or the GPU (bit-identical).')
     g.add_argument('--queue_size', type=int, default=100, help='Maximum size of data queue.')
     g = parser.add_argument_group('Output parameters')
     g.add_argument('--model_dump', type=str, default=None,
@@ -129,7 +131,7 @@ def main(argv=None):
     # Load and L2-normalize class embeddings (learn_devise.py:57-62), load dataset (:65)
     embed_labels, embedding = load_class_embedding(args.embedding)
     data = get_data_generator(args.dataset, args.data_root, classes=embed_labels, device='cuda:0',
-                              read_workers=args.read_workers)
+                              read_workers=args.read_workers, decoder=args.decoder)
     D = embedding.shape[1]
 
     # Construct model (learn_devise.py:67-74)

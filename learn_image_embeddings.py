@@ -63,6 +63,8 @@ def build_parser():
     g.add_argument('--finetune_init', type=int, default=8)
     g.add_argument('--gpus', type=int, default=1)
     g.add_argument('--read_workers', type=int, default=8)
+    g.add_argument('--decoder', choices=('pil', 'gpu'), default='pil',
+                   help='JPEG decoding of the file datasets: PIL on the read threads, or the GPU (bit-identical).')
     g.add_argument('--queue_size', type=int, default=100)
     g.add_argument('--gpu_merge', action='store_true', default=False)
     g = parser.add_argument_group('Output parameters')
@@ -100,7 +102,7 @@ def main(argv=None):
     local, rank, world, say = trainer.init_distributed(args)
 
     data = get_data_generator(args.dataset, args.data_root, classes=embed_labels, device='cuda:%d' % local,
-                              read_workers=args.read_workers)
+                              read_workers=args.read_workers, decoder=args.decoder)
     if embedding is None:
         embedding = np.eye(data.num_classes)
 

@@ -60,6 +60,33 @@ class ResampleDesc(ctypes.Structure):
                                                                      'ew', 'cy', 'cx', 'noise_id')]
 
 
+class JpegHuff(ctypes.Structure):
+    """se_jpeg_huff: one Huffman table in lookup form."""
+    _fields_ = [('lookup', ctypes.c_uint16 * 512), ('maxcode', c_int32 * 18), ('valoffset', c_int32 * 18),
+                ('huffval', ctypes.c_uint8 * 256)]
+
+
+class JpegInfo(ctypes.Structure):
+    """se_jpeg_info: what se_jpeg_parse reads from a JPEG file's headers."""
+    _fields_ = ([(n, c_int32) for n in ('status', 'width', 'height', 'ncomp')] +
+                [(n, c_int32 * 3) for n in ('comp_id', 'h', 'v', 'tq', 'td', 'ta')] +
+                [(n, c_int32) for n in ('hmax', 'vmax', 'mcus_x', 'mcus_y', 'restart_interval', 'n_intervals', 'n_subseq',
+                                        'saw_jfif', 'saw_adobe', 'adobe_transform', 'qt_mask', 'reserved')] +
+                [(n, c_int64) for n in ('scan_begin', 'scan_end', 'data_bytes', 'packed_bytes')] +
+                [('qt', (ctypes.c_uint16 * 64) * 4), ('dc', JpegHuff * 4), ('ac', JpegHuff * 4)])
+
+
+class JpegJob(ctypes.Structure):
+    """se_jpeg_job: one image of se_jpeg_decode_batch."""
+    _fields_ = [(n, c_int64) for n in ('info_offset', 'packed_offset', 'out_offset', 'ws_offset')]
+
+
+# se_jpeg_info.status (include/se_b200.h): why a file is not decoded on the device
+JPEG_REASONS = ('ok', 'not_jpeg', 'truncated', 'malformed', 'progressive', 'arithmetic', 'other_process', 'precision',
+                'components', 'colorspace', 'sampling', 'multiscan', 'size', 'restart')
+SE_JPEG_OK, SE_JPEG_DEV_CORRUPT, SE_JPEG_SUBSEQ_BYTES = 0, 1, 128
+
+
 class Op(ctypes.Structure):
     _fields_ = [('opcode', c_int32), ('i', c_int32 * 15), ('f', c_float * 8), ('p', c_void_p * 16)]
 
@@ -131,6 +158,11 @@ _SIGS = {
     'se_augment_batch': (c_int, [_P, c_int, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'se_resample_crop_batch': (c_int, [_P, _P, _P, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_int,
                                        ctypes.c_uint64, _P, _P]),
+    'se_jpeg_parse': (c_int, [_P, c_int64, POINTER(JpegInfo)]),
+    'se_jpeg_pack': (c_int64, [_P, c_int64, POINTER(JpegInfo), _P, c_int64]),
+    'se_jpeg_workspace_bytes': (c_int64, [_P, _P, c_int]),
+    'se_jpeg_decode_batch': (c_int, [_P, _P, _P, _P, c_int, _P, _P, _P, c_int64, _P]),
+    'se_jpeg_layout': (c_int, [POINTER(c_int64), c_int]),
     'se_sgd_step': (c_int, [_P, _P, _P, c_int64, POINTER(L2Segment), c_int, c_float, c_float, c_int, c_float, _P, _P]),
     'se_sgd_prepare': (c_int, [_P, _P, c_int64, POINTER(L2Segment), c_int, _P, _P]),
     'se_sgd_apply': (c_int, [_P, _P, _P, c_int64, c_float, c_float, c_int, c_float, _P, _P]),

@@ -10,10 +10,15 @@ in the product; tests compare the kernel with oracle/augment.py.
 
 The NABirds / CUB file datasets (FileDatasetGenerator) decode JPEG / PNG files on host threads and hand each batch to
 one CUDA launch (se_resample_crop_batch, csrc/file_augment.cu) that resizes exactly like PIL, standardises, flips,
-erases and crops.
+erases and crops.  With decoder='gpu' the host threads only read the files and parse the JPEG headers
+(se_jpeg_parse); the device decodes the batch's JPEGs bit-identically to load_img (se_jpeg_decode_batch,
+csrc/jpeg_decode.cu), and the files it does not support go through load_img as before.
 """
+import collections
+import ctypes
 import os
 import pickle
+import threading
 
 import numpy as np
 
@@ -163,6 +168,52 @@ def load_img(path):
         return np.asarray(img, dtype=np.uint8)
 
 
+class DeviceJpeg:
+    """A JPEG file the device decodes: its parsed header (_lib.JpegInfo), its scan packed by se_jpeg_pack (uint8
+    array) and its path (for the host decode when the device reports corrupt data).  `shape` is the (H, W, 3) of the
+    image load_img returns."""
+    __slots__ = ('info', 'packed', 'path', 'shape')
+
+    def __init__(self, info, packed, path):
+        self.info, self.packed, self.path = info, packed, path
+        self.shape = (info.height, info.width, 3)
+
+
+def parse_jpeg(data):
+    """se_jpeg_parse on the bytes of a file: the _lib.JpegInfo (status 0 when the device decodes the file, else the
+    index of the reason in _lib.JPEG_REASONS)."""
+    info = _lib.JpegInfo()
+    _lib.load().se_jpeg_parse(data, len(data), ctypes.byref(info))
+    return info
+
+
+def read_for_device(path):
+    """Reads a file for the device decoder: a DeviceJpeg when se_jpeg_parse supports it, else (load_img's array, the
+    reason's name)."""
+    with open(path, 'rb') as f:
+        data = f.read()
+    info = parse_jpeg(data)
+    if info.status == _lib.SE_JPEG_OK:
+        packed = np.empty(info.packed_bytes, np.uint8)
+        if _lib.load().se_jpeg_pack(data, len(data), ctypes.byref(info), packed.ctypes.data, packed.size) == packed.size:
+            return DeviceJpeg(info, packed, path), None
+    return load_img(path), _lib.JPEG_REASONS[info.status] if info.status else 'pack'
+
+
+class _DecoderState:
+    """decoder='gpu': the side stream the decodes run on and their workspace."""
+    __slots__ = ('stream', 'workspace')
+
+    def __init__(self, stream, workspace):
+        self.stream, self.workspace = stream, workspace
+
+
+# A batch sent to the device decoder: its key, images, staging slot (pinned host, device, event), bytes of descriptors
+# before the source area, source offset of every image, (image, byte offset in the slot) of the device's outputs, the
+# status words on the device and their pinned host copy, and the event that ends its decode.
+_DecodedBatch = collections.namedtuple('_DecodedBatch', 'key imgs slot dbytes src device_out status_dev status_host done')
+
+
 def resized_size(h, w, target):
     """datasets/common.py:468-469: the shorter side becomes `target`, the longer one round(other * target / shorter)
     (Python 3 round, half to even); a square image takes the second branch.  Returns (rh, rw)."""
@@ -205,8 +256,11 @@ class FileDatasetGenerator:
 
     def __init__(self, train_files, train_labels, test_files, test_labels, classes, cropsize=224, default_target_size=256,
                  randzoom_range=None, mean=NAB_MEAN, std=NAB_STD, color_mode='rgb', randerase_prob=0.5,
-                 randerase_params=RANDERASE_PARAMS, read_workers=8, prefetch=2, device='cuda'):
+                 randerase_params=RANDERASE_PARAMS, read_workers=8, prefetch=2, device='cuda', decoder='pil'):
         import torch
+        if decoder not in ('pil', 'gpu'):
+            raise ValueError('Unknown decoder: {} (pil or gpu)'.format(decoder))
+        self.decoder = decoder
         self.dev = torch.device(device)
         self.train_img_files, self.test_img_files = list(train_files), list(test_files)
         self.y_train, self.y_test = np.asarray(train_labels, dtype=np.int64), np.asarray(test_labels, dtype=np.int64)
@@ -227,6 +281,11 @@ class FileDatasetGenerator:
         self._sizes = {}                                                # (train, index) -> decoded (h, w)
         self._slots = [None, None]                                      # (pinned host, device, event) per staging slot
         self._slot = 0
+        self._fallbacks = collections.Counter()                         # decoder='gpu': files load_img decoded, by reason
+        self._fallback_lock = threading.Lock()
+        self._jpeg = None                                               # decoder='gpu': _DecoderState
+        self._ahead = None                                              # decoder='gpu': the _DecodedBatch sent ahead
+        self._upcoming = None                                           # (train, indices) of the iteration's next batch
 
     # ---- properties of the reference interface
     @property
@@ -274,13 +333,35 @@ class FileDatasetGenerator:
         if self._pool is None:
             self._pool = ThreadPoolExecutor(self.read_workers)
         files = self._files(train)
-        return [self._pool.submit(load_img, files[i]) for i in indices]
+        fn = self._read_for_device if self.decoder == 'gpu' else load_img
+        return [self._pool.submit(fn, files[i]) for i in indices]
+
+    def _read_for_device(self, path):
+        item, reason = read_for_device(path)
+        if reason is not None:
+            self._count_fallback(reason)
+        return item
+
+    def _count_fallback(self, reason):
+        with self._fallback_lock:
+            self._fallbacks[reason] += 1
+
+    def take_fallback_counts(self):
+        """decoder='gpu': {reason: count} of the files load_img decoded instead of the device since the last call --
+        the se_jpeg_parse reasons of _lib.JPEG_REASONS, 'device' for data the device found corrupt.  Empty with
+        decoder='pil'."""
+        with self._fallback_lock:
+            out = dict(self._fallbacks)
+            self._fallbacks.clear()
+        return out
 
     def _key(self, train, indices):
         return (bool(train), np.asarray(indices, dtype=np.int64).tobytes())
 
     def _prefetch(self, train, indices):
         key = self._key(train, indices)
+        if self._ahead is not None and self._ahead.key == key:
+            return                                                      # read, and on the device already
         if key not in self._pending:
             self._pending[key] = self._submit(train, indices)
 
@@ -317,6 +398,11 @@ class FileDatasetGenerator:
         from concurrent.futures import ThreadPoolExecutor
 
         def header(path):
+            if self.decoder == 'gpu':                                   # the SOF of a file the device decodes
+                with open(path, 'rb') as f:
+                    info = parse_jpeg(f.read())
+                if info.status == _lib.SE_JPEG_OK:
+                    return info.height, info.width
             with PIL.Image.open(path) as im:
                 return im.size[1], im.size[0]
         files = self._files(train)
@@ -413,46 +499,215 @@ class FileDatasetGenerator:
             self._slots[k] = slot
         return slot
 
-    def compose_batch(self, indices, train, out, augment=False, rng=None, params=None, images=None):
-        """datasets/common.py:380-432 for the images `indices` of the training or test set: writes the (B, crop, crop, 3)
-        float32 batch into `out` (a CUDA tensor).  params: a dict of draw_params instead of fresh draws (tests);
-        images: the decoded images instead of reading the files (tests)."""
-        import ctypes
-        import torch
-        imgs = images if images is not None else self.decode(indices, train)
+    def _resample_descs(self, imgs, params, src_offsets):
+        """The se_resample_desc array of a batch: image i at src_offsets[i] of the source area, its draws in `params`."""
         n = len(imgs)
-        if params is None:
-            params = self.batch_params(indices, train, augment, rng, imgs)
         noise_id = params.get('noise_id', np.arange(n))
-        ch = self.cropsize
         descs = (_lib.ResampleDesc * n)()
-        dbytes = (ctypes.sizeof(descs) + 255) // 256 * 256
-        off = dbytes
         for i, im in enumerate(imgs):
             d = descs[i]
-            d.src_offset, d.src_h, d.src_w = off - dbytes, im.shape[0], im.shape[1]
+            d.src_offset, d.src_h, d.src_w = src_offsets[i], im.shape[0], im.shape[1]
             d.rh, d.rw = (int(v) for v in params['size'][i])
             d.flip = int(params['flip'][i])
             d.ey, d.ex, d.eh, d.ew = (int(v) for v in params['erase'][i])
             d.cy, d.cx = (int(v) for v in params['crop'][i])
             d.noise_id = int(noise_id[i])
-            off += im.size
+        return descs
+
+    def _resample(self, dev, dbytes, descs, params, out):
+        """se_resample_crop_batch on the current stream: descriptors at dev[0:], sources at dev[dbytes:]."""
+        mean = (ctypes.c_float * 3)(*self.mean.tolist())
+        std = (ctypes.c_float * 3)(*self.std.tolist())
+        _lib.call('se_resample_crop_batch', dev.data_ptr() + dbytes, ctypes.addressof(descs), dev.data_ptr(), len(descs),
+                  self.cropsize, self.cropsize, mean, std, 1 if self.color_mode == 'bgr' else 0,
+                  ctypes.c_uint64(params['seed'] & (2 ** 64 - 1)), out.data_ptr(), _lib.stream_ptr())
+
+    def compose_batch(self, indices, train, out, augment=False, rng=None, params=None, images=None):
+        """datasets/common.py:380-432 for the images `indices` of the training or test set: writes the (B, crop, crop, 3)
+        float32 batch into `out` (a CUDA tensor).  params: a dict of draw_params instead of fresh draws (tests);
+        images: the decoded images instead of reading the files (tests).  With decoder='gpu' the batch's JPEGs were
+        usually decoded on the device while the previous batch trained (_decode_ahead); the next batch's decode is
+        started before returning."""
+        import torch
+        batch = None
+        if self.decoder == 'gpu' and images is None:
+            batch = self._take_ahead(train, indices)
+        if batch is None:
+            imgs = images if images is not None else self.decode(indices, train)
+            if any(isinstance(im, DeviceJpeg) for im in imgs):
+                batch = self._send_and_decode(self._key(train, indices), imgs)
+        if batch is not None:
+            self._compose_decoded(batch, indices, train, out, augment, rng, params)
+            if images is None:
+                self._decode_ahead()
+            return out
+        n = len(imgs)
+        if params is None:
+            params = self.batch_params(indices, train, augment, rng, imgs)
+        dbytes = (ctypes.sizeof(_lib.ResampleDesc) * n + 255) // 256 * 256
+        offs = np.concatenate([[0], np.cumsum([im.size for im in imgs])]).tolist()
+        descs = self._resample_descs(imgs, params, offs)
+        off = dbytes + offs[-1]
         host, dev, ev = self._staging(off)
         buf = host.numpy()
         buf[:ctypes.sizeof(descs)] = np.frombuffer(descs, dtype=np.uint8)
-        pos = dbytes
-        for im in imgs:
-            buf[pos:pos + im.size] = im.reshape(-1)
-            pos += im.size
-        mean = (ctypes.c_float * 3)(*self.mean.tolist())
-        std = (ctypes.c_float * 3)(*self.std.tolist())
+        for im, o in zip(imgs, offs):
+            buf[dbytes + o:dbytes + o + im.size] = im.reshape(-1)
         with torch.cuda.device(self.dev):
             dev[:off].copy_(host[:off], non_blocking=True)                # one host-to-device copy per batch
-            _lib.call('se_resample_crop_batch', dev.data_ptr() + dbytes, ctypes.addressof(descs), dev.data_ptr(), n, ch, ch,
-                      mean, std, 1 if self.color_mode == 'bgr' else 0, ctypes.c_uint64(params['seed'] & (2 ** 64 - 1)),
-                      out.data_ptr(), _lib.stream_ptr())
+            self._resample(dev, dbytes, descs, params, out)
             ev.record()
+        if self.decoder == 'gpu' and images is None:
+            self._decode_ahead()
         return out
+
+    # ---- device JPEG decoding (decoder='gpu')
+    def _decoder_state(self, ws_bytes):
+        """The side stream of the device decoder and its workspace (grown as needed)."""
+        import torch
+        st = self._jpeg
+        if st is None:
+            with torch.cuda.device(self.dev):
+                st = self._jpeg = _DecoderState(torch.cuda.Stream(self.dev), None)
+        if st.workspace is None or st.workspace.numel() < ws_bytes:
+            st.workspace = None
+            with torch.cuda.device(self.dev), torch.cuda.stream(st.stream):   # allocated for the stream that uses it
+                st.workspace = torch.empty(ws_bytes + ws_bytes // 4, dtype=torch.uint8, device=self.dev)
+        return st
+
+    def _send_and_decode(self, key, imgs):
+        """Stages the batch `imgs` (DeviceJpeg or decoded arrays) in the next staging slot -- [resample descriptors
+        (written by _compose_decoded) | decoded arrays | jobs | headers | packed scans], then the device's RGB output --
+        copies everything but the descriptors to the device in one copy and starts se_jpeg_decode_batch and the copy of
+        its status words to the host, all on the side stream, which does not wait for the training on the main
+        stream (the slot's previous readers have completed, _staging).  An image repeated in the batch (a padded last
+        batch) is sent and decoded once.  Returns the _DecodedBatch."""
+        import torch
+        L = _lib
+        n = len(imgs)
+        dbytes = (ctypes.sizeof(L.ResampleDesc) * n + 255) // 256 * 256
+        first = {}                                                      # id(image) -> its first position
+        uniq = [i for i, im in enumerate(imgs) if first.setdefault(id(im), i) == i]
+        src = [0] * n
+        pos = dbytes
+        for i in uniq:
+            if not isinstance(imgs[i], DeviceJpeg):
+                src[i] = pos - dbytes
+                pos += imgs[i].size
+        dev_idx = [i for i in uniq if isinstance(imgs[i], DeviceJpeg)]
+        nd = len(dev_idx)
+        isz = ctypes.sizeof(L.JpegInfo)
+        jobs, infos = (L.JpegJob * nd)(), (L.JpegInfo * nd)()
+        job_off = (pos + 255) // 256 * 256
+        info_off = job_off + (ctypes.sizeof(jobs) + 255) // 256 * 256
+        pos = info_off + nd * isz
+        for k, i in enumerate(dev_idx):
+            infos[k] = imgs[i].info
+            pos = (pos + 15) // 16 * 16
+            jobs[k].info_offset = info_off + k * isz
+            jobs[k].packed_offset = pos
+            pos += imgs[i].packed.size
+        copy_end = (pos + 255) // 256 * 256
+        rgb = copy_end
+        for k, i in enumerate(dev_idx):
+            h, w, _ = imgs[i].shape
+            jobs[k].out_offset = rgb
+            src[i] = rgb - dbytes
+            rgb += h * w * 3
+        for i in range(n):
+            src[i] = src[first[id(imgs[i])]]
+        ws_bytes = int(L.load().se_jpeg_workspace_bytes(infos, jobs, nd))
+        L.check(0 if ws_bytes >= 0 else ws_bytes, 'se_jpeg_workspace_bytes')
+        host, dev, ev = self._staging(rgb)
+        buf = host.numpy()
+        for i in uniq:
+            if not isinstance(imgs[i], DeviceJpeg):
+                o = dbytes + src[i]
+                buf[o:o + imgs[i].size] = imgs[i].reshape(-1)
+        buf[job_off:job_off + ctypes.sizeof(jobs)] = np.frombuffer(jobs, dtype=np.uint8)
+        buf[info_off:info_off + ctypes.sizeof(infos)] = np.frombuffer(infos, dtype=np.uint8)
+        for k, i in enumerate(dev_idx):
+            o = jobs[k].packed_offset
+            buf[o:o + imgs[i].packed.size] = imgs[i].packed
+        st = self._decoder_state(ws_bytes)
+        with torch.cuda.device(self.dev), torch.cuda.stream(st.stream):
+            # the status words belong to the side stream's allocations: a batch dropped by _take_ahead frees them
+            # while its decode may still run
+            batch = _DecodedBatch(key, imgs, (host, dev, ev), dbytes, src,
+                                  [(i, jobs[k].out_offset) for k, i in enumerate(dev_idx)],
+                                  torch.empty(max(nd, 1), dtype=torch.int32, device=self.dev),
+                                  torch.empty(max(nd, 1), dtype=torch.int32).pin_memory(), torch.cuda.Event())
+            dev[dbytes:copy_end].copy_(host[dbytes:copy_end], non_blocking=True)
+            L.call('se_jpeg_decode_batch', dev.data_ptr(), ctypes.addressof(infos), ctypes.addressof(jobs),
+                   dev.data_ptr() + job_off, nd, dev.data_ptr(), batch.status_dev.data_ptr(), st.workspace.data_ptr(),
+                   st.workspace.numel(), st.stream.cuda_stream)
+            batch.status_host[:nd].copy_(batch.status_dev[:nd], non_blocking=True)   # one small copy per batch
+            batch.done.record(st.stream)
+            ev.record(st.stream)            # the slot is busy until the decode ends, even if the batch is never composed
+        return batch
+
+    def _compose_decoded(self, batch, indices, train, out, augment, rng, params):
+        """compose_batch for a batch sent by _send_and_decode: waits for its decode (already over when it ran while
+        the previous batch trained), has load_img decode again any image whose status is not OK and copies it over the
+        device's output, then writes the descriptors and runs se_resample_crop_batch on the main stream."""
+        import torch
+        imgs = batch.imgs
+        if params is None:
+            params = self.batch_params(indices, train, augment, rng, imgs)
+        host, dev, ev = batch.slot
+        batch.done.synchronize()
+        status = batch.status_host.numpy()
+        with torch.cuda.device(self.dev):
+            for k, (i, o) in enumerate(batch.device_out):
+                if status[k] != _lib.SE_JPEG_OK:
+                    self._count_fallback('device')
+                    im = load_img(imgs[i].path)
+                    dev[o:o + im.size].copy_(torch.from_numpy(im.reshape(-1)).to(self.dev))
+            descs = self._resample_descs(imgs, params, batch.src)
+            host.numpy()[:ctypes.sizeof(descs)] = np.frombuffer(descs, dtype=np.uint8)
+            stream = torch.cuda.current_stream()
+            stream.wait_event(batch.done)
+            dev[:ctypes.sizeof(descs)].copy_(host[:ctypes.sizeof(descs)], non_blocking=True)
+            self._resample(dev, batch.dbytes, descs, params, out)
+            ev.record()
+
+    def _take_ahead(self, train, indices):
+        """The batch _decode_ahead sent for `indices` -- or for their prefix when `indices` is that batch padded with
+        repeats of its last index (run_validation, dump_features) -- else None; a batch sent for other indices is
+        dropped (its slot frees itself when its decode ends)."""
+        batch, self._ahead = self._ahead, None
+        if batch is None:
+            return None
+        indices = np.asarray(indices, dtype=np.int64)
+        if batch.key == self._key(train, indices):
+            return batch
+        m = len(indices)
+        while m > 1 and indices[m - 2] == indices[-1]:
+            m -= 1
+        if m < len(indices) and batch.key == self._key(train, indices[:m]):
+            imgs = batch.imgs + [batch.imgs[-1]] * (len(indices) - m)
+            return batch._replace(imgs=imgs, src=batch.src + [batch.src[-1]] * (len(indices) - m))
+        return None
+
+    def _decode_ahead(self):
+        """Sends the next batch of the running iteration (_iterate) to the device decoder when its files have been
+        read, so that its decode runs while the current batch trains; its status words are read when it is
+        composed."""
+        nxt, self._upcoming = self._upcoming, None
+        if nxt is None or self._ahead is not None:
+            return
+        key = self._key(*nxt)
+        futs = self._pending.get(key)
+        if futs is None or not all(f.done() for f in futs):
+            return
+        imgs = [f.result() for f in futs]
+        if not any(isinstance(im, DeviceJpeg) for im in imgs):
+            return                                                      # stays with decode(): no device work
+        del self._pending[key]
+        train, idx = nxt
+        for i, im in zip(np.asarray(idx).tolist(), imgs):
+            self._sizes[(bool(train), i)] = im.shape[:2]
+        self._ahead = self._send_and_decode(key, imgs)
 
     def train_batches(self, batch_size, rng, rank=0, world=1):
         """As TinyDatasetGenerator.train_batches (shuffled, trailing partial batch dropped); the images of the next
@@ -480,6 +735,7 @@ class FileDatasetGenerator:
             for k, idx in enumerate(batches):
                 for ahead in batches[k:k + 1 + self.prefetch]:
                     self._prefetch(train, ahead)
+                self._upcoming = (train, batches[k + 1]) if k + 1 < len(batches) else None
                 yield idx, labels[idx]
         finally:
             self._forget(train, batches)
@@ -488,7 +744,7 @@ class FileDatasetGenerator:
 FILE_DATASETS = ('nab', 'cub')
 
 
-def _file_generator(dataset, data_root, classes, device, read_workers):
+def _file_generator(dataset, data_root, classes, device, read_workers, decoder='pil'):
     """datasets/__init__.py:60-117 for NABirds / CUB: the suffixes '-ilsvrcmean' / '-caffe' (then '-large') and the
     per-dataset crop, target size, zoom range and statistics.  None for names that are not file datasets."""
     name = dataset.lower()
@@ -519,15 +775,18 @@ def _file_generator(dataset, data_root, classes, device, read_workers):
     classes, tr_files, tr_labels, te_files, te_labels = parse_nab(data_root, classes, 'images')
     print('Found {} training and {} validation images from {} classes.'.format(len(tr_files), len(te_files), len(classes)))
     return FileDatasetGenerator(tr_files, tr_labels, te_files, te_labels, classes, read_workers=read_workers, device=device,
-                                **kw)
+                                decoder=decoder, **kw)
 
 
-def get_data_generator(dataset, data_root, classes=None, device='cuda', read_workers=8):
+def get_data_generator(dataset, data_root, classes=None, device='cuda', read_workers=8, decoder='pil'):
     """datasets/__init__.py:21-166, CIFAR branch (:85-87), the NABirds / CUB branches (:101-117: 'nab', 'nab-large',
     'cub', each optionally followed by '-ilsvrcmean' or '-caffe'; FileDatasetGenerator, decoding on `read_workers`
     threads), plus 'synthetic[:n]' (uint8 images = a fixed random colour template per class blended with pixel noise,
     for machines without data).  The other file datasets of the reference (ILSVRC, iNat, Cars, Flowers, subdirectories)
-    are not supported."""
+    are not supported.  decoder: 'pil' (load_img on the read threads) or 'gpu' (the device decodes the JPEGs it
+    supports, bit-identically); it only concerns the file datasets, the others hold decoded pixels."""
+    if decoder not in ('pil', 'gpu'):
+        raise ValueError('Unknown decoder: {} (pil or gpu)'.format(decoder))
     name = dataset.lower()
     if name in ('cifar-100', 'cifar-10'):
         return TinyDatasetGenerator(*_load_cifar(data_root, name, classes), device=device)
@@ -541,7 +800,7 @@ def get_data_generator(dataset, data_root, classes=None, device='cuda', read_wor
         ytr, yte = rng.randint(0, ncls, n), rng.randint(0, ncls, max(n // 4, 1))
         make = lambda y: np.clip(0.6 * templates[y] + 0.4 * rng.randint(0, 256, (len(y), 32, 32, 3)), 0, 255).astype(np.uint8)
         return TinyDatasetGenerator(make(ytr), make(yte), ytr, yte, device=device)
-    gen = _file_generator(dataset, data_root, classes, device, read_workers)
+    gen = _file_generator(dataset, data_root, classes, device, read_workers, decoder)
     if gen is not None:
         return gen
     raise ValueError('Unknown dataset: {}'.format(dataset))

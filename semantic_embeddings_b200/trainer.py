@@ -151,6 +151,15 @@ def run_validation(eng, data, ks, embed_dst):
     return out, (np.concatenate(cls_pred) if cls_pred else None)
 
 
+def report_fallbacks(data, say):
+    """With the device JPEG decoder: one line with the files load_img decoded instead since the last line, by
+    reason (FileDatasetGenerator.take_fallback_counts).  Nothing with decoder='pil' or in-memory datasets."""
+    if getattr(data, 'decoder', 'pil') != 'gpu':
+        return
+    counts = data.take_fallback_counts()
+    say('Decoder fallbacks: ' + (', '.join('{} {}'.format(k, counts[k]) for k in sorted(counts)) or 'none'))
+
+
 def format_logs(logs):
     return ' - '.join('{}: {:.4f}'.format(k, logs[k]) for k in sorted(logs))
 
@@ -169,6 +178,7 @@ def pretrain_new_layers(eng, data, args, new_layers, rng, rank, world, ks, say, 
         val, _ = run_validation(eng, data, ks, None)
         logs.update({'val_' + k: v for k, v in val.items()})
         say('Epoch {}/{} - '.format(ep + 1, args.finetune_init) + format_logs(logs))
+        report_fallbacks(data, say)
     eng.set_trainable(None)
     eng.V.zero_()
     eng.set_iterations(0)
@@ -192,6 +202,7 @@ def fit_constant_lr(eng, data, batch_size, lr, epochs, rng, ks, say, rank=0, wor
         val, _ = run_validation(eng, data, ks, None)
         logs.update({'val_' + k: v for k, v in val.items()})
         say('Epoch {}/{} - '.format(epoch + 1, epochs) + format_logs(logs))
+        report_fallbacks(data, say)
 
 
 def fit(eng, data, args, sched, epochs, rng, rank, world, ks, say, train_ks=()):
@@ -209,6 +220,7 @@ def fit(eng, data, args, sched, epochs, rng, rank, world, ks, say, train_ks=()):
         logs['val_loss'] = val.get('total', val['loss'])
         if rank == 0:
             say('Epoch {}/{} - lr {:.6f} - '.format(epoch + 1, epochs, sched.lr) + format_logs(logs))
+            report_fallbacks(data, say)
             if args.snapshot:
                 cur = logs.get(monitor) if monitor else None
                 better = monitor is None or best is None or cur is None or \
