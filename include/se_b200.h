@@ -543,6 +543,21 @@ int64_t se_row_argsort_workspace_bytes(int rows, int n);
 int se_row_argsort(const float* dist, int64_t ld, int rows, int n, int32_t* out_idx, int64_t ldo, void* workspace,
                    void* stream);
 
+/* Recall-precision of plot_recall_precision.py:59-77 (flat relevance: same label).
+ * se_class_index: labels [N] int32 -> offsets [C+1] int32 (class c owns members[offsets[c], offsets[c+1])) and
+ * members [N] int32 (the items of each class in ascending index order).  SE_ERR_ARG for a label outside [0, C); it
+ * waits for the stream to report that.  Built once per feature set.
+ * se_relevant_positions: for query i (database index q = q0 + i) of dist [rows, ld] (the rows se_pairwise_dist
+ * writes), the 1-based positions of the n_i = offsets[c+1] - offsets[c] - 1 other members of q's class c in the ranking
+ * of row i with q removed (the order of se_row_argsort: ascending distance, ties by ascending index, -0.0 == +0.0),
+ * ascending, at out + out_offsets[i] (int64 [rows], device).  offsets / members come from se_class_index of the same
+ * labels.  SE_ERR_ARG for negative sizes, ld < n or q0 + rows > n.  No workspace; integer atomics only, reruns give the
+ * same output. */
+int se_class_index(const int32_t* labels, int N, int C, int32_t* offsets, int32_t* members, void* stream);
+int se_relevant_positions(const float* dist, int64_t ld, int rows, int n, int q0, const int32_t* labels, int C,
+                          const int32_t* offsets, const int32_t* members, const int64_t* out_offsets, int32_t* out,
+                          void* stream);
+
 /* ------------------------------------------------------------------ classification (evaluate_classification_accuracy.py)
  * One-vs-rest linear SVM of the reference's train_and_predict (:20-48, sklearn LinearSVC(C): squared hinge loss, L2
  * penalty, intercept as a constant feature 1 that is regularised like the weights).  For class c, y_i = +1 where

@@ -155,6 +155,8 @@ _SIGS = {
     'se_hier_metrics': (c_int, [_P, c_int64, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P]),
     'se_row_argsort_workspace_bytes': (c_int64, [c_int, c_int]),
     'se_row_argsort': (c_int, [_P, c_int64, c_int, c_int, _P, c_int64, _P, _P]),
+    'se_class_index': (c_int, [_P, c_int, c_int, _P, _P, _P]),
+    'se_relevant_positions': (c_int, [_P, c_int64, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P, _P]),
     'se_augment_batch': (c_int, [_P, c_int, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'se_resample_crop_batch': (c_int, [_P, _P, _P, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_int,
                                        ctypes.c_uint64, _P, _P]),

@@ -17,12 +17,6 @@ namespace se {
 constexpr int AS_THREADS = 1024;
 constexpr int AS_CHUNK = 4096;                 // words per shared-memory sub-sort (32 KB)
 
-__device__ __forceinline__ uint32_t as_key(float f) {
-  if (f == 0.f) f = 0.f;                                  // -0.0 ties with +0.0 as in numpy
-  uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
 // compare-exchange steps j = j_hi, j_hi/2, ..., 1 of merge level k on a chunk held in shared memory.
 // `base` = global index of the chunk's first word (direction of a pair depends on the global index)
 __device__ __forceinline__ void smem_steps(unsigned long long* s, int base, int k, int j_hi) {

@@ -114,6 +114,14 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// Ranking order of the retrieval kernels (se_row_argsort, se_relevant_positions): ascending distance, -0.0 == +0.0,
+// as an ascending unsigned key; (as_key(d) << 32 | index) also breaks ties by ascending index.
+__device__ __forceinline__ uint32_t as_key(float f) {
+  if (f == 0.f) f = 0.f;                                  // -0.0 ties with +0.0 as in numpy
+  uint32_t u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
 // 128-bit streaming load/store (read-once / write-once data: keep L1 for reused tiles)
 __device__ __forceinline__ float4 ldg_nc_f4(const float* p) {
   float4 r;
