@@ -75,7 +75,7 @@ __device__ __forceinline__ void put_t(uint8_t* hi, uint8_t* lo, int c4, int px, 
   }
 }
 
-template <int BN, int X3>
+template <int BN, int X3, int NP>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 conv_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dy, WgTcParams p) {
   pdl_grid_sync();
@@ -127,8 +127,11 @@ conv_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dy, 
     }
   };
 
-  // X3: each chunk's MMAs go into a fresh register tile that is then added into `acc` (see conv_tc.cu)
-  float acc[BN / 2], part[BN / 2];
+  // X3: each chunk's MMAs go into NP fresh register tiles (of 32 / NP pixels each) that are then added into `acc`.  The
+  // tensor core keeps fewer bits of a sum than an fp32 add: long reductions (NP = 4, see the host side) start a fresh
+  // tile every 8 pixels and add the small terms first
+  constexpr int KPP = (WG_PX / 8) / NP;
+  float acc[BN / 2], part[NP][BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -151,9 +154,16 @@ conv_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dy, 
     for (int ks = 0; ks < WG_PX / 8; ++ks) {
       const uint64_t da = wgmma_desc(smem_u32(sx) + ks * 32, 128), db = wgmma_desc(smem_u32(sy) + ks * 32, 128);
       if (X3) {
-        wgmma_tf32<BN>(part, da, db, ks > 0);
-        wgmma_tf32<BN>(part, da, wgmma_desc(smem_u32(syl) + ks * 32, 128), 1);
-        wgmma_tf32<BN>(part, wgmma_desc(smem_u32(sxl) + ks * 32, 128), db, 1);
+        float (&pt)[BN / 2] = part[ks / KPP];
+        if (NP > 1) {
+          wgmma_tf32<BN>(pt, da, wgmma_desc(smem_u32(syl) + ks * 32, 128), ks % KPP > 0);
+          wgmma_tf32<BN>(pt, wgmma_desc(smem_u32(sxl) + ks * 32, 128), db, 1);
+          wgmma_tf32<BN>(pt, da, db, 1);
+        } else {
+          wgmma_tf32<BN>(pt, da, db, ks > 0);
+          wgmma_tf32<BN>(pt, da, wgmma_desc(smem_u32(syl) + ks * 32, 128), 1);
+          wgmma_tf32<BN>(pt, wgmma_desc(smem_u32(sxl) + ks * 32, 128), db, 1);
+        }
       } else {
         wgmma_tf32<BN>(acc, da, db, first == 0 || ks > 0);
       }
@@ -162,7 +172,9 @@ conv_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dy, 
     wgmma_wait<0>();
     if (X3) {
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+      for (int j = 0; j < NP; ++j)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += part[j][i];
     }
     named_bar_sync(1 + wg, 128);            // every warp's MMAs have read the tiles before they are rewritten
     first = 0;
@@ -211,8 +223,9 @@ conv_wgrad_reduce_kernel(const float* __restrict__ ws, int splits, long long T, 
 // ---------------------------------------------------------------------------------------- host side
 template <int BN>
 static bool set_smem_limit() {
-  return cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess &&
-         cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess;
+  return cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, 0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess &&
+         cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, 1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess &&
+         cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, 1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess;
 }
 
 int init_conv_wgrad_tc() {
@@ -306,11 +319,20 @@ bool conv_wgrad_tc_fixed_order(const se_conv_desc* d, cudaStream_t st) {
   return wgrad_workspace(2 * (T + d->Cout), st, &ws) == SE_OK && ws != nullptr;
 }
 
+// Error-compensated sums over at least this many pixels take four partial tiles per chunk (NP = 4).  Measured on an H100
+// on ResNet-50's res2a_branch2a at 448 px (B = 32, 394 272 pixels, in front of a BatchNorm: dY sums to zero per channel,
+// X >= 0): 3.6e-5 of the largest dW with one tile and the big term first, 2.9e-5 small terms first, 5.7e-6 with four
+// tiles and small terms first (2.0e-5 big term first), against 7e-7 for the float64 sum of the split operands.  Four
+// tiles cost 2-6 % on such layers, and up to 20 % on the short reductions of the CIFAR networks, which keep the one tile
+// and the arithmetic they had.
+constexpr long long WG_LONG_PX = 1LL << 18;
+
 template <int BN>
 static void wgrad_go(int x3, dim3 grid, cudaStream_t st, const float* x, const float* dy, const WgTcParams& p) {
   const size_t smem = 1024 + 2 * (size_t)(WG_MT * 128 + BN * 128) * (x3 ? 2 : 1);
-  if (x3) launch(conv_wgrad_tc_kernel<BN, 1>, grid, dim3(WG_THREADS), smem, st, x, dy, p);
-  else launch(conv_wgrad_tc_kernel<BN, 0>, grid, dim3(WG_THREADS), smem, st, x, dy, p);
+  if (x3 && p.npx >= WG_LONG_PX) launch(conv_wgrad_tc_kernel<BN, 1, 4>, grid, dim3(WG_THREADS), smem, st, x, dy, p);
+  else if (x3) launch(conv_wgrad_tc_kernel<BN, 1, 1>, grid, dim3(WG_THREADS), smem, st, x, dy, p);
+  else launch(conv_wgrad_tc_kernel<BN, 0, 1>, grid, dim3(WG_THREADS), smem, st, x, dy, p);
 }
 
 int conv_wgrad_tc(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias, int x3, cudaStream_t st) {

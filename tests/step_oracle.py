@@ -527,17 +527,36 @@ CONFIGS = [
 ]
 
 
+# ResNet-50 at 448 x 448, the crops of the NAB-large and CUB datasets (learn_image_embeddings.py, learn_classifier.py;
+# test_gpu_step_layers_448.py).  The recipes' per-GPU batch of 64 (README: 128 on 2 GPUs) needs about 44 GB of engine
+# buffers before the float64 checks, so the batch is 32 (B = 24 for the classifier: 96 on 4 GPUs).  Six convolutions leave
+# the tensor cores at this size (test_cpu_plan_448.py); test_gpu_step_layers_448.py also runs them alone at B = 64.
+CONFIGS_448 = [
+    # README, NAB from scratch: the 555-d nab embedding, inv_corr, cls_weight 0.1
+    ('resnet-50', 32, 'tf32x3', dict(tag='nab-large', input_size=448, cls_weight=0.1)),
+    # NAB fine-tuned, the --finetune_init phase: only the new layers train, 'embedding' (also the embedding model's
+    # last layer) and the classifier branch's 'prob' (learn_image_embeddings.py:132-133)
+    ('resnet-50', 32, 'tf32x3', dict(tag='nab-large-finetune-init', input_size=448, cls_weight=0.1,
+                                     train=('embedding', 'prob'))),
+    # CosineLoss.md section 4.1 on CUB with --label_smoothing 0.1 (learn_classifier.py, --clipgrad 10 by default)
+    ('resnet-50', 24, 'tf32x3', dict(tag='cub-softmax', input_size=448, objective='softmax', num_classes=200,
+                                     label_smoothing=0.1, clipnorm=10.0)),
+]
+
+
 def config_id(cfg):
     arch, B, mode, opts = cfg
-    return ('%s-' % opts['tag'] if 'tag' in opts else '') + '%s-b%d-%s' % (arch, B, mode)
+    size = '-%dpx' % opts['input_size'] if opts.get('input_size') else ''
+    return ('%s-' % opts['tag'] if 'tag' in opts else '') + '%s%s-b%d-%s' % (arch, size, B, mode)
 
 
 def build_engine(cfg, device='cuda:0', use_cuda_graph=True):
     """The Engine of a configuration (arch, batch, mode, options), built the way its trainer builds it.  Options are
     Engine's, plus: 'tag' (the name of the case), 'devise_classes' (learn_devise.py --init_weights: the network of
     utils.build_devise_network with that many classes before), 'embed_dim' (learn_labelembedding.py /
-    learn_center_loss.py), 'fixed_centroids' (--centroids: a seeded C x D array, which the engine freezes) and 'train'
-    (the layers that train, as set_trainable(lambda name: name.split('/')[0] in train))."""
+    learn_center_loss.py), 'fixed_centroids' (--centroids: a seeded C x D array, which the engine freezes), 'train'
+    (the layers that train, as set_trainable(lambda name: name.split('/')[0] in train)) and 'input_size' (the side of
+    the square input, as the file datasets pass it; None: the architecture's default)."""
     import os
     from semantic_embeddings_b200 import _lib as L, utils
     from semantic_embeddings_b200.engine import Engine
@@ -546,18 +565,19 @@ def build_engine(cfg, device='cuda:0', use_cuda_graph=True):
     opts.pop('tag', None)
     devise_classes, embed_dim = opts.pop('devise_classes', None), opts.pop('embed_dim', None)
     fixed, train = opts.pop('fixed_centroids', False), opts.pop('train', None)
+    size = opts.pop('input_size', None)
     objective = opts.get('objective', 'embedding')
     if objective == 'embedding':
         key = 'nab' if arch == 'resnet-50' else 'cifar100'
         emb = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'class_matrices.npz'))[key + '_embedding']
         D = emb.shape[1]
-        graph = utils.build_devise_network(D, arch, devise_classes, input_channels=3) if devise_classes else \
-            utils.build_network(D, arch, input_channels=3)
+        graph = utils.build_devise_network(D, arch, devise_classes, input_channels=3, input_size=size) if devise_classes \
+            else utils.build_network(D, arch, input_channels=3, input_size=size)
         opts.update(embedding=emb, num_classes=emb.shape[0])
     elif objective == 'softmax':
-        graph = utils.build_network(opts['num_classes'], arch, classification=True, input_channels=3)
+        graph = utils.build_network(opts['num_classes'], arch, classification=True, input_channels=3, input_size=size)
     else:
-        graph = utils.build_network(embed_dim, arch, input_channels=3)
+        graph = utils.build_network(embed_dim, arch, input_channels=3, input_size=size)
         if fixed:
             C, D = opts['num_classes'], graph.output.shape[0]
             opts['centroids'] = np.random.RandomState(C + D).uniform(-0.05, 0.05, (C, D))
