@@ -34,7 +34,9 @@ Deviations, all stated at run time when they apply:
   * --gpus N > 1: launch with `python -m torch.distributed.run --nproc-per-node N learn_center_loss.py ...`;
   * --centroids whose width differs from the network's output (e.g. resnet-110's 64) raise a ValueError naming both
     sizes, where the reference fails inside Keras;
-  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles) and 'synthetic[:n]'; LR schedule: SGDR;
+  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles), the file datasets of get_data_generator ('NAB',
+    'CUB', 'CUB-sub<X>', 'ILSVRC', 'iNat[_<super-category>]', 'iNat2019', 'Cars', 'Flowers', 'MIT67Scenes', 'UCMLU',
+    'RESISC45', with '-large' / '-ilsvrcmean' / '-caffe') and 'synthetic[:n]'; LR schedule: SGDR;
   * --arith selects the arithmetic of the convolutions (see learn_image_embeddings.py).
 """
 import argparse

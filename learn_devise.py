@@ -23,7 +23,9 @@ Deviations, all stated at run time when they apply:
   * --init_weights reads this package's classifier dumps (learn_classifier.py --weight_dump / --model_dump pickles, or
     an .npz of Keras-named arrays), not Keras HDF5; the architecture and the class count come from the dump;
   * --log_dir is accepted and ignored with a message; validation runs with --batch_size;
-  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles) and 'synthetic[:n]'; one GPU, as in the reference;
+  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles), the file datasets of get_data_generator ('NAB',
+    'CUB', 'CUB-sub<X>', 'ILSVRC', 'iNat[_<super-category>]', 'iNat2019', 'Cars', 'Flowers', 'MIT67Scenes', 'UCMLU',
+    'RESISC45', with '-large' / '-ilsvrcmean' / '-caffe') and 'synthetic[:n]'; one GPU, as in the reference;
   * --arith selects the arithmetic of the convolutions (see learn_image_embeddings.py).
 """
 import argparse

@@ -16,8 +16,10 @@ Deviations, all stated at run time when they apply:
     with a message;
   * --gpus N > 1: launch with `python -m torch.distributed.run --nproc-per-node N learn_image_embeddings.py ...`
     (one process per GPU, NCCL all-reduce; the reference's in-graph towers have the same arithmetic);
-  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles, datasets/cifar.py), 'NAB' / 'NAB-large' / 'CUB' (+ '-ilsvrcmean'
-    / '-caffe'; image files decoded on --read_workers threads, the network built for the crop size) and 'synthetic[:n]';
+  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles, datasets/cifar.py), the file datasets of get_data_generator
+    ('NAB', 'CUB', 'CUB-sub<X>', 'ILSVRC', 'iNat[_<super-category>]', 'iNat2019', 'Cars', 'Flowers', 'MIT67Scenes', 'UCMLU',
+    'RESISC45', with '-large' / '-ilsvrcmean' / '-caffe'; image files decoded on --read_workers threads, the network
+    built for the crop size) and 'synthetic[:n]';
   * --arith selects the arithmetic of the convolutions: tf32x3 (default: tensor-core tiles with error compensation, fp32-level
     results), f32 (fp32 FFMA kernels), tf32 (single-pass TF32, ~1e-3 relative deviation: NOT the reference's arithmetic).
 """

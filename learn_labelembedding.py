@@ -29,7 +29,9 @@ Deviations, all stated at run time when they apply:
     accepted and ignored with a message; validation runs with --batch_size (its last batch is padded with rows that
     take no part in the loss's normalisation);
   * --gpus N > 1: launch with `python -m torch.distributed.run --nproc-per-node N learn_labelembedding.py ...`;
-  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles) and 'synthetic[:n]'; LR schedule: SGDR;
+  * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles), the file datasets of get_data_generator ('NAB',
+    'CUB', 'CUB-sub<X>', 'ILSVRC', 'iNat[_<super-category>]', 'iNat2019', 'Cars', 'Flowers', 'MIT67Scenes', 'UCMLU',
+    'RESISC45', with '-large' / '-ilsvrcmean' / '-caffe') and 'synthetic[:n]'; LR schedule: SGDR;
   * --arith selects the arithmetic of the convolutions (see learn_image_embeddings.py).
 """
 import argparse

@@ -8,7 +8,8 @@ TinyDatasetGenerator.compose_batch's per-image Python loop around Keras' ImageDa
 Only the random draws (three numbers per image) are made on the host.  There is no CPU implementation of the transform
 in the product; tests compare the kernel with oracle/augment.py.
 
-The NABirds / CUB file datasets (FileDatasetGenerator) decode JPEG / PNG files on host threads and hand each batch to
+The file datasets (FileDatasetGenerator: NABirds, CUB and its CUB-subX splits, ILSVRC, iNaturalist, Stanford Cars,
+Flowers-102, MIT-67 Scenes, UCMLU, RESISC45) decode JPEG / PNG files on host threads and hand each batch to
 one CUDA launch (se_resample_crop_batch, csrc/file_augment.cu) that resizes exactly like PIL, standardises, flips,
 erases and crops.  With decoder='gpu' the host threads only read the files and parse the JPEG headers
 (se_jpeg_parse); the device decodes the batch's JPEGs bit-identically to load_img (se_jpeg_decode_batch,
@@ -16,6 +17,8 @@ csrc/jpeg_decode.cu), and the files it does not support go through load_img as b
 """
 import collections
 import ctypes
+import glob
+import json
 import os
 import pickle
 import threading
@@ -156,6 +159,36 @@ IMAGENET_MEAN, IMAGENET_STD = [122.65435242, 116.6545058, 103.99789959], [71.405
 NAB_MEAN, NAB_STD = [125.30513277, 129.66606421, 118.45121113], [57.0045467, 56.70059436, 68.44430446]
 CUB_MEAN, CUB_STD = [123.82988033, 127.35116805, 110.25606303], [59.2230949, 58.0736071, 67.80251684]
 RANDERASE_PARAMS = {'sl': 0.02, 'sh': 0.3, 'r1': 0.3, 'r2': 1. / 0.3}                     # nab.py:11
+# FileDatasetGenerator's own erase defaults (datasets/common.py:129-130), which ILSVRC and iNat keep: no erasing
+NO_RANDERASE = {'randerase_prob': 0.0, 'randerase_params': {'sl': 0.02, 'sh': 0.4, 'r1': 0.3, 'r2': 1. / 0.3}}
+INAT2019_MEAN, INAT2019_STD = [115.77492586, 120.84414891, 93.51744386], [60.46127213, 58.63136496, 63.5872299]
+CARS_MEAN, CARS_STD = [120.03730636, 117.33780928, 116.0130335], [75.40415763, 75.15394251, 77.28286728]
+FLOWERS_MEAN, FLOWERS_STD = [110.7799141, 97.65648664, 75.32889973], [74.90387818, 62.70218863, 69.7656359]
+# datasets/__init__.py:142-164: name -> (image directory, training list, test list, mean, std)
+SUBDIRECTORY_DATASETS = {
+    'mit67scenes': ('Images', 'TrainImages.txt', 'TestImages.txt',
+                    [124.62788179, 110.01028625, 94.95780545], [68.56923599, 66.86607736, 67.35944349]),
+    'ucmlu': ('.', 'train.txt', 'test.txt', [122.65409223, 124.40230701, 114.25659171], [55.74499679, 51.65585669, 50.16527551]),
+    'resisc45': ('.', 'train.txt', 'test.txt', [94.17769482, 97.40967803, 87.80359702], [51.92246172, 47.22081475, 47.07685676]),
+}
+# datasets/inat.py:7-23: channel statistics of iNaturalist 2018 and of each of its super-categories
+INAT_SUPERCATEGORY_STATS = {
+    None: ([119.99310088, 122.86333725, 102.38318464], [60.83471124, 59.33123704, 65.92057842]),
+    'actinopterygii': ([95.60659929, 109.21340134, 99.53273934], [62.64981594, 56.77583425, 57.79043402]),
+    'amphibia': ([120.38820316, 112.09448704, 93.57291079], [64.38971069, 60.88945117, 60.689195]),
+    'animalia': ([117.86148813, 112.27558493, 100.76823038], [65.10786879, 60.9941875, 61.3212783]),
+    'arachnida': ([123.05328454, 123.11786486, 99.49669769], [62.10607939, 59.69295922, 64.12102046]),
+    'aves': ([125.68554284, 131.58931007, 123.51576605], [56.91926625, 57.04151665, 67.97284604]),
+    'bacteria': ([130.44253929, 118.58949652, 100.64353881], [63.52655078, 61.3866035, 62.52496727]),
+    'chromista': ([126.63609004, 120.30744082, 103.69842308], [61.3142875, 60.35121831, 64.33445667]),
+    'fungi': ([105.4904181, 98.20844854, 81.95195412], [66.43803547, 63.26916273, 61.75505097]),
+    'insecta': ([126.79141945, 126.55725101, 94.4626541], [62.46710552, 59.70656548, 64.38703598]),
+    'mammalia': ([119.32537707, 119.28610021, 105.22655576], [60.25561291, 58.86410094, 60.85549787]),
+    'mollusca': ([119.15865454, 107.82338741, 93.65438902], [65.54171188, 62.00986655, 62.64830566]),
+    'plantae': ([109.4558912, 115.78290918, 84.83970548], [60.36177593, 59.17162815, 60.81183456]),
+    'protozoa': ([99.4855571, 90.12976005, 71.67906874], [69.23439903, 63.83415135, 59.1059619]),
+    'reptilia': ([126.42469824, 119.44987437, 103.84680809], [63.4749642, 60.19704406, 60.20556052]),
+}
 
 
 def load_img(path):
@@ -245,18 +278,151 @@ def parse_nab(root_dir, classes=None, img_dir='images', img_list_file='images.tx
     return (classes,) + out
 
 
+def list_pictures(directory, ext='jpeg'):
+    """The file-listing rule ILSVRCGenerator relies on (keras_preprocessing.image.list_pictures, Keras 2.2 and later),
+    restated so that it no longer depends on the Keras version: every file below `directory` -- os.walk, recursive,
+    symbolic links to directories not followed, nothing when the directory does not exist -- whose name, lower-cased,
+    ends in '.' + ext.  So 'x.JPEG' and 'x.jpeg' are listed, 'x.jpg' is not, and names with characters other than
+    letters, digits and '_' ('a-b c.JPEG', 'a.b.JPEG') are listed too (earlier Keras versions matched the name against a
+    regular expression of word characters, which drops those).  The file's contents are not looked at: a PNG named
+    '.JPEG' is listed.  Returns the paths in os.walk order."""
+    ext = '.' + ext.lower()
+    return [os.path.join(root, f) for root, _, files in os.walk(directory) for f in files if f.lower().endswith(ext)]
+
+
+def parse_ilsvrc(root_dir, classes=None):
+    """ILSVRCGenerator.__init__ (datasets/ilsvrc.py:34-55): the synsets -- `classes` in the order given, else the sorted
+    sub-directories of ILSVRC2012_img_train -- enumerated in that order; the images of a synset are the sorted
+    list_pictures(<split dir>/<synset>, 'jpeg') of ILSVRC2012_img_train and ILSVRC2012_img_val.  Returns
+    (classes, train_files, train_labels, test_files, test_labels)."""
+    train_dir = os.path.join(root_dir, 'ILSVRC2012_img_train')
+    test_dir = os.path.join(root_dir, 'ILSVRC2012_img_val')
+    if classes is None:
+        classes = [d for d in sorted(os.listdir(train_dir)) if os.path.isdir(os.path.join(train_dir, d))]
+    classes = list(classes)
+    out = ([], [], [], [])
+    for lbl, synset in enumerate(classes):
+        for k, d in ((0, train_dir), (2, test_dir)):
+            files = sorted(list_pictures(os.path.join(d, synset), 'jpeg'))
+            out[k].extend(files)
+            out[k + 1].extend([lbl] * len(files))
+    return (classes,) + out
+
+
+def _inat_annotations(fname, root_dir, supercategory):
+    """INatGenerator.get_tuples_for_supercategory (datasets/inat.py:96-134): [(label, absolute path)] of the images of
+    the kept categories (all, or those of `supercategory`), the label being the rank of the category id among the kept
+    ones; and {category name: label}."""
+    with open(fname) as f:
+        data = json.load(f)
+    id_to_image = {image['id']: image for image in data['images']}
+    kept = {c['id']: c for c in data['categories']
+            if supercategory is None or c['supercategory'].lower() == supercategory}
+    ids = sorted(kept)
+    old_to_new = {old: new for new, old in enumerate(ids)}
+    mapping = {kept[old]['name']: new for new, old in enumerate(ids)}
+    tuples = [(old_to_new[a['category_id']], os.path.abspath(os.path.join(root_dir, id_to_image[a['image_id']]['file_name'])))
+              for a in data['annotations'] if a['category_id'] in kept]
+    return tuples, mapping
+
+
+def parse_inat(root_dir, train_file='train2018.json', val_file='val2018.json', supercategory=None):
+    """INatGenerator.__init__ (datasets/inat.py:63-93) for iNaturalist 2018 / 2019: the images of the training and
+    validation JSON files (COCO-style 'images', 'categories', 'annotations'), restricted to `supercategory`
+    (lower-cased) when given.  The classes are the category names ordered by label (those of the training file).
+    Raises ValueError when a file lists no image of the kept categories (the reference fails to unpack there too)."""
+    supercategory = supercategory.lower() if supercategory is not None else None
+    out = []
+    for fn in (train_file, val_file):
+        tuples, mapping = _inat_annotations(fn if os.path.isabs(fn) else os.path.join(root_dir, fn), root_dir, supercategory)
+        if not tuples:
+            raise ValueError('{} lists no image{}'.format(fn, '' if supercategory is None else
+                                                           ' of the super-category ' + supercategory))
+        if not out:
+            classes = [c for c, _ in sorted(mapping.items(), key=lambda t: t[1])]
+        out += [[p for _, p in tuples], [lbl for lbl, _ in tuples]]
+    return (classes,) + tuple(out)
+
+
+def parse_cars(root_dir, classes=None, annotation_file='cars_annos.mat'):
+    """CarsGenerator.__init__ (datasets/cars.py:55-75): the 'annotations' struct array of the MATLAB file
+    (relative_im_path, class, test); classes in the order given, else the sorted set of class numbers.  Images of other
+    classes are skipped."""
+    import scipy.io
+    fn = annotation_file if os.path.isabs(annotation_file) else os.path.join(root_dir, annotation_file)
+    annotations = scipy.io.loadmat(fn, squeeze_me=True)['annotations']
+    classes = list(classes) if classes is not None else sorted(set(annotations['class']))
+    class_indices = dict(zip(classes, range(len(classes))))
+    out = ([], [], [], [])
+    for sample in annotations:
+        if sample['class'] in class_indices:
+            path = sample['relative_im_path']
+            k = 2 if sample['test'] else 0
+            out[k].append(path if os.path.isabs(path) else os.path.join(root_dir, path))
+            out[k + 1].append(class_indices[sample['class']])
+    return (classes,) + out
+
+
+def parse_flowers(root_dir, classes=None, img_dir='jpg', label_file='imagelabels.mat', split_file='setid.mat',
+                  train_splits=('trnid', 'valid'), test_splits=('tstid',)):
+    """FlowersGenerator.__init__ (datasets/flowers.py:60-84): image i (1-based) is <img_dir>/image_%05d.jpg with label
+    'labels'[i - 1] of label_file; the training images are the ids of the train_splits arrays of split_file, the test
+    images those of test_splits.  Unlike the other parsers this one does not skip images of classes left out of
+    `classes`: the reference raises KeyError there, this function ValueError."""
+    import scipy.io
+    rel = lambda p: p if os.path.isabs(p) else os.path.join(root_dir, p)
+    img_labels = scipy.io.loadmat(rel(label_file), squeeze_me=True)['labels']
+    splits = scipy.io.loadmat(rel(split_file), squeeze_me=True)
+    classes = list(classes) if classes is not None else sorted(set(img_labels))
+    class_indices = dict(zip(classes, range(len(classes))))
+    out = ([], [], [], [])
+    for k, names in ((0, train_splits), (2, test_splits)):
+        for split in names:
+            for i in splits[split]:
+                lbl = img_labels[i - 1]
+                if lbl not in class_indices:
+                    raise ValueError('image {} of the {} split has class {}, which is not among the classes {}'
+                                     .format(i, split, lbl, classes))
+                out[k].append(os.path.join(rel(img_dir), 'image_{:05d}.jpg'.format(i)))
+                out[k + 1].append(class_indices[lbl])
+    return (classes,) + out
+
+
+def parse_subdirectory(root_dir, classes=None, img_dir='.', train_list='train.txt', test_list='test.txt'):
+    """SubDirectoryGenerator.__init__ (datasets/subdirectory.py:51-80): one sub-directory of img_dir per class (the
+    sorted directory names not starting with '.', unless `classes` is given); the lists name one image per line relative
+    to img_dir, and an image's class is the directory part of its line.  Lines of other classes are skipped."""
+    img_dir = img_dir if os.path.isabs(img_dir) else os.path.join(root_dir, img_dir)
+    if classes is None:
+        classes = sorted(os.path.basename(d) for d in glob.glob(os.path.join(img_dir, '*'))
+                         if not os.path.basename(d).startswith('.') and os.path.isdir(d))
+    classes = list(classes)
+    class_indices = dict(zip(classes, range(len(classes))))
+    out = ([], [], [], [])
+    for k, fn in ((0, train_list), (2, test_list)):
+        with open(fn if os.path.isabs(fn) else os.path.join(root_dir, fn)) as f:
+            for l in f:
+                if l.strip() != '' and os.path.dirname(l.strip()) in class_indices:
+                    out[k].append(os.path.join(img_dir, l.strip()))
+                    out[k + 1].append(class_indices[os.path.dirname(l.strip())])
+    return (classes,) + out
+
+
 class FileDatasetGenerator:
-    """FileDatasetGenerator of datasets/common.py:126-632 for the NABirds / CUB layout, with the interface of
+    """FileDatasetGenerator of datasets/common.py:126-632 over a parsed file list (parse_nab, parse_ilsvrc, ...), with the
+    interface of
     TinyDatasetGenerator.  Images are decoded on `read_workers` host threads (PIL releases the GIL), the batches of
     train_batches / test_batches ahead of the one being composed; everything after the decode -- resize, standardisation,
     BGR, flip, random erasing, crop -- is one se_resample_crop_batch launch per batch that writes the engine's input
     tensor.  The random draws are made on the host `rng` in the reference's order (draw_params); the erase noise is the
-    one deliberate departure: the device computes it from a per-batch seed (include/se_b200.h).  Constructing the
-    generator reads the file lists only."""
+    one deliberate departure: the device computes it from a per-batch seed (include/se_b200.h).  train_repeats: passes
+    over the training set per epoch (NABGenerator's train_repeats, the CUB-subX splits).  Constructing the generator
+    reads the file lists only."""
 
     def __init__(self, train_files, train_labels, test_files, test_labels, classes, cropsize=224, default_target_size=256,
                  randzoom_range=None, mean=NAB_MEAN, std=NAB_STD, color_mode='rgb', randerase_prob=0.5,
-                 randerase_params=RANDERASE_PARAMS, read_workers=8, prefetch=2, device='cuda', decoder='pil'):
+                 randerase_params=RANDERASE_PARAMS, read_workers=8, prefetch=2, device='cuda', decoder='pil',
+                 train_repeats=1):
         import torch
         if decoder not in ('pil', 'gpu'):
             raise ValueError('Unknown decoder: {} (pil or gpu)'.format(decoder))
@@ -273,6 +439,7 @@ class FileDatasetGenerator:
         self.color_mode = color_mode.lower()
         self.randerase_prob = randerase_prob
         self.randerase_params = dict(randerase_params)
+        self.train_repeats = int(train_repeats)
         self.read_workers = max(1, int(read_workers))
         self.prefetch = max(0, int(prefetch))
         self._pool = None
@@ -415,12 +582,13 @@ class FileDatasetGenerator:
         return [self._sizes[(bool(train), i)] for i in np.asarray(indices).tolist()]
 
     # ---- host draws
-    def draw_params(self, sizes, augment, rng=None):
+    def draw_params(self, sizes, augment, rng=None, files=None):
         """The random draws of FileDatasetGenerator.compose_batch (datasets/common.py:408-425) for images of decoded
         sizes `sizes` [(h, w)], in the reference's order on `rng`: per image the zoom (:467), the flip (:523) and the
         erase decision and geometry (:530-537); then per image the crop row and column (:417, :422).  With augment=False:
         the default target size and the centre crop.  A last draw gives the seed of the erase noise when erasing is on.
-        Returns a dict of int arrays: size [n, 2] (rh, rw), flip [n], erase [n, 4] (ey, ex, eh, ew; eh = 0: none),
+        An image with a side above SE_RESAMPLE_MAX_SIDE raises ValueError naming it (its path in `files`, when given)
+        before anything is drawn.  Returns a dict of int arrays: size [n, 2] (rh, rw), flip [n], erase [n, 4] (ey, ex, eh, ew; eh = 0: none),
         crop [n, 2] (cy, cx), and the int `seed`."""
         n, ch = len(sizes), self.cropsize
         size = np.zeros((n, 2), np.int64)
@@ -430,6 +598,11 @@ class FileDatasetGenerator:
         rng = rng if rng is not None else np.random
         erase_on = augment and self.randerase_prob > 0
         p = self.randerase_params
+        for i, (h, w) in enumerate(sizes):
+            if max(h, w) > _lib.SE_RESAMPLE_MAX_SIDE:
+                raise ValueError('{} is {}x{} pixels (width x height): images with a side above {} are not supported'
+                                 .format(files[i] if files is not None else 'image %d' % i, w, h,
+                                         _lib.SE_RESAMPLE_MAX_SIDE))
         for i, (h, w) in enumerate(sizes):
             target = self.default_target_size
             if augment and self.randzoom_range is not None:
@@ -467,16 +640,17 @@ class FileDatasetGenerator:
         later epochs stay identical on all ranks, and the slices together are exactly the single-GPU batch (the erase
         noise is keyed by the image's position in the global batch, `noise_id`)."""
         ctx = self._global.get(self._key(train, indices)) if augment else None
+        files = self._files(train)
         if ctx is None:
             if images is None:
                 images = self.decode(indices, train)
-            return self.draw_params([im.shape[:2] for im in images], augment, rng)
+            return self.draw_params([im.shape[:2] for im in images], augment, rng, [files[i] for i in indices])
         g, off = ctx
         n = len(indices)
         sizes = self.image_sizes(g, train)
         if images is not None:
             assert [im.shape[:2] for im in images] == sizes[off:off + n]
-        p = self.draw_params(sizes, augment, rng)
+        p = self.draw_params(sizes, augment, rng, [files[i] for i in g])
         out = {k: v[off:off + n] for k, v in p.items() if k != 'seed'}
         out['seed'] = p['seed']
         return out
@@ -712,19 +886,29 @@ class FileDatasetGenerator:
     def train_batches(self, batch_size, rng, rank=0, world=1):
         """As TinyDatasetGenerator.train_batches (shuffled, trailing partial batch dropped); the images of the next
         `prefetch` batches are decoded while the current one trains.  With world > 1 each rank's slice remembers its
-        global batch, so that compose_batch draws for all of it (batch_params) and `rng` stays the same on every rank."""
-        perm = rng.permutation(self.num_train)
+        global batch, so that compose_batch draws for all of it (batch_params) and `rng` stays the same on every rank.
+        With train_repeats = R the epoch is R passes, as DataSequence(repeats=R) makes it (datasets/common.py:29-118):
+        the R permutations are drawn first, in pass order, then pass r takes the batches of permutation r, each pass
+        dropping its own trailing partial batch."""
+        perms = [rng.permutation(self.num_train) for _ in range(self.train_repeats)]
         per = batch_size // world
         starts = range(0, self.num_train - batch_size + 1, batch_size)
-        batches = [perm[i + rank * per:i + (rank + 1) * per] for i in starts]
-        if world > 1:
-            for i, idx in zip(starts, batches):
-                self._global[self._key(True, idx)] = (perm[i:i + world * per], rank * per)
+        batches = [perm[i + rank * per:i + (rank + 1) * per] for perm in perms for i in starts]
+        ctxs = [(perm[i:i + world * per], rank * per) for perm in perms for i in starts]
+        # a slice's global batch is registered while the slice is the current batch only: with several passes the
+        # same slice can recur with other images around it
+        it = self._iterate(batches, True, self.y_train)
         try:
-            yield from self._iterate(batches, True, self.y_train)
+            for k, (idx, y) in enumerate(it):
+                key = self._key(True, idx)
+                if world > 1:
+                    self._global[key] = ctxs[k]
+                try:
+                    yield idx, y
+                finally:
+                    self._global.pop(key, None)
         finally:
-            for idx in batches:
-                self._global.pop(self._key(True, idx), None)
+            it.close()
 
     def test_batches(self, batch_size):
         batches = [np.arange(i, min(i + batch_size, self.num_test)) for i in range(0, self.num_test, batch_size)]
@@ -741,13 +925,17 @@ class FileDatasetGenerator:
             self._forget(train, batches)
 
 
-FILE_DATASETS = ('nab', 'cub')
+FILE_DATASETS = ('nab', 'cub', 'ilsvrc', 'inat', 'inat2019', 'cars', 'flowers', 'mit67scenes', 'ucmlu', 'resisc45')
 
 
 def _file_generator(dataset, data_root, classes, device, read_workers, decoder='pil'):
-    """datasets/__init__.py:60-117 for NABirds / CUB: the suffixes '-ilsvrcmean' / '-caffe' (then '-large') and the
-    per-dataset crop, target size, zoom range and statistics.  None for names that are not file datasets."""
+    """datasets/__init__.py:58-164 for the file datasets: 'inat2018' read as 'inat', then the suffixes '-ilsvrcmean' /
+    '-caffe', then '-large', and the per-dataset parser, crop, target size, zoom range, random erasing and statistics.
+    None for names that are not file datasets; ValueError for the names the reference refuses (with TypeError,
+    ValueError or ZeroDivisionError there) and when `data_root` lacks a file or directory the dataset needs."""
     name = dataset.lower()
+    if name.startswith('inat2018'):
+        name = 'inat' + name[8:]
     kw = {}
     if name.endswith('-ilsvrcmean'):
         kw['mean'], kw['std'] = IMAGENET_MEAN, IMAGENET_STD
@@ -759,31 +947,79 @@ def _file_generator(dataset, data_root, classes, device, read_workers, decoder='
     if large:
         kw['cropsize'], kw['default_target_size'] = 448, 512
         name = name[:-6]
+
+    def refuse(why):
+        raise ValueError('Unknown dataset: {} ({})'.format(dataset, why))
+
+    # defaults of the reference's generator classes, under the suffixes' settings
+    default = lambda **d: kw.update({k: v for k, v in d.items() if k not in kw})
     if name == 'nab':
         if not large:
             kw['cropsize'], kw['default_target_size'], kw['randzoom_range'] = 224, 256, (256, 480)
-    elif name == 'cub':
+        parse = lambda: parse_nab(data_root, classes, 'images')
+    elif name == 'cub' or name.startswith('cub-sub'):
         if large:       # the reference passes cropsize / default_target_size twice here (TypeError)
-            raise ValueError('Unknown dataset: {} (the reference rejects -large for CUB)'.format(dataset))
-        kw.setdefault('mean', CUB_MEAN)
-        kw.setdefault('std', CUB_STD)
+            refuse('the reference rejects -large for CUB')
+        default(mean=CUB_MEAN, std=CUB_STD)
         kw['cropsize'], kw['default_target_size'] = 448, 512
-    elif name.startswith('cub-sub'):
-        raise ValueError('Unknown dataset: {} (the cub-sub* splits are not supported)'.format(dataset))
+        split_file = 'train_test_split.txt'
+        if name != 'cub':
+            try:
+                samples = int(name[7:])
+            except ValueError:
+                refuse('cub-sub is followed by the number of training images per class')
+            if not 1 <= samples <= 30:      # 30 // samples passes per epoch; the reference divides by zero at 0
+                refuse('cub-sub<X> needs 1 <= X <= 30')
+            split_file = 'train_test_split_{}.txt'.format(samples)
+            kw['train_repeats'] = 30 // samples
+        parse = lambda: parse_nab(data_root, classes, 'images', split_file=split_file)
+    elif name == 'ilsvrc':
+        if large:       # ILSVRCGenerator takes no cropsize / default_target_size (TypeError)
+            refuse('the reference rejects -large for ILSVRC')
+        default(mean=IMAGENET_MEAN, std=IMAGENET_STD, cropsize=224, default_target_size=256, randzoom_range=(256, 480),
+                **NO_RANDERASE)
+        parse = lambda: parse_ilsvrc(data_root, classes)
+    elif name in ('inat', 'inat2019') or name.startswith('inat_'):
+        # `classes` is not passed on: the categories of the JSON files define the classes
+        sup = name[5:] if name.startswith('inat_') else None
+        if not large:
+            kw['randzoom_range'] = (256, 480)
+        if name == 'inat2019':
+            default(mean=INAT2019_MEAN, std=INAT2019_STD)
+        elif 'mean' not in kw:
+            if sup not in INAT_SUPERCATEGORY_STATS:     # the reference decodes every training image to compute them
+                refuse('no channel statistics for the super-category {}'.format(sup))
+            kw['mean'], kw['std'] = INAT_SUPERCATEGORY_STATS[sup]
+        default(cropsize=224, default_target_size=256, **NO_RANDERASE)
+        files = ('train2019.json', 'val2019.json') if name == 'inat2019' else ('train2018.json', 'val2018.json')
+        parse = lambda: parse_inat(data_root, *files, supercategory=sup)
+    elif name in ('cars', 'flowers'):
+        default(mean=CARS_MEAN if name == 'cars' else FLOWERS_MEAN, std=CARS_STD if name == 'cars' else FLOWERS_STD,
+                cropsize=448, default_target_size=512)
+        parse = lambda: (parse_cars if name == 'cars' else parse_flowers)(data_root, classes)
+    elif name in SUBDIRECTORY_DATASETS:
+        img_dir, train_list, test_list, mean, std = SUBDIRECTORY_DATASETS[name]
+        default(mean=mean, std=std, cropsize=224, default_target_size=256)
+        parse = lambda: parse_subdirectory(data_root, classes, img_dir, train_list, test_list)
     else:
         return None
-    classes, tr_files, tr_labels, te_files, te_labels = parse_nab(data_root, classes, 'images')
+    try:
+        classes, tr_files, tr_labels, te_files, te_labels = parse()
+    except OSError as e:
+        raise ValueError('{}: {} does not hold the dataset ({})'.format(dataset, data_root, e)) from e
     print('Found {} training and {} validation images from {} classes.'.format(len(tr_files), len(te_files), len(classes)))
     return FileDatasetGenerator(tr_files, tr_labels, te_files, te_labels, classes, read_workers=read_workers, device=device,
                                 decoder=decoder, **kw)
 
 
 def get_data_generator(dataset, data_root, classes=None, device='cuda', read_workers=8, decoder='pil'):
-    """datasets/__init__.py:21-166, CIFAR branch (:85-87), the NABirds / CUB branches (:101-117: 'nab', 'nab-large',
-    'cub', each optionally followed by '-ilsvrcmean' or '-caffe'; FileDatasetGenerator, decoding on `read_workers`
-    threads), plus 'synthetic[:n]' (uint8 images = a fixed random colour template per class blended with pixel noise,
-    for machines without data).  The other file datasets of the reference (ILSVRC, iNat, Cars, Flowers, subdirectories)
-    are not supported.  decoder: 'pil' (load_img on the read threads) or 'gpu' (the device decodes the JPEGs it
+    """datasets/__init__.py:21-166: 'cifar-10', 'cifar-100' (:85-87) and the file datasets (FileDatasetGenerator,
+    decoding on `read_workers` threads): 'nab', 'cub', 'cub-sub<X>' (X training images per class from
+    train_test_split_<X>.txt, 30 // X passes per epoch), 'ilsvrc', 'inat' / 'inat2018' (optionally '_<super-category>';
+    `classes` is ignored), 'inat2019', 'cars', 'flowers', 'mit67scenes', 'ucmlu', 'resisc45', each optionally followed
+    by '-large' (448-pixel crops of 512-pixel images; not for ILSVRC and CUB) and then by '-ilsvrcmean' or '-caffe';
+    plus 'synthetic[:n]' (uint8 images = a fixed random colour template per class blended with pixel noise, for
+    machines without data).  'cifar-100-a' / 'cifar-100-b' are not supported.  decoder: 'pil' (load_img on the read threads) or 'gpu' (the device decodes the JPEGs it
     supports, bit-identically); it only concerns the file datasets, the others hold decoded pixels."""
     if decoder not in ('pil', 'gpu'):
         raise ValueError('Unknown decoder: {} (pil or gpu)'.format(decoder))
