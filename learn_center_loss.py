@@ -15,7 +15,7 @@ What each part of the reference script maps to:
                                                      fixed centroids (Engine(centroids=...), frozen), D = their width
   loss_weights {prob: 1, center_loss: w} (:137-139, :162-165)
                                                   -> loss = CE(prob) + w * mean 1/2 ||z - c_y||^2 (+ the base network's L2)
-  SGD(sgd_lr, decay, momentum 0.9, nesterov, clipnorm) under SGDR (:151-172)
+  SGD(sgd_lr, decay, momentum 0.9, nesterov, clipnorm) under --lr_schedule (:151-172)
                                                   -> the engine's SGD; the centroids' gradient is part of the clip norm
   --finetune / --finetune_init (:129-148)         -> Engine.set_trainable: only embedding, embedding_bn, prob,
                                                      cls_centroids and the base network's last layer train; afterwards
@@ -36,7 +36,7 @@ Deviations, all stated at run time when they apply:
     sizes, where the reference fails inside Keras;
   * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles), the file datasets of get_data_generator ('NAB',
     'CUB', 'CUB-sub<X>', 'ILSVRC', 'iNat[_<super-category>]', 'iNat2019', 'Cars', 'Flowers', 'MIT67Scenes', 'UCMLU',
-    'RESISC45', with '-large' / '-ilsvrcmean' / '-caffe') and 'synthetic[:n]'; LR schedule: SGDR;
+    'RESISC45', with '-large' / '-ilsvrcmean' / '-caffe') and 'synthetic[:n]';
   * --arith selects the arithmetic of the convolutions (see learn_image_embeddings.py).
 """
 import argparse

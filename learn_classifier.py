@@ -19,7 +19,7 @@ Deviations, all stated at run time when they apply:
   * --gpus N > 1: launch with `python -m torch.distributed.run --nproc-per-node N learn_classifier.py ...`;
   * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles), the file datasets of get_data_generator ('NAB',
     'CUB', 'CUB-sub<X>', 'ILSVRC', 'iNat[_<super-category>]', 'iNat2019', 'Cars', 'Flowers', 'MIT67Scenes', 'UCMLU',
-    'RESISC45', with '-large' / '-ilsvrcmean' / '-caffe') and 'synthetic[:n]'; LR schedule: SGDR;
+    'RESISC45', with '-large' / '-ilsvrcmean' / '-caffe') and 'synthetic[:n]';
   * --arith selects the arithmetic of the convolutions (see learn_image_embeddings.py).
 """
 import argparse

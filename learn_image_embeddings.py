@@ -4,7 +4,7 @@ H100-native engine.  Reference: learn_image_embeddings.py:54-275.
 
 What each part of the reference script maps to:
   model construction + compile (:123-150, 224-236)  -> semantic_embeddings_b200.utils.build_network + engine.Engine
-  fit_generator (:238-243): train batches, validation pass per epoch, SGDR callback, ModelCheckpoint
+  fit_generator (:238-243): train batches, validation pass per epoch, LR schedule callback, ModelCheckpoint
                                                      -> the epoch loop below (device-side augmentation: datasets.py)
   evaluate_generator / Average Accuracy (:245-254)  -> final_evaluation()
   model / weight dumps (:257-267)                   -> pickles of {Keras weight name: array} (Keras HDF5 needs h5py; names

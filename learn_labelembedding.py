@@ -11,7 +11,7 @@ What each part of the reference script maps to:
                                                      'embedding_bn' -> 'prob' / stop-gradient 'out2', the identity-initialised
                                                      table 'labelembeddings/embeddings'; the five-term loss, its mask
                                                      normalisation and every gradient are one op (se_labelembed_fwd_bwd)
-  SGD(sgd_lr, decay, momentum 0.9, nesterov, clipnorm) under SGDR (:158-178)
+  SGD(sgd_lr, decay, momentum 0.9, nesterov, clipnorm) under --lr_schedule (:158-178)
                                                   -> the engine's SGD; the table's gradient is part of the clip norm
   --finetune / --finetune_init (:137-155)         -> Engine.set_trainable: only embedding, embedding_bn, prob, out2,
                                                      labelembeddings and the base network's last layer train
@@ -31,7 +31,7 @@ Deviations, all stated at run time when they apply:
   * --gpus N > 1: launch with `python -m torch.distributed.run --nproc-per-node N learn_labelembedding.py ...`;
   * datasets: 'CIFAR-100' / 'CIFAR-10' (python pickles), the file datasets of get_data_generator ('NAB',
     'CUB', 'CUB-sub<X>', 'ILSVRC', 'iNat[_<super-category>]', 'iNat2019', 'Cars', 'Flowers', 'MIT67Scenes', 'UCMLU',
-    'RESISC45', with '-large' / '-ilsvrcmean' / '-caffe') and 'synthetic[:n]'; LR schedule: SGDR;
+    'RESISC45', with '-large' / '-ilsvrcmean' / '-caffe') and 'synthetic[:n]';
   * --arith selects the arithmetic of the convolutions (see learn_image_embeddings.py).
 """
 import argparse

@@ -99,14 +99,17 @@ def resume(eng, path, say):
         eng.set_iterations(snap.get('iterations', 0))
 
 
-def train_epoch(eng, data, batch_size, rng, rank, world, ks=()):
-    """One pass over the training set; running means of the per-batch metrics (Keras progress bar)."""
+def train_epoch(eng, data, batch_size, rng, rank, world, ks=(), on_step=None):
+    """One pass over the training set; running means of the per-batch metrics (Keras progress bar).  `on_step(batch)`,
+    if given, runs after every training step (where fit_generator calls on_batch_end)."""
     import torch
     sums, nb, pending = {}, 0, None
-    for idx, y in data.train_batches(batch_size, rng, rank, world):
+    for batch, (idx, y) in enumerate(data.train_batches(batch_size, rng, rank, world)):
         data.compose_batch(idx, True, eng.x, augment=True, rng=rng)
         eng.labels.copy_(torch.from_numpy(np.asarray(y, dtype=np.int32)), non_blocking=True)
         eng.train_step()
+        if on_step is not None:
+            on_step(batch)
         h = eng.metrics_async(ks)                # without stalling the device
         if pending is not None:
             for k, v in eng.metrics_result(pending).items():
@@ -206,20 +209,52 @@ def fit_constant_lr(eng, data, batch_size, lr, epochs, rng, ks, say, rank=0, wor
 
 
 def fit(eng, data, args, sched, epochs, rng, rank, world, ks, say, train_ks=()):
-    """The epochs of fit_generator: SGDR learning rate per epoch, a training pass, a validation pass, and the
-    ModelCheckpoint of --snapshot / --snapshot_best (monitor 'val_loss' by default; metrics containing 'acc' are
-    maximised)."""
-    sched.on_train_begin()          # like the reference, a resumed run starts a fresh SGDR cycle (the callback is new)
+    """The epochs of fit_generator: the schedule callback's hooks where Keras calls them, a training pass, a validation
+    pass, and the ModelCheckpoint of --snapshot / --snapshot_best (monitor 'val_loss' by default; metrics containing
+    'acc' are maximised).
+
+    Callbacks other than SGDR read and write the optimizer's float32 rate, which starts at --sgd_lr.  The rate is pushed
+    to the device (Engine.set_lr) at the start of every epoch and, for a schedule with `on_batch_end` (CyclicLR), after
+    every step; the device applies Keras SGD's `decay` to it.  `on_epoch_begin` gets the absolute epoch, so a step
+    schedule resumed with --initial_epoch continues where it left off; like the reference, a resumed run otherwise
+    starts with fresh callback state (a new SGDR or CLR cycle, an empty plateau history).  ReduceLROnPlateau monitors
+    Keras' val_loss, which includes the L2 regularisation term (the logged val_loss does not).  With data parallelism
+    rank 0's rate is broadcast to every rank at the start of every epoch: the ranks validate with their own BatchNorm
+    statistics and could otherwise disagree on a plateau."""
+    from .keras_callbacks import OptimizerLR
+    from .parallel import broadcast_parameters
+    optimizer_lr = None
+    if hasattr(sched, 'set_optimizer_lr'):
+        optimizer_lr = OptimizerLR(args.sgd_lr)
+        sched.set_optimizer_lr(optimizer_lr)
+    if rank != 0 and hasattr(sched, 'verbose'):
+        sched.verbose = 0                       # the "reducing learning rate" message comes from rank 0 only
+    per_batch = getattr(sched, 'on_batch_end', None)
+
+    def on_step(batch):
+        per_batch(batch)
+        eng.set_lr(sched.lr)
+
     monitor = args.snapshot_best
     best = None
+    sched.on_train_begin()
     for epoch in range(args.initial_epoch, epochs):
-        eng.set_lr(sched.lr)
-        logs = train_epoch(eng, data, args.batch_size, rng, rank, world, train_ks)
+        if hasattr(sched, 'on_epoch_begin'):
+            sched.on_epoch_begin(epoch)
+        lr = sched.lr
+        eng.set_lr(lr)
+        if world > 1:
+            broadcast_parameters([eng.lr_dev])
+            if rank != 0 and optimizer_lr is not None:
+                optimizer_lr.set_value(float(eng.lr_dev[0].item()))
+                lr = sched.lr
+        logs = train_epoch(eng, data, args.batch_size, rng, rank, world, train_ks,
+                           on_step if per_batch is not None else None)
         val, _ = run_validation(eng, data, ks, None)
         logs.update({'val_' + k: v for k, v in val.items()})
         logs['val_loss'] = val.get('total', val['loss'])
         if rank == 0:
-            say('Epoch {}/{} - lr {:.6f} - '.format(epoch + 1, epochs, sched.lr) + format_logs(logs))
+            say('Epoch {}/{} - lr {:.6f} - '.format(epoch + 1, epochs, lr) + format_logs(logs))
             report_fallbacks(data, say)
             if args.snapshot:
                 cur = logs.get(monitor) if monitor else None
@@ -230,7 +265,10 @@ def fit(eng, data, args, sched, epochs, rng, rank, world, ks, say, train_ks=()):
                     with open(args.snapshot, 'wb') as f:
                         pickle.dump({'weights': eng.get_weights(), 'velocity': eng.get_velocity(), 'epoch': epoch + 1,
                                      'iterations': eng.iterations, 'architecture': args.architecture}, f)
-        sched.on_epoch_end(epoch)
+        cb_logs = dict(logs)
+        if getattr(sched, 'monitor', None) == 'val_loss':
+            cb_logs['val_loss'] = logs['val_loss'] + l2_term(eng)
+        sched.on_epoch_end(epoch, cb_logs)
 
 
 def average_accuracy(pred, labels):

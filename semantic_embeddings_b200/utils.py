@@ -9,6 +9,8 @@ import numpy as np
 
 from . import _lib
 from .models import cifar_resnet, plainnet, resnet50, wide_residual_network as wrn
+from .clr_callback import CyclicLR
+from .keras_callbacks import LearningRateScheduler, ReduceLROnPlateau
 from .sgdr_callback import SGDR
 
 # utils.py:26-28 lists more names; the ones below are the architectures of the hot path (BASELINE.json configs)
@@ -157,9 +159,44 @@ def feature_layer(graph):
 
 
 def get_lr_schedule(schedule, num_samples, batch_size, schedule_args={}):
-    """utils.py:288-399.  Returns ([schedule objects], suggested number of epochs).  Only the SGDR branch
-    (utils.py:357-368, the default of learn_image_embeddings.py:67) is on the hot path."""
-    if schedule.lower() == 'sgdr':
+    """utils.py:288-399.  Returns ([schedule objects], suggested number of epochs); fills the defaults of the chosen
+    branch into `schedule_args` in place, as the reference does.
+      'sgd' with an `sgd_schedule` of 1-based `epoch:lr` points (a point without a rate keeps the current rate; the
+            last point may be a bare epoch count): LearningRateScheduler, last point + 1 epochs;
+      'sgd' otherwise: ReduceLROnPlateau on val_loss (sgd_patience 10, sgd_min_lr 1e-4), 200 epochs;
+      'sgdr': SGDR (sgdr_base_len 12, sgdr_mul 2, sgdr_max_lr 0.1), five cycles;
+      'clr': triangular CyclicLR (clr_step_len 12 epochs per half cycle, clr_min_lr 1e-5, clr_max_lr 0.1),
+             clr_step_len * 20 epochs;
+      'resnet-schedule': 0.01 for epoch 0, 0.1 until 80, 0.01 until 120, then 0.001; 164 epochs.
+    The SGD-step and plateau schedules start from the optimizer's rate (--sgd_lr).  One deviation: an `sgd_schedule`
+    whose bare epoch count equals the epoch of a point with a rate ('1:0.1,2:0.01,2') trains, where the reference's sort
+    fails to compare None with a float."""
+    if schedule.lower() == 'sgd':
+        if ('sgd_schedule' in schedule_args) and (schedule_args['sgd_schedule'] is not None) and \
+                (schedule_args['sgd_schedule'] != ''):
+
+            def lr_scheduler(schedule, epoch, cur_lr):
+                if schedule[0][0] > epoch:
+                    return cur_lr
+                for i in range(1, len(schedule)):
+                    if schedule[i][0] > epoch:
+                        return schedule[i - 1][1] if schedule[i - 1][1] is not None else cur_lr
+                return schedule[-1][1] if schedule[-1][1] is not None else cur_lr
+
+            points = [(int(point[0]) - 1, float(point[1]) if len(point) > 1 else None)
+                      for sched_tuple in schedule_args['sgd_schedule'].split(',') for point in [sched_tuple.split(':')]]
+            # the reference's points.sort() raises TypeError under Python 3 when a point without a rate shares its epoch
+            # with one that has a rate (e.g. the trailing count of '1:0.1,2:0.01,2'); rate-less points go first there
+            points.sort(key=lambda p: (p[0], p[1] is not None, p[1] or 0.0))
+            return [LearningRateScheduler(lambda ep, cur_lr: lr_scheduler(points, ep, cur_lr))], points[-1][0] + 1
+        else:
+            if 'sgd_patience' not in schedule_args:
+                schedule_args['sgd_patience'] = 10
+            if 'sgd_min_lr' not in schedule_args:
+                schedule_args['sgd_min_lr'] = 1e-4
+            return [ReduceLROnPlateau('val_loss', patience=schedule_args['sgd_patience'], epsilon=1e-4,
+                                      min_lr=schedule_args['sgd_min_lr'], verbose=True)], 200
+    elif schedule.lower() == 'sgdr':
         if 'sgdr_base_len' not in schedule_args:
             schedule_args['sgdr_base_len'] = 12
         if 'sgdr_mul' not in schedule_args:
@@ -170,9 +207,31 @@ def get_lr_schedule(schedule, num_samples, batch_size, schedule_args={}):
             [SGDR(1e-6, schedule_args['sgdr_max_lr'], schedule_args['sgdr_base_len'], schedule_args['sgdr_mul'])],
             sum(schedule_args['sgdr_base_len'] * (schedule_args['sgdr_mul'] ** i) for i in range(5))
         )
-    elif schedule.lower() in ('sgd', 'clr', 'resnet-schedule'):
-        raise NotImplementedError('LR schedule {} exists in the reference (utils.py:326-391) but is outside the '
-                                  'accelerated hot path'.format(schedule))
+    elif schedule.lower() == 'clr':
+        if 'clr_step_len' not in schedule_args:
+            schedule_args['clr_step_len'] = 12
+        if 'clr_min_lr' not in schedule_args:
+            schedule_args['clr_min_lr'] = 1e-5
+        if 'clr_max_lr' not in schedule_args:
+            schedule_args['clr_max_lr'] = 0.1
+        return (
+            [CyclicLR(schedule_args['clr_min_lr'], schedule_args['clr_max_lr'],
+                      schedule_args['clr_step_len'] * (num_samples // batch_size), mode='triangular')],
+            schedule_args['clr_step_len'] * 20
+        )
+    elif schedule.lower() == 'resnet-schedule':
+
+        def resnet_scheduler(epoch):
+            if epoch >= 120:
+                return 0.001
+            elif epoch >= 80:
+                return 0.01
+            elif epoch >= 1:
+                return 0.1
+            else:
+                return 0.01
+
+        return [LearningRateScheduler(resnet_scheduler)], 164
     else:
         raise ValueError('Unknown learning rate schedule: {}'.format(schedule))
 
