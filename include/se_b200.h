@@ -254,6 +254,23 @@ int se_embed_head_fwd_bwd_ex(const float* z, int ldz, const int32_t* labels, con
 int se_devise_rank_fwd_bwd(const float* z, int ldz, const int32_t* labels, const float* E, int ldE, int B, int D, int C,
                            int loss_kind, float loss_scale, const float* extra_dx, float* x_out, float* loss, float* acc,
                            float* dz, float* rank_out, float margin, void* stream);
+/* Which launch configuration the three head entry points above take for (B, D, C, loss_kind): pure host-side planning,
+ * callable without a GPU; the launcher decides by the same function.  want_metrics: acc or rank_out is requested; for
+ * SE_LOSS_DEVISE_RANK the loss or dz is taken to be requested (the ranking loss' pass over the classes).  vec: z, E and
+ * x_out are 16-byte aligned and ldz, ldE are multiples of 4.  Bits 0-1 name the configuration, bit 2 the float4 variant
+ * (vec and D % 4 == 0, else scalar loads):
+ *   SE_HEAD_SMEM   one warp per row, the class matrix staged in shared memory (pitch D+1): needs
+ *                  16 Dp + 4 C (D+1) [+ 4 * 4 ceil(C/32) for the ranking loss' masks] <= 48 KB, Dp = D rounded up to 4
+ *   SE_HEAD_SPLIT  one CTA of 8 warps per row, the warps share the loop over the classes, E read from global memory:
+ *                  Dp <= 1536, or Dp <= 1532 with the ranking loss' mask (32 Dp + 4 ceil(C/32) <= 48 KB)
+ *   SE_HEAD_WARP   one warp per row, E (if read) from global memory: every other D <= 3072 (16 Dp [+ 16 ceil(C/32)]
+ *                  <= 48 KB), and every call that reads no class matrix (no metrics, SE_LOSS_SOFTMAX_CORR)
+ * Returns SE_ERR_ARG where the entry points refuse: D > 3072, a ranking loss whose masks do not fit, B, D or C <= 0. */
+#define SE_HEAD_WARP 0
+#define SE_HEAD_SMEM 1
+#define SE_HEAD_SPLIT 2
+#define SE_HEAD_VEC 4
+int se_embed_head_path(int B, int D, int C, int loss_kind, int want_metrics, int vec);
 /* softmax + Keras categorical_crossentropy (clip 1e-7) + argmax accuracy + backward
  * (learn_image_embeddings.py:44,230-231): dlogits = scale * dCE/dlogits. */
 int se_softmax_xent_fwd_bwd(const float* logits, int ld, const int32_t* labels, int B, int C, float scale,

@@ -24,6 +24,9 @@ SE_COL_SQNORM, SE_COL_CENTER = 0, 1
 SE_DEV_SIM, SE_DEV_DIST = 0, 1
 # se_bn_bwd_path: bits 0-1 = path (0 reduce + apply, 1 shared-memory slab, 2 register slab), bit 2 = float4 / fixed quad
 SE_BN_BWD_SCALAR, SE_BN_BWD_SLAB_ATOMIC, SE_BN_BWD_SLAB_REG, SE_BN_BWD_VEC, SE_BN_BWD_SLAB_QUAD = 0, 1, 2, 4, 5
+# se_embed_head_path: bits 0-1 = configuration (one warp per row, class matrix in shared memory, one CTA per row),
+# bit 2 = float4 loads
+SE_HEAD_WARP, SE_HEAD_SMEM, SE_HEAD_SPLIT, SE_HEAD_VEC = 0, 1, 2, 4
 
 # opcodes of se_run_ops (csrc/opcodes.h)
 OP_CONV_FWD, OP_CONV_DGRAD, OP_CONV_WGRAD, OP_BN_STATS, OP_BN_FWD_TRAIN, OP_BN_FWD_INFER, OP_BN_BWD, \
@@ -137,6 +140,7 @@ _SIGS = {
     'se_embed_head_fwd_bwd_ex': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P]),
     'se_devise_rank_fwd_bwd': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P,
                                        c_float, _P]),
+    'se_embed_head_path': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int]),
     'se_labelembed_workspace_bytes': (c_int64, [c_int, c_int]),
     'se_labelembed_fwd_bwd': (c_int, [_P, _P, c_int, _P, _P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, _P, _P,
                                       _P, _P, _P, _P, _P]),

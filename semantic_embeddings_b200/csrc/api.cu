@@ -75,7 +75,7 @@ extern "C" const char* se_version(void) { return "se_b200 0.1 (sm_90a)"; }
 extern "C" const char* se_last_error(void) { return g_err; }
 extern "C" int64_t se_launch_count(void) { return g_launches.load(); }
 extern "C" int se_device_sm_count(void) { return sm_count(); }
-namespace se { int init_conv_simt(); int init_pairwise_tc(); int init_conv_tc(); int init_conv_wgrad_tc(); }
+namespace se { int init_conv_simt(); int init_pairwise_tc(); int init_conv_tc(); int init_conv_wgrad_tc(); int init_head(); }
 // One-time per-process setup that must not happen inside a CUDA-graph capture: device query and the
 // cudaFuncSetAttribute calls of every kernel that needs more than 48 KB of dynamic shared memory.
 static bool side_stream_ready();
@@ -87,6 +87,7 @@ extern "C" int se_init(void) {
   if (rc == SE_OK) rc = se::init_pairwise_tc();
   if (rc == SE_OK) rc = se::init_conv_tc();
   if (rc == SE_OK) rc = se::init_conv_wgrad_tc();
+  if (rc == SE_OK) rc = se::init_head();
   if (rc == SE_OK) side_stream_ready();      // side stream + fork/join events of se_run_ops exist before any graph capture
   if (rc == SE_OK) rc = prepare_side_workspace();   // and the weight-gradient workspace of that stream
   return rc;

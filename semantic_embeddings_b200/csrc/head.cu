@@ -76,10 +76,12 @@ embed_head_kernel(const float* __restrict__ z, int ldz, const int* __restrict__ 
     for (int i = lane; i < (D >> 2); i += 32) {
       float4 v = ldg_nc_f4(zr + 4 * i);
       *reinterpret_cast<float4*>(xs + 4 * i) = v;
-      ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+      // an explicit chain, so that the mse metric's |x|^2 can be restated bit for bit (a bare x*x + y*y + ... may be
+      // contracted either way; this is the order nvcc chose for it, so the bits are those of that expression)
+      ss += fmaf(v.w, v.w, fmaf(v.z, v.z, fmaf(v.x, v.x, __fmul_rn(v.y, v.y))));
     }
   } else {
-    for (int i = lane; i < D; i += 32) { float v = zr[i]; xs[i] = v; ss += v * v; }
+    for (int i = lane; i < D; i += 32) { float v = zr[i]; xs[i] = v; ss = fmaf(v, v, ss); }
   }
   ss = warp_sum(ss);
   float inv = 1.f;
@@ -394,40 +396,81 @@ extern "C" int se_embed_head_fwd_bwd(const float* z, int ldz, const int32_t* lab
                                   nullptr, stream);
 }
 
+// The launch configuration of embed_head_kernel (se_embed_head_path): host arithmetic only, shared by the launcher and
+// the query so that the two cannot differ.  want_metrics: acc or rank_out is written; rank: the ranking loss' pass over
+// the classes (its bit mask of active classes takes (C+31)/32 words per row).  Either reads the class matrix.
+struct HeadPlan {
+  int path = SE_HEAD_WARP;   // SE_HEAD_WARP / SE_HEAD_SMEM / SE_HEAD_SPLIT, | SE_HEAD_VEC
+  int nwarps = HEAD_WARPS, split = 0, es_classes = 0, grid = 0;
+  size_t smem = 0;
+};
+
+static int head_plan(int B, int D, int C, int loss_kind, bool want_metrics, bool rank, bool vec, HeadPlan* hp) {
+  SE_REQUIRE(B > 0 && D > 0 && C > 0, "bad arguments");
+  const int Dp = (D + 3) & ~3;
+  size_t smem = (size_t)HEAD_WARPS * Dp * sizeof(float);
+  SE_REQUIRE(smem <= 48 * 1024, "D too large for the fused head (max 3072)");
+  HeadPlan p;
+  p.grid = ceil_div(B, HEAD_WARPS);
+  const size_t es_bytes = (size_t)C * (D + 1) * sizeof(float);
+  const size_t mask_row = rank ? (size_t)((C + 31) / 32) * sizeof(unsigned) : 0;
+  const bool need_E = (want_metrics || rank) && loss_kind != SE_LOSS_SOFTMAX_CORR;
+  if (need_E && smem + es_bytes + HEAD_WARPS * mask_row <= 48 * 1024) {
+    p.path = SE_HEAD_SMEM; p.es_classes = C; smem += es_bytes + HEAD_WARPS * mask_row;
+  } else if (need_E && (size_t)HEAD_WARPS_SPLIT * Dp * sizeof(float) + mask_row <= 48 * 1024) {
+    // the class matrix stays in global memory: the loop over it is latency-bound per warp, so a row gets a whole CTA
+    p.path = SE_HEAD_SPLIT; p.split = 1; p.nwarps = HEAD_WARPS_SPLIT; p.grid = B;
+    smem = (size_t)HEAD_WARPS_SPLIT * Dp * sizeof(float) + mask_row;
+  } else {
+    smem += HEAD_WARPS * mask_row;
+  }
+  SE_REQUIRE(smem <= 48 * 1024, "too many classes for the ranking loss' active-set mask");
+  p.smem = smem;
+  if (vec && D % 4 == 0) p.path |= SE_HEAD_VEC;
+  *hp = p;
+  return p.path;
+}
+
+extern "C" int se_embed_head_path(int B, int D, int C, int loss_kind, int want_metrics, int vec) {
+  SE_REQUIRE(loss_kind >= 0 && loss_kind <= SE_LOSS_DEVISE_RANK, "unknown loss kind");
+  HeadPlan p;
+  return head_plan(B, D, C, loss_kind, want_metrics != 0, loss_kind == SE_LOSS_DEVISE_RANK, vec != 0, &p);
+}
+
+// The plans allow up to 48 KB of dynamic shared memory; the kernel's static s_red / s_hinge come on top of that, past
+// the default limit of 48 KB in all (a row split over 8 warps at Dp = 1532 or 1536, and a warp per row at Dp > 3060,
+// failed to launch).  Called by se_init, before any graph capture; a standalone first call makes it then.
+static bool g_head_inited = false;
+namespace se {
+int init_head() {
+  for (const void* k : {(const void*)embed_head_kernel<true>, (const void*)embed_head_kernel<false>})
+    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024) != cudaSuccess) {
+      set_error("init_head: cannot raise the shared-memory limit");
+      return SE_ERR_CUDA;
+    }
+  g_head_inited = true;
+  return SE_OK;
+}
+}  // namespace se
+
 static int embed_head(const float* z, int ldz, const int32_t* labels, const float* E, int ldE, int B, int D, int C,
                       int loss_kind, float loss_scale, const float* extra_dx, float* x_out, float* loss, float* acc,
                       float* dz, float* rank_out, float margin, void* stream) {
   SE_REQUIRE(z && labels && E && B > 0 && D > 0 && C > 0, "bad arguments");
   SE_REQUIRE(ldz >= D && ldE >= D, "leading dimension smaller than D");
-  SE_REQUIRE(loss_kind != SE_LOSS_SOFTMAX_CORR || C >= 1, "bad arguments");
-  const int Dp = (D + 3) & ~3;
-  size_t smem = (size_t)HEAD_WARPS * Dp * sizeof(float);
-  SE_REQUIRE(smem <= 48 * 1024, "D too large for the fused head (max 3072)");
-  int nwarps = HEAD_WARPS, split = 0;
   auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-  bool vec = (D % 4 == 0) && (ldz % 4 == 0) && (ldE % 4 == 0) && al16(z) && al16(E) && (!x_out || al16(x_out));
-  int grid = ceil_div(B, HEAD_WARPS);
-  int es_classes = 0;
-  const size_t es_bytes = (size_t)C * (D + 1) * sizeof(float);
-  // the ranking loss reads the class matrix for its hinge terms and keeps a bit mask of the active classes per row
-  const bool rank = loss_kind == SE_LOSS_DEVISE_RANK && (loss || dz);
-  const size_t mask_row = rank ? (size_t)((C + 31) / 32) * sizeof(unsigned) : 0;
-  const bool need_E = (acc || rank_out || rank) && loss_kind != SE_LOSS_SOFTMAX_CORR;
-  if (need_E && smem + es_bytes + HEAD_WARPS * mask_row <= 48 * 1024) {
-    es_classes = C; smem += es_bytes + HEAD_WARPS * mask_row;
-  } else if (need_E && (size_t)HEAD_WARPS_SPLIT * Dp * sizeof(float) + mask_row <= 48 * 1024) {
-    // the class matrix stays in global memory: the loop over it is latency-bound per warp, so a row gets a whole CTA
-    split = 1; nwarps = HEAD_WARPS_SPLIT; grid = B; smem = (size_t)HEAD_WARPS_SPLIT * Dp * sizeof(float) + mask_row;
-  } else {
-    smem += HEAD_WARPS * mask_row;
-  }
-  SE_REQUIRE(smem <= 48 * 1024, "too many classes for the ranking loss' active-set mask");
-  if (vec)
-    launch(embed_head_kernel<true>, dim3(grid), dim3(nwarps * 32), smem, as_stream(stream), z, ldz, labels, E, ldE, B, D, C, loss_kind,
-           loss_scale, extra_dx, x_out, loss, acc, dz, rank_out, es_classes, split, margin);
+  const bool vec = (D % 4 == 0) && (ldz % 4 == 0) && (ldE % 4 == 0) && al16(z) && al16(E) && (!x_out || al16(x_out));
+  HeadPlan p;
+  const int rc = head_plan(B, D, C, loss_kind, acc || rank_out, loss_kind == SE_LOSS_DEVISE_RANK && (loss || dz), vec,
+                           &p);
+  if (rc < 0) return rc;
+  if (!g_head_inited) { const int irc = init_head(); if (irc) return irc; }
+  if (p.path & SE_HEAD_VEC)
+    launch(embed_head_kernel<true>, dim3(p.grid), dim3(p.nwarps * 32), p.smem, as_stream(stream), z, ldz, labels, E, ldE, B,
+           D, C, loss_kind, loss_scale, extra_dx, x_out, loss, acc, dz, rank_out, p.es_classes, p.split, margin);
   else
-    launch(embed_head_kernel<false>, dim3(grid), dim3(nwarps * 32), smem, as_stream(stream), z, ldz, labels, E, ldE, B, D, C, loss_kind,
-           loss_scale, extra_dx, x_out, loss, acc, dz, rank_out, es_classes, split, margin);
+    launch(embed_head_kernel<false>, dim3(p.grid), dim3(p.nwarps * 32), p.smem, as_stream(stream), z, ldz, labels, E, ldE,
+           B, D, C, loss_kind, loss_scale, extra_dx, x_out, loss, acc, dz, rank_out, p.es_classes, p.split, margin);
   return check_launch("embed_head_kernel");
 }
 

@@ -180,6 +180,12 @@ class Engine:
             self.C, self.D = emb.shape
             if graph.output.shape != (self.D,):
                 raise ValueError('network output %s does not match the %d-d class embeddings' % (graph.output.shape, self.D))
+            # the fused head takes at most 3072 dimensions (fewer for the ranking loss' active-set masks): refuse such a
+            # matrix here, not with an error from inside the first captured step
+            if self.lib.se_embed_head_path(self.B, self.D, self.C, LOSS_KINDS[loss], 1, 1) < 0:
+                raise ValueError('the class embedding is %d x %d: the fused embedding head takes at most 3072 dimensions, '
+                                 'fewer with the ranking loss (%s)'
+                                 % (self.C, self.D, self.lib.se_last_error().decode('utf-8', 'replace')))
             self.E = torch.from_numpy(np.ascontiguousarray(emb)).to(self.dev)
         self.num_classes = int(num_classes or self.C)
         self._extend_graph()

@@ -51,34 +51,95 @@ def _f32_fma(s, a, b):
     return np.where(fix, nb, r).astype(np.float32)
 
 
-def kernel_similarities(E, Z):
-    """The head kernels' fp32 scores <z,E_c>: one sequential fmaf chain over the dimensions (float32 numpy (B, C))."""
+def _f32_fma_t(s, a, b):
+    """_f32_fma on float32 torch tensors (CPU or CUDA): the same float64 arithmetic, element by element."""
+    s64 = s.double()
+    p = a.double() * b.double()
+    hi = s64 + p
+    bb = hi - s64
+    lo = (s64 - (hi - bb)) + (p - bb)
+    r = hi.float()
+    d = hi - r.double()
+    nb = torch.nextafter(r, torch.where(d > 0, torch.full_like(r, math.inf), torch.full_like(r, -math.inf)))
+    fix = (d != 0) & (2.0 * d == nb.double() - r.double()) & (lo != 0) & (torch.sign(lo) == torch.sign(d))
+    return torch.where(fix, nb, r)
+
+
+def kernel_similarities(E, Z, device=None):
+    """The head kernels' fp32 scores <z,E_c>: one sequential fmaf chain over the dimensions (float32 numpy (B, C)).
+    device: compute with torch there (the same values; a CUDA device makes the 8142-class matrices cheap)."""
     E, Z = np.asarray(E, np.float32), np.asarray(Z, np.float32)
+    if device is not None:
+        Et, Zt = torch.as_tensor(E, device=device), torch.as_tensor(Z, device=device)
+        sim = torch.zeros((Z.shape[0], E.shape[0]), dtype=torch.float32, device=device)
+        for i in range(Z.shape[1]):
+            sim = _f32_fma_t(sim, Zt[:, i:i + 1], Et[None, :, i])
+        return sim.cpu().numpy()
     sim = np.zeros((Z.shape[0], E.shape[0]), np.float32)
     for i in range(Z.shape[1]):
         sim = _f32_fma(sim, Z[:, i:i + 1], E[None, :, i])
     return sim
 
 
-def kernel_hinges(E, T, Z, margin):
-    """se_devise_rank_fwd_bwd's fp32 hinge arguments: (m - <t,z>) + <z,E_c> with <t,z> summed as warp_dot does
-    (lane-strided float4 or scalar chains, then the xor-shuffle tree) and <z,E_c> as kernel_similarities."""
-    E, T, Z = (np.asarray(a, np.float32) for a in (E, T, Z))
-    B, D = Z.shape
-    vec = D % 4 == 0
-    lanes = np.zeros((B, 32), np.float32)
+def kernel_warp_chains(A, Bm, vec):
+    """The 32 lane sums of the head kernel's lane-strided fmaf chains over a row pair (float32 (rows, 32)): lane l takes
+    the float4 groups g = l, l+32, ... in the order x, y, z, w (vec), or the elements i = l, l+32, ... (scalar)."""
+    A, Bm = np.asarray(A, np.float32), np.asarray(Bm, np.float32)
+    rows, D = A.shape
+    lanes = np.zeros((rows, 32), np.float32)
     for lane in range(32):
         if vec:
             for g in range(lane, D // 4, 32):
                 for j in range(4):
-                    lanes[:, lane] = _f32_fma(lanes[:, lane], Z[:, 4 * g + j], T[:, 4 * g + j])
+                    lanes[:, lane] = _f32_fma(lanes[:, lane], A[:, 4 * g + j], Bm[:, 4 * g + j])
         else:
             for i in range(lane, D, 32):
-                lanes[:, lane] = _f32_fma(lanes[:, lane], Z[:, i], T[:, i])
+                lanes[:, lane] = _f32_fma(lanes[:, lane], A[:, i], Bm[:, i])
+    return lanes
+
+
+def warp_sum(lanes):
+    """common.cuh warp_sum: the xor-shuffle tree over the 32 lanes, lane 0's result (float32 (rows,))."""
+    lanes = np.asarray(lanes, np.float32)
     for o in (16, 8, 4, 2, 1):
         lanes = (lanes + lanes[:, np.arange(32) ^ o]).astype(np.float32)
-    base = (np.float32(margin) - lanes[:, 0]).astype(np.float32)
-    return (base[:, None] + kernel_similarities(E, Z)).astype(np.float32)
+    return lanes[:, 0]
+
+
+def kernel_hinges(E, T, Z, margin, device=None):
+    """se_devise_rank_fwd_bwd's fp32 hinge arguments: (m - <t,z>) + <z,E_c> with <t,z> summed as warp_dot does
+    (lane-strided float4 or scalar chains, then the xor-shuffle tree) and <z,E_c> as kernel_similarities."""
+    E, T, Z = (np.asarray(a, np.float32) for a in (E, T, Z))
+    tz = warp_sum(kernel_warp_chains(Z, T, Z.shape[1] % 4 == 0))
+    base = (np.float32(margin) - tz).astype(np.float32)
+    return (base[:, None] + kernel_similarities(E, Z, device)).astype(np.float32)
+
+
+def kernel_sqnorm(Z, vec):
+    """The head kernel's fp32 sum of squares of z (embed_head_kernel's ss: per lane y*y, then fmaf of x, z, w per float4
+    group, or one fmaf chain (scalar); then warp_sum).  The mse metric's |x|^2 (float32 (B,))."""
+    Z = np.asarray(Z, np.float32)
+    if not vec:
+        return warp_sum(kernel_warp_chains(Z, Z, False))
+    rows, D = Z.shape
+    lanes = np.zeros((rows, 32), np.float32)
+    for lane in range(32):
+        for g in range(lane, D // 4, 32):
+            x, y, z, w = (Z[:, 4 * g + j] for j in range(4))
+            t = (y * y).astype(np.float32)
+            for v in (x, z, w):
+                t = _f32_fma(t, v, v)
+            lanes[:, lane] = (lanes[:, lane] + t).astype(np.float32)
+    return warp_sum(lanes)
+
+
+def kernel_class_sqnorms(E):
+    """The accuracy loop's fp32 |E_c|^2: one sequential fmaf chain over the dimensions (float32 (C,))."""
+    E = np.asarray(E, np.float32)
+    en = np.zeros(E.shape[0], np.float32)
+    for i in range(E.shape[1]):
+        en = _f32_fma(en, E[:, i], E[:, i])
+    return en
 
 
 def gradient_from_active(E, T, active, scale):

@@ -399,7 +399,13 @@ def metrics(ctx, node, out):
                   the target's (utils.top_k_acc)
       labelembed  out1: acc = argmax == label, 0 on padding rows
       head        the wrapped output: fp32 scores <x,E_c> (devise_oracle.kernel_similarities); acc = the best score within
-                  1e-6 of the true class' (utils.nn_accuracy), rank = classes better by >= 1e-6, or C when none is within"""
+                  1e-6 of the true class' (utils.nn_accuracy), rank = classes better by >= 1e-6, or C when none is within.
+                  mse: the score is -(|x|^2 + |E_c|^2 - 2 <x,E_c>) in fp32, each term summed as the kernel sums it
+                  (devise_oracle.kernel_sqnorm with the float4 chains when D % 4 == 0: the engine's tensors are 16-byte
+                  aligned; kernel_class_sqnorms).  softmax_corr: Keras categorical accuracy, argmax x == argmax t (first
+                  maximum), rank = outputs strictly above the one at argmax t
+    The fp32 scores are computed on out's device."""
+    dev = out.device if torch.is_tensor(out) and out.is_cuda else None
     o = out.detach().float().cpu().numpy()
     y = ctx.labels.cpu().numpy()
     rows = np.arange(len(y))
@@ -410,9 +416,16 @@ def metrics(ctx, node, out):
     if node.op == 'labelembed':
         return ((o.argmax(-1) == y) & (y >= 0)).astype(np.float64), None
     if node.op == 'head':
-        if ctx.kind not in ('inv_corr', 'unnorm_corr', 'devise_rank'):
-            raise NotImplementedError('metrics of the %s head' % ctx.kind)
-        sim = devise_oracle.kernel_similarities(_np(ctx.E), o)
+        E = _np(ctx.E).astype(np.float32)
+        if ctx.kind == 'softmax_corr':
+            tgt = E[y].argmax(-1)
+            own = o[rows, tgt]
+            return (o.argmax(-1) == tgt).astype(np.float64), (o > own[:, None]).sum(-1).astype(np.float64)
+        sim = devise_oracle.kernel_similarities(E, o, dev)
+        if ctx.kind == 'mse':
+            xn = devise_oracle.kernel_sqnorm(o, o.shape[1] % 4 == 0)
+            en = devise_oracle.kernel_class_sqnorms(E)
+            sim = -((xn[:, None] + en[None, :]).astype(np.float32) - np.float32(2) * sim)
         mine = sim[rows, y]
         acc = np.abs(sim.max(-1) - mine) < np.float32(1e-6)
         within = np.abs(sim - mine[:, None]) < np.float32(1e-6)
@@ -544,6 +557,54 @@ CONFIGS_448 = [
 ]
 
 
+# ResNet-50 at 224 px with the large class matrices (learn_image_embeddings.py / learn_classifier.py on ILSVRC and
+# iNaturalist; test_gpu_step_layers_classes.py) at the recipes' per-GPU batch of 64 (README: 128 on 2 GPUs).  The head
+# takes one CTA per row (SE_HEAD_SPLIT) on all three embedding matrices, with float4 loads except at iNat2019's 1010
+# dimensions; test_cpu_plan_classes.py pins that.
+CONFIGS_CLASSES = [
+    # README: ILSVRC with imagenet_mintree.unitsphere, inv_corr, --cls_weight 0.1
+    ('resnet-50', 64, 'tf32x3', dict(tag='ilsvrc', class_matrix='ilsvrc', cls_weight=0.1)),
+    # iNaturalist 2018 with inat.sim1024 (8142 classes of 1024 dimensions) and the 8142-way classifier branch
+    ('resnet-50', 64, 'tf32x3', dict(tag='inat2018', class_matrix='inat2018-sim1024', cls_weight=0.1)),
+    # iNaturalist 2019 with its unitsphere matrix (1010 dimensions: scalar loads)
+    ('resnet-50', 64, 'tf32x3', dict(tag='inat2019', class_matrix='inat2019', cls_weight=0.1)),
+    # learn_classifier.py on iNaturalist 2018: 8142 classes, label smoothing 0.1
+    ('resnet-50', 64, 'tf32x3', dict(tag='inat2018-softmax', objective='softmax', num_classes=8142, label_smoothing=0.1,
+                                     clipnorm=10.0)),
+]
+
+_CLASS_MATRICES = {}
+
+
+def class_matrix(name, device='cuda'):
+    """A class-embedding matrix of the large-class recipes (float64 (C, D)), built once per process from the fixture's
+    hierarchies (tests/golden/class_embedding_ref.npz):
+      'ilsvrc'            imagenet_mintree.unitsphere: the Cholesky factor of 1 - D on the WordNet mintree, 1000 x 1000
+      'inat2019'          the same on the iNaturalist 2019 hierarchy, 1010 x 1010
+      'inat2018-sim1024'  inat.sim1024: approx_sim with 1024 dimensions of the 8142-class iNaturalist hierarchy, computed
+                          by class_embedding.embed_classes (its Jacobi solver runs on the GPU).  With device='cpu' (the
+                          plan tests, which depend on shapes only) a seeded stand-in of the same shape."""
+    import tempfile
+    import class_embedding_oracle as ceo
+    if name in ('ilsvrc', 'inat2019'):
+        key = name
+    elif name == 'inat2018-sim1024':
+        key = name if device != 'cpu' else name + '-standin'
+    else:
+        raise ValueError('unknown class matrix %r' % name)
+    if key not in _CLASS_MATRICES:
+        if name != 'inat2018-sim1024':
+            _CLASS_MATRICES[key] = ceo.unitsphere(1.0 - ceo.distance({'ilsvrc': 'mintree'}.get(name, name)))
+        elif device == 'cpu':
+            _CLASS_MATRICES[key] = np.random.RandomState(8142).randn(8142, 1024) / 32.0
+        else:
+            from semantic_embeddings_b200 import class_embedding
+            with tempfile.TemporaryDirectory() as tmp:
+                h, labels, _ = ceo.hierarchy('inat', tmp)
+                _CLASS_MATRICES[key] = class_embedding.embed_classes(h, labels, 'approx_sim', num_dim=1024)['embedding']
+    return _CLASS_MATRICES[key]
+
+
 def config_id(cfg):
     arch, B, mode, opts = cfg
     size = '-%dpx' % opts['input_size'] if opts.get('input_size') else ''
@@ -556,7 +617,8 @@ def build_engine(cfg, device='cuda:0', use_cuda_graph=True):
     utils.build_devise_network with that many classes before), 'embed_dim' (learn_labelembedding.py /
     learn_center_loss.py), 'fixed_centroids' (--centroids: a seeded C x D array, which the engine freezes), 'train'
     (the layers that train, as set_trainable(lambda name: name.split('/')[0] in train)) and 'input_size' (the side of
-    the square input, as the file datasets pass it; None: the architecture's default)."""
+    the square input, as the file datasets pass it; None: the architecture's default) and 'class_matrix' (a name of
+    class_matrix(); default: NAB's 555-d matrix for ResNet-50, CIFAR-100's for the CIFAR networks)."""
     import os
     from semantic_embeddings_b200 import _lib as L, utils
     from semantic_embeddings_b200.engine import Engine
@@ -566,10 +628,14 @@ def build_engine(cfg, device='cuda:0', use_cuda_graph=True):
     devise_classes, embed_dim = opts.pop('devise_classes', None), opts.pop('embed_dim', None)
     fixed, train = opts.pop('fixed_centroids', False), opts.pop('train', None)
     size = opts.pop('input_size', None)
+    matrix = opts.pop('class_matrix', None)
     objective = opts.get('objective', 'embedding')
     if objective == 'embedding':
-        key = 'nab' if arch == 'resnet-50' else 'cifar100'
-        emb = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'class_matrices.npz'))[key + '_embedding']
+        if matrix is not None:
+            emb = class_matrix(matrix, device)
+        else:
+            key = 'nab' if arch == 'resnet-50' else 'cifar100'
+            emb = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'class_matrices.npz'))[key + '_embedding']
         D = emb.shape[1]
         graph = utils.build_devise_network(D, arch, devise_classes, input_channels=3, input_size=size) if devise_classes \
             else utils.build_network(D, arch, input_channels=3, input_size=size)
