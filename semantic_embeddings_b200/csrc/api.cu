@@ -7,6 +7,7 @@
 #include <atomic>
 
 #include "common.cuh"
+#include "conv_plan.cuh"
 #include "opcodes.h"
 
 namespace se {
@@ -46,11 +47,6 @@ int sm_count() {
 int conv_fwd_simt(const se_conv_desc*, const float*, const float*, const float*, const float*, float*, int, double*, cudaStream_t);
 int conv_dgrad_simt(const se_conv_desc*, const float*, const float*, float*, float, cudaStream_t);
 int conv_wgrad_simt(const se_conv_desc*, const float*, const float*, float*, float*, cudaStream_t);
-// conv_tc.cu / conv_wgrad_tc.cu (wgmma TF32); each returns SE_ERR_UNSUPPORTED for shapes it does not cover
-int conv_fwd_tc(const se_conv_desc*, const float*, const float*, const float*, const float*, const float*, float*, int, double*,
-                cudaStream_t);
-int conv_dgrad_tc(const se_conv_desc*, const float*, const float*, const float*, float*, float, cudaStream_t);
-int conv_wgrad_tc(const se_conv_desc*, const float*, const float*, float*, float*, int x3, cudaStream_t);
 
 static int check_desc(const se_conv_desc* d) {
   if (!d) { set_error("null conv descriptor"); return SE_ERR_ARG; }
@@ -101,20 +97,15 @@ extern "C" int se_conv2d_fwd_aux(const se_conv_desc* d, const float* x, const fl
   int rc = check_desc(d);
   if (rc) return rc;
   SE_REQUIRE(x && w && y, "null pointer");
-  const bool tc1 = mode == SE_MODE_TF32 && aux && aux->w_t;
-  const bool tc3 = mode == SE_MODE_TF32X3 && aux && aux->w_t && aux->w_t_lo;
-  if (tc1 || tc3) {
-    const float* lo = tc3 ? aux->w_t_lo : nullptr;
-    rc = conv_fwd_tc(d, x, aux->w_t, lo, bias, residual, y, relu, stats, as_stream(stream));
-    if (rc == SE_ERR_UNSUPPORTED && stats) {
-      // wide layers (640 output channels): the per-warp statistics slots of the fused epilogue do not fit in shared
-      // memory -- run the tensor-core convolution without them and take the BatchNorm sums in a separate pass over y
-      rc = conv_fwd_tc(d, x, aux->w_t, lo, bias, residual, y, relu, nullptr, as_stream(stream));
-      if (rc == SE_OK) return se_bn_stats(y, (int64_t)d->N * d->Ho * d->Wo, d->Cout, stats, stream);
-    }
-    if (rc != SE_ERR_UNSUPPORTED) return rc;
-  }
-  return conv_fwd_simt(d, x, w, bias, residual, y, relu, stats, as_stream(stream));
+  ConvCall c;
+  c.w_t = aux && aux->w_t;
+  c.w_t_lo = aux && aux->w_t_lo;
+  c.stats = stats != nullptr;
+  ConvPlan pl;
+  if (conv_plan(d, 0, mode, c, &pl) == CONV_FP32) return conv_fwd_simt(d, x, w, bias, residual, y, relu, stats, as_stream(stream));
+  rc = conv_fwd_tc(pl, d, x, aux->w_t, aux->w_t_lo, bias, residual, y, relu, pl.fused_stats ? stats : nullptr, as_stream(stream));
+  if (rc || !stats || pl.fused_stats) return rc;
+  return se_bn_stats(y, (int64_t)d->N * d->Ho * d->Wo, d->Cout, stats, stream);
 }
 
 extern "C" int se_conv2d_fwd_ex(const se_conv_desc* d, const float* x, const float* w, const float* w_t,
@@ -162,31 +153,24 @@ extern "C" int se_conv2d_dgrad_aux(const se_conv_desc* d, const float* dy, const
   int rc = check_desc(d);
   if (rc) return rc;
   SE_REQUIRE(dy && w && dx, "null pointer");
-  if (mode == SE_MODE_TF32) {
-    rc = conv_dgrad_tc(d, dy, w, nullptr, dx, beta, as_stream(stream));
-    if (rc != SE_ERR_UNSUPPORTED) return rc;
-  } else if (mode == SE_MODE_TF32X3 && aux && aux->w_lo) {
-    rc = conv_dgrad_tc(d, dy, w, aux->w_lo, dx, beta, as_stream(stream));
-    if (rc != SE_ERR_UNSUPPORTED) return rc;
-  }
-  return conv_dgrad_simt(d, dy, w, dx, beta, as_stream(stream));
+  ConvCall c;
+  c.w_lo = aux && aux->w_lo;
+  c.beta = beta;
+  ConvPlan pl;
+  if (conv_plan(d, 1, mode, c, &pl) == CONV_FP32) return conv_dgrad_simt(d, dy, w, dx, beta, as_stream(stream));
+  return conv_dgrad_tc(pl, d, dy, w, c.w_lo ? aux->w_lo : nullptr, dx, beta, as_stream(stream));
 }
 extern "C" int se_conv2d_dgrad(const se_conv_desc* d, const float* dy, const float* w, float* dx, float beta, int mode,
                                void* stream) {
   return se_conv2d_dgrad_aux(d, dy, w, nullptr, dx, beta, mode, stream);
 }
 
-namespace se {
-bool conv_tc_would_run(const se_conv_desc* d, int dir, int x3);
-bool conv_wgrad_tc_would_run(const se_conv_desc* d, int x3);
-}
 extern "C" int se_conv2d_path(const se_conv_desc* d, int mode, int direction) {
   int rc = check_desc(d);
   if (rc) return rc;
   SE_REQUIRE(direction >= 0 && direction <= 2, "direction: 0 forward, 1 backward data, 2 weight gradient");
-  if (mode != SE_MODE_TF32 && mode != SE_MODE_TF32X3) return 0;
-  const int x3 = mode == SE_MODE_TF32X3;
-  return (direction == 2 ? conv_wgrad_tc_would_run(d, x3) : conv_tc_would_run(d, direction, x3)) ? 1 : 0;
+  ConvPlan pl;
+  return conv_plan(d, direction, mode, ConvCall(), &pl) == CONV_FP32 ? 0 : 1;
 }
 
 extern "C" int se_conv2d_wgrad(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias, int mode,
@@ -194,11 +178,13 @@ extern "C" int se_conv2d_wgrad(const se_conv_desc* d, const float* x, const floa
   int rc = check_desc(d);
   if (rc) return rc;
   SE_REQUIRE(x && dy && dw, "null pointer");
-  if (mode == SE_MODE_TF32 || mode == SE_MODE_TF32X3) {
-    rc = conv_wgrad_tc(d, x, dy, dw, dbias, mode == SE_MODE_TF32X3, as_stream(stream));
-    if (rc != SE_ERR_UNSUPPORTED) return rc;
-  }
-  return conv_wgrad_simt(d, x, dy, dw, dbias, as_stream(stream));
+  // the kernel stores dW / dbias as float2 / float4
+  ConvCall c;
+  c.aligned = (reinterpret_cast<uintptr_t>(dw) & 15) == 0 && (reinterpret_cast<uintptr_t>(dbias) & 15) == 0;
+  c.sms = sm_count();
+  ConvPlan pl;
+  if (conv_plan(d, 2, mode, c, &pl) == CONV_FP32) return conv_wgrad_simt(d, x, dy, dw, dbias, as_stream(stream));
+  return conv_wgrad_tc(pl, x, dy, dw, dbias, as_stream(stream));
 }
 
 static se_conv_desc dense_desc(int B, int Cin, int Cout) {

@@ -35,6 +35,7 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "conv_plan.cuh"
 #include "tc.cuh"
 
 namespace se {
@@ -45,27 +46,6 @@ constexpr int CT_BM = 128;
 constexpr int CT_THREADS = 384;        // warpgroup 0: TMA producer (one thread), warpgroups 1 and 2: MMA + epilogue
 constexpr int CT_MAX_STAGES = 6;
 constexpr int CT_SMEM_LIMIT = 227 * 1024;
-
-struct ConvTcParams {
-  int N, H, W;              // extent of the grid the pixel tiles cover (images, rows, pixels)
-  int Kc, Nc, BN;           // GEMM K channels (A tensor channels), GEMM N channels, output channels per tile
-  int Wb, Hb, Nb;           // pixel box, Wb*Hb*Nb == 128
-  int tw, th;               // tiles along a row / along the rows of an image
-  int cblk, kblocks;        // channels per pipeline stage (16 or 32), Kc / cblk
-  int taps, pad, flip;      // filter size (3 or 1), 'same' padding rows (1 or 0), 1: dgrad (tap order reversed for B)
-  int res;                  // 1: resident box (A loaded once per tile, stages hold B only), 0: per-tap stages
-  int ring_off;             // bytes of shared memory before the stage ring (the resident box)
-  int stages, stage_bytes, b_bytes;   // stage = [A of one tap (per-tap only)] B [B_lo (X3)]
-  int a_bytes, a_tx;        // one A tile (per-tap stage / channel block of the resident box): slot size, TMA bytes
-  long long o_sn, o_sh, o_sw;   // output (and residual) element strides of an image, a row, a pixel
-  int ovh, ovw;             // rows / pixels of the output view that exist (a strided view may be one short)
-  int relu;
-  float beta;               // dgrad: out = beta*out + D
-  const float* bias;
-  const float* residual;
-  float* out;
-  double* stats;
-};
 
 template <int BN>
 __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a, uint64_t b, int acc) {
@@ -342,34 +322,25 @@ static int pow2_ge(int v) { int q = 1; while (q < v) q <<= 1; return q; }
 // image sizes the 3x3 tiles take: rows of 4..56 pixels (every layer of the reference networks at their input sizes)
 static bool geometry_ok(int W) { return W >= 4 && W <= 56; }
 
-static bool tc_shape_ok(const se_conv_desc* d, int Kc, int Nc) {
-  if (d->kh != 3 || d->kw != 3 || d->stride != 1 || d->pad_t != 1 || d->pad_l != 1 || d->Ho != d->H || d->Wo != d->W)
-    return false;
-  if (Kc % 16 != 0 || Nc % 16 != 0) return false;
-  if (Kc > 16 && Kc % 32 != 0) return false;
-  return geometry_ok(d->W);
-}
+// GEMM channels the tiles take: K in one stage block of 16 or in blocks of 32, N in wgmma tiles of 16 or more
+static bool channels_ok(int Kc, int Nc) { return Kc % 16 == 0 && Nc % 16 == 0 && (Kc <= 16 || Kc % 32 == 0); }
 
-// 1x1 / stride 1 / no padding: a GEMM over the flat pixel list, any image size
-static bool tc_shape_ok_1x1(const se_conv_desc* d, int Kc, int Nc) {
-  if (d->kh != 1 || d->kw != 1 || d->stride != 1 || d->pad_t != 0 || d->pad_l != 0 || d->Ho != d->H || d->Wo != d->W)
-    return false;
-  if (Kc % 16 != 0 || Nc % 16 != 0) return false;
-  if (Kc > 16 && Kc % 32 != 0) return false;
-  return (long long)d->N * d->H * d->W >= CT_BM;
-}
-
-// 1x1 / stride 2 / no padding (the first convolution and the projection shortcut of a ResNet-50 stage, the shortcuts of
-// wide_residual_network.py:28): the GEMM of the 1x1 case over the (Ho, Wo) grid, the input (forward) or the output
-// (backward data) addressed through a tensor map of the sub-sampled VIEW x[:, ::2, ::2, :] (pixel and row strides
-// doubled) -- no gather pass.
-static bool tc_shape_ok_1x1_s2(const se_conv_desc* d, int Kc, int Nc) {
-  if (d->kh != 1 || d->kw != 1 || d->stride != 2 || d->pad_t != 0 || d->pad_l != 0 || d->Ho != (d->H + 1) / 2 ||
-      d->Wo != (d->W + 1) / 2)
-    return false;
-  if (Kc % 16 != 0 || Nc % 16 != 0) return false;
-  if (Kc > 16 && Kc % 32 != 0) return false;
-  return d->Wo <= 32 && geometry_ok(d->Wo);
+// The conv_tc_kernel family of a forward or data-gradient layer with GEMM channels Kc x Nc, by shape alone
+static ConvFamily tc_family(const se_conv_desc* d, int Kc, int Nc) {
+  if (!channels_ok(Kc, Nc)) return CONV_FP32;
+  if (d->kh == 3 && d->kw == 3 && d->stride == 1 && d->pad_t == 1 && d->pad_l == 1 && d->Ho == d->H && d->Wo == d->W)
+    return geometry_ok(d->W) ? CONV_TC_3X3 : CONV_FP32;
+  if (d->kh != 1 || d->kw != 1 || d->pad_t != 0 || d->pad_l != 0) return CONV_FP32;
+  // 1x1 / stride 1: a GEMM over the flat pixel list, any image size
+  if (d->stride == 1 && d->Ho == d->H && d->Wo == d->W)
+    return (long long)d->N * d->H * d->W >= CT_BM ? CONV_TC_1X1 : CONV_FP32;
+  // 1x1 / stride 2 (the first convolution and the projection shortcut of a ResNet-50 stage, the shortcuts of
+  // wide_residual_network.py:28): the GEMM of the 1x1 case over the (Ho, Wo) grid, the input (forward) or the output
+  // (backward data) addressed through a tensor map of the sub-sampled VIEW x[:, ::2, ::2, :] (pixel and row strides
+  // doubled) -- no gather pass.
+  if (d->stride == 2 && d->Ho == (d->H + 1) / 2 && d->Wo == (d->W + 1) / 2)
+    return d->Wo <= 32 && geometry_ok(d->Wo) ? CONV_TC_1X1_S2 : CONV_FP32;
+  return CONV_FP32;
 }
 
 // output channels per tile: the widest wgmma N that divides the channel count (<= 128; <= 64 in the error-compensated
@@ -380,35 +351,19 @@ static int pick_bn(int Nc, int x3) {
   return 0;
 }
 
-template <int BN>
-static void conv_tc_go(int x3, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& ma, const CUtensorMap& mb,
-                       const CUtensorMap& mbl, const ConvTcParams& p) {
-  if constexpr (BN <= 64)       // pick_bn: <= 64 channels per tile in the error-compensated mode
-    if (x3) return launch(conv_tc_kernel<BN, 1>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
-  launch(conv_tc_kernel<BN, 0>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
-}
-
-static int conv_tc_launch(const se_conv_desc* d, const float* a_tensor, int Kc, const float* bmat, int Nc, int flip,
-                          const float* bias, const float* residual, float* out, int relu, float beta, double* stats,
-                          cudaStream_t st, const float* bmat_lo = nullptr, int taps = 3, int s2 = 0, int x3_plan = -1,
-                          int out_view_w = 0, int out_view_h = 0) {
-  // out_view_w / out_view_h (s2 backward data only, 0 = Wo x Ho): extent of the sub-sampled output view that starts at
-  // `out` -- a caller that passes dx + (r*W + s)*Cin writes dx[:, r::2, s::2, :], whose last column / row may not exist:
-  // one tap of a 3x3 / stride 2 data gradient, conv_dgrad_tc below
-  // x3_plan >= 0: plan only (se_conv2d_path) -- the shape / shared-memory decisions below for arithmetic mode x3_plan,
-  // no pointers touched, nothing launched: SE_OK when this kernel would take the layer
-  // s2 (1x1 / stride 2): tiles over the (Ho, Wo) grid; forward reads the sub-sampled view of a_tensor, backward data
-  // (flip) writes the sub-sampled view of out (after zeroing it: the other three quarters of dx are zero)
-  ConvTcParams p;
+// The launch configuration of conv_tc_kernel for family f (of one tap, for the nine-tap data gradient): false when the
+// tiles, the grid or the shared memory do not fit.  flip: data gradient.
+static bool tc_config(const se_conv_desc* d, ConvFamily f, int Kc, int Nc, int flip, int x3, ConvPlan* pl) {
+  ConvTcParams& p = pl->tc;
+  const int taps = f == CONV_TC_3X3 ? 3 : 1;
+  const bool s2 = f == CONV_TC_1X1_S2 || f == CONV_TC_DGRAD_3X3S2;
   const int gW = s2 ? d->Wo : d->W, gH = s2 ? d->Ho : d->H;      // the grid the pixel tiles cover
-  const int x3 = x3_plan >= 0 ? x3_plan : (bmat_lo ? 1 : 0);   // error-compensated mode: bmat_lo = the low parts of bmat (se_split_filters)
   const long long total_px = (long long)d->N * gH * gW;
-  const bool flat = taps == 1 && !s2;
   p.taps = taps; p.pad = taps == 3 ? 1 : 0; p.flip = flip;
   p.N = d->N; p.H = gH; p.W = gW; p.Kc = Kc; p.Nc = Nc;
-  if (flat) {
+  if (f == CONV_TC_1X1) {
     // a 128-pixel tile is a run of the flat [N*H*W][C] matrix: the kernel sees one "image" of 1 x total_px pixels
-    if (total_px > 0x7fffffffLL) return SE_ERR_UNSUPPORTED;
+    if (total_px > 0x7fffffffLL) return false;
     p.N = 1; p.H = 1; p.W = (int)total_px; p.Wb = CT_BM; p.Hb = 1; p.Nb = 1;
   } else {
     p.Wb = min(pow2_ge(gW), CT_BM);
@@ -418,7 +373,7 @@ static int conv_tc_launch(const se_conv_desc* d, const float* a_tensor, int Kc, 
   p.tw = ceil_div(p.W, p.Wb); p.th = ceil_div(p.H, p.Hb);
   const long long tiles_m = (long long)p.tw * p.th * ceil_div(p.N, p.Nb);
   p.BN = pick_bn(Nc, x3);
-  if (p.BN == 0 || tiles_m > 0x7fffffffLL || Nc / p.BN > 65535) return SE_ERR_UNSUPPORTED;
+  if (p.BN == 0 || tiles_m > 0x7fffffffLL || Nc / p.BN > 65535) return false;
   p.cblk = Kc >= 32 ? 32 : 16;
   p.kblocks = Kc / p.cblk;
   // The order in which the products reach the accumulator -- filter tap, then channel block, then k-step -- is the
@@ -440,53 +395,81 @@ static int conv_tc_launch(const se_conv_desc* d, const float* a_tensor, int Kc, 
   }
   p.ring_off = p.res ? p.kblocks * p.a_bytes : 0;
   p.stages = min(CT_MAX_STAGES, (CT_SMEM_LIMIT - smem_fixed - p.ring_off) / p.stage_bytes);
-  if (p.stages < 2) return SE_ERR_UNSUPPORTED;
+  if (p.stages < 2) return false;
   // a CTA runs one tile: a ring longer than the tile's stages would only hold shared memory that other CTAs can use
   p.stages = min(p.stages, taps * taps * p.kblocks);
-  p.relu = relu; p.beta = beta;
-  p.bias = bias; p.residual = residual; p.out = out; p.stats = stats;
-  if (stats && (size_t)16 * Nc * sizeof(float) > 24 * 1024) return SE_ERR_UNSUPPORTED;   // wide layers: separate statistics pass
-  if (beta != 0.f && (beta != 1.f || residual || relu)) return SE_ERR_UNSUPPORTED;
-  const size_t smem = (size_t)p.ring_off + (size_t)p.stages * p.stage_bytes + smem_fixed;
-  if (smem > CT_SMEM_LIMIT) return SE_ERR_UNSUPPORTED;
-  if (x3_plan >= 0) return SE_OK;
+  pl->smem = (size_t)p.ring_off + (size_t)p.stages * p.stage_bytes + smem_fixed;
+  if (pl->smem > CT_SMEM_LIMIT) return false;
   // output (and residual) addressing: NHWC over the tile grid, or the strided view dx[:, ::2, ::2, :] (s2 backward data)
   p.o_sw = Nc; p.o_sh = (long long)p.W * Nc; p.o_sn = (long long)p.H * p.W * Nc;
   p.ovw = p.W; p.ovh = p.H;
-  if (s2 && flip) {
-    p.o_sw = 2LL * Nc; p.o_sh = 2LL * d->W * Nc; p.o_sn = (long long)d->H * d->W * Nc;
-    if (out_view_w) p.ovw = out_view_w;
-    if (out_view_h) p.ovh = out_view_h;
+  if (s2 && flip) { p.o_sw = 2LL * Nc; p.o_sh = 2LL * d->W * Nc; p.o_sn = (long long)d->H * d->W * Nc; }
+  pl->grid = dim3((unsigned)tiles_m, (unsigned)(Nc / p.BN));
+  return true;
+}
+
+bool conv3x3s2_tc_ok(const se_conv_desc* d);                                 // conv_wgrad_tc.cu
+bool wgrad_config(const se_conv_desc* d, int x3, int sms, ConvPlan* pl);    // conv_wgrad_tc.cu
+
+ConvFamily conv_plan(const se_conv_desc* d, int dir, int mode, const ConvCall& c, ConvPlan* pl) {
+  *pl = ConvPlan();
+  if (mode != SE_MODE_TF32 && mode != SE_MODE_TF32X3) return CONV_FP32;
+  const int x3 = pl->x3 = mode == SE_MODE_TF32X3;
+  if (dir == 2) return c.aligned && wgrad_config(d, x3, c.sms, pl) ? (pl->family = CONV_TC_WGRAD) : CONV_FP32;
+  // the B operands: the transposed kernel copy (forward) or the kernel itself (data gradient), and their low parts
+  if (dir == 0 && (!c.w_t || (x3 && !c.w_t_lo))) return CONV_FP32;
+  if (dir == 1 && x3 && !c.w_lo) return CONV_FP32;
+  if (dir == 1 && c.beta != 0.f && c.beta != 1.f) return CONV_FP32;     // overwrite or accumulate only
+  const int Kc = dir == 0 ? d->Cin : d->Cout, Nc = dir == 0 ? d->Cout : d->Cin;
+  ConvFamily f = tc_family(d, Kc, Nc);
+  if (dir == 1 && conv3x3s2_tc_ok(d)) {
+    // every filter tap is a 1x1 / stride 2 data gradient over the same grid, added into its own view of dx
+    se_conv_desc d1 = *d;
+    d1.kh = 1; d1.kw = 1;
+    f = tc_family(&d1, Kc, Nc) == CONV_TC_1X1_S2 ? CONV_TC_DGRAD_3X3S2 : CONV_FP32;
   }
+  if (f == CONV_FP32 || !tc_config(d, f, Kc, Nc, dir, x3, pl)) return CONV_FP32;
+  pl->tc.beta = f == CONV_TC_DGRAD_3X3S2 ? 1.f : c.beta;
+  // wide layers (640 output channels): the per-warp statistics slots of the fused epilogue do not fit in shared memory,
+  // the BatchNorm sums come from a separate pass over y
+  pl->fused_stats = c.stats && (size_t)16 * Nc * sizeof(float) <= 24 * 1024;
+  return pl->family = f;
+}
+
+template <int BN>
+static void conv_tc_go(int x3, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& ma, const CUtensorMap& mb,
+                       const CUtensorMap& mbl, const ConvTcParams& p) {
+  if constexpr (BN <= 64)       // pick_bn: <= 64 channels per tile in the error-compensated mode
+    if (x3) return launch(conv_tc_kernel<BN, 1>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
+  launch(conv_tc_kernel<BN, 0>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
+}
+
+// conv_tc_kernel with the planned configuration and the pointers of p: A = a_tensor (x, or dy for the data gradient),
+// B = bmat and, in the error-compensated mode, its low parts bmat_lo (se_split_filters)
+static int conv_tc_launch(const ConvPlan& pl, const ConvTcParams& p, const se_conv_desc* d, const float* a_tensor,
+                          const float* bmat, const float* bmat_lo, cudaStream_t st) {
+  const int Kc = p.Kc, Nc = p.Nc;
   CUtensorMap ma, mb, mbl;
-  {
-    uint64_t dims[4] = {(uint64_t)Kc, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.N};
-    uint64_t strides[3] = {(uint64_t)Kc * 4, (uint64_t)p.W * Kc * 4, (uint64_t)p.H * p.W * Kc * 4};
-    if (s2 && !flip) {      // forward: x[:, ::2, ::2, :]
-      strides[0] = (uint64_t)2 * Kc * 4; strides[1] = (uint64_t)2 * d->W * Kc * 4; strides[2] = (uint64_t)d->H * d->W * Kc * 4;
-    }
-    uint32_t box[4] = {(uint32_t)p.cblk, (uint32_t)(p.Wb + 2 * p.res), (uint32_t)(p.Hb + 2 * p.res), (uint32_t)p.Nb};
-    CUtensorMapSwizzle sw = p.cblk == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-    if (!make_tmap(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(a_tensor), dims, strides, box, sw)) return SE_ERR_CUDA;
-    uint64_t bdims[2] = {(uint64_t)Kc, (uint64_t)taps * taps * Nc};
-    uint64_t bstrides[1] = {(uint64_t)Kc * 4};
-    uint32_t bbox[2] = {(uint32_t)p.cblk, (uint32_t)p.BN};
-    if (!make_tmap(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(bmat), bdims, bstrides, bbox, sw)) return SE_ERR_CUDA;
-    mbl = mb;
-    if (x3 && !make_tmap(&mbl, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(bmat_lo), bdims, bstrides, bbox, sw))
-      return SE_ERR_CUDA;
+  uint64_t dims[4] = {(uint64_t)Kc, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.N};
+  uint64_t strides[3] = {(uint64_t)Kc * 4, (uint64_t)p.W * Kc * 4, (uint64_t)p.H * p.W * Kc * 4};
+  if (pl.family == CONV_TC_1X1_S2 && !p.flip) {      // forward: x[:, ::2, ::2, :]
+    strides[0] = (uint64_t)2 * Kc * 4; strides[1] = (uint64_t)2 * d->W * Kc * 4; strides[2] = (uint64_t)d->H * d->W * Kc * 4;
   }
-  if (s2 && flip && beta == 0.f &&
-      cudaMemsetAsync(out, 0, (size_t)d->N * d->H * d->W * Nc * sizeof(float), st) != cudaSuccess) {
-    set_error("conv_tc: cudaMemsetAsync failed");
+  uint32_t box[4] = {(uint32_t)p.cblk, (uint32_t)(p.Wb + 2 * p.res), (uint32_t)(p.Hb + 2 * p.res), (uint32_t)p.Nb};
+  CUtensorMapSwizzle sw = p.cblk == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+  if (!make_tmap(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(a_tensor), dims, strides, box, sw)) return SE_ERR_CUDA;
+  uint64_t bdims[2] = {(uint64_t)Kc, (uint64_t)p.taps * p.taps * Nc};
+  uint64_t bstrides[1] = {(uint64_t)Kc * 4};
+  uint32_t bbox[2] = {(uint32_t)p.cblk, (uint32_t)p.BN};
+  if (!make_tmap(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(bmat), bdims, bstrides, bbox, sw)) return SE_ERR_CUDA;
+  mbl = mb;
+  if (pl.x3 && !make_tmap(&mbl, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(bmat_lo), bdims, bstrides, bbox, sw))
     return SE_ERR_CUDA;
-  }
-  const dim3 grid((unsigned)tiles_m, (unsigned)(Nc / p.BN));
   switch (p.BN) {
-    case 16: conv_tc_go<16>(x3, grid, smem, st, ma, mb, mbl, p); break;
-    case 32: conv_tc_go<32>(x3, grid, smem, st, ma, mb, mbl, p); break;
-    case 64: conv_tc_go<64>(x3, grid, smem, st, ma, mb, mbl, p); break;
-    default: conv_tc_go<128>(x3, grid, smem, st, ma, mb, mbl, p); break;
+    case 16: conv_tc_go<16>(pl.x3, pl.grid, pl.smem, st, ma, mb, mbl, p); break;
+    case 32: conv_tc_go<32>(pl.x3, pl.grid, pl.smem, st, ma, mb, mbl, p); break;
+    case 64: conv_tc_go<64>(pl.x3, pl.grid, pl.smem, st, ma, mb, mbl, p); break;
+    default: conv_tc_go<128>(pl.x3, pl.grid, pl.smem, st, ma, mb, mbl, p); break;
   }
   return check_launch("conv_tc_kernel");
 }
@@ -513,69 +496,41 @@ static int ensure_init() {
   return SE_OK;
 }
 
-// forward needs the transposed kernel copy w_t = [tap][co][ci]; without it the caller falls back to the fp32 kernels
-// w_t_lo != null selects the error-compensated arithmetic (w_t_lo = low parts of w_t, se_split_filters)
-int conv_fwd_tc(const se_conv_desc* d, const float* x, const float* w_t, const float* w_t_lo, const float* bias,
-                const float* residual, float* y, int relu, double* stats, cudaStream_t st) {
-  if (!w_t) return SE_ERR_UNSUPPORTED;
-  const bool k2 = tc_shape_ok_1x1_s2(d, d->Cin, d->Cout);
-  const bool k1 = k2 || tc_shape_ok_1x1(d, d->Cin, d->Cout);
-  if (!k1 && !tc_shape_ok(d, d->Cin, d->Cout)) return SE_ERR_UNSUPPORTED;
+// w_t = the transposed kernel copy [tap][co][ci], w_t_lo its low parts (error-compensated mode)
+int conv_fwd_tc(const ConvPlan& pl, const se_conv_desc* d, const float* x, const float* w_t, const float* w_t_lo,
+                const float* bias, const float* residual, float* y, int relu, double* stats, cudaStream_t st) {
   int rc = ensure_init();
   if (rc) return rc;
-  return conv_tc_launch(d, x, d->Cin, w_t, d->Cout, 0, bias, residual, y, relu, 0.f, stats, st, w_t_lo, k1 ? 1 : 3, k2);
+  ConvTcParams p = pl.tc;
+  p.relu = relu; p.bias = bias; p.residual = residual; p.out = y; p.stats = stats;
+  return conv_tc_launch(pl, p, d, x, w_t, w_t_lo, st);
 }
 
-bool conv3x3s2_tc_ok(const se_conv_desc* d);      // conv_wgrad_tc.cu
-
-// 3x3 / stride 2 / no leading padding, wide layers (see conv3x3s2_tc_ok): nine 1x1 / stride 2 data gradients, one per
-// filter tap, each added into its own sub-sampled view of dx:   dx[:, r::2, s::2, :] += dY W[r, s]^T
-static int conv_dgrad_tc_3x3s2(const se_conv_desc* d, const float* dy, const float* w, const float* w_lo, float* dx, float beta,
-                               cudaStream_t st) {
-  if (beta != 0.f && beta != 1.f) return SE_ERR_UNSUPPORTED;
+// dx = beta * dx + conv^T(dy, w), beta 0 or 1.  The stride-2 families write sub-sampled views of dx, which is zeroed
+// first when beta = 0: the 1x1 layer dx[:, ::2, ::2, :], and every filter tap (r, s) of a wide 3x3 layer (see
+// conv3x3s2_tc_ok) adds dY W[r, s]^T into dx[:, r::2, s::2, :], whose last column / row may not exist.
+int conv_dgrad_tc(const ConvPlan& pl, const se_conv_desc* d, const float* dy, const float* w, const float* w_lo, float* dx,
+                  float beta, cudaStream_t st) {
   int rc = ensure_init();
   if (rc) return rc;
-  se_conv_desc d1 = *d;
-  d1.kh = 1; d1.kw = 1;
-  if (!tc_shape_ok_1x1_s2(&d1, d->Cout, d->Cin)) return SE_ERR_UNSUPPORTED;
-  if (beta == 0.f && cudaMemsetAsync(dx, 0, (size_t)d->N * d->H * d->W * d->Cin * sizeof(float), st) != cudaSuccess) {
+  const bool nine = pl.family == CONV_TC_DGRAD_3X3S2;
+  if ((nine || pl.family == CONV_TC_1X1_S2) && beta == 0.f &&
+      cudaMemsetAsync(dx, 0, (size_t)d->N * d->H * d->W * d->Cin * sizeof(float), st) != cudaSuccess) {
     set_error("conv_dgrad_tc: cudaMemsetAsync failed");
     return SE_ERR_CUDA;
   }
+  ConvTcParams p = pl.tc;
+  p.out = dx;
+  if (!nine) return conv_tc_launch(pl, p, d, dy, w, w_lo, st);
   for (int r = 0; r < 3; ++r)
     for (int s = 0; s < 3; ++s) {
       const long long woff = (long long)(r * 3 + s) * d->Cin * d->Cout;
-      rc = conv_tc_launch(&d1, dy, d->Cout, w + woff, d->Cin, 1, nullptr, nullptr, dx + ((long long)r * d->W + s) * d->Cin, 0, 1.f,
-                          nullptr, st, w_lo ? w_lo + woff : nullptr, 1, 1, -1, d->Wo - (s == 2), d->Ho - (r == 2));
+      p.out = dx + ((long long)r * d->W + s) * d->Cin;
+      p.ovw = d->Wo - (s == 2); p.ovh = d->Ho - (r == 2);
+      rc = conv_tc_launch(pl, p, d, dy, w + woff, w_lo ? w_lo + woff : nullptr, st);
       if (rc != SE_OK) return rc;
     }
   return SE_OK;
-}
-
-int conv_dgrad_tc(const se_conv_desc* d, const float* dy, const float* w, const float* w_lo, float* dx, float beta,
-                  cudaStream_t st) {
-  if (conv3x3s2_tc_ok(d)) return conv_dgrad_tc_3x3s2(d, dy, w, w_lo, dx, beta, st);
-  const bool k2 = tc_shape_ok_1x1_s2(d, d->Cout, d->Cin);
-  const bool k1 = k2 || tc_shape_ok_1x1(d, d->Cout, d->Cin);
-  if (!k1 && !tc_shape_ok(d, d->Cout, d->Cin)) return SE_ERR_UNSUPPORTED;
-  int rc = ensure_init();
-  if (rc) return rc;
-  return conv_tc_launch(d, dy, d->Cout, w, d->Cin, 1, nullptr, nullptr, dx, 0, beta, nullptr, st, w_lo, k1 ? 1 : 3, k2);
-}
-
-// se_conv2d_path: would the tensor-core kernel of this file take the layer?  (dir 0 forward, 1 backward data; x3 = 0 / 1)
-bool conv_tc_would_run(const se_conv_desc* d, int dir, int x3) {
-  if (dir == 1 && conv3x3s2_tc_ok(d)) {
-    se_conv_desc d1 = *d;
-    d1.kh = 1; d1.kw = 1;
-    return conv_tc_would_run(&d1, 1, x3);
-  }
-  const int Kc = dir == 0 ? d->Cin : d->Cout, Nc = dir == 0 ? d->Cout : d->Cin;
-  const bool k2 = tc_shape_ok_1x1_s2(d, Kc, Nc);
-  const bool k1 = k2 || tc_shape_ok_1x1(d, Kc, Nc);
-  if (!k1 && !tc_shape_ok(d, Kc, Nc)) return false;
-  return conv_tc_launch(d, nullptr, Kc, nullptr, Nc, dir, nullptr, nullptr, nullptr, 0, 0.f, nullptr, nullptr, nullptr, k1 ? 1 : 3,
-                        k2, x3) == SE_OK;
 }
 
 int transpose_filters(const float* P, float* PT, float* PL, float* PTL, const long long* table, int n, cudaStream_t st) {

@@ -20,6 +20,7 @@
 #include <mutex>
 
 #include "common.cuh"
+#include "conv_plan.cuh"
 #include "tc.cuh"
 
 namespace se {
@@ -29,17 +30,6 @@ using namespace tc;
 constexpr int WG_PX = 32;              // pixels per chunk: one 128-byte swizzle row per channel
 constexpr int WG_MT = 64;              // rows of dW ((filter tap, input channel) pairs) per warpgroup tile
 constexpr int WG_THREADS = 256;
-
-struct WgTcParams {
-  int N, H, W, Cin, Cout, Ho, Wo, kw, stride, pad_t, pad_l;
-  int KK;                      // rows of dW: kh * kw * Cin, row = tap * Cin + ci
-  int npx;                     // N * Ho * Wo
-  int chunks;                  // ceil(npx / 32)
-  int per_cta;                 // chunks per CTA (even)
-  float* ws;                   // [2 * gridDim.x][KK * Cout] partial dW, then [2 * gridDim.x][Cout] partial dbias
-  float* dw;                   // direct mode (ws == nullptr): atomics straight into dW / dbias
-  float* dbias;
-};
 
 // Workspaces of the split-K partial sums: one per (device, stream), 32 MB each, allocated outside graph captures (se_init
 // prepares the one of se_run_ops' side stream).  A request that does not fit, or a stream that first appears inside a
@@ -304,21 +294,6 @@ static bool conv3x3_wgrad_tc_ok(const se_conv_desc* d) {
          d->Cin % 16 == 0 && d->Cout % 16 == 0 && d->W >= 4 && d->W <= 64;
 }
 
-// se_conv2d_path: would the tensor-core weight-gradient kernel take the layer?
-bool conv_wgrad_tc_would_run(const se_conv_desc* d, int x3) {
-  (void)x3;
-  return conv1x1_wgrad_tc_ok(d) || conv3x3s2_tc_ok(d) || conv3x3_wgrad_tc_ok(d);
-}
-
-// se_linear_svm_fit: does the tensor-core kernel take this shape on stream `st` and add its split-K slices in a fixed
-// order, i.e. does at least one pair of slices fit a workspace that exists or can be allocated now?
-bool conv_wgrad_tc_fixed_order(const se_conv_desc* d, cudaStream_t st) {
-  if (!conv_wgrad_tc_would_run(d, 1)) return false;
-  const long long T = (long long)d->kh * d->kw * d->Cin * d->Cout;
-  float* ws = nullptr;
-  return wgrad_workspace(2 * (T + d->Cout), st, &ws) == SE_OK && ws != nullptr;
-}
-
 // Error-compensated sums over at least this many pixels take four partial tiles per chunk (NP = 4).  Measured on an H100
 // on ResNet-50's res2a_branch2a at 448 px (B = 32, 394 272 pixels, in front of a BatchNorm: dY sums to zero per channel,
 // X >= 0): 3.6e-5 of the largest dW with one tile and the big term first, 2.9e-5 small terms first, 5.7e-6 with four
@@ -327,54 +302,70 @@ bool conv_wgrad_tc_fixed_order(const se_conv_desc* d, cudaStream_t st) {
 // and the arithmetic they had.
 constexpr long long WG_LONG_PX = 1LL << 18;
 
-template <int BN>
-static void wgrad_go(int x3, dim3 grid, cudaStream_t st, const float* x, const float* dy, const WgTcParams& p) {
-  const size_t smem = 1024 + 2 * (size_t)(WG_MT * 128 + BN * 128) * (x3 ? 2 : 1);
-  if (x3 && p.npx >= WG_LONG_PX) launch(conv_wgrad_tc_kernel<BN, 1, 4>, grid, dim3(WG_THREADS), smem, st, x, dy, p);
-  else if (x3) launch(conv_wgrad_tc_kernel<BN, 1, 1>, grid, dim3(WG_THREADS), smem, st, x, dy, p);
-  else launch(conv_wgrad_tc_kernel<BN, 0, 1>, grid, dim3(WG_THREADS), smem, st, x, dy, p);
-}
-
-int conv_wgrad_tc(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias, int x3, cudaStream_t st) {
-  if (!conv_wgrad_tc_would_run(d, x3)) return SE_ERR_UNSUPPORTED;
-  if ((reinterpret_cast<uintptr_t>(dw) & 15) != 0 || (dbias && (reinterpret_cast<uintptr_t>(dbias) & 15) != 0))
-    return SE_ERR_UNSUPPORTED;
-  static bool inited = false;
-  if (!inited) { int rc0 = init_conv_wgrad_tc(); if (rc0) return rc0; inited = true; }
+// The launch configuration of conv_wgrad_tc_kernel (conv_plan): false for the shapes it does not take
+bool wgrad_config(const se_conv_desc* d, int x3, int sms, ConvPlan* pl) {
+  if (!conv1x1_wgrad_tc_ok(d) && !conv3x3s2_tc_ok(d) && !conv3x3_wgrad_tc_ok(d)) return false;
   const long long npx = (long long)d->N * d->Ho * d->Wo, KK = (long long)d->kh * d->kw * d->Cin;
-  if (npx > 0x7fffffffLL - 64 || KK > 0x7fffffffLL) return SE_ERR_UNSUPPORTED;
-  WgTcParams p;
+  if (npx > 0x7fffffffLL - 64 || KK > 0x7fffffffLL) return false;
+  int BN = x3 ? 64 : 128;                   // error-compensated mode: a second accumulator tile, see the kernel
+  while (d->Cout % BN != 0) BN >>= 1;
+  const int gy = (int)ceil_div<long long>(KK, WG_MT), gz = d->Cout / BN;
+  if (gy > 65535 || gz > 65535) return false;
+  WgTcParams& p = pl->wg;
   p.N = d->N; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.Cout = d->Cout; p.Ho = d->Ho; p.Wo = d->Wo;
   p.kw = d->kw; p.stride = d->stride; p.pad_t = d->pad_t; p.pad_l = d->pad_l;
   p.KK = (int)KK;
   p.npx = (int)npx;
   p.chunks = (int)ceil_div<long long>(npx, WG_PX);
-  p.dw = dw; p.dbias = dbias;
-  int BN = x3 ? 64 : 128;                   // error-compensated mode: a second accumulator tile, see the kernel
-  while (d->Cout % BN != 0) BN >>= 1;
-  const int gy = (int)ceil_div<long long>(KK, WG_MT), gz = d->Cout / BN;
   // about eight CTAs per SM over all row / column tiles, each with at least 4 chunks: a warpgroup's chunks are
   // latency-bound round trips (load, transpose, MMA), so the pixel range is cut finely
-  long long gx = ceil_div<long long>(8LL * sm_count(), (long long)gy * gz);
+  long long gx = ceil_div<long long>(8LL * sms, (long long)gy * gz);
   gx = std::max(1LL, std::min(gx, ceil_div<long long>(p.chunks, 4)));
-  const long long T = KK * d->Cout;
-  gx = std::max(1LL, wgrad_fit_splits(2 * gx, T, d->Cout) / 2);      // the slices fit the workspace
-  int rc = wgrad_workspace(2 * gx * (T + d->Cout), st, &p.ws);
-  if (rc) return rc;
+  gx = std::max(1LL, wgrad_fit_splits(2 * gx, KK * d->Cout, d->Cout) / 2);      // the slices fit the workspace
   p.per_cta = (int)ceil_div<long long>(p.chunks, gx);
   p.per_cta += p.per_cta & 1;
   gx = ceil_div<long long>(p.chunks, p.per_cta);
-  if (gy > 65535 || gz > 65535) return SE_ERR_UNSUPPORTED;
-  const dim3 grid((unsigned)gx, (unsigned)gy, (unsigned)gz);
-  switch (BN) {
-    case 16: wgrad_go<16>(x3, grid, st, x, dy, p); break;
-    case 32: wgrad_go<32>(x3, grid, st, x, dy, p); break;
-    case 64: wgrad_go<64>(x3, grid, st, x, dy, p); break;
-    default: wgrad_go<128>(x3, grid, st, x, dy, p); break;
+  pl->grid = dim3((unsigned)gx, (unsigned)gy, (unsigned)gz);
+  pl->wg_bn = BN;
+  pl->wg_np = x3 && npx >= WG_LONG_PX ? 4 : 1;
+  pl->smem = 1024 + 2 * (size_t)(WG_MT * 128 + BN * 128) * (x3 ? 2 : 1);
+  return true;
+}
+
+// se_linear_svm_fit: does the tensor-core kernel take this shape on stream `st` and add its split-K slices in a fixed
+// order, i.e. does at least one pair of slices fit a workspace that exists or can be allocated now?
+bool conv_wgrad_tc_fixed_order(const se_conv_desc* d, cudaStream_t st) {
+  ConvPlan pl;
+  if (conv_plan(d, 2, SE_MODE_TF32X3, ConvCall(), &pl) != CONV_TC_WGRAD) return false;
+  const long long T = (long long)d->kh * d->kw * d->Cin * d->Cout;
+  float* ws = nullptr;
+  return wgrad_workspace(2 * (T + d->Cout), st, &ws) == SE_OK && ws != nullptr;
+}
+
+template <int BN>
+static void wgrad_go(const ConvPlan& pl, cudaStream_t st, const float* x, const float* dy, const WgTcParams& p) {
+  if (pl.wg_np == 4) launch(conv_wgrad_tc_kernel<BN, 1, 4>, pl.grid, dim3(WG_THREADS), pl.smem, st, x, dy, p);
+  else if (pl.x3) launch(conv_wgrad_tc_kernel<BN, 1, 1>, pl.grid, dim3(WG_THREADS), pl.smem, st, x, dy, p);
+  else launch(conv_wgrad_tc_kernel<BN, 0, 1>, pl.grid, dim3(WG_THREADS), pl.smem, st, x, dy, p);
+}
+
+int conv_wgrad_tc(const ConvPlan& pl, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st) {
+  static bool inited = false;
+  if (!inited) { int rc0 = init_conv_wgrad_tc(); if (rc0) return rc0; inited = true; }
+  WgTcParams p = pl.wg;
+  p.dw = dw; p.dbias = dbias;
+  const long long T = (long long)p.KK * p.Cout, splits = 2LL * pl.grid.x;
+  int rc = wgrad_workspace(splits * (T + p.Cout), st, &p.ws);
+  if (rc) return rc;
+  switch (pl.wg_bn) {
+    case 16: wgrad_go<16>(pl, st, x, dy, p); break;
+    case 32: wgrad_go<32>(pl, st, x, dy, p); break;
+    case 64: wgrad_go<64>(pl, st, x, dy, p); break;
+    default: wgrad_go<128>(pl, st, x, dy, p); break;
   }
   rc = check_launch("conv_wgrad_tc_kernel");
   if (rc || !p.ws) return rc;
-  return wgrad_reduce(p.ws, (int)(2 * gx), T, d->Cout, dw, dbias, st);
+  return wgrad_reduce(p.ws, (int)splits, T, p.Cout, dw, dbias, st);
 }
 
 }  // namespace se

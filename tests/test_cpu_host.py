@@ -418,15 +418,15 @@ CONV_PLAN = {
     (1, 5, 65, 32, 16, 3, 1, 'same'): (0, 0, 0),          # conv3x3_wgrad_tc_ok: W = 65
     (4, 3, 3, 32, 32, 3, 1, 'same'): (0, 0, 0),           # W = 3
     (3, 5, 4, 16, 32, 3, 1, 'same'): (1, 1, 1),           # W = 4
-    (1, 4, 64, 32, 32, 1, 2, 'valid'): (1, 1, 1),         # tc_shape_ok_1x1_s2: Wo = 32
+    (1, 4, 64, 32, 32, 1, 2, 'valid'): (1, 1, 1),         # tc_family (1x1 / stride 2): Wo = 32
     (1, 4, 66, 32, 32, 1, 2, 'valid'): (0, 0, 0),         # Wo = 33
     (2, 6, 6, 32, 64, 1, 2, 'valid'): (0, 0, 1),          # Wo = 3: geometry_ok; conv1x1_wgrad_tc_ok has no lower limit
     (2, 8, 8, 32, 64, 1, 2, 'valid'): (1, 1, 1),          # Wo = 4
-    (1, 1, 127, 32, 32, 1, 1, 'valid'): (0, 0, 1),        # tc_shape_ok_1x1: 127 pixels
+    (1, 1, 127, 32, 32, 1, 1, 'valid'): (0, 0, 1),        # tc_family (1x1): 127 pixels
     (1, 2, 64, 32, 32, 1, 1, 'valid'): (1, 1, 1),         # 128 pixels
     (1, 1, 31, 32, 48, 1, 1, 'valid'): (0, 0, 0),         # conv1x1_wgrad_tc_ok: 31 pixels
     (2, 4, 4, 32, 48, 1, 1, 'valid'): (0, 0, 1),          # 32 pixels
-    (2, 8, 8, 48, 32, 3, 1, 'same'): (0, 1, 1),           # tc_shape_ok: forward K = 48
+    (2, 8, 8, 48, 32, 3, 1, 'same'): (0, 1, 1),           # channels_ok: forward K = 48
     (2, 8, 8, 32, 80, 3, 1, 'same'): (1, 0, 1),           # pick_bn -> 16; dgrad K = 80
     (2, 8, 8, 32, 192, 3, 1, 'same'): (1, 1, 1),          # pick_bn -> 64
     (2, 4, 4, 128, 128, 3, 2, 'same'): (0, 0, 1),         # conv3x3s2_tc_ok at Wo = 2; dgrad tiles need Wo >= 4

@@ -30,7 +30,7 @@ OFF_TENSOR_CORES = {
     'res2a_branch2b': (3, 1, 111, 64, 64),      # geometry_ok: W <= 56; conv3x3_wgrad_tc_ok: W <= 64
     'res2b_branch2b': (3, 1, 111, 64, 64),
     'res2c_branch2b': (3, 1, 111, 64, 64),
-    'res3a_branch1': (1, 2, 111, 256, 512),     # tc_shape_ok_1x1_s2 / conv1x1_wgrad_tc_ok: Wo = 56 > 32
+    'res3a_branch1': (1, 2, 111, 256, 512),     # tc_family (1x1 / stride 2) / conv1x1_wgrad_tc_ok: Wo = 56 > 32
     'res3a_branch2a': (1, 2, 111, 256, 128),
 }
 

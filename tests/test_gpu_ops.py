@@ -95,15 +95,15 @@ CONV_CASES = [
     (1, 5, 65, 32, 16, 3, 1, 'same', True),      # conv3x3_wgrad_tc_ok: W = 65 -> fp32 in every direction
     (4, 3, 3, 32, 32, 3, 1, 'same', True),       # geometry_ok / conv3x3_wgrad_tc_ok: W = 3 < 4 -> fp32
     (3, 5, 4, 16, 32, 3, 1, 'same', True),       # geometry_ok / conv3x3_wgrad_tc_ok: W = 4, the narrowest tensor-core row
-    (1, 4, 64, 32, 32, 1, 2, 'valid', True),     # tc_shape_ok_1x1_s2: Wo = 32, the widest strided 1x1 grid
-    (1, 4, 66, 32, 32, 1, 2, 'valid', False),    # tc_shape_ok_1x1_s2 / conv1x1_wgrad_tc_ok: Wo = 33 -> fp32
-    (2, 6, 6, 32, 64, 1, 2, 'valid', True),      # tc_shape_ok_1x1_s2: Wo = 3 < 4 -> fp32 forward / dgrad; wgrad has no lower limit
-    (2, 8, 8, 32, 64, 1, 2, 'valid', False),     # tc_shape_ok_1x1_s2: Wo = 4
-    (1, 1, 127, 32, 32, 1, 1, 'valid', True),    # tc_shape_ok_1x1: 127 pixels < CT_BM -> fp32 forward / dgrad
-    (1, 2, 64, 32, 32, 1, 1, 'valid', False),    # tc_shape_ok_1x1: 128 pixels, one flat GEMM tile
+    (1, 4, 64, 32, 32, 1, 2, 'valid', True),     # tc_family (1x1 / stride 2): Wo = 32, the widest strided 1x1 grid
+    (1, 4, 66, 32, 32, 1, 2, 'valid', False),    # tc_family (1x1 / stride 2) / conv1x1_wgrad_tc_ok: Wo = 33 -> fp32
+    (2, 6, 6, 32, 64, 1, 2, 'valid', True),      # tc_family (1x1 / stride 2): Wo = 3 < 4 -> fp32 forward / dgrad; wgrad has no lower limit
+    (2, 8, 8, 32, 64, 1, 2, 'valid', False),     # tc_family (1x1 / stride 2): Wo = 4
+    (1, 1, 127, 32, 32, 1, 1, 'valid', True),    # tc_family (1x1): 127 pixels < CT_BM -> fp32 forward / dgrad
+    (1, 2, 64, 32, 32, 1, 1, 'valid', False),    # tc_family (1x1): 128 pixels, one flat GEMM tile
     (1, 1, 31, 32, 48, 1, 1, 'valid', True),     # conv1x1_wgrad_tc_ok: 31 pixels < 32 -> fp32 wgrad
     (2, 4, 4, 32, 48, 1, 1, 'valid', True),      # conv1x1_wgrad_tc_ok: 32 pixels, one wgrad chunk
-    (2, 8, 8, 48, 32, 3, 1, 'same', True),       # tc_shape_ok: K = Cin = 48 (neither 16 nor whole 32-blocks) -> fp32 forward
+    (2, 8, 8, 48, 32, 3, 1, 'same', True),       # channels_ok: K = Cin = 48 (neither 16 nor whole 32-blocks) -> fp32 forward
     (2, 8, 8, 32, 80, 3, 1, 'same', False),      # pick_bn: N = 80 -> 16-channel tiles; dgrad K = 80 -> fp32
     (2, 8, 8, 32, 192, 3, 1, 'same', True),      # pick_bn: N = 192 -> 64-channel tiles (the X3 cap, and 192 % 128 != 0)
     (2, 4, 4, 128, 128, 3, 2, 'same', True),     # conv3x3s2_tc_ok: Wo = 2 (wgrad); the dgrad's 1x1 / stride 2 tiles need Wo >= 4

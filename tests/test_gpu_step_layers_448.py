@@ -8,7 +8,7 @@ stage-2 maps leave them in six layers, in all three directions (test_cpu_plan_44
 - res2a/b/c_branch2b, 3x3 64 -> 64 at 111 x 111: geometry_ok (W <= 56) and conv3x3_wgrad_tc_ok (W <= 64) fail, so the
   forward runs launch_fwd<64, 64, 4, 4>, the data gradient conv_dgrad_kernel and the weight gradient
   conv_wgrad3x3_kernel<16, 16> with one-row tiles (TH = 128 / W = 1);
-- res3a_branch1 and res3a_branch2a, 1x1 / 2 on 111 -> 56 (Wo = 56 > 32: tc_shape_ok_1x1_s2, conv1x1_wgrad_tc_ok): the
+- res3a_branch1 and res3a_branch2a, 1x1 / 2 on 111 -> 56 (Wo = 56 > 32: tc_family (1x1 / stride 2), conv1x1_wgrad_tc_ok): the
   data gradient without the parity ordering (odd input), the weight gradient on the generic conv_wgrad_kernel.
 The tensor-core layers sum four times the pixels they sum at 224 (the weight gradient of res2a_branch2a: 32 * 111^2 =
 394 272 at B = 32, 788 544 at B = 64), BatchNorm sees up to 1.6 M rows, max-pooling maps 224 to 111 and the global
