@@ -17,7 +17,7 @@
  *     into a CUDA graph.
  *   - process-wide state is limited to what se_init() / se_comm_init() create: the low-priority
  *     side stream and the fork/join events se_run_ops uses for weight gradients, and the NCCL
- *     communicator with its stream.  Kernels keep no state between calls.
+ *     communicator with its stream and event.  Kernels keep no state between calls.
  *   - activations are float32 NHWC; conv kernels are float32 HWIO (Keras layout); dense
  *     kernels are (in,out).  `mode` selects the arithmetic of contraction kernels:
  *     SE_MODE_F32 = fp32 FFMA; SE_MODE_TF32 = TF32 wgmma (operands read with a
@@ -61,7 +61,9 @@ const char* se_last_error(void);
 /* number of kernel launches issued by this library since load (for bench.py's gpu_launches) */
 int64_t se_launch_count(void);
 int se_device_sm_count(void);
-/* one-time per-process setup (device query, shared-memory attributes); call before capturing CUDA graphs */
+/* one-time per-process setup (device query, shared-memory attributes, se_run_ops' side stream); call before capturing
+ * CUDA graphs.  Entry points that depend on it run it themselves if it has not run; a failure (SE_ERR_CUDA, for example
+ * when the side stream cannot be created) is returned again by every later call. */
 int se_init(void);
 /* bit mask of the tensor-core kernels compiled in: 1 conv fwd, 2 conv dgrad, 4 conv wgrad, 8 pairwise */
 int se_tc_capabilities(void);
@@ -184,8 +186,8 @@ int se_bn_bwd(const float* x, const float* y, const float* dout, int64_t rows, i
               float beta_dx, float* dres, float beta_res, float* dgamma, float* dbeta, double* scratch,
               void* stream);
 /* Which implementation se_bn_bwd runs for (rows, C) on a device with `sms` SMs (sms <= 0: the current device; a positive
- * sms is pure host-side planning, callable without a GPU).  se_bn_bwd decides by the same function, and SE_BN_NO_FUSE /
- * SE_BN_NO_REG in the environment move both alike.  Bits 0-1 name the path, bit 2 its float4 / fixed-quad variant:
+ * sms is pure host-side planning, callable without a GPU).  se_bn_bwd decides by the same function.  Bits 0-1 name the
+ * path, bit 2 its float4 / fixed-quad variant:
  *   SE_BN_BWD_SCALAR       bn_bwd_reduce_kernel + bn_bwd_apply_kernel, scalar branch (C % 4 != 0)          2 launches
  *   SE_BN_BWD_VEC          the same two kernels, float4 branch                                             2 launches
  *   SE_BN_BWD_SLAB_ATOMIC  bn_bwd_fused_kernel (slab in shared memory, grid barrier), per-element shared

@@ -22,10 +22,6 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
-bool pdl_enabled() {
-  static const bool on = getenv("SE_NO_PDL") == nullptr;
-  return on;
-}
 bool coop_enabled() {
   static const bool on = getenv("SE_BN_COOP") != nullptr;
   return on;
@@ -71,23 +67,50 @@ extern "C" const char* se_version(void) { return "se_b200 0.1 (sm_90a)"; }
 extern "C" const char* se_last_error(void) { return g_err; }
 extern "C" int64_t se_launch_count(void) { return g_launches.load(); }
 extern "C" int se_device_sm_count(void) { return sm_count(); }
-namespace se { int init_conv_simt(); int init_pairwise_tc(); int init_conv_tc(); int init_conv_wgrad_tc(); int init_head(); }
-// One-time per-process setup that must not happen inside a CUDA-graph capture: device query and the
-// cudaFuncSetAttribute calls of every kernel that needs more than 48 KB of dynamic shared memory.
-static bool side_stream_ready();
-static int prepare_side_workspace();
+// Weight gradients are off the critical path of the backward pass (nothing reads dW before the optimizer), so a
+// multi-op plan issues them on a second, lowest-priority stream (see Streams below).  Inside a CUDA-graph capture this
+// becomes a parallel branch.  The backward-data / BatchNorm-backward chain and the wgrad kernels can share an SM (shared
+// memory, registers; see conv_tc.cu / conv_wgrad_tc.cu), so the side branch fills the latency bubbles of the main chain.
+static cudaStream_t g_side = nullptr;
+static cudaEvent_t g_ev_fork = nullptr, g_ev_join = nullptr;
 
-extern "C" int se_init(void) {
+namespace se {
+int init_conv_simt(); int init_pairwise_tc(); int init_conv_tc(); int init_conv_wgrad_tc(); int init_head();
+int init_bn_bwd(); int init_row_topk(); int init_resample_crop();
+int wgrad_workspace_prepare(cudaStream_t st);
+
+static int setup() {
   sm_count();
-  int rc = se::init_conv_simt();
-  if (rc == SE_OK) rc = se::init_pairwise_tc();
-  if (rc == SE_OK) rc = se::init_conv_tc();
-  if (rc == SE_OK) rc = se::init_conv_wgrad_tc();
-  if (rc == SE_OK) rc = se::init_head();
-  if (rc == SE_OK) side_stream_ready();      // side stream + fork/join events of se_run_ops exist before any graph capture
-  if (rc == SE_OK) rc = prepare_side_workspace();   // and the weight-gradient workspace of that stream
+  for (int (*init)() : {init_conv_simt, init_pairwise_tc, init_conv_tc, init_conv_wgrad_tc, init_head, init_bn_bwd,
+                        init_row_topk, init_resample_crop}) {
+    const int rc = init();
+    if (rc) return rc;
+  }
+  int lo = 0, hi = 0;
+  cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&g_side, cudaStreamNonBlocking, lo);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g_ev_fork, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g_ev_join, cudaEventDisableTiming);
+  if (e != cudaSuccess) {
+    set_error("se_init: cannot create the side stream of se_run_ops: %s", cudaGetErrorString(e));
+    return SE_ERR_CUDA;
+  }
+  return wgrad_workspace_prepare(g_side);
+}
+
+int ensure_setup() {
+  static char msg[sizeof(g_err)];
+  static const int rc = [] {
+    const int r = setup();
+    if (r) snprintf(msg, sizeof(msg), "%s", g_err);
+    return r;
+  }();
+  if (rc) set_error("%s", msg);
   return rc;
 }
+}  // namespace se
+
+extern "C" int se_init(void) { return ensure_setup(); }
 namespace se { int tc_capabilities(); }
 extern "C" int se_tc_capabilities(void) { return se::tc_capabilities(); }
 
@@ -221,76 +244,79 @@ static se_conv_desc desc_from(const int32_t* i) {
 extern "C" int se_sgd_apply_devlr(float* p, const float* g, float* v, int64_t n, const float* lr_dev, float momentum,
                                   int nesterov, float clipnorm, const double* out, void* stream);
 
-// Weight gradients are off the critical path of the backward pass (nothing reads dW before the optimizer), so a
-// multi-op plan issues them on a second, lowest-priority stream: fork after the op that produced dY, join at the end of
-// the plan.  Inside a CUDA-graph capture this becomes a parallel branch.  The backward-data / BatchNorm-backward
-// chain and the wgrad kernels can share an SM (shared memory, registers; see
-// conv_tc.cu / conv_wgrad_tc.cu), so the side branch fills the latency bubbles of the main chain.  SE_NO_SIDE_STREAM=1
-// keeps everything on one stream.
-static cudaStream_t g_side = nullptr;
-static cudaEvent_t g_ev_fork = nullptr, g_ev_join = nullptr;
-static bool side_stream_ready() {
-  static const bool off = getenv("SE_NO_SIDE_STREAM") != nullptr;
-  if (off) return false;
-  if (!g_side) {
-    int lo = 0, hi = 0;
-    if (cudaDeviceGetStreamPriorityRange(&lo, &hi) != cudaSuccess) return false;
-    if (cudaStreamCreateWithPriority(&g_side, cudaStreamNonBlocking, lo) != cudaSuccess) { g_side = nullptr; return false; }
-    if (cudaEventCreateWithFlags(&g_ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&g_ev_join, cudaEventDisableTiming) != cudaSuccess) {
-      g_side = nullptr;
-      return false;
-    }
-  }
-  return true;
-}
-
-namespace se { int wgrad_workspace_prepare(cudaStream_t st); }
-static int prepare_side_workspace() { return g_side ? se::wgrad_workspace_prepare(g_side) : SE_OK; }
-
 namespace se {
 cudaStream_t comm_stream();
+cudaEvent_t comm_event();
 bool comm_ready();
 int comm_allreduce_ranges(float* base, const long long* off, const long long* cnt, int nranges, cudaStream_t st);
 }
-static cudaEvent_t g_ev_comm_main = nullptr, g_ev_comm_side = nullptr, g_ev_comm_done = nullptr;
-static bool g_comm_pending = false;      // all-reduces in flight on the communication stream (joined before the optimizer)
-static bool comm_events_ready() {
-  if (!g_ev_comm_main) {
-    if (cudaEventCreateWithFlags(&g_ev_comm_main, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&g_ev_comm_side, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&g_ev_comm_done, cudaEventDisableTiming) != cudaSuccess) {
-      g_ev_comm_main = nullptr;
-      return false;
-    }
-  }
-  return true;
-}
-static void join_comm(void* stream) {
-  if (g_comm_pending) {
-    cudaEventRecord(g_ev_comm_done, se::comm_stream());
-    cudaStreamWaitEvent(as_stream(stream), g_ev_comm_done, 0);
-    g_comm_pending = false;
-  }
+
+// `waiter` waits for the work issued so far on `st`
+static void wait_for(cudaStream_t waiter, cudaStream_t st, cudaEvent_t ev) {
+  cudaEventRecord(ev, st);
+  cudaStreamWaitEvent(waiter, ev, 0);
 }
 
-static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* forked);
+// The stream ordering of one se_run_ops call.  Besides the caller's (main) stream a multi-op plan uses two branches:
+// the side stream (weight gradients, and the filter transposition at the start of a step) and the communication stream
+// (all-reduces).  These joins are what keeps the optimizer from racing the gradient writes, so the rule is:
+//   - an op that reads or clears gradient memory -- MEMSET with i[0] bit 0 set, SGD_PREPARE, SGD_APPLY, ADAGRAD_APPLY --
+//     first joins both branches;
+//   - the first CONV_FWD / CONV_BN_FWD that reads a transposed filter joins the transposition;
+//   - an ALLREDUCE waits for the main stream, and for the side stream when that branch is open;
+//   - the end of the call joins everything, on every path (an unjoined fork would invalidate an ongoing capture).
+struct Streams {
+  cudaStream_t main;
+  bool use_side;              // a multi-op plan
+  bool side_open = false;     // side-stream work not yet joined
+  bool transposing = false;   // ... and it is the filter transposition
+  bool comm_pending = false;  // all-reduces not yet joined
+
+  cudaStream_t fork_side() {
+    if (!use_side) return main;
+    wait_for(g_side, main, g_ev_fork);
+    side_open = true;
+    return g_side;
+  }
+  void join_side() {
+    if (!side_open) return;
+    wait_for(main, g_side, g_ev_join);
+    side_open = transposing = false;
+  }
+  cudaStream_t fork_comm() {
+    const cudaStream_t cs = comm_stream();
+    wait_for(cs, main, comm_event());
+    if (side_open) wait_for(cs, g_side, comm_event());
+    comm_pending = true;
+    return cs;
+  }
+  void join_comm() {
+    if (!comm_pending) return;
+    wait_for(main, comm_stream(), comm_event());
+    comm_pending = false;
+  }
+  void join_all() {
+    join_comm();
+    join_side();
+  }
+};
+
+// the arithmetic mode of a convolution op: its own (i[13] >= 0) or the plan's
+static int op_mode(const int32_t* i, int mode) { return i[13] >= 0 ? i[13] : mode; }
+
+static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, Streams& st);
 
 extern "C" int se_run_ops(const se_op* ops, int n, int mode, void* stream) {
   SE_REQUIRE(ops && n >= 0, "bad arguments");
-  bool forked = false;
-  int rc = run_ops_impl(ops, n, mode, stream, &forked);
-  if (forked) {   // join on every path (an unjoined fork would invalidate an ongoing capture)
-    cudaEventRecord(g_ev_join, g_side);
-    cudaStreamWaitEvent(as_stream(stream), g_ev_join, 0);
-  }
-  join_comm(stream);
+  int rc = ensure_setup();
+  if (rc) return rc;
+  Streams st{as_stream(stream), n > 1};
+  rc = run_ops_impl(ops, n, mode, stream, st);
+  st.join_all();
   return rc;
 }
 
-static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* forked) {
-  const bool use_side = n > 1 && side_stream_ready();
-  bool transposing = false;          // filter transposition in flight on the side stream
+static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, Streams& st) {
   for (int k = 0; k < n; ++k) {
     const se_op& o = ops[k];
     const int32_t* i = o.i;
@@ -300,50 +326,34 @@ static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* f
     switch (o.opcode) {
       case SE_OP_CONV_FWD: {
         se_conv_desc d = desc_from(i);
-        if (transposing && p[6]) {   // first consumer of the transposed filters: the side branch joins here
-          cudaEventRecord(g_ev_join, g_side);
-          cudaStreamWaitEvent(as_stream(stream), g_ev_join, 0);
-          transposing = false;
-          *forked = false;
-        }
+        if (st.transposing && p[6]) st.join_side();
         se_conv_aux aux = {(const float*)p[6], (const float*)p[7], nullptr};
         rc = se_conv2d_fwd_aux(&d, (const float*)p[0], (const float*)p[1], &aux, (const float*)p[2],
-                               (const float*)p[3], (float*)p[4], i[12], (double*)p[5], i[13] >= 0 ? i[13] : mode, stream);
+                               (const float*)p[3], (float*)p[4], i[12], (double*)p[5], op_mode(i, mode), stream);
         break;
       }
       case SE_OP_CONV_BN_FWD: {
         // p: 0 x, 1 w, 2 bias, 3 y, 4 stats, 5 w_t, 6 gamma, 7 beta, 8 moving_mean, 9 moving_var, 10 save_mean,
         //    11 save_invstd, 12 residual, 13 bn_out, 14 counter;  i[12] conv relu, i[14] bn relu;  f: eps, momentum
         se_conv_desc d = desc_from(i);
-        if (transposing && p[5]) {
-          cudaEventRecord(g_ev_join, g_side);
-          cudaStreamWaitEvent(as_stream(stream), g_ev_join, 0);
-          transposing = false;
-          *forked = false;
-        }
+        if (st.transposing && p[5]) st.join_side();
         rc = se_conv_bn_fwd(&d, (const float*)p[0], (const float*)p[1], (const float*)p[5], (const float*)p[2], (float*)p[3],
                             i[12], (double*)p[4], (const float*)p[6], (const float*)p[7], f[0], f[1], (float*)p[8],
                             (float*)p[9], (float*)p[10], (float*)p[11], (const float*)p[12], i[14], (float*)p[13], p[14],
-                            i[13] >= 0 ? i[13] : mode, stream);
+                            op_mode(i, mode), stream);
         break;
       }
       case SE_OP_CONV_DGRAD: {
         se_conv_desc d = desc_from(i);
         se_conv_aux aux = {nullptr, nullptr, (const float*)p[3]};
-        rc = se_conv2d_dgrad_aux(&d, (const float*)p[0], (const float*)p[1], &aux, (float*)p[2], f[0],
-                                 i[13] >= 0 ? i[13] : mode, stream);
+        rc = se_conv2d_dgrad_aux(&d, (const float*)p[0], (const float*)p[1], &aux, (float*)p[2], f[0], op_mode(i, mode),
+                                 stream);
         break;
       }
       case SE_OP_CONV_WGRAD: {
         se_conv_desc d = desc_from(i);
-        void* ws = stream;
-        if (use_side) {
-          cudaEventRecord(g_ev_fork, as_stream(stream));
-          cudaStreamWaitEvent(g_side, g_ev_fork, 0);
-          ws = g_side;
-          *forked = true;
-        }
-        rc = se_conv2d_wgrad(&d, (const float*)p[0], (const float*)p[1], (float*)p[2], (float*)p[3], i[13] >= 0 ? i[13] : mode, ws);
+        rc = se_conv2d_wgrad(&d, (const float*)p[0], (const float*)p[1], (float*)p[2], (float*)p[3], op_mode(i, mode),
+                             st.fork_side());
         break;
       }
       case SE_OP_BN_STATS:
@@ -431,16 +441,7 @@ static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* f
                                     i[4], f[0], (float*)p[3], (float*)p[4], (float*)p[5], stream);
         break;
       case SE_OP_MEMSET: {
-        if (i[0] & 1) {
-          // a memset of GRADIENT memory (frozen parameters, Engine.set_trainable): the weight-gradient kernels of the side
-          // stream and the all-reduces of the communication stream write that memory -- join them first
-          join_comm(stream);
-          if (*forked) {
-            cudaEventRecord(g_ev_join, g_side);
-            cudaStreamWaitEvent(as_stream(stream), g_ev_join, 0);
-            *forked = false;
-          }
-        }
+        if (i[0] & 1) st.join_all();   // gradient memory (frozen parameters, Engine.set_trainable)
         cudaError_t e = cudaMemsetAsync(p[0], 0, (size_t)(uintptr_t)p[1], as_stream(stream));
         if (e != cudaSuccess) { set_error("memset: %s", cudaGetErrorString(e)); rc = SE_ERR_CUDA; }
         break;
@@ -449,13 +450,10 @@ static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* f
         if (mode == SE_MODE_TF32 || mode == SE_MODE_TF32X3) {
           // the transposed filter copies are first needed by the first tensor-core convolution: the transposition runs
           // on the side stream beside the statistics memset, the stem convolution and its BatchNorm
-          void* ts = stream;
-          if (use_side && !*forked) {
-            cudaEventRecord(g_ev_fork, as_stream(stream));
-            cudaStreamWaitEvent(g_side, g_ev_fork, 0);
-            ts = g_side;
-            *forked = true;
-            transposing = true;
+          cudaStream_t ts = st.main;
+          if (!st.side_open) {
+            ts = st.fork_side();
+            st.transposing = st.side_open;
           }
           if (mode == SE_MODE_TF32X3 && p[3] && p[4])
             rc = se_split_filters((const float*)p[0], (float*)p[1], (float*)p[3], (float*)p[4], (const int64_t*)p[2], i[0], ts);
@@ -468,37 +466,20 @@ static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* f
         // The ranges hold gradients that every op up to here has finished writing: weight gradients on the side stream,
         // BatchNorm / bias gradients on the main stream.  The exchange runs on the communication stream behind both and
         // overlaps the rest of the backward pass; the optimizer joins it.
-        if (!se::comm_ready() || !comm_events_ready()) { set_error("SE_OP_ALLREDUCE without a communicator (se_comm_init)"); return SE_ERR_ARG; }
-        cudaStream_t cs = se::comm_stream();
-        cudaEventRecord(g_ev_comm_main, as_stream(stream));
-        cudaStreamWaitEvent(cs, g_ev_comm_main, 0);
-        if (*forked) {
-          cudaEventRecord(g_ev_comm_side, g_side);
-          cudaStreamWaitEvent(cs, g_ev_comm_side, 0);
-        }
+        if (!se::comm_ready()) { set_error("SE_OP_ALLREDUCE without a communicator (se_comm_init)"); return SE_ERR_ARG; }
         long long off[7], cnt[7];
         const int nr = i[0] < 7 ? i[0] : 7;
         for (int r = 0; r < nr; ++r) { off[r] = (long long)(uintptr_t)p[1 + 2 * r]; cnt[r] = (long long)(uintptr_t)p[2 + 2 * r]; }
-        rc = se::comm_allreduce_ranges((float*)p[0], off, cnt, nr, cs);
-        g_comm_pending = true;
+        rc = se::comm_allreduce_ranges((float*)p[0], off, cnt, nr, st.fork_comm());
         break;
       }
       case SE_OP_SGD_PREPARE:
-        join_comm(stream);
-        if (*forked) {   // the optimizer reads every gradient: the side branch joins here
-          cudaEventRecord(g_ev_join, g_side);
-          cudaStreamWaitEvent(as_stream(stream), g_ev_join, 0);
-          *forked = false;
-        }
+        st.join_all();
         rc = se_sgd_prepare((const float*)p[0], (float*)p[1], (int64_t)(uintptr_t)p[2], (const se_l2_segment*)p[3], i[0],
                             (double*)p[4], stream);
         break;
       case SE_OP_SGD_APPLY:
-        if (*forked) {
-          cudaEventRecord(g_ev_join, g_side);
-          cudaStreamWaitEvent(as_stream(stream), g_ev_join, 0);
-          *forked = false;
-        }
+        st.join_all();
         // p[3] = lr_state {lr, decay, iterations, lr_t}: the schedule kernel derives this step's lr_t, the update reads it
         rc = se_sgd_schedule((float*)p[3], stream);
         if (rc == SE_OK)
@@ -507,11 +488,7 @@ static int run_ops_impl(const se_op* ops, int n, int mode, void* stream, bool* f
         break;
       case SE_OP_ADAGRAD_APPLY:
         // the Adagrad update in place of SGD_APPLY: same p[0..5] (p[5] = accumulators), f[0] = epsilon, f[1] = clipnorm
-        if (*forked) {
-          cudaEventRecord(g_ev_join, g_side);
-          cudaStreamWaitEvent(as_stream(stream), g_ev_join, 0);
-          *forked = false;
-        }
+        st.join_all();
         rc = se_sgd_schedule((float*)p[3], stream);
         if (rc == SE_OK)
           rc = se_adagrad_apply_devlr((float*)p[0], (const float*)p[1], (float*)p[5], (int64_t)(uintptr_t)p[2],

@@ -764,14 +764,20 @@ static int bn_bwd_plan(long long rows, int C, int sms, long long* per_cta, int* 
   if (per_cta) *per_cta = per_l;
   if (grid) *grid = gridf;
   if (smem) *smem = bytes;
-  static const bool no_fuse = getenv("SE_BN_NO_FUSE") != nullptr;
-  static const bool no_reg = getenv("SE_BN_NO_REG") != nullptr;
   const int C4 = C >> 2;
-  if (!no_fuse && !no_reg && gridf <= sms && C <= BNR_MAXC && (512 % C4) == 0 && per_l * C4 <= (long long)BNR * 512)
+  if (gridf <= sms && C <= BNR_MAXC && (512 % C4) == 0 && per_l * C4 <= (long long)BNR * 512)
     return SE_BN_BWD_SLAB_REG;
-  if (!no_fuse && bytes <= BNF_MAX_SMEM && gridf <= sms)
+  if (bytes <= BNF_MAX_SMEM && gridf <= sms)
     return (512 % C4) == 0 ? SE_BN_BWD_SLAB_QUAD : SE_BN_BWD_SLAB_ATOMIC;   // bn_bwd_fused_kernel's fixed_quad (512 threads)
   return SE_BN_BWD_VEC;
+}
+
+int init_bn_bwd() {
+  if (cudaFuncSetAttribute(bn_bwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BNF_MAX_SMEM) != cudaSuccess) {
+    set_error("init_bn_bwd: cannot raise the shared-memory limit");
+    return SE_ERR_CUDA;
+  }
+  return SE_OK;
 }
 
 }  // namespace se
@@ -833,19 +839,13 @@ int se::bn_bwd(const float* x, const float* y, const float* dout, int64_t rows, 
   long long* bn_trace = bn_trace_env ? reinterpret_cast<long long*>(strtoull(bn_trace_env, nullptr, 0)) : nullptr;
   if (path == SE_BN_BWD_SLAB_REG) {
     launch_grid_barrier(bn_bwd_reg_kernel, dim3(gridf), dim3(512), 0, as_stream(stream), x, y ? y : x, dout, rows, C, gamma, save_mean, save_invstd,
-           relu, relu_in, dx, beta_dx, dres, beta_res, dgamma, dbeta, scratch, (int)per_l, early && pdl_enabled() ? 1 : 0, bn_trace);
+           relu, relu_in, dx, beta_dx, dres, beta_res, dgamma, dbeta, scratch, (int)per_l, early ? 1 : 0, bn_trace);
     return check_launch("bn_bwd_reg_kernel");
   }
   if (path == SE_BN_BWD_SLAB_QUAD || path == SE_BN_BWD_SLAB_ATOMIC) {
     // fused single-launch path: every CTA's slab of x and g fits in shared memory (one CTA per SM)
-    static bool configured = false;
-    if (!configured) {
-      if (cudaFuncSetAttribute(bn_bwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BNF_MAX_SMEM) != cudaSuccess) {
-        set_error("bn_bwd_fused: cannot raise the shared-memory limit");
-        return SE_ERR_CUDA;
-      }
-      configured = true;
-    }
+    const int rc = ensure_setup();
+    if (rc) return rc;
     // at least 116 KB per CTA would be needed to force one CTA per SM; co-residency only needs grid <= #SMs
     launch_grid_barrier(bn_bwd_fused_kernel, dim3(gridf), dim3(512), smem, as_stream(stream), x, y, dout, rows, C, gamma, save_mean, save_invstd, relu,
                                                                   relu_in, dx, beta_dx, dres, beta_res, dgamma, dbeta,

@@ -25,31 +25,33 @@ struct NcclApi {
   bool ok;
 };
 
-static NcclApi* nccl_api() {
-  static NcclApi api = {};
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD);          // the copy PyTorch already loaded
-    if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
-    if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
-    if (h) {
-      api.GetUniqueId = (decltype(api.GetUniqueId))dlsym(h, "ncclGetUniqueId");
-      api.CommInitRank = (decltype(api.CommInitRank))dlsym(h, "ncclCommInitRank");
-      api.CommDestroy = (decltype(api.CommDestroy))dlsym(h, "ncclCommDestroy");
-      api.AllReduce = (decltype(api.AllReduce))dlsym(h, "ncclAllReduce");
-      api.GroupStart = (decltype(api.GroupStart))dlsym(h, "ncclGroupStart");
-      api.GroupEnd = (decltype(api.GroupEnd))dlsym(h, "ncclGroupEnd");
-      api.GetErrorString = (decltype(api.GetErrorString))dlsym(h, "ncclGetErrorString");
-      api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllReduce && api.GroupStart && api.GroupEnd;
-    }
+static NcclApi load_nccl() {
+  NcclApi api = {};
+  void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD);          // the copy PyTorch already loaded
+  if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
+  if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
+  if (h) {
+    api.GetUniqueId = (decltype(api.GetUniqueId))dlsym(h, "ncclGetUniqueId");
+    api.CommInitRank = (decltype(api.CommInitRank))dlsym(h, "ncclCommInitRank");
+    api.CommDestroy = (decltype(api.CommDestroy))dlsym(h, "ncclCommDestroy");
+    api.AllReduce = (decltype(api.AllReduce))dlsym(h, "ncclAllReduce");
+    api.GroupStart = (decltype(api.GroupStart))dlsym(h, "ncclGroupStart");
+    api.GroupEnd = (decltype(api.GroupEnd))dlsym(h, "ncclGroupEnd");
+    api.GetErrorString = (decltype(api.GetErrorString))dlsym(h, "ncclGetErrorString");
+    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllReduce && api.GroupStart && api.GroupEnd;
   }
+  return api;
+}
+
+static NcclApi* nccl_api() {
+  static NcclApi api = load_nccl();
   return &api;
 }
 
 static ncclComm_t g_comm = nullptr;
 static int g_rank = 0, g_world = 1;
 static cudaStream_t g_comm_stream = nullptr;
+static cudaEvent_t g_comm_event = nullptr;   // orders the communication stream against se_run_ops' streams
 
 static int nccl_fail(const char* what, ncclResult_t r) {
   NcclApi* a = nccl_api();
@@ -58,6 +60,7 @@ static int nccl_fail(const char* what, ncclResult_t r) {
 }
 
 cudaStream_t comm_stream() { return g_comm_stream; }
+cudaEvent_t comm_event() { return g_comm_event; }
 bool comm_ready() { return g_comm != nullptr; }
 
 // sum all-reduce (in place) of `nranges` element ranges of a float buffer on stream `st`, one NCCL group
@@ -97,19 +100,21 @@ extern "C" int se_comm_init(int rank, int world, const void* unique_id, int byte
   NcclApi* a = nccl_api();
   if (!a->ok) { set_error("se_comm_init: libnccl.so.2 is not available in this process"); return SE_ERR_UNSUPPORTED; }
   if (g_comm) { set_error("se_comm_init: a communicator already exists (se_comm_destroy first)"); return SE_ERR_ARG; }
+  if (!g_comm_stream) {   // the stream and event outlive a communicator: se_comm_destroy keeps them for the next one
+    int lo = 0, hi = 0;
+    cudaDeviceGetStreamPriorityRange(&lo, &hi);
+    if (cudaStreamCreateWithPriority(&g_comm_stream, cudaStreamNonBlocking, hi) != cudaSuccess ||
+        cudaEventCreateWithFlags(&g_comm_event, cudaEventDisableTiming) != cudaSuccess) {
+      g_comm_stream = nullptr;
+      set_error("se_comm_init: cannot create the communication stream");
+      return SE_ERR_CUDA;
+    }
+  }
   ncclUniqueId id;
   memcpy(&id, unique_id, sizeof(id));
   ncclResult_t r = a->CommInitRank(&g_comm, world, id, rank);
   if (r != ncclSuccess) { g_comm = nullptr; return nccl_fail("ncclCommInitRank", r); }
   g_rank = rank; g_world = world;
-  if (!g_comm_stream) {
-    int lo = 0, hi = 0;
-    cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    if (cudaStreamCreateWithPriority(&g_comm_stream, cudaStreamNonBlocking, hi) != cudaSuccess) {
-      set_error("se_comm_init: cannot create the communication stream");
-      return SE_ERR_CUDA;
-    }
-  }
   return SE_OK;
 }
 

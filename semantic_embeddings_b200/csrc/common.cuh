@@ -16,6 +16,10 @@ int bn_bwd(const float* x, const float* y, const float* dout, int64_t rows, int 
            float* dbeta, double* scratch, int early, void* stream);
 void count_launch(int n = 1);
 int sm_count();
+// The library's one-time set-up (api.cu), run by se_init and by every entry point that depends on it: the shared-memory
+// limits of the kernels that need more than 48 KB, and se_run_ops' side stream with its events and weight-gradient
+// workspace.  Runs once per process, thread-safe; a failure is returned, with its message, by every later call.
+int ensure_setup();
 // weight gradients without atomics (conv_wgrad_tc.cu): split-K partial sums go to slices of a workspace of the library
 // (one per device and stream) and wgrad_reduce adds the slices into dW / dbias in slice order, so the result is the same
 // on every run.  Slice k holds [T = kh*kw*Cin*Cout] dW partials at ws + k*T; the bias partials follow all slices,
@@ -48,12 +52,11 @@ inline int check_launch(const char* what) {
 // (barrier init, descriptor prefetch) while the preceding grid drains, and it blocks in
 // griddepcontrol.wait -- which returns only when ALL prerequisite grids have completed and flushed their writes --
 // before it touches global memory.  Invariant that keeps this safe at any chain depth: no kernel reads or writes
-// global memory before its griddepcontrol.wait.  SE_NO_PDL=1 turns the attribute off (kernels then serialise fully).
+// global memory before its griddepcontrol.wait.
 // One documented exception: bn_bwd_reg_kernel with its `early` hint READS (never writes) x, y and the saved statistics
 // before the wait.  That is safe only because those tensors were produced by the forward pass and the backward plan
 // starts with a cudaMemsetAsync of the gradient buffer -- a full stream dependency that drains every forward kernel;
 // Engine._build_plans asserts that memset when it sets the hint (removing it would turn the prefetch into a race).
-bool pdl_enabled();
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_grid_sync() { pdl_trigger(); pdl_wait(); }
@@ -69,7 +72,7 @@ inline void launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, c
   attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr.val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = &attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);   // errors surface through check_launch()
 }
 

@@ -27,7 +27,6 @@ static ConvP to_p(const se_conv_desc* d) {
 }
 
 constexpr size_t WGRAD3X3_MAX_SMEM = 160 * 1024;
-int init_conv_simt();
 
 // ---------------------------------------------------------------------------------------- forward
 template <int BM, int BN, int TM, int TN, bool VEC>
@@ -759,12 +758,10 @@ static int launch_wgrad3x3(const ConvP& p, const float* x, const float* dy, floa
   int gx = (int)wgrad_fit_splits(min(num_tiles, max(1, (2 * sm_count()) / (cy * cz))), T, p.Cout);
   auto kern = conv_wgrad3x3_kernel<NCI, NCO>;
   if (smem > WGRAD3X3_MAX_SMEM) return SE_ERR_UNSUPPORTED;
-  if (smem > 48 * 1024) {   // attribute normally raised by se_init(); direct C-ABI callers get it lazily
-    static bool inited = false;
-    if (!inited) { int rc = init_conv_simt(); if (rc) return rc; inited = true; }
-  }
+  int rc = ensure_setup();
+  if (rc) return rc;
   float* ws = nullptr;
-  int rc = wgrad_workspace(gx * (T + p.Cout), st, &ws);
+  rc = wgrad_workspace(gx * (T + p.Cout), st, &ws);
   if (rc) return rc;
   launch(kern, dim3(gx, cy, cz), dim3(256), smem, st, p, x, dy, ws ? ws : dw, ws ? (dbias ? ws + gx * T : nullptr) : dbias, TH,
          tiles_per_img, num_tiles, ws ? 0 : 1);

@@ -490,16 +490,10 @@ int init_conv_tc() {
   return SE_OK;
 }
 
-static bool g_tc_inited = false;
-static int ensure_init() {
-  if (!g_tc_inited) { int rc = init_conv_tc(); if (rc) return rc; g_tc_inited = true; }
-  return SE_OK;
-}
-
 // w_t = the transposed kernel copy [tap][co][ci], w_t_lo its low parts (error-compensated mode)
 int conv_fwd_tc(const ConvPlan& pl, const se_conv_desc* d, const float* x, const float* w_t, const float* w_t_lo,
                 const float* bias, const float* residual, float* y, int relu, double* stats, cudaStream_t st) {
-  int rc = ensure_init();
+  int rc = ensure_setup();
   if (rc) return rc;
   ConvTcParams p = pl.tc;
   p.relu = relu; p.bias = bias; p.residual = residual; p.out = y; p.stats = stats;
@@ -511,7 +505,7 @@ int conv_fwd_tc(const ConvPlan& pl, const se_conv_desc* d, const float* x, const
 // conv3x3s2_tc_ok) adds dY W[r, s]^T into dx[:, r::2, s::2, :], whose last column / row may not exist.
 int conv_dgrad_tc(const ConvPlan& pl, const se_conv_desc* d, const float* dy, const float* w, const float* w_lo, float* dx,
                   float beta, cudaStream_t st) {
-  int rc = ensure_init();
+  int rc = ensure_setup();
   if (rc) return rc;
   const bool nine = pl.family == CONV_TC_DGRAD_3X3S2;
   if ((nine || pl.family == CONV_TC_1X1_S2) && beta == 0.f &&

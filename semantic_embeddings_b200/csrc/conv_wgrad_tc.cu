@@ -350,12 +350,12 @@ static void wgrad_go(const ConvPlan& pl, cudaStream_t st, const float* x, const 
 }
 
 int conv_wgrad_tc(const ConvPlan& pl, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st) {
-  static bool inited = false;
-  if (!inited) { int rc0 = init_conv_wgrad_tc(); if (rc0) return rc0; inited = true; }
+  int rc = ensure_setup();
+  if (rc) return rc;
   WgTcParams p = pl.wg;
   p.dw = dw; p.dbias = dbias;
   const long long T = (long long)p.KK * p.Cout, splits = 2LL * pl.grid.x;
-  int rc = wgrad_workspace(splits * (T + p.Cout), st, &p.ws);
+  rc = wgrad_workspace(splits * (T + p.Cout), st, &p.ws);
   if (rc) return rc;
   switch (pl.wg_bn) {
     case 16: wgrad_go<16>(pl, st, x, dy, p); break;

@@ -202,6 +202,15 @@ resample_crop_kernel(const unsigned char* __restrict__ src, const se_resample_de
 
 }  // namespace
 
+// plan() asks for at most kSmemBudget bytes
+int init_resample_crop() {
+  if (cudaFuncSetAttribute(resample_crop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget) != cudaSuccess) {
+    set_error("init_resample_crop: cannot raise the shared-memory limit");
+    return SE_ERR_CUDA;
+  }
+  return SE_OK;
+}
+
 }  // namespace se
 
 using namespace se;
@@ -251,7 +260,8 @@ extern "C" int se_resample_crop_batch(const unsigned char* src, const se_resampl
   int KH, KV, S;
   const int smem = plan(desc_host, B, crop_h, crop_w, &KH, &KV, &S);
   if (smem < 0) return smem;
-  cudaFuncSetAttribute(resample_crop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  const int rc = ensure_setup();
+  if (rc) return rc;
   const dim3 grid((crop_h + kRows - 1) / kRows, B);
   launch(resample_crop_kernel, grid, dim3(kThreads), (size_t)smem, as_stream(stream), src, desc_dev, crop_h, crop_w, KH, KV,
          S, mean[0], mean[1], mean[2], std[0], std[1], std[2], bgr, (unsigned long long)seed, out);

@@ -439,8 +439,7 @@ extern "C" int se_embed_head_path(int B, int D, int C, int loss_kind, int want_m
 
 // The plans allow up to 48 KB of dynamic shared memory; the kernel's static s_red / s_hinge come on top of that, past
 // the default limit of 48 KB in all (a row split over 8 warps at Dp = 1532 or 1536, and a warp per row at Dp > 3060,
-// failed to launch).  Called by se_init, before any graph capture; a standalone first call makes it then.
-static bool g_head_inited = false;
+// failed to launch).  Called once by ensure_setup.
 namespace se {
 int init_head() {
   for (const void* k : {(const void*)embed_head_kernel<true>, (const void*)embed_head_kernel<false>})
@@ -448,7 +447,6 @@ int init_head() {
       set_error("init_head: cannot raise the shared-memory limit");
       return SE_ERR_CUDA;
     }
-  g_head_inited = true;
   return SE_OK;
 }
 }  // namespace se
@@ -464,7 +462,8 @@ static int embed_head(const float* z, int ldz, const int32_t* labels, const floa
   const int rc = head_plan(B, D, C, loss_kind, acc || rank_out, loss_kind == SE_LOSS_DEVISE_RANK && (loss || dz), vec,
                            &p);
   if (rc < 0) return rc;
-  if (!g_head_inited) { const int irc = init_head(); if (irc) return irc; }
+  const int irc = ensure_setup();
+  if (irc) return irc;
   if (p.path & SE_HEAD_VEC)
     launch(embed_head_kernel<true>, dim3(p.grid), dim3(p.nwarps * 32), p.smem, as_stream(stream), z, ldz, labels, E, ldE, B,
            D, C, loss_kind, loss_scale, extra_dx, x_out, loss, acc, dz, rank_out, p.es_classes, p.split, margin);

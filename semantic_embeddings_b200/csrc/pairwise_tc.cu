@@ -301,15 +301,11 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_const
 
 // ---- host side
 int init_pairwise_tc() {
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(pairwise_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, PW_SMEM) != cudaSuccess ||
-        cudaFuncSetAttribute(pairwise_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, PW_SMEM) != cudaSuccess ||
-        cudaFuncSetAttribute(pairwise_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, PW_SMEM) != cudaSuccess) {
-      set_error("pairwise_tc: cannot reserve %d bytes of shared memory", PW_SMEM);
-      return SE_ERR_CUDA;
-    }
-    configured = true;
+  if (cudaFuncSetAttribute(pairwise_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, PW_SMEM) != cudaSuccess ||
+      cudaFuncSetAttribute(pairwise_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, PW_SMEM) != cudaSuccess ||
+      cudaFuncSetAttribute(pairwise_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, PW_SMEM) != cudaSuccess) {
+    set_error("pairwise_tc: cannot reserve %d bytes of shared memory", PW_SMEM);
+    return SE_ERR_CUDA;
   }
   return SE_OK;
 }
@@ -374,7 +370,7 @@ static int pw_launch(const PwLayout& L, int N, int row0, int rows, const __half*
   p.sq = L.sq; p.sq_b = sq_b; p.scal = L.scal; p.ncols = ncols;
   p.tau_sum = nullptr; p.tau_scale = 0.f; p.cnt = nullptr; p.cand_val = nullptr; p.cand_idx = nullptr; p.capr = 0; p.jsel = 1;
   if (e1) { p.jsel = e1->jsel; p.tau_sum = e1->tau_sum; p.tau_scale = e1->tau_scale; p.cnt = e1->cnt; p.cand_val = e1->cand_val; p.cand_idx = e1->cand_idx; p.capr = e1->capr; }
-  int rc0 = init_pairwise_tc();
+  int rc0 = ensure_setup();
   if (rc0) return rc0;
   int grid = min(sm_count(), p.tiles_m * p.tiles_n);
   // candidate sweep: a row block may be shared by at most two CTAs (regions are per (row, column half, part))

@@ -157,6 +157,14 @@ row_topk_kernel(const float* __restrict__ dist, long long ld, int rows, int n, i
   }
 }
 
+int init_row_topk() {
+  if (cudaFuncSetAttribute(row_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
+    set_error("init_row_topk: cannot raise the shared-memory limit");
+    return SE_ERR_CUDA;
+  }
+  return SE_OK;
+}
+
 }  // namespace se
 
 using namespace se;
@@ -173,14 +181,8 @@ extern "C" int se_row_topk(const float* dist, int64_t ld, int rows, int n, int k
     set_error("se_row_topk: a row of %d values does not fit in shared memory (max ~52000)", n);
     return SE_ERR_UNSUPPORTED;
   }
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(row_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
-      set_error("se_row_topk: cannot raise the shared-memory limit");
-      return SE_ERR_CUDA;
-    }
-    configured = true;
-  }
+  const int rc = ensure_setup();
+  if (rc) return rc;
   const int grid = min(rows, sm_count());
   launch(row_topk_kernel, dim3(grid), dim3(TK_THREADS), smem, as_stream(stream), dist, (long long)ld, rows, n, k, out_val, out_idx, ldo);
   return check_launch("row_topk_kernel");

@@ -878,7 +878,7 @@ class Engine:
         cg = self._graphs.get(which)
         if cg is None:
             # capture only (no warm-up run: a plan has side effects -- optimizer step, moving statistics);
-            # se_init() has already done every lazy per-kernel attribute setup the library needs
+            # se_init() has already done the library's one-time set-up, which must not happen inside a capture
             torch.cuda.synchronize(self.dev)
             cg = torch.cuda.CUDAGraph()
             with torch.cuda.graph(cg):

@@ -2,7 +2,10 @@
 for every BatchNorm layer of the benchmarked networks and at the edges of its rule, and the float64 BatchNorm reference
 of tests/test_gpu_bn_pool.py against torch.autograd."""
 import collections
+import json
 import os
+import subprocess
+import sys
 
 import pytest
 import torch
@@ -121,6 +124,22 @@ def test_bn_backward_path_boundaries(built_lib):
     # the register-slab limit at 114 SMs: 114 x 1024 rows
     assert lib.se_bn_bwd_path(114 * 1024, 16, PCIE) == REG and lib.se_bn_bwd_path(114 * 1024 + 1, 16, PCIE) == QUAD
     assert lib.se_bn_bwd_path(0, 16, SXM) < 0 and lib.se_bn_bwd_path(16, 0, SXM) < 0
+
+
+def test_bn_backward_path_ignores_the_environment(built_lib):
+    """The plan depends on (rows, C, sms) alone: a process with SE_BN_NO_FUSE and SE_BN_NO_REG set (switches the library
+    once read) picks the same path for every layer of the tables above."""
+    cases = sorted(set(BOUNDARY_PLAN) | {rc for plan in NETWORK_PLAN.values() for rc in plan})
+    cases = [(rows, C, sms) for rows, C in cases for sms in (SXM, PCIE)]
+    code = ('import ctypes, json, sys\n'
+            'f = ctypes.CDLL(sys.argv[1]).se_bn_bwd_path\n'
+            'f.argtypes = [ctypes.c_int64, ctypes.c_int, ctypes.c_int]\n'
+            'print(json.dumps([f(*c) for c in json.loads(sys.argv[2])]))\n')
+    env = dict(os.environ, SE_BN_NO_FUSE='1', SE_BN_NO_REG='1')
+    out = subprocess.run([sys.executable, '-c', code, built_lib.LIB_PATH, json.dumps(cases)], env=env, capture_output=True,
+                         text=True, check=True).stdout
+    lib = built_lib.load()
+    assert json.loads(out) == [lib.se_bn_bwd_path(*c) for c in cases]
 
 
 BN_REF_CASES = [
