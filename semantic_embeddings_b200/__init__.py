@@ -6,7 +6,7 @@ all-pairs retrieval distance matrix, as hand-written sm_90a CUDA behind a C ABI
   utils.py              build_network, l2norm, inv_correlation, nn_accuracy, get_lr_schedule  (reference utils.py)
   sgdr_callback.py      SGDR                                                                    (reference sgdr_callback.py)
   evaluate_retrieval.py pairwise_retrieval                                                      (reference evaluate_retrieval.py)
-  models/               plainnet, cifar_resnet, wide_residual_network, resnet50                 (reference models/)
+  models/               plainnet, cifar_resnet, wide_residual_network, resnet50, resnet_v1      (reference models/)
   engine.py             the layer-list executor that replaces Keras' compile/fit/predict
 """
 __version__ = '0.1'
