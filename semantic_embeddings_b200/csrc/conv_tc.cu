@@ -98,7 +98,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                const __grid_constant__ CUtensorMap map_bl, ConvTcParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  // 1024-byte aligned (the swizzle pattern starts over), as an offset from smem_raw rather than a rounded integer: the
+  // compiler then knows that every pointer derived from it is in shared memory and reads A with LDS.  (From a rounded
+  // uintptr_t it cannot tell, and emits generic loads, whose longer latency sits on every stage's critical path.)
+  uint8_t* smem = smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023);
   uint8_t* ring = smem + p.ring_off;
   uint64_t* full = reinterpret_cast<uint64_t*>(ring + (size_t)p.stages * p.stage_bytes);
   uint64_t* empty = full + CT_MAX_STAGES;
@@ -171,10 +174,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   if (p.res) mbar_wait(abar, 0);
-  int stage = 0, phase = 0;
+  // stage it = (filter tap (r, s), channel block kb), counted along instead of divided out: the A addresses of a
+  // stage are on its critical path
+  int stage = 0, phase = 0, kb = 0, r = 0, s = 0;
   for (int it = 0; it < nk; ++it) {
-    const int tap = it / p.kblocks, kb = it - tap * p.kblocks;
-    const int r = tap / p.taps, s = tap - r * p.taps;
     mbar_wait(&full[stage], phase);
     const uint8_t* sst = ring + (size_t)stage * p.stage_bytes;
     const uint8_t* abase = p.res ? smem + (size_t)kb * p.a_bytes : sst;
@@ -221,6 +224,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[stage]);
     if (++stage == p.stages) { stage = 0; phase ^= 1; }
+    if (++kb == p.kblocks) { kb = 0; if (++s == p.taps) { s = 0; ++r; } }
   }
 
   // ===================== epilogue on the registers: the two rows of this thread, BN/8 column pairs each
