@@ -33,6 +33,7 @@ import center_loss_oracle
 import classifier_oracle
 import devise_oracle
 import labelembed_oracle
+import reduction_oracle
 from oracle import nn as onn
 from oracle import train as otrain
 
@@ -172,14 +173,18 @@ def maxpool_backward(node, x, y, dy):
     return dxp[:, pt:pt + x.shape[1], pl:pl + x.shape[2]]
 
 
-def backward(node, ins, y, dy, p, ctx=None, need=None, fwd=None):
+def backward(node, ins, y, dy, p, ctx=None, need=None, fwd=None, mags=False):
     """Local gradients of one node.  ins: its float64 inputs; y: its output (the ReLU masks are y > 0); dy: the upstream
     gradient of its output (None for a loss node without consumers); need[i]: whether input i takes a gradient (None:
     all).  fwd: the node's forward() dict, if at hand (BatchNorm statistics).
-    Returns {'dx': [contribution to input i, or None], <param name>: gradient}."""
+    Returns {'dx': [contribution to input i, or None], <param name>: gradient}; with mags, also 'mag': {<param name>:
+    the same sum over the magnitudes of its terms} for the conv / dense kernels and biases and BatchNorm's gamma / beta
+    (reduction_oracle: the M their errors are measured against)."""
     op, a, nm = node.op, node.attrs, node.name
     need = [True] * len(ins) if need is None else need
     out = {'dx': [None] * len(ins)}
+    if mags:
+        out['mag'] = {}
     if op in ('conv', 'dense'):
         x, W = ins[0], p[nm + '/kernel']
         want_dx = need[0] and not a.get('stop_gradient')
@@ -196,6 +201,14 @@ def backward(node, ins, y, dy, p, ctx=None, need=None, fwd=None):
                 out['dx'][0] = gs[1]
         if a['use_bias']:
             out[nm + '/bias'] = dy.reshape(-1, dy.shape[-1]).sum(0)
+        if mags:
+            if op == 'dense':
+                out['mag'][nm + '/kernel'] = x.abs().t() @ dy.abs()
+            else:
+                pt, _, pl, _ = pads(node)
+                out['mag'][nm + '/kernel'] = reduction_oracle.conv_wgrad(x.abs(), dy.abs(), a['k'], a['stride'], pt, pl)
+            if a['use_bias']:
+                out['mag'][nm + '/bias'] = dy.abs().reshape(-1, dy.shape[-1]).sum(0)
         if a.get('residual') and need[1]:
             out['dx'][1] = dy
         return out
@@ -207,6 +220,8 @@ def backward(node, ins, y, dy, p, ctx=None, need=None, fwd=None):
         dx, dgamma, dbeta, g = bn_oracle.backward(x, fwd['xhat'], fwd['invstd'], p[nm + '/gamma'], dy, keep, relu_in(node))
         out['dx'][0] = dx if need[0] else None
         out[nm + '/gamma'], out[nm + '/beta'] = dgamma, dbeta
+        if mags:
+            _, out['mag'][nm + '/gamma'], _, out['mag'][nm + '/beta'] = reduction_oracle.bn_ref(g, fwd['xhat'])
         if a['residual'] and need[1]:
             out['dx'][1] = bn_oracle.shortcut_backward(g, ins[1].shape[-1], a['res_pad_lo'], a['res_pool'])
         return out
@@ -288,10 +303,10 @@ def grad_class(ops):
     raise ValueError(ops)
 
 
-def backward_walk(eng, act, upstream, p, ctx):
+def backward_walk(eng, act, upstream, p, ctx, mags=False):
     """The backward pass node by node, last node first.  act(name) -> float64 activation; upstream(name) -> the
     float64 gradient to feed the producer of that tensor (the engine's own in the GPU test; pass None to use the
-    walk's own sums); p: float64 parameters.  Yields, in order:
+    walk's own sums); p: float64 parameters; mags: backward(mags=True).  Yields, in order:
       ('grad', tensor name, expected gradient, contributing ops)   once every consumer has contributed
       ('node', node, local gradients of backward())
     """
@@ -311,7 +326,7 @@ def backward_walk(eng, act, upstream, p, ctx):
         need = [has_gradient(eng, i) for i in n.inputs]
         ins = [act(i.name) for i in n.inputs]
         y = act(t.name) if n.op in ('bn', 'maxpool', 'add', 'relu') else None
-        local = backward(n, ins, y, dy, p, ctx, need)
+        local = backward(n, ins, y, dy, p, ctx, need, mags=mags)
         del ins, y, dy
         for k, c in enumerate(local['dx']):
             if c is None:

@@ -27,8 +27,12 @@ The configurations cover every objective and optimizer of Engine at the trainers
 networks (resnet-110-wfc: 32/64/128 channels): the label-smoothed classifier, DeViSE with Adagrad (both phases), the
 label embedding network and the center loss with learned and fixed centroids.
 
-Errors are max-norm relative.  Bounds (TOL) are about 3x the largest value measured on an H100 80GB HBM3 (132 SMs) over
-the configurations, never above the 2e-5 per-op contract of DESIGN.md section 2; the measured value stands beside each.
+Errors are max-norm relative, except those of the gradient reductions -- conv / dense weight and bias gradients,
+BatchNorm dgamma / dbeta -- which are err_cond: each element against the float64 sum over the magnitudes of its terms
+(tests/reduction_oracle.py, DESIGN.md section 2); the report line also has each of their largest max-norm errors, the
+kappa of the worst element, and err_cond / kappa / max-norm error of every parameter (`layers`).  Bounds (TOL) are about
+3x the largest value measured on an H100 80GB HBM3 (132 SMs) over the configurations, never above the 2e-5 per-op
+contract of DESIGN.md section 2; the measured value stands beside each.
 The classes up to 'add_infer_y' were measured over the first five configurations at a 400 W power limit (the new
 configurations stay within them); the classes after it, over all configurations at a 700 W power limit.  The whole file
 runs in about 25 s there."""
@@ -39,6 +43,7 @@ import numpy as np
 import pytest
 import torch
 
+import reduction_oracle as ro
 import step_oracle as so
 from oracle import nn as onn
 from test_gpu_ops import _lib, report
@@ -48,16 +53,27 @@ pytestmark = pytest.mark.gpu
 G = os.path.join(os.path.dirname(__file__), 'golden')
 
 TOL = {
-    # convolutions and dense layers (fp32 / error-compensated TF32 kernels).  The weight gradient is the one bound at the
-    # contract: 1.54e-5 on ResNet-50's res2a_branch2a (1x1, 100352 pixels summed), 1.04e-5 on ResNet-110's stage-1 3x3
-    # layers in SE_MODE_TF32X3 (1.6e-6 in SE_MODE_F32)
+    # the gradient reductions -- conv / dense weight and bias gradients, BatchNorm dgamma / dbeta -- are held to err_cond
+    # (reduction_oracle: each element against the same sum over the magnitudes of its terms), about 3x the largest value
+    # measured over every configuration of this file, test_gpu_step_layers_448.py, _classes.py and
+    # test_deep_resnets_gpu.py (H100 80GB HBM3, 700 W), where they stand; the upstream atomics vary the inputs from run
+    # to run.  One bound holds at every size: no configuration needs a raise
+    'conv_dw': 4e-6,          # 1.25e-6 (DeViSE res3-18y); <= 4.7e-7 elsewhere
+    # tensor-core weight gradients that sum at least 2^18 pixels (LONG_PX: the stride-1 1x1 layers of stage 2 at 448
+    # px, kappa up to 400): one accumulator tile per 32-pixel chunk in conv_wgrad_tc_kernel (NP = 1) takes them to
+    # 1.5e-7 .. 1.8e-7, past this bound
+    'conv_dw_long_tc': 1.4e-7,    # 4.9e-8 (res2c_branch2c, CUB at B = 24)
+    # ... and their max-norm error: one tile per chunk takes res2a_branch2a to 2.1e-5 .. 3.4e-5 of the largest dW
+    'conv_dw_long_tc_norm': 1e-5,  # max-norm, 5.2e-6 (res2a_branch2a, NAB at B = 32)
+    'conv_db': 7.5e-7,        # 3.5e-7 (conv1/bias, ResNet-50 at B = 64)
+    'dense_dw': 6.5e-6,       # 2.15e-6 (iNat-2018 embedding/kernel: 64 rows)
+    'dense_db': 1.5e-6,       # 4.8e-7
+    'bn_dgamma': 3e-6,        # 1.23e-6 (cls_bn/gamma, resnet-101 ILSVRC); 1.05e-6 on embedding_bn/gamma (100 rows)
+    'bn_dbeta': 5e-7,         # 1.6e-7
+    # convolutions and dense layers (fp32 / error-compensated TF32 kernels), max-norm
     'conv_y': 5e-6,           # measured 1.5e-6
-    'conv_dw': 2e-5,          # 1.54e-5
-    'conv_db': 1.5e-7,        # 4.3e-8 (against the sum of |dy|)
     'conv_dx': 4e-6,          # 1.3e-6
     'dense_y': 2.5e-6,        # 7.7e-7
-    'dense_dw': 2.5e-6,       # 8.6e-7
-    'dense_db': 6e-7,         # 2.1e-7
     'dense_dx': 4.5e-6,       # 1.5e-6
     # BatchNorm: training forward, saved and moving statistics, backward
     'bn_y': 6e-7,             # 2.0e-7
@@ -66,8 +82,6 @@ TOL = {
     'bn_moving_mean': 1e-6,   # 3.4e-7
     'bn_moving_variance': 4.5e-7,  # 1.4e-7
     'bn_dx': 5e-7,            # 1.7e-7
-    'bn_dgamma': 8e-7,        # 2.6e-7
-    'bn_dbeta': 4.5e-6,       # 1.4e-6
     # float64 sums of the BatchNorm input (fused convolution epilogue or se_bn_stats) against the sums of the stored input
     'stats_sum': 2e-7,        # 5.9e-8
     'stats_sumsq': 8e-8,      # 2.6e-8
@@ -106,9 +120,8 @@ TOL = {
     # f32decay class above holds the same layers to 8e-8)
     'bn_moving_variance_adagrad': 3e-6,    # 9.5e-7
     # 'embedding_bn', the BatchNorm behind relu(z) in the label embedding and center loss branches (100 rows): 2.3e-6
-    # in its output and 2.0e-6 in dgamma.  Every other BatchNorm, the 2-D ones included (<= 2e-7), keeps bn_y / bn_dgamma
+    # in its output.  Every other BatchNorm, the 2-D ones included (<= 2e-7), keeps bn_y
     'embedding_bn_y': 7e-6,       # 2.3e-6
-    'embedding_bn_dgamma': 6e-6,  # 2.0e-6
     # label-smoothed cross-entropy (learn_classifier.py)
     'xent_ls_y': 2e-7,        # 6.9e-8
     'xent_ls_loss': 2e-7,     # 6.9e-8
@@ -153,6 +166,7 @@ TOL = {
 }
 
 CONFIGS = so.CONFIGS
+LONG_PX = 1 << 18       # the pixel count from which the weight-gradient kernels switch to their long-sum arithmetic
 PAD = 28            # padding rows of the label embedding validation batch
 
 
@@ -162,16 +176,28 @@ def derr(got, ref):
 
 
 class Errors:
-    """Largest error per class (and where), every check counted by plan and opcode; `tol` holds the bounds."""
+    """Largest error per class (and where), every check counted by plan and opcode; `tol` holds the bounds.  `info`
+    holds report-only values: the kappa of the worst element of each reduction class, and the largest max-norm error."""
 
     def __init__(self, tol=None):
         self.tol = TOL if tol is None else tol
         self.worst = {}
+        self.info = {}
+        self.layers = {}
         self.ops = collections.defaultdict(collections.Counter)
 
     def add(self, key, err, where):
         if key not in self.worst or err > self.worst[key][0]:
             self.worst[key] = (err, where)
+
+    def add_cond(self, key, e, where):
+        """a reduction_oracle.cond_errors result: err_cond is held to the bound of `key`; every parameter's err_cond,
+        kappa and max-norm error go to the report (`layers`)"""
+        if key not in self.worst or e['err_cond'] > self.worst[key][0]:
+            self.info[key + '_kappa'] = e['kappa']
+        self.add(key, e['err_cond'], where)
+        self.info[key + '_maxnorm'] = max(self.info.get(key + '_maxnorm', 0.0), e['err_max'])
+        self.layers[where] = [float('%.3g' % e[k]) for k in ('err_cond', 'kappa', 'err_max')]
 
     def covered(self, plan, opcodes):
         self.ops[plan].update(opcodes)
@@ -365,7 +391,7 @@ def _check_backward(eng, errs, p, ctx):
     from semantic_embeddings_b200 import _lib as L
     A, Gd = eng.act, eng.grad
     covered = torch.zeros(eng.nparams, dtype=torch.bool, device='cuda')
-    walk = so.backward_walk(eng, lambda t: A[t].double(), lambda t: Gd[t].double(), p, ctx)
+    walk = so.backward_walk(eng, lambda t: A[t].double(), lambda t: Gd[t].double(), p, ctx, mags=True)
     for ev in walk:
         if ev[0] == 'grad':
             _, name, ref, ops = ev
@@ -376,6 +402,7 @@ def _check_backward(eng, errs, p, ctx):
             continue
         _, n, local = ev
         errs.covered('bwd', so.bwd_ops(eng, n))
+        mags = local.pop('mag')
         for pname, ref in local.items():
             if pname == 'dx':
                 continue
@@ -385,14 +412,18 @@ def _check_backward(eng, errs, p, ctx):
                 'dgamma' if pname.endswith('/gamma') else 'dbeta' if pname.endswith('/beta') else \
                 {so.TABLE: 'dtable', so.CENTROIDS: 'dc'}[pname]
             got = eng._pview(pname, eng.G)
-            if kind == 'db':
-                # a bias in front of a BatchNorm has a gradient that is zero in exact arithmetic (BatchNorm's dx sums to
-                # zero per channel): its error is measured against the sum of the magnitudes of the summed terms
-                dy = Gd[n.output.name]
-                mag = dy.double().abs().reshape(-1, dy.shape[-1]).sum(0).max()
-                errs.add('%s_db' % n.op, float((got.double() - ref).abs().max() / mag.clamp_min(1e-30)), pname)
+            key = '%s_%s' % (n.op, kind)
+            if key == 'conv_dw' and Gd[n.output.name].numel() // Gd[n.output.name].shape[-1] >= LONG_PX and \
+                    int(L.load().se_conv2d_path(L.ConvDesc(*eng._conv_desc(n)), eng.mode, 2)) == 1:
+                key = 'conv_dw_long_tc'
+            if key == 'conv_dw_long_tc':
+                # the second guard of these layers: their max-norm error, which their deep cancellation magnifies
+                errs.add('conv_dw_long_tc_norm', derr(got, ref), pname)
+            if pname in mags:
+                # a sum of terms that cancel (dY of a layer in front of a BatchNorm sums to zero per channel, X >= 0
+                # after a ReLU): each element against the same sum over the magnitudes of its terms (reduction_oracle)
+                errs.add_cond(key, ro.cond_errors(got, ref, mags[pname]), pname)
             else:
-                key = 'embedding_bn_dgamma' if pname == 'embedding_bn/gamma' else '%s_%s' % (n.op, kind)
                 errs.add(key, derr(got, ref), pname)
         if n.op in ('conv', 'dense'):
             d = L.ConvDesc(*eng._conv_desc(n))
@@ -491,7 +522,8 @@ def check_captured_step(cfg, tol=None, report_name='step_layers'):
     names = {v: k for k, v in vars(L).items() if k.startswith('OP_')}
     counts = {k: {names[o]: c for o, c in sorted(errs.ops[k].items())} for k in plans}
     report(report_name, case=so.config_id(cfg), seconds=round(time.time() - t0, 1), ops=counts,
-           **{k: v[0] for k, v in sorted(errs.worst.items())}, worst_at={k: v[1] for k, v in errs.worst.items()})
+           **{k: v[0] for k, v in sorted(errs.worst.items())}, worst_at={k: v[1] for k, v in errs.worst.items()},
+           **dict(sorted(errs.info.items())), layers=errs.layers)
     for k in plans:
         assert errs.ops[k] == plans[k], (k, counts[k], {names[o]: c for o, c in sorted(plans[k].items())})
     bad = errs.failures()

@@ -14,11 +14,13 @@ The tensor-core layers sum four times the pixels they sum at 224 (the weight gra
 394 272 at B = 32, 788 544 at B = 64), BatchNorm sees up to 1.6 M rows, max-pooling maps 224 to 111 and the global
 average pool averages 14 x 14.
 
-The step checks hold every class to test_gpu_step_layers.TOL except those of TOL_448, which the larger sums and the
-32-row BatchNorm of the classifier branch take close to their 224 px bounds; the report line of each configuration has
-the worst value of every class and where it occurred.  The weight gradients of the stride-1 1x1 layers stay at 5.7e-6
+The step checks hold every class to test_gpu_step_layers.TOL except those of TOL_448, which the 32-row BatchNorm of the
+classifier branch and the 14 x 14 average pool take close to their 224 px bounds; the gradient reductions keep TOL's
+err_cond bounds (reduction_oracle) at this size.  The report line of each configuration has the worst value of every
+class and where it occurred.  The weight gradients of the stride-1 1x1 layers stay at 5.7e-6 of the largest dW
 (res2a_branch2a): conv_wgrad_tc.cu starts a fresh accumulator tile every 8 pixels on such long sums (4.4e-5 with one tile
-per 32 pixels).  Measured on an H100 80GB HBM3 at a 700 W power limit, where the configurations take 9.1 s (nab-large),
+per 32 pixels), and TOL's conv_dw_long_tc (err_cond) and conv_dw_long_tc_norm (max-norm) fail without them, as does
+test_gpu_reductions.py on this step's own activations.  Measured on an H100 80GB HBM3 at a 700 W power limit, where the configurations take 9.1 s (nab-large),
 4.0 s (nab-large-finetune-init) and 2.6 s (cub-softmax), and the standalone convolutions about 110 s together (float64
 references on the host).  The engines need about 22 GB (B = 32), the device snapshot of the eval check 11 GB more."""
 import gc
@@ -35,11 +37,9 @@ from test_gpu_step_layers import TOL, check_captured_step
 pytestmark = pytest.mark.gpu
 
 # classes whose 224 px bound the 448 px configurations come close to or exceed, about 3x the largest value measured
-# over CONFIGS_448 (all within the 2e-5 per-op contract)
+# over CONFIGS_448 (all within the 2e-5 per-op contract).  The reductions need no raise under err_cond (TOL)
 TOL_448 = dict(TOL, **{
     'bn_y': 2e-6,             # 6.6e-7 on cls_bn: 32 rows (2.0e-7 at 224 px)
-    'bn_dgamma': 2e-6,        # 7.1e-7 on cls_bn/gamma
-    'conv_db': 7e-7,          # 2.4e-7 (conv1/bias: 1.6 M pixels summed in splits of 2048)
     'gap_infer_y': 2.5e-6,    # 8.8e-7: 14 x 14 maps
     'xent_y': 5e-7,           # 1.6e-7: 555 classes
 })

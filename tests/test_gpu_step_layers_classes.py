@@ -13,11 +13,16 @@ Every class is held to test_gpu_step_layers.TOL except those of TOL_CLASSES; the
 the worst value of every class and where it occurred.  Measured on an H100 80GB HBM3 at a 700 W power limit, where
 the configurations take 3 to 15 s each.
 
-The weight gradient of res2a_branch2a (1x1, 64 -> 64 at 56 x 56) sums 200 704 pixels at this batch, twice what the
-B = 32 step of test_gpu_step_layers.py sums, in front of a BatchNorm whose dY sums to zero per channel: in
-SE_MODE_TF32X3 it comes to 2.9e-5 of the largest dW, past the 2e-5 per-op bound that every other op keeps.  (Four
-partial tiles per chunk, which conv_wgrad_tc.cu takes from 2^18 pixels on, measured 2.7e-5 on it: not the remedy.)
-TOL_CLASSES holds it to 3x that, so that it cannot grow unnoticed."""
+The weight gradients are held to err_cond (reduction_oracle), like every gradient reduction of the step checks.  Under
+the max-norm measure the weight gradient of res2a_branch2a (1x1, 64 -> 64 at 56 x 56, 200 704 pixels) comes to
+2.1e-5 .. 3.4e-5 of the largest dW here, past the 2e-5 per-op bound: its dY sums to zero per channel (a BatchNorm
+follows) and X >= 0, so the largest |dW| is a small part of the sums of magnitudes (kappa = max M / max |dW| = 234 ..
+348 in two runs of the four configurations).  Its err_cond is 1.2e-7 .. 1.3e-7.  The other tensor-core weight gradients
+of the same steps, all below 2^18 pixels like it, reach 3.2e-7 .. 3.4e-7 (res4f / res5c_branch2b) and 1.9e-7 .. 2.1e-7
+in stage 2 (res2c_branch2b / 2c): by the contract it is in line, within bounds.  Like for like, with the four partial
+tiles of NP = 4 forced at this length (one measurement, not a shipped setting) it comes to 2.3e-8 .. 2.6e-8: the one
+accumulator tile per chunk that conv_wgrad_tc_kernel keeps below 2^18 pixels costs it a factor of 5, on top of the
+conditioning.  Moving that switch down is a speed trade (DESIGN.md section 5.1) left out of this test."""
 import gc
 
 import pytest
@@ -29,14 +34,12 @@ from test_gpu_step_layers import TOL, check_captured_step
 pytestmark = pytest.mark.gpu
 
 # classes whose bound the large class counts exceed or come close to, about 3x the largest value measured over
-# CONFIGS_CLASSES in two runs (dense_dx: the 2e-5 per-op contract, 2.1x).  The classifier branch's BatchNorm normalises the 1000 / 1010 / 1024 head outputs over
+# CONFIGS_CLASSES in two runs (dense_dx: the 2e-5 per-op contract, 2.1x); the reductions need none (TOL).  The classifier branch's BatchNorm normalises the 1000 / 1010 / 1024 head outputs over
 # 64 rows (cls_bn); its dense layer sums 8142 classes into each data gradient (cls_bn:2 and, in the classifier, avg_pool)
 TOL_CLASSES = dict(TOL, **{
-    'conv_dw': 9e-5,              # 2.9e-5 on res2a_branch2a (inat2019): above the 2e-5 per-op bound (docstring)
     'bn_y': 4e-6,                 # 1.4e-6 on cls_bn (ilsvrc)
     'bn_mean': 3.5e-7,            # 1.1e-7 on cls_bn
     'bn_invstd': 3.5e-6,          # 1.1e-6 on cls_bn
-    'bn_dgamma': 5e-6,            # 1.6e-6 on cls_bn/gamma
     'bn_dx': 2.5e-6,              # 7.6e-7 on cls_relu
     'stats_sum': 3.5e-7,          # 1.1e-7 on cls_bn
     'stats_sumsq': 3.5e-7,        # 1.1e-7 on cls_bn
