@@ -76,7 +76,9 @@ int se_tc_capabilities(void);
  * In SE_MODE_TF32 / SE_MODE_TF32X3 the tensor-core kernels take: 3x3 / stride 1 / pad 1 on image widths 4..56 (weight
  * gradient: ..64), 1x1 / stride 1 / pad 0 on any image size (>= 128 pixels per call), 1x1 / stride 2 / pad 0 with
  * Wo <= 32 -- channel counts in multiples of 16 (the GEMM K dimension: 16 or a multiple of 32); backward data and weight
- * gradient of 3x3 / stride 2 / pad 0 on even image sizes with >= 128 channels on both sides (nine strided 1x1 GEMMs).
+ * gradient of 3x3 / stride 2 / pad 0 on even image sizes with >= 128 channels on both sides (nine strided 1x1 GEMMs);
+ * and 3x3 / stride 1 / pad 1 on image widths 8..32 with both channel counts >= 16 and at least one of them not a
+ * multiple of 8 (PyramidNet's widths), in all three directions.
  * Every other shape (3-channel stems, the forward pass and the narrow layers of 3x3 / stride 2, 7x7, dense layers) runs on
  * the fp32 kernels in every mode; se_conv2d_path() tells which. */
 typedef struct {

@@ -125,8 +125,10 @@ extern "C" int se_conv2d_fwd_aux(const se_conv_desc* d, const float* x, const fl
   c.w_t_lo = aux && aux->w_t_lo;
   c.stats = stats != nullptr;
   ConvPlan pl;
-  if (conv_plan(d, 0, mode, c, &pl) == CONV_FP32) return conv_fwd_simt(d, x, w, bias, residual, y, relu, stats, as_stream(stream));
-  rc = conv_fwd_tc(pl, d, x, aux->w_t, aux->w_t_lo, bias, residual, y, relu, pl.fused_stats ? stats : nullptr, as_stream(stream));
+  const ConvFamily f = conv_plan(d, 0, mode, c, &pl);
+  if (f == CONV_FP32) return conv_fwd_simt(d, x, w, bias, residual, y, relu, stats, as_stream(stream));
+  rc = f == CONV_TC_ODD_3X3 ? conv_fwd_odd_tc(pl, x, aux->w_t, aux->w_t_lo, bias, residual, y, relu, as_stream(stream))
+                            : conv_fwd_tc(pl, d, x, aux->w_t, aux->w_t_lo, bias, residual, y, relu, pl.fused_stats ? stats : nullptr, as_stream(stream));
   if (rc || !stats || pl.fused_stats) return rc;
   return se_bn_stats(y, (int64_t)d->N * d->Ho * d->Wo, d->Cout, stats, stream);
 }
@@ -180,7 +182,9 @@ extern "C" int se_conv2d_dgrad_aux(const se_conv_desc* d, const float* dy, const
   c.w_lo = aux && aux->w_lo;
   c.beta = beta;
   ConvPlan pl;
-  if (conv_plan(d, 1, mode, c, &pl) == CONV_FP32) return conv_dgrad_simt(d, dy, w, dx, beta, as_stream(stream));
+  const ConvFamily f = conv_plan(d, 1, mode, c, &pl);
+  if (f == CONV_FP32) return conv_dgrad_simt(d, dy, w, dx, beta, as_stream(stream));
+  if (f == CONV_TC_ODD_3X3) return conv_dgrad_odd_tc(pl, dy, w, c.w_lo ? aux->w_lo : nullptr, dx, beta, as_stream(stream));
   return conv_dgrad_tc(pl, d, dy, w, c.w_lo ? aux->w_lo : nullptr, dx, beta, as_stream(stream));
 }
 extern "C" int se_conv2d_dgrad(const se_conv_desc* d, const float* dy, const float* w, float* dx, float beta, int mode,
@@ -206,7 +210,9 @@ extern "C" int se_conv2d_wgrad(const se_conv_desc* d, const float* x, const floa
   c.aligned = (reinterpret_cast<uintptr_t>(dw) & 15) == 0 && (reinterpret_cast<uintptr_t>(dbias) & 15) == 0;
   c.sms = sm_count();
   ConvPlan pl;
-  if (conv_plan(d, 2, mode, c, &pl) == CONV_FP32) return conv_wgrad_simt(d, x, dy, dw, dbias, as_stream(stream));
+  const ConvFamily f = conv_plan(d, 2, mode, c, &pl);
+  if (f == CONV_FP32) return conv_wgrad_simt(d, x, dy, dw, dbias, as_stream(stream));
+  if (f == CONV_TC_ODD_3X3) return conv_wgrad_odd_tc(pl, x, dy, dw, dbias, as_stream(stream));
   return conv_wgrad_tc(pl, x, dy, dw, dbias, as_stream(stream));
 }
 

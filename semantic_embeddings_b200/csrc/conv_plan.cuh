@@ -38,6 +38,26 @@ struct WgTcParams {
   float* dbias;
 };
 
+// conv_odd_tc_kernel: forward (flip 0) or data gradient (flip 1) of a 3x3 / stride 1 / 'same' layer, any channel counts
+struct OddTcParams {
+  int H, W, npx;            // image rows and pixels, N * H * W
+  int Kc, Nc;               // GEMM K channels (A tensor channels), GEMM N channels (output channels)
+  int flip;                 // 1: dgrad (B = the HWIO kernel, tap order reversed)
+  int relu;
+  float beta;               // out = beta * out + D (dgrad; 0 in the forward pass)
+  const float* bias;
+  const float* residual;
+  float* out;
+};
+
+// conv_odd_wgrad_tc_kernel: split z sums the pixels [z * per_split, (z + 1) * per_split)
+struct OddWgParams {
+  int H, W, Cin, Cout, npx, per_split;
+  float* ws;                   // [gridDim.z][9 * Cin * Cout] partial dW, then [gridDim.z][Cout] partial dbias
+  float* dw;                   // direct mode (ws == nullptr): atomics straight into dW / dbias
+  float* dbias;
+};
+
 enum ConvFamily {
   CONV_FP32,             // conv_simt.cu
   CONV_TC_3X3,           // conv_tc_kernel: 3x3 / stride 1 / 'same'
@@ -45,6 +65,7 @@ enum ConvFamily {
   CONV_TC_1X1_S2,        // conv_tc_kernel: 1x1 / stride 2 through the sub-sampled view
   CONV_TC_DGRAD_3X3S2,   // data gradient of a wide 3x3 / stride 2 layer: nine 1x1 / stride 2 launches, one per tap
   CONV_TC_WGRAD,         // conv_wgrad_tc_kernel
+  CONV_TC_ODD_3X3,       // conv_odd_tc.cu: 3x3 / stride 1 / 'same' with channel counts that are not multiples of 8
 };
 
 // The facts about one call that the choice depends on, besides descriptor, direction and mode.  The defaults are what
@@ -66,6 +87,9 @@ struct ConvPlan {
   ConvTcParams tc = {};       // conv_tc_kernel: every field but relu and the pointers
   WgTcParams wg = {};         // conv_wgrad_tc_kernel: every field but the pointers
   int wg_bn = 0, wg_np = 1;   // conv_wgrad_tc_kernel<BN, X3, NP>
+  OddTcParams od = {};        // conv_odd_tc_kernel: every field but relu, beta and the pointers
+  OddWgParams owg = {};       // conv_odd_wgrad_tc_kernel: every field but the pointers
+  int od_bn = 0;              // N tile of the conv_odd_tc kernels (32 or 64)
 };
 
 // dir 0 forward, 1 backward data, 2 weight gradient; the descriptor is valid (check_desc)
@@ -76,5 +100,10 @@ int conv_fwd_tc(const ConvPlan& p, const se_conv_desc* d, const float* x, const 
 int conv_dgrad_tc(const ConvPlan& p, const se_conv_desc* d, const float* dy, const float* w, const float* w_lo, float* dx,
                   float beta, cudaStream_t st);
 int conv_wgrad_tc(const ConvPlan& p, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st);
+int conv_fwd_odd_tc(const ConvPlan& p, const float* x, const float* w_t, const float* w_t_lo, const float* bias,
+                    const float* residual, float* y, int relu, cudaStream_t st);
+int conv_dgrad_odd_tc(const ConvPlan& p, const float* dy, const float* w, const float* w_lo, float* dx, float beta,
+                      cudaStream_t st);
+int conv_wgrad_odd_tc(const ConvPlan& p, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st);
 
 }  // namespace se

@@ -414,8 +414,11 @@ static bool tc_config(const se_conv_desc* d, ConvFamily f, int Kc, int Nc, int f
 
 bool conv3x3s2_tc_ok(const se_conv_desc* d);                                 // conv_wgrad_tc.cu
 bool wgrad_config(const se_conv_desc* d, int x3, int sms, ConvPlan* pl);    // conv_wgrad_tc.cu
+bool conv_odd_tc_ok(const se_conv_desc* d);                                  // conv_odd_tc.cu
+bool odd_config(const se_conv_desc* d, int dir, int sms, ConvPlan* pl);     // conv_odd_tc.cu
 
-ConvFamily conv_plan(const se_conv_desc* d, int dir, int mode, const ConvCall& c, ConvPlan* pl) {
+// The families of conv_tc_kernel and conv_wgrad_tc_kernel
+static ConvFamily conv_plan_wide(const se_conv_desc* d, int dir, int mode, const ConvCall& c, ConvPlan* pl) {
   *pl = ConvPlan();
   if (mode != SE_MODE_TF32 && mode != SE_MODE_TF32X3) return CONV_FP32;
   const int x3 = pl->x3 = mode == SE_MODE_TF32X3;
@@ -438,6 +441,21 @@ ConvFamily conv_plan(const se_conv_desc* d, int dir, int mode, const ConvCall& c
   // the BatchNorm sums come from a separate pass over y
   pl->fused_stats = c.stats && (size_t)16 * Nc * sizeof(float) <= 24 * 1024;
   return pl->family = f;
+}
+
+ConvFamily conv_plan(const se_conv_desc* d, int dir, int mode, const ConvCall& c, ConvPlan* pl) {
+  const ConvFamily f = conv_plan_wide(d, dir, mode, c, pl);
+  if (f != CONV_FP32 || !conv_odd_tc_ok(d)) return f;
+  // only shapes every family above declines: channel counts that are not all multiples of 8 (see conv_odd_tc_ok)
+  *pl = ConvPlan();
+  if (mode != SE_MODE_TF32 && mode != SE_MODE_TF32X3) return CONV_FP32;
+  const int x3 = pl->x3 = mode == SE_MODE_TF32X3;
+  if (dir == 0 && (!c.w_t || (x3 && !c.w_t_lo))) return CONV_FP32;
+  if (dir == 1 && ((x3 && !c.w_lo) || (c.beta != 0.f && c.beta != 1.f))) return CONV_FP32;
+  if (dir == 2 && !c.aligned) return CONV_FP32;
+  if (!odd_config(d, dir, c.sms, pl)) return CONV_FP32;
+  pl->fused_stats = false;                // se_bn_stats sums the BatchNorm statistics after the forward launch
+  return pl->family = CONV_TC_ODD_3X3;
 }
 
 template <int BN>

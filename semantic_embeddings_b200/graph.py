@@ -189,6 +189,19 @@ class Graph:
                 fan_in, fan_out = rf * p.shape[-2], rf * p.shape[-1]
                 lim = math.sqrt(6.0 / (fan_in + fan_out))
                 a = rng.uniform(-lim, lim, p.shape).astype(np.float32)
+            elif p.init == 'glorot_normal':
+                # Keras 2.2.4 VarianceScaling(1, 'fan_avg', 'normal'): a normal truncated at +-2 sigma (values outside
+                # are redrawn), with sigma = sqrt(2 / (fan_in + fan_out)) / 0.87962566103423978 so that the truncated
+                # distribution keeps the variance 2 / (fan_in + fan_out)
+                rf = int(np.prod(p.shape[:-2])) if len(p.shape) > 2 else 1
+                fan_in, fan_out = rf * p.shape[-2], rf * p.shape[-1]
+                std = math.sqrt(2.0 / (fan_in + fan_out)) / 0.87962566103423978
+                z = rng.randn(*p.shape)
+                out_of_range = np.abs(z) > 2
+                while out_of_range.any():
+                    z[out_of_range] = rng.randn(int(out_of_range.sum()))
+                    out_of_range = np.abs(z) > 2
+                a = (z * std).astype(np.float32)
             elif p.init == 'he_normal':
                 rf = int(np.prod(p.shape[:-2])) if len(p.shape) > 2 else 1
                 std = math.sqrt(2.0 / (rf * p.shape[-2]))

@@ -8,14 +8,14 @@ forms of what the fused head kernel computes inside a training step; they run th
 import numpy as np
 
 from . import _lib
-from .models import cifar_resnet, plainnet, resnet50, resnet_v1, wide_residual_network as wrn
+from .models import cifar_resnet, plainnet, pyramidnet, resnet50, resnet_v1, wide_residual_network as wrn
 from .clr_callback import CyclicLR
 from .keras_callbacks import LearningRateScheduler, ReduceLROnPlateau
 from .sgdr_callback import SGDR
 
 # utils.py:26-28 lists more names; the ones below are the architectures of the hot path (BASELINE.json configs)
 ARCHITECTURES = ['simple', 'resnet-32', 'resnet-110', 'resnet-110-fc', 'resnet-110-wfc', 'wrn-28-10', 'resnet-50',
-                 'resnet-101', 'resnet-152']
+                 'resnet-101', 'resnet-152', 'pyramidnet-110-270']
 REFERENCE_ARCHITECTURES = ['simple', 'resnet-32', 'resnet-110', 'resnet-110-fc', 'resnet-110-wfc', 'wrn-28-10',
                            'densenet-100-12', 'densenet-100-24', 'densenet-bc-190-40', 'pyramidnet-272-200',
                            'pyramidnet-110-270', 'resnet-50', 'resnet-101', 'resnet-152', 'rn18', 'rn34', 'rn50', 'rn101',
@@ -58,6 +58,10 @@ def build_network(num_outputs, architecture, classification=False, no_softmax=Fa
         return plainnet.PlainNet(num_outputs, input_shape=(hw or 32, hw or 32, ic), name=name, top_name=top)
     elif architecture == 'resnet-50':
         return resnet50.ResNet50(num_outputs, input_shape=(hw or 224, hw or 224, ic), name=name, top_name=top)
+    elif architecture == 'pyramidnet-110-270':
+        # utils.py:213-216: the Dense top always exists, 'embedding' or 'prob' by top_activation
+        return pyramidnet.PyramidNet(110, 270, input_shape=(hw or 32, hw or 32, ic), classes=num_outputs, name=name,
+                                     top_name=top)
     elif architecture in ('resnet-101', 'resnet-152'):
         # utils.py:230-233: keras_applications.resnet.ResNet101 / ResNet152
         return resnet_v1.ResNetV1(int(architecture[7:]), num_outputs, input_shape=(hw or 224, hw or 224, ic), name=name,
