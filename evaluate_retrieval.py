@@ -8,6 +8,9 @@ H100 kernels.  Reference: evaluate_retrieval.py:157-208.
   print_performance / write_performance (:76-102)  -> the same table and the same `k;<labels>` CSV of P@k (--prec_type)
   plot_performance (:105-141)                      -> skipped with a message (matplotlib is not a dependency); use --csv
 `pairwise_retrieval` is re-exported with the reference's signature (plot_recall_precision.py:9 imports it from here).
+--db_feat (new) ranks a separate database for every query instead of the query set itself -- e.g. the test images against
+the training images (extract_features.py --split train writes such a dump): hierarchical_precision(...,
+ignore_qids=False) of those rankings via database_metrics.  --db_split says whose labels the database ids index.
 Multi-GPU: launch with torch.distributed.run; query rows are sharded over the processes, rank 0 prints.
 """
 import argparse
@@ -24,7 +27,8 @@ if ROOT not in sys.path:
 
 from semantic_embeddings_b200.class_hierarchy import ClassHierarchy  # noqa: E402
 from semantic_embeddings_b200.datasets import get_data_generator  # noqa: E402
-from semantic_embeddings_b200.evaluate_retrieval import pairwise_retrieval, retrieval_metrics  # noqa: E402,F401
+from semantic_embeddings_b200.evaluate_retrieval import (  # noqa: E402,F401
+    database_metrics, database_retrieval, pairwise_retrieval, retrieval_metrics)
 
 METRICS = ['P@1 (WUP)', 'P@10 (WUP)', 'P@50 (WUP)', 'P@100 (WUP)', 'AHP (WUP)', 'P@1 (LCS_HEIGHT)', 'P@10 (LCS_HEIGHT)',
            'P@50 (LCS_HEIGHT)', 'P@100 (LCS_HEIGHT)', 'AHP (LCS_HEIGHT)', 'AP']
@@ -66,10 +70,7 @@ def evaluate_features(feat_dump, normalize, hierarchy, labels_test, ks, clip_ahp
     """hierarchy.hierarchical_precision(pairwise_retrieval(feat_dump, normalize), labels_test, ks, compute_ahp=clip or
     True, compute_ap=True, all_ids=range(num_test))[0] of evaluate_retrieval.py:195 on the device.
     Returns the averages dict with the reference's metric names (summed over this rank's queries when world > 1)."""
-    from semantic_embeddings_b200.evaluate_retrieval import _features_to_array
-    features, ind2id = _features_to_array(feat_dump)
-    if ind2id is not None and not np.array_equal(ind2id, np.arange(len(ind2id))):
-        raise ValueError('feature ids must be 0..N-1 in order (the --feature_dump format of learn_image_embeddings.py)')
+    features = _dump_rows(feat_dump)
     classes = sorted(set(labels_test), key=lambda v: (str(type(v)), v))
     cix = {c: i for i, c in enumerate(classes)}
     lab_ix = np.array([cix[c] for c in labels_test], dtype=np.int32)
@@ -77,6 +78,10 @@ def evaluate_features(feat_dump, normalize, hierarchy, labels_test, ks, clip_ahp
     kmax = max(ks)
     res, (row0, rows) = retrieval_metrics(features, lab_ix, wup, lcsh, kcurve=kmax, clip_ahp=clip_ahp, compute_ap=True,
                                           normalize=normalize, rank=rank, world=world)
+    return _metric_sums(res, ks, clip_ahp), rows
+
+
+def _metric_sums(res, ks, clip_ahp):
     sfx = '@{}'.format(clip_ahp) if clip_ahp else ''
     sums = OrderedDict()
     for k in ks:
@@ -85,10 +90,50 @@ def evaluate_features(feat_dump, normalize, hierarchy, labels_test, ks, clip_ahp
     sums['AHP{} (WUP)'.format(sfx)] = res['ahp'][:, 0].sum()
     sums['AHP{} (LCS_HEIGHT)'.format(sfx)] = res['ahp'][:, 1].sum()
     sums['AP'] = res['ap'].sum()
-    return sums, rows
+    return sums
 
 
-def main(argv=None):
+def _dump_rows(dump):
+    """Features of a --feature_dump pickle whose ids are 0..N-1 in order."""
+    from semantic_embeddings_b200.evaluate_retrieval import _features_to_array
+    features, ind2id = _features_to_array(dump)
+    if ind2id is not None and not np.array_equal(ind2id, np.arange(len(ind2id))):
+        raise ValueError('feature ids must be 0..N-1 in order (the --feature_dump format of learn_image_embeddings.py)')
+    return features
+
+
+def evaluate_database(feat_dump, db_dump, normalize, hierarchy, labels_query, labels_db, ks, clip_ahp, rank=0, world=1):
+    """hierarchy.hierarchical_precision(database_retrieval(feat_dump, db_dump, normalize), labels, ks, compute_ahp=clip or
+    True, compute_ap=True, ignore_qids=False, all_ids=database ids)[0] on the device, where query id i has the class
+    labels_query[i] and database id j the class labels_db[j].  Returns the sums over this rank's queries and their count."""
+    queries, database = _dump_rows(feat_dump), _dump_rows(db_dump)
+    if len(queries) > len(labels_query) or len(database) > len(labels_db):
+        raise ValueError('{} queries / {} database items, but {} / {} labels'.format(len(queries), len(database),
+                                                                                   len(labels_query), len(labels_db)))
+    labels_query, labels_db = list(labels_query)[:len(queries)], list(labels_db)[:len(database)]
+    classes = sorted(set(labels_query) | set(labels_db), key=lambda v: (str(type(v)), v))
+    cix = {c: i for i, c in enumerate(classes)}
+    q_ix = np.array([cix[c] for c in labels_query], dtype=np.int32)
+    x_ix = np.array([cix[c] for c in labels_db], dtype=np.int32)
+    wup, lcsh = hierarchy.similarity_luts(classes)
+    res, (row0, rows) = database_metrics(queries, q_ix, database, x_ix, wup, lcsh, kcurve=max(ks), clip_ahp=clip_ahp,
+                                         compute_ap=True, normalize=normalize, rank=rank, world=world)
+    return _metric_sums(res, ks, clip_ahp), rows
+
+
+def db_dumps(feat, db_feat):
+    """The database dump of every --feat: one --db_feat for all of them, or one per --feat (None without --db_feat)."""
+    if not db_feat:
+        return [None] * len(feat)
+    if len(db_feat) == 1:
+        return list(db_feat) * len(feat)
+    if len(db_feat) != len(feat):
+        raise ValueError('--db_feat given {} times for {} --feat: give it once, or once per --feat'.format(
+            len(db_feat), len(feat)))
+    return list(db_feat)
+
+
+def build_parser():
     parser = argparse.ArgumentParser(description='Evaluates hierarchical precision of nearest neighbour search performed on '
                                      'different image embeddings.', formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     g = parser.add_argument_group('Dataset')
@@ -102,12 +147,22 @@ def main(argv=None):
     g.add_argument('--feat', type=str, action='append', required=True)
     g.add_argument('--label', type=str, action='append')
     g.add_argument('--norm', type=str2bool, action='append')
+    g.add_argument('--db_feat', type=str, action='append', default=None,
+                   help='(new) Pickle of database features to rank for every query instead of the query set itself: '
+                   'once for all --feat, or once per --feat')
+    g.add_argument('--db_split', type=str, default='train', choices=['train', 'test'],
+                   help='(new) Split whose labels the --db_feat ids index')
     g = parser.add_argument_group('Output')
     g.add_argument('--plot_max', type=int, default=250)
     g.add_argument('--prec_type', type=str, default='LCS_HEIGHT', choices=['WUP', 'LCS_HEIGHT'])
     g.add_argument('--clip_ahp', type=int, default=None)
     g.add_argument('--csv', type=str, default=None)
-    args = parser.parse_args(argv)
+    return parser
+
+
+def main(argv=None):
+    args = build_parser().parse_args(argv)
+    dbs = db_dumps(args.feat, args.db_feat)
 
     import torch
     from semantic_embeddings_b200.parallel import init_process_group
@@ -123,6 +178,9 @@ def main(argv=None):
     data_generator = get_data_generator(args.dataset, args.data_root, classes=embed_labels, device='cuda:%d' % local)
     labels_test = [embed_labels[lbl] for lbl in data_generator.labels_test] if embed_labels is not None \
         else [int(v) for v in data_generator.labels_test]
+    if args.db_feat:
+        db_src = data_generator.labels_train if args.db_split == 'train' else data_generator.labels_test
+        labels_db = [embed_labels[lbl] for lbl in db_src] if embed_labels is not None else [int(v) for v in db_src]
     id_type = str if args.str_ids else int
     hierarchy = ClassHierarchy.from_file(args.hierarchy, is_a_relations=args.is_a, id_type=id_type)
 
@@ -135,7 +193,11 @@ def main(argv=None):
         feat_name = args.label[i] if (args.label is not None) and (i < len(args.label)) \
             else os.path.splitext(os.path.basename(feat_dump))[0]
         normalize = args.norm[i] if (args.norm is not None) and (i < len(args.norm)) else False
-        sums, rows = evaluate_features(feat_dump, normalize, hierarchy, labels_test, ks, args.clip_ahp, rank, world)
+        if dbs[i] is None:
+            sums, rows = evaluate_features(feat_dump, normalize, hierarchy, labels_test, ks, args.clip_ahp, rank, world)
+        else:
+            sums, rows = evaluate_database(feat_dump, dbs[i], normalize, hierarchy, labels_test, labels_db, ks, args.clip_ahp,
+                                           rank, world)
         keys = list(sums.keys())
         vec = torch.tensor([sums[k] for k in keys] + [float(rows)], dtype=torch.float64, device='cuda')
         if world > 1:

@@ -528,6 +528,30 @@ int64_t se_pairwise_topk_workspace_bytes(int N, int D, int rows);
 int se_pairwise_topk(const float* F, int ldF, int N, int D, int row0, int rows, int pdist_mode, int normalize, int k,
                      int32_t* out_idx, float* out_val, int ldo, void* workspace, int32_t* status, void* stream);
 
+/* Distances between two feature sets: rows [row0, row0+rows) of the Nq x Nd matrix of the queries Q [Nq, ldQ] against
+ * the database X [Nd, ldX] (fp32, D columns each) with the semantics of evaluate_retrieval.py:56-63; out [rows, ldout].
+ * normalize=1 L2-normalises both sets on the fly without mutating them.  SE_MODE_TF32 / SE_MODE_TF32X3 with D <= 128:
+ * the split-fp16 x3 tensor-core tiles, each set scaled by its own power of two; SE_MODE_F32 and D > 128: the fp32
+ * tiles.  se_cross_dist(F, F) gives the bits of se_pairwise_dist(F).  workspace: se_cross_workspace_bytes bytes of
+ * device memory.  SE_ERR_ARG for non-positive sizes, ld < D or a row range outside [0, Nq). */
+int64_t se_cross_workspace_bytes(int Nq, int Nd, int D, int mode);
+int se_cross_dist(const float* Q, int ldQ, int Nq, const float* X, int ldX, int Nd, int D, int row0, int rows,
+                  int pdist_mode, int normalize, float* out, int64_t ldout, void* workspace, int mode, void* stream);
+
+/* The first k database items of every query row [row0, row0+rows) (ascending distance, ties by index, -0.0 == +0.0)
+ * without writing the matrix: the fused path of se_pairwise_topk for two sets.  When the query blocks do not fill the
+ * GPU, the sweep splits the database columns over the CTAs.  status [1] device int32: 0 = exact, i.e. out_idx equals the
+ * first k entries of se_row_argsort of the se_cross_dist matrix (tensor-core mode); non-zero = some row found fewer
+ * than k or too many candidates and the caller must use the matrix path.  (se_cross_dist stores with the tensor-core
+ * kernel when ldout is a multiple of 4 and out is 16-byte aligned; with any other layout it takes the fp32 tiles, as
+ * se_pairwise_dist does, and its values may differ from these in the last bits.)  SE_ERR_UNSUPPORTED for D > 128, k > 1024 or
+ * k > Nd (the matrix path serves those).  out_idx [rows, ldo] int32, out_val [rows, ldo] float32 (may be NULL).
+ * workspace: se_cross_topk_workspace_bytes(Nq, Nd, D, rows) bytes of device memory. */
+int64_t se_cross_topk_workspace_bytes(int Nq, int Nd, int D, int rows);
+int se_cross_topk(const float* Q, int ldQ, int Nq, const float* X, int ldX, int Nd, int D, int row0, int rows,
+                  int pdist_mode, int normalize, int k, int32_t* out_idx, float* out_val, int ldo, void* workspace,
+                  int32_t* status, void* stream);
+
 /* Ranking step of evaluate_retrieval.py:67 (`np.argsort(pdist, axis=-1)`) restricted to what the metrics read
  * (class_hierarchy.py:242-244,273,283: the first clip_ahp+1 ranks): for each of `rows` rows of dist [rows, ld] the k
  * smallest of its n values in ascending order, ties by ascending index (a stable argsort's prefix; -0.0 == +0.0).
@@ -557,6 +581,15 @@ int se_hier_metrics(const int32_t* ranks, int64_t ldr, int Q, int n_ret, int q0,
                     const double* wup_lut, const double* lcs_height_lut, const double* best_wup, const double* best_lcs,
                     int kcurve, int clip, double* curve, double* ahp, double* ap, void* stream);
 
+/* se_hier_metrics for queries that are not database items (hierarchical_precision(..., ignore_qids=False)): the class of
+ * query i is query_labels[i] (int32 [Q], < C) and no ranking entry is removed.  ranks index the database, labels [N]
+ * are the database's classes and best_wup / best_lcs [C, n_ret] its ideal gains.  kcurve, clip <= n_ret; the outputs
+ * are those of se_hier_metrics. */
+int se_hier_metrics_q(const int32_t* ranks, int64_t ldr, int Q, int n_ret, const int32_t* query_labels,
+                      const int32_t* labels, int C, const double* wup_lut, const double* lcs_height_lut,
+                      const double* best_wup, const double* best_lcs, int kcurve, int clip, double* curve, double* ahp,
+                      double* ap, void* stream);
+
 /* Full-length ranking of evaluate_retrieval.py:67 (`np.argsort(pdist, axis=-1)`; ascending distance, ties by ascending
  * index, -0.0 == +0.0): out_idx [rows, ldo] int32 = the n column indices of every row of dist [rows, ld] in rank order.
  * workspace: se_row_argsort_workspace_bytes(rows, n) bytes of device memory (one padded row of 64-bit words per row). */
@@ -578,6 +611,12 @@ int se_class_index(const int32_t* labels, int N, int C, int32_t* offsets, int32_
 int se_relevant_positions(const float* dist, int64_t ld, int rows, int n, int q0, const int32_t* labels, int C,
                           const int32_t* offsets, const int32_t* members, const int64_t* out_offsets, int32_t* out,
                           void* stream);
+/* se_relevant_positions for queries that are not database items: row i of dist [rows, ld] (se_cross_dist) belongs to a
+ * query of class query_labels[i], and the output is the positions of all offsets[c+1] - offsets[c] database members of
+ * that class in the row's ranking, nothing removed.  offsets / members: se_class_index of the database labels. */
+int se_relevant_positions_q(const float* dist, int64_t ld, int rows, int n, const int32_t* query_labels,
+                            const int32_t* labels, int C, const int32_t* offsets, const int32_t* members,
+                            const int64_t* out_offsets, int32_t* out, void* stream);
 
 /* ------------------------------------------------------------------ classification (evaluate_classification_accuracy.py)
  * One-vs-rest linear SVM of the reference's train_and_predict (:20-48, sklearn LinearSVC(C): squared hinge loss, L2

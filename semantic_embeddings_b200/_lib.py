@@ -176,6 +176,14 @@ _SIGS = {
     'se_adagrad_apply_devlr': (c_int, [_P, _P, _P, c_int64, _P, c_float, c_float, _P, _P]),
     'se_pairwise_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'se_pairwise_dist': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, c_int, _P]),
+    'se_cross_workspace_bytes': (c_int64, [c_int, c_int, c_int, c_int]),
+    'se_cross_dist': (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, c_int,
+                              _P]),
+    'se_cross_topk_workspace_bytes': (c_int64, [c_int, c_int, c_int, c_int]),
+    'se_cross_topk': (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P,
+                              _P, _P]),
+    'se_hier_metrics_q': (c_int, [_P, c_int64, c_int, c_int, _P, _P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P]),
+    'se_relevant_positions_q': (c_int, [_P, c_int64, c_int, c_int, _P, _P, c_int, _P, _P, _P, _P, _P]),
     'se_lcs_height_table': (c_int, [_P, _P, _P, c_int, c_int, c_int, _P, c_int64, _P]),
     'se_cholesky_f64': (c_int, [_P, c_int64, c_int, _P, _P]),
     'se_class_gram_f64': (c_int, [_P, c_int64, c_int, c_int, _P, c_int64, _P]),

@@ -130,13 +130,17 @@ class ClassHierarchy(object):
         """class_hierarchy.py:211-316 with the same arguments, metric names and return value
         (averages dict, dict metric -> {query id: value}).  `retrieved`: dict or generator of (query id, ranked id list);
         `labels`: dict / sequence id -> class label.  Lists shorter than the database are completed from `all_ids` (:259-
-        262) -- in database order, where the reference's completion order is that of all_ids as well.  ignore_qids=False
-        is not supported by the kernels (the reference's scripts never use it)."""
+        262) -- in database order, where the reference's completion order is that of all_ids as well.
+        ignore_qids=False keeps every ranking whole (se_hier_metrics_q): the database is all_ids (or the retrieved ids),
+        a query need not be one of its items, and its class is labels[query id]."""
         import torch
-        if not ignore_qids:
-            raise NotImplementedError('ignore_qids=False is outside the accelerated path')
         items = list(retrieved) if isinstance(retrieved, types.GeneratorType) else list(retrieved.items())
-        ids = list(all_ids) if all_ids else sorted({r for _, ret in items for r in ret} | {q for q, _ in items})
+        if all_ids:
+            ids = list(all_ids)
+        elif ignore_qids:
+            ids = sorted({r for _, ret in items for r in ret} | {q for q, _ in items})
+        else:
+            ids = sorted({r for _, ret in items for r in ret})
         pos = {v: i for i, v in enumerate(ids)}
         N = len(ids)
         ranks = np.empty((len(items), N), dtype=np.int32)
@@ -148,15 +152,19 @@ class ClassHierarchy(object):
                 seen[r] = True
                 r = np.concatenate([r, np.nonzero(~seen)[0].astype(np.int32)])
             ranks[row] = r
-            qidx[row] = pos[q]
+            if ignore_qids:
+                qidx[row] = pos[q]
         lab = [labels[v] for v in ids]
-        classes = sorted(set(lab), key=lambda v: (str(type(v)), v))
+        q_lab = [labels[q] for q, _ in items]
+        classes = sorted(set(lab) | set(q_lab), key=lambda v: (str(type(v)), v))
         cix = {c: i for i, c in enumerate(classes)}
         lab_ix = np.array([cix[c] for c in lab], dtype=np.int32)
         wup, lcsh = self.similarity_luts(classes)
         ks = [ks] if isinstance(ks, int) else list(ks)
         clip = 0 if compute_ahp is False else (-1 if compute_ahp is True else int(compute_ahp))
-        res = hierarchical_metrics(torch.as_tensor(ranks).to(device), qidx, lab_ix, wup, lcsh, max(ks), clip, bool(compute_ap))
+        res = hierarchical_metrics(torch.as_tensor(ranks).to(device), qidx if ignore_qids else None, lab_ix, wup, lcsh, max(ks),
+                                   clip, bool(compute_ap),
+                                   query_labels=None if ignore_qids else np.array([cix[c] for c in q_lab], dtype=np.int32))
         prec = {}
         for k in ks:
             prec['P@{} (WUP)'.format(k)] = res['curve'][:, 0, k - 1]
@@ -201,11 +209,13 @@ def ideal_gains(labels_ix, wup, lcsh, n):
     return bw, bl
 
 
-def hierarchical_metrics(ranks, query_index, labels_ix, wup, lcsh, kcurve, clip, compute_ap, block=4096):
+def hierarchical_metrics(ranks, query_index, labels_ix, wup, lcsh, kcurve, clip, compute_ap, block=4096, query_labels=None):
     """se_hier_metrics over device rankings.  ranks: int32 CUDA tensor [Q, n_ret] of database indices; query_index: the
     database index of every row's query (int array, or None for rows q0.. = 0..Q-1); labels_ix: class index of every
-    database item.  clip: 0 no AHP, > 0 AHP@clip, < 0 AHP over the whole list.  Returns numpy arrays
-    {'curve' [Q, 2, kcurve], 'ahp' [Q, 2], 'ap' [Q]} (absent keys for what was not requested)."""
+    database item.  clip: 0 no AHP, > 0 AHP@clip, < 0 AHP over the whole list.  With query_labels (class index of every
+    row's query) the queries are not database items and nothing is removed from the rankings (se_hier_metrics_q;
+    query_index is ignored).  Returns numpy arrays {'curve' [Q, 2, kcurve], 'ahp' [Q, 2], 'ap' [Q]} (absent keys for
+    what was not requested)."""
     import torch
     dev = ranks.device
     Q, n_ret = ranks.shape
@@ -225,6 +235,12 @@ def hierarchical_metrics(ranks, query_index, labels_ix, wup, lcsh, kcurve, clip,
     qi = np.arange(Q) if query_index is None else np.asarray(query_index)
     start = 0
     with torch.cuda.device(dev):
+        if query_labels is not None:
+            ql_d = t(np.ascontiguousarray(query_labels, dtype=np.int32))
+            _lib.call('se_hier_metrics_q', ranks.data_ptr(), ranks.stride(0), Q, n_ret, ql_d.data_ptr(), lab_d.data_ptr(), C,
+                      wup_d.data_ptr(), lcs_d.data_ptr(), bw_d.data_ptr(), bl_d.data_ptr(), kcurve, clip, _lib.ptr(curve),
+                      _lib.ptr(ahp), _lib.ptr(ap), _lib.stream_ptr())
+            start = Q
         while start < Q:
             end = start + 1
             while end < Q and qi[end] == qi[end - 1] + 1:

@@ -99,25 +99,28 @@ hier_precision_kernel(const int* __restrict__ ranks, int ldr, int Q, int K1, int
 //                      of the list without the query when clip < 0                           (:303-309)
 //   ap[q]            = average_precision_score(same class?, -rank) = mean over the same-class items of
 //                      (same-class items up to and including this rank) / rank, query removed     (:310-314)
+// With query_labels (se_hier_metrics_q, ignore_qids=False) the query's class is query_labels[qi] and nothing is removed:
+// the queries need not be database items.
 // One warp per query walks the list in blocks of 32 ranks with warp scans (float64 for the gains, integers for the hits).
 __global__ void __launch_bounds__(128)
-hier_metrics_kernel(const int* __restrict__ ranks, long long ldr, int Q, int n_ret, int q0, const int* __restrict__ labels,
-                    int C, const double* __restrict__ wup, const double* __restrict__ lcsh, const double* __restrict__ best_wup,
-                    const double* __restrict__ best_lcs, int kcurve, int clip, double* __restrict__ curve,
-                    double* __restrict__ ahp, double* __restrict__ ap) {
+hier_metrics_kernel(const int* __restrict__ ranks, long long ldr, int Q, int n_ret, int q0, const int* __restrict__ query_labels,
+                    const int* __restrict__ labels, int C, const double* __restrict__ wup, const double* __restrict__ lcsh,
+                    const double* __restrict__ best_wup, const double* __restrict__ best_lcs, int kcurve, int clip,
+                    double* __restrict__ curve, double* __restrict__ ahp, double* __restrict__ ap) {
   pdl_grid_sync();
   const int lane = threadIdx.x & 31;
   const int qi = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (qi >= Q) return;
-  const int q = q0 + qi;
+  const int q = query_labels ? -1 : q0 + qi;           // -1: no database item is the query
   const int* r = ranks + (long long)qi * ldr;
-  const int L = labels[q];
+  const int L = query_labels ? query_labels[qi] : labels[q];
   const double* wrow = wup + (long long)L * C;
   const double* lrow = lcsh + (long long)L * C;
   const double* bw = best_wup + (long long)L * n_ret;
   const double* bl = best_lcs + (long long)L * n_ret;
   int p = n_ret;                                       // position of the query in its own list (first occurrence)
-  for (int j = lane; j < n_ret; j += 32) if (r[j] == q) p = min(p, j);
+  if (q >= 0)
+    for (int j = lane; j < n_ret; j += 32) if (r[j] == q) p = min(p, j);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) p = min(p, __shfl_xor_sync(0xffffffffu, p, o));
   const int n_eff = (p < n_ret) ? n_ret - 1 : n_ret;
@@ -198,7 +201,23 @@ extern "C" int se_hier_metrics(const int32_t* ranks, int64_t ldr, int Q, int n_r
   SE_REQUIRE(clip == 0 || ahp, "ahp output missing");
   const int warps = 4;
   launch(hier_metrics_kernel, dim3(ceil_div(Q, warps)), dim3(32 * warps), 0, as_stream(stream), ranks, (long long)ldr, Q, n_ret, q0,
-         labels, C, wup_lut, lcs_height_lut, best_wup, best_lcs, kcurve, clip, curve, clip != 0 ? ahp : nullptr, ap);
+         (const int*)nullptr, labels, C, wup_lut, lcs_height_lut, best_wup, best_lcs, kcurve, clip, curve, clip != 0 ? ahp : nullptr,
+         ap);
+  return check_launch("hier_metrics_kernel");
+}
+
+extern "C" int se_hier_metrics_q(const int32_t* ranks, int64_t ldr, int Q, int n_ret, const int32_t* query_labels,
+                                 const int32_t* labels, int C, const double* wup_lut, const double* lcs_height_lut,
+                                 const double* best_wup, const double* best_lcs, int kcurve, int clip, double* curve, double* ahp,
+                                 double* ap, void* stream) {
+  SE_REQUIRE(ranks && query_labels && labels && wup_lut && lcs_height_lut && best_wup && best_lcs, "null pointer");
+  SE_REQUIRE(Q > 0 && n_ret > 0 && ldr >= n_ret && C > 0 && kcurve >= 0 && kcurve <= n_ret, "bad sizes");
+  SE_REQUIRE(kcurve == 0 || curve, "curve output missing");
+  SE_REQUIRE(clip <= n_ret, "clip (compute_ahp) needs clip retrieved ranks");
+  SE_REQUIRE(clip == 0 || ahp, "ahp output missing");
+  const int warps = 4;
+  launch(hier_metrics_kernel, dim3(ceil_div(Q, warps)), dim3(32 * warps), 0, as_stream(stream), ranks, (long long)ldr, Q, n_ret, 0,
+         query_labels, labels, C, wup_lut, lcs_height_lut, best_wup, best_lcs, kcurve, clip, curve, clip != 0 ? ahp : nullptr, ap);
   return check_launch("hier_metrics_kernel");
 }
 

@@ -32,10 +32,12 @@ pairwise_prep_kernel(const float* __restrict__ F, int ldF, int N, int D, int nor
   if (lane == 0) { sq[warp] = s; invn[warp] = inv; }
 }
 
+// rows [row0, row0+rows) of the queries F against the N database items X (X == F for the all-pairs matrix)
 template <int BM, int BN, int TM, int TN>
 __global__ void __launch_bounds__((BM / TM) * (BN / TN))
-pairwise_f32_kernel(const float* __restrict__ F, int ldF, int N, int D, int row0, int rows, int pmode,
-                    const float* __restrict__ sq, const float* __restrict__ invn, float* __restrict__ out,
+pairwise_f32_kernel(const float* __restrict__ F, int ldF, const float* __restrict__ X, int ldX, int N, int D, int row0,
+                    int rows, int pmode, const float* __restrict__ sq, const float* __restrict__ invn,
+                    const float* __restrict__ sq_x, const float* __restrict__ invn_x, float* __restrict__ out,
                     long long ldout) {
   pdl_grid_sync();
   constexpr int NT = (BM / TM) * (BN / TN);
@@ -64,7 +66,7 @@ pairwise_f32_kernel(const float* __restrict__ F, int ldF, int N, int D, int row0
     for (int idx = tid; idx < BN * BK; idx += NT) {
       int r = idx / BK, k = idx % BK;
       float v = 0.f;
-      if (j0 + r < N && k0 + k < D) v = F[(long long)(j0 + r) * ldF + k0 + k] / invn[j0 + r];
+      if (j0 + r < N && k0 + k < D) v = X[(long long)(j0 + r) * ldX + k0 + k] / invn_x[j0 + r];
       Bs[k][r] = v;
     }
     __syncthreads();
@@ -81,7 +83,7 @@ pairwise_f32_kernel(const float* __restrict__ F, int ldF, int N, int D, int row0
       int gj = j0 + tn * TN + j;
       if (gj >= N) continue;
       float c = acc[i][j];
-      float v = (pmode == SE_PDIST_NEGDOT) ? -c : (a + sq[gj]) - 2.f * c;
+      float v = (pmode == SE_PDIST_NEGDOT) ? -c : (a + sq_x[gj]) - 2.f * c;
       out[(long long)(gi - row0) * ldout + gj] = v;
     }
   }
@@ -93,6 +95,12 @@ long long pairwise_tc_workspace_floats(int N, int D);
 long long pairwise_topk_extra_bytes(int N, int D, int rows);
 int pairwise_tc_topk(const float* F, int ldF, int N, int D, int row0, int rows, int pmode, int k, int* out_idx, float* out_val,
                      int ldo, float* ws, int* status, cudaStream_t st);
+int pairwise_tc_cross(const float* Q, int ldQ, int Nq, const float* X, int ldX, int Nd, int D, int row0, int rows, int pmode,
+                      float* out, long long ldout, float* ws_q, float* ws_x, cudaStream_t st);
+long long cross_topk_extra_bytes(int Nd, int D, int rows);
+int pairwise_tc_cross_topk(const float* Q, int ldQ, int Nq, const float* X, int ldX, int Nd, int D, int row0, int rows,
+                           int pmode, int k, int* out_idx, float* out_val, int ldo, float* ws_q, float* ws_x, void* extra,
+                           int* status, cudaStream_t st);
 
 }  // namespace se
 
@@ -122,7 +130,8 @@ extern "C" int se_pairwise_dist(const float* F, int ldF, int N, int D, int row0,
   }
   constexpr int BM = 64, BN = 64;
   dim3 grid(ceil_div(N, BN), ceil_div(rows, BM));
-  launch(pairwise_f32_kernel<BM, BN, 4, 4>, dim3(grid), dim3(256), 0, st, F, ldF, N, D, row0, rows, pdist_mode, sq, invn, out, ldout);
+  launch(pairwise_f32_kernel<BM, BN, 4, 4>, dim3(grid), dim3(256), 0, st, F, ldF, F, ldF, N, D, row0, rows, pdist_mode, sq, invn,
+         sq, invn, out, ldout);
   return check_launch("pairwise_f32_kernel");
 }
 
@@ -141,4 +150,72 @@ extern "C" int se_pairwise_topk(const float* F, int ldF, int N, int D, int row0,
   int rc = check_launch("pairwise_prep_kernel");
   if (rc) return rc;
   return pairwise_tc_topk(F, ldF, N, D, row0, rows, pdist_mode, k, out_idx, out_val, ldo, ws, status, st);
+}
+
+// Two feature sets share one workspace: the queries' region (the all-pairs layout for Nq items), then the database's
+// region (the same layout for Nd items) at the next 256-byte boundary, then (se_cross_topk) the fused path's own part.
+static int64_t cross_region_bytes(int N, int D, int mode) { return (se_pairwise_workspace_bytes(N, D, mode) + 255) & ~255LL; }
+static float* cross_ws_x(void* ws, int Nq, int D, int mode) {
+  return reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ws) + cross_region_bytes(Nq, D, mode));
+}
+
+extern "C" int64_t se_cross_workspace_bytes(int Nq, int Nd, int D, int mode) {
+  return cross_region_bytes(Nq, D, mode) + cross_region_bytes(Nd, D, mode);
+}
+
+// row norms (and, with normalize, the normalised squared norms) of both sets into their regions
+static int cross_prep(const float* Q, int ldQ, int Nq, const float* X, int ldX, int Nd, int D, int normalize, float* wq,
+                      float* wx, cudaStream_t st) {
+  launch(pairwise_prep_kernel, dim3(ceil_div(Nq, 8)), dim3(256), 0, st, Q, ldQ, Nq, D, normalize, wq, wq + Nq);
+  int rc = check_launch("pairwise_prep_kernel");
+  if (rc) return rc;
+  launch(pairwise_prep_kernel, dim3(ceil_div(Nd, 8)), dim3(256), 0, st, X, ldX, Nd, D, normalize, wx, wx + Nd);
+  return check_launch("pairwise_prep_kernel");
+}
+
+extern "C" int se_cross_dist(const float* Q, int ldQ, int Nq, const float* X, int ldX, int Nd, int D, int row0, int rows,
+                             int pdist_mode, int normalize, float* out, int64_t ldout, void* workspace, int mode, void* stream) {
+  SE_REQUIRE(Q && X && out && workspace, "null pointer");
+  SE_REQUIRE(Nq > 0 && Nd > 0 && D > 0 && ldQ >= D && ldX >= D && rows > 0 && ldout >= Nd, "bad shape");
+  SE_REQUIRE(row0 >= 0 && (int64_t)row0 + rows <= Nq, "query rows outside [0, Nq)");
+  SE_REQUIRE(pdist_mode == SE_PDIST_SQEUCLID || pdist_mode == SE_PDIST_NEGDOT, "unknown pairwise mode");
+  cudaStream_t st = as_stream(stream);
+  float* wq = reinterpret_cast<float*>(workspace);
+  float* wx = cross_ws_x(workspace, Nq, D, mode);
+  int rc = cross_prep(Q, ldQ, Nq, X, ldX, Nd, D, normalize, wq, wx, st);
+  if (rc) return rc;
+  if (mode != SE_MODE_F32) {
+    rc = pairwise_tc_cross(Q, ldQ, Nq, X, ldX, Nd, D, row0, rows, pdist_mode, out, ldout, wq, wx, st);
+    if (rc != SE_ERR_UNSUPPORTED) return rc;   // D > 128 (or unaligned output rows): the fp32 tiles
+  }
+  constexpr int BM = 64, BN = 64;
+  dim3 grid(ceil_div(Nd, BN), ceil_div(rows, BM));
+  launch(pairwise_f32_kernel<BM, BN, 4, 4>, dim3(grid), dim3(256), 0, st, Q, ldQ, X, ldX, Nd, D, row0, rows, pdist_mode, wq,
+         wq + Nq, wx, wx + Nd, out, ldout);
+  return check_launch("pairwise_f32_kernel");
+}
+
+extern "C" int64_t se_cross_topk_workspace_bytes(int Nq, int Nd, int D, int rows) {
+  return se_cross_workspace_bytes(Nq, Nd, D, SE_MODE_TF32X3) + cross_topk_extra_bytes(Nd, D, rows) + 8192;
+}
+
+extern "C" int se_cross_topk(const float* Q, int ldQ, int Nq, const float* X, int ldX, int Nd, int D, int row0, int rows,
+                             int pdist_mode, int normalize, int k, int32_t* out_idx, float* out_val, int ldo, void* workspace,
+                             int32_t* status, void* stream) {
+  SE_REQUIRE(Q && X && out_idx && workspace && status, "null pointer");
+  SE_REQUIRE(Nq > 0 && Nd > 0 && D > 0 && ldQ >= D && ldX >= D && rows > 0 && k > 0 && ldo >= k, "bad shape");
+  SE_REQUIRE(row0 >= 0 && (int64_t)row0 + rows <= Nq, "query rows outside [0, Nq)");
+  SE_REQUIRE(pdist_mode == SE_PDIST_SQEUCLID || pdist_mode == SE_PDIST_NEGDOT, "unknown pairwise mode");
+  if (D > 128 || k > 1024 || k > Nd) {
+    set_error("se_cross_topk: D = %d, k = %d, Nd = %d outside the fused path (D <= 128, k <= min(1024, Nd))", D, k, Nd);
+    return SE_ERR_UNSUPPORTED;
+  }
+  cudaStream_t st = as_stream(stream);
+  float* wq = reinterpret_cast<float*>(workspace);
+  float* wx = cross_ws_x(workspace, Nq, D, SE_MODE_TF32X3);
+  void* extra = reinterpret_cast<uint8_t*>(workspace) + se_cross_workspace_bytes(Nq, Nd, D, SE_MODE_TF32X3);
+  int rc = cross_prep(Q, ldQ, Nq, X, ldX, Nd, D, normalize, wq, wx, st);
+  if (rc) return rc;
+  return pairwise_tc_cross_topk(Q, ldQ, Nq, X, ldX, Nd, D, row0, rows, pdist_mode, k, out_idx, out_val, ldo, wq, wx, extra,
+                                status, st);
 }

@@ -7,6 +7,10 @@
 // <= 2^-24).  fp16 wgmma moves 2 bytes per element and runs at twice the TF32 rate, which is what keeps the
 // contraction hidden behind the fp32 output stream (4 bytes per pair -- the HBM roofline of this kernel).
 //
+// Two feature sets (se_cross_dist, se_cross_topk): the queries are A and the database is B, and each set gets its own
+// power-of-two scaling 2^-e_q, 2^-e_x (the sets may differ in magnitude by orders); the epilogue undoes 2^(e_q + e_x),
+// which is the 4^e of the all-pairs matrix when both sets are the same.
+//
 // Structure (one persistent CTA per SM, 384 threads, warp-specialised):
 //   warpgroup 0 : one thread issues the TMA loads -- the A row block (128 rows, h and l, all K) stays RESIDENT while
 //                 the CTA sweeps the column tiles; B tiles (128 rows) stream through a 2-stage ring, one 64-wide K
@@ -38,18 +42,20 @@ struct PwParams {
   float* out;
   const float* sq;       // squared norms of the (normalised) query rows, [N]
   const float* sq_b;     // squared norms of the column items (== sq for the all-pairs matrix; a sample's norms otherwise)
-  const float* scal;     // scal[1] = 4^e: undoes the power-of-two input scaling
+  const float* scal;     // scal[1] = 2^(e_q + e_x): undoes the power-of-two input scaling
   // fused ranking (se_pairwise_topk).  EPI == 2, sample pass: every (row, 64-column half tile with >= 8 columns) adds the
   // j-th smallest of its distances to tau_sum[row] -- the mean of those order statistics is the row's candidate threshold.  EPI == 1,
   // sweep: entries below the threshold become (value, column) candidates in the region of the writing (row, column
   // half, part of the row block) -- a thread owns its row for the CTA's whole stretch of the row block, so the fill
-  // count lives in a register and no atomics are needed.
+  // count lives in a register and no atomics are needed.  Part = the CTA's place among the CTAs that share the row block
+  // (regions: half * nparts + part).
   float* tau_sum;        // [rows]   EPI 2: accumulates; EPI 1: threshold = tau_sum[row] * tau_scale
   float tau_scale;       // 1 / (number of half tiles of the sample pass with >= 8 columns)
-  int* cnt;              // [rows, 4] candidates per region (may exceed capr: the finishing kernel reports it)
-  float* cand_val;       // [rows, 4, capr]
-  int* cand_idx;         // [rows, 4, capr]
+  int* cnt;              // [rows, 2 * nparts] candidates per region (may exceed capr: the finishing kernel reports it)
+  float* cand_val;       // [rows, 2 * nparts, capr]
+  int* cand_idx;         // [rows, 2 * nparts, capr]
   int capr, ncols;       // ncols: number of valid columns
+  int nparts;            // EPI 1: the most CTAs that share one row block
   int jsel;              // EPI 2: which order statistic (0-based, < 8) of a half tile feeds the threshold
 };
 
@@ -70,14 +76,20 @@ pairwise_absmax_kernel(const float* __restrict__ F, int ldF, int N, int D, const
 
 __global__ void __launch_bounds__(256)
 pairwise_split_kernel(const float* __restrict__ F, int ldF, int N, int D, int KW, const float* __restrict__ norms,
-                      float* __restrict__ scal, __half* __restrict__ Fh, __half* __restrict__ Fl) {
+                      const float* scal, const float* scal_other, float* scale_out, __half* __restrict__ Fh,
+                      __half* __restrict__ Fl) {
   pdl_grid_sync();
-  // scal[0] holds the bit pattern of max|f| (0 if the matrix is all zero)
-  float amax = __uint_as_float(reinterpret_cast<const unsigned*>(scal)[0]);
-  int e = 0;
-  if (amax > 0.f) frexpf(amax, &e);            // amax = m * 2^e, m in [0.5, 1)  =>  amax * 2^-e < 1
+  // scal[0] / scal_other[0] hold the bit patterns of max|f| of this set / of the other operand's set (0 if all zero);
+  // scale_out (may be NULL) receives 2^(e + e_other), the factor the epilogue multiplies the dot products by
+  auto exponent = [](const float* sc) {
+    const float amax = __uint_as_float(reinterpret_cast<const unsigned*>(sc)[0]);
+    int e = 0;
+    if (amax > 0.f) frexpf(amax, &e);          // amax = m * 2^e, m in [0.5, 1)  =>  amax * 2^-e < 1
+    return e;
+  };
+  const int e = exponent(scal);
   const float s = ldexpf(1.f, -e);
-  if (blockIdx.x == 0 && threadIdx.x == 0) scal[1] = ldexpf(1.f, 2 * e);
+  if (scale_out && blockIdx.x == 0 && threadIdx.x == 0) *scale_out = ldexpf(1.f, e + exponent(scal_other));
   const long long total = (long long)N * KW;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
     int r = (int)(idx / KW), k = (int)(idx % KW);
@@ -209,9 +221,9 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_const
     if (EPI == 1) {
       tau = row_ok ? p.tau_sum[lrow] * p.tau_scale : 0.f;
       if (tm != e_tm) {                                // a new row block: flush the previous block's fill count
-        if (e_tm >= 0 && e_tm * PW_BM + r_local < p.rows) p.cnt[(long long)(e_tm * PW_BM + r_local) * 4 + e_region] = e_pos;
+        if (e_tm >= 0 && e_tm * PW_BM + r_local < p.rows) p.cnt[(long long)(e_tm * PW_BM + r_local) * 2 * p.nparts + e_region] = e_pos;
         e_tm = tm; e_pos = 0;
-        e_region = half * 2 + ((t_begin > tm * p.tiles_n) ? 1 : 0);
+        e_region = half * p.nparts + (blockIdx.x - (tm * p.tiles_n) / per_cta);
       }
     }
     float ms[8];                                       // EPI 2: the eight smallest distances of this half tile, ascending
@@ -243,8 +255,8 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_const
         if (mask) {
 #pragma unroll
           for (int q = 0; q < 8; ++q) *reinterpret_cast<float4*>(myrow + col + 4 * q) = o[q];     // own row only
-          float* cv = p.cand_val + ((long long)lrow * 4 + e_region) * p.capr;
-          int* ci = p.cand_idx + ((long long)lrow * 4 + e_region) * p.capr;
+          float* cv = p.cand_val + ((long long)lrow * 2 * p.nparts + e_region) * p.capr;
+          int* ci = p.cand_idx + ((long long)lrow * 2 * p.nparts + e_region) * p.capr;
           while (mask) {
             const int i = __ffs(mask) - 1;
             mask &= mask - 1;
@@ -296,7 +308,7 @@ pairwise_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_const
     }
     named_bar_sync(1 + wg, 128);                      // the staging rows are free for the next tile
   }
-  if (EPI == 1 && e_tm >= 0 && e_tm * PW_BM + r_local < p.rows) p.cnt[(long long)(e_tm * PW_BM + r_local) * 4 + e_region] = e_pos;
+  if (EPI == 1 && e_tm >= 0 && e_tm * PW_BM + r_local < p.rows) p.cnt[(long long)(e_tm * PW_BM + r_local) * 2 * p.nparts + e_region] = e_pos;
 }
 
 // ---- host side
@@ -321,7 +333,8 @@ struct PwLayout {
   float* sq; float* norms; float* scal; __half* Fh; __half* Fl; int KW, kblocks;
 };
 
-static int pw_prepare(const float* F, int ldF, int N, int D, float* ws, cudaStream_t st, PwLayout* L) {
+// one feature set's region of the workspace: [sq N][norms N] | 256-aligned: scalars (256 bytes), Fh, Fl
+static int pw_carve(float* ws, int N, int D, PwLayout* L) {
   L->KW = ceil_div(D, 16) * 16;
   L->kblocks = ceil_div(L->KW, PW_KB);
   if (L->kblocks > PW_MAXKB) return SE_ERR_UNSUPPORTED;                    // D > 128: fp32 tiles
@@ -331,19 +344,50 @@ static int pw_prepare(const float* F, int ldF, int N, int D, float* ws, cudaStre
   L->scal = reinterpret_cast<float*>(base);
   L->Fh = reinterpret_cast<__half*>(base + 256);
   L->Fl = L->Fh + (long long)N * L->KW;
-  if (cudaMemsetAsync(L->scal, 0, 256, st) != cudaSuccess) { set_error("pairwise_tc: memset failed"); return SE_ERR_CUDA; }
+  return SE_OK;
+}
+
+static int pw_absmax(const float* F, int ldF, int N, int D, const PwLayout& L, cudaStream_t st) {
+  if (cudaMemsetAsync(L.scal, 0, 256, st) != cudaSuccess) { set_error("pairwise_tc: memset failed"); return SE_ERR_CUDA; }
   long long w1 = ceil_div<long long>((long long)N * D, 256), cap = (long long)sm_count() * 8;
   int g1 = (int)(w1 < cap ? w1 : cap);
-  launch(pairwise_absmax_kernel, dim3(g1), dim3(256), 0, st, F, ldF, N, D, L->norms, reinterpret_cast<unsigned*>(L->scal));
-  int rc = check_launch("pairwise_absmax_kernel");
-  if (rc) return rc;
-  long long w2 = ceil_div<long long>((long long)N * L->KW, 256);
+  launch(pairwise_absmax_kernel, dim3(g1), dim3(256), 0, st, F, ldF, N, D, L.norms, reinterpret_cast<unsigned*>(L.scal));
+  return check_launch("pairwise_absmax_kernel");
+}
+
+// scal_other: the other operand's scalars (its max|f| at [0]); scale_out: where 2^(e + e_other) goes (NULL: nowhere)
+static int pw_split(const float* F, int ldF, int N, int D, const PwLayout& L, const float* scal_other, float* scale_out,
+                    cudaStream_t st) {
+  long long w2 = ceil_div<long long>((long long)N * L.KW, 256), cap = (long long)sm_count() * 8;
   int g2 = (int)(w2 < cap ? w2 : cap);
-  launch(pairwise_split_kernel, dim3(g2), dim3(256), 0, st, F, ldF, N, D, L->KW, L->norms, L->scal, L->Fh, L->Fl);
+  launch(pairwise_split_kernel, dim3(g2), dim3(256), 0, st, F, ldF, N, D, L.KW, L.norms, (const float*)L.scal, scal_other,
+         scale_out, L.Fh, L.Fl);
   return check_launch("pairwise_split_kernel");
 }
 
-struct PwEpi { int kind; float* tau_sum; float tau_scale; int* cnt; float* cand_val; int* cand_idx; int capr; int jsel; };
+static int pw_prepare(const float* F, int ldF, int N, int D, float* ws, cudaStream_t st, PwLayout* L) {
+  int rc = pw_carve(ws, N, D, L);
+  if (!rc) rc = pw_absmax(F, ldF, N, D, *L, st);
+  if (!rc) rc = pw_split(F, ldF, N, D, *L, L->scal, L->scal + 1, st);
+  return rc;
+}
+
+// two feature sets: queries Q (A, region ws_q) and database X (B, region ws_x), each scaled by its own power of two
+static int cw_prepare(const float* Q, int ldQ, int Nq, const float* X, int ldX, int Nd, int D, float* ws_q, float* ws_x,
+                      cudaStream_t st, PwLayout* A, PwLayout* B) {
+  int rc = pw_carve(ws_q, Nq, D, A);
+  if (!rc) rc = pw_carve(ws_x, Nd, D, B);
+  if (!rc) rc = pw_absmax(Q, ldQ, Nq, D, *A, st);
+  if (!rc) rc = pw_absmax(X, ldX, Nd, D, *B, st);
+  if (!rc) rc = pw_split(Q, ldQ, Nq, D, *A, B->scal, A->scal + 1, st);
+  if (!rc) rc = pw_split(X, ldX, Nd, D, *B, A->scal, nullptr, st);
+  return rc;
+}
+
+struct PwEpi {
+  int kind; float* tau_sum; float tau_scale; int* cnt; float* cand_val; int* cand_idx; int capr; int jsel;
+  int grid, nparts;      // kind 1: the sweep's grid and the most CTAs sharing a row block (pt_sweep_shape)
+};
 
 // rows [row0, row0+rows) of the N query items against `ncols` column items given by (Bh, Bl, sq_b)
 static int pw_launch(const PwLayout& L, int N, int row0, int rows, const __half* Bh, const __half* Bl, const float* sq_b,
@@ -369,12 +413,12 @@ static int pw_launch(const PwLayout& L, int N, int row0, int rows, const __half*
   p.out = out; p.ldout = ldout;
   p.sq = L.sq; p.sq_b = sq_b; p.scal = L.scal; p.ncols = ncols;
   p.tau_sum = nullptr; p.tau_scale = 0.f; p.cnt = nullptr; p.cand_val = nullptr; p.cand_idx = nullptr; p.capr = 0; p.jsel = 1;
+  p.nparts = 2;
   if (e1) { p.jsel = e1->jsel; p.tau_sum = e1->tau_sum; p.tau_scale = e1->tau_scale; p.cnt = e1->cnt; p.cand_val = e1->cand_val; p.cand_idx = e1->cand_idx; p.capr = e1->capr; }
   int rc0 = ensure_setup();
   if (rc0) return rc0;
   int grid = min(sm_count(), p.tiles_m * p.tiles_n);
-  // candidate sweep: a row block may be shared by at most two CTAs (regions are per (row, column half, part))
-  if (e1 && e1->kind == 1) grid = max(1, min(grid, p.tiles_m));
+  if (e1 && e1->kind == 1) { grid = e1->grid; p.nparts = e1->nparts; }   // candidate sweep: regions per (row, half, part)
   if (e1 && e1->kind == 1) launch(pairwise_tc_kernel<1>, dim3(grid), dim3(PW_THREADS), PW_SMEM, st, mh, ml, mbh, mbl, p);
   else if (e1) launch(pairwise_tc_kernel<2>, dim3(grid), dim3(PW_THREADS), PW_SMEM, st, mh, ml, mbh, mbl, p);
   else launch(pairwise_tc_kernel<0>, dim3(grid), dim3(PW_THREADS), PW_SMEM, st, mh, ml, mbh, mbl, p);
@@ -389,6 +433,14 @@ int pairwise_tc(const float* F, int ldF, int N, int D, int row0, int rows, int p
   return pw_launch(L, N, row0, rows, L.Fh, L.Fl, L.sq, N, pmode, out, ldout, nullptr, st);
 }
 
+int pairwise_tc_cross(const float* Q, int ldQ, int Nq, const float* X, int ldX, int Nd, int D, int row0, int rows, int pmode,
+                      float* out, long long ldout, float* ws_q, float* ws_x, cudaStream_t st) {
+  PwLayout A, B;
+  int rc = cw_prepare(Q, ldQ, Nq, X, ldX, Nd, D, ws_q, ws_x, st, &A, &B);
+  if (rc) return rc;
+  return pw_launch(A, Nq, row0, rows, B.Fh, B.Fl, B.sq, Nd, pmode, out, ldout, nullptr, st);
+}
+
 // ---------------------------------------------------------------------------------------- fused distance + top-k
 // SURVEY.md section 8(f) rank 1: the k nearest items of every query WITHOUT the rows x N distance matrix in HBM.
 //   1. sample pass (EPI 2): distances to a strided sample of S <= 4096 column items; every (row, 64-column half tile)
@@ -401,7 +453,16 @@ int pairwise_tc(const float* F, int ldF, int N, int D, int row0, int rows, int p
 // written matrix -- provided every row found at least k candidates and no region overflowed, which status[0] reports
 // (0 = exact; otherwise the caller falls back to the matrix path).  The threshold is a statistical estimate; exactness
 // never depends on it, only the fallback rate does.
-constexpr int PT_SAMPLE = 4096, PT_CAPR = 1024, PT_CAP = 4 * PT_CAPR, PT_THREADS = 512;
+// The all-pairs sweep gives a row block to at most two CTAs.  Against a separate database (se_cross_topk) a few query
+// blocks would then leave most SMs idle, so that sweep spreads the tiles of all row blocks evenly over every SM: a row
+// block is split into column ranges, each CTA keeps its own regions (smaller ones when there are many parts), and the
+// finishing sort merges them.
+// Thresholds of a large database: the half-tile statistic resolves no quantile below 2/65 of the row, i.e. ~N/32
+// candidates, too many for the sort beyond ~65 000 items.  Above PT_NEST_S items (two sets only) the threshold of a row
+// is instead the exact k2-th smallest distance to a strided sample of PT_NEST_S database items, with k2 chosen so that
+// ~3k of the row's entries are expected below it -- found by this same fused path run on the sample.
+constexpr int PT_SAMPLE = 4096, PT_CAPR = 1024, PT_CAP = 4 * PT_CAPR, PT_THREADS = 512, PT_MIN_CAPR = 256;
+constexpr int PT_NEST_S = 65536, PT_NEST_MAXK = 1024;
 
 __global__ void __launch_bounds__(256)
 pairwise_sample_kernel(const __half* __restrict__ Fh, const __half* __restrict__ Fl, const float* __restrict__ sq, int KW,
@@ -424,33 +485,37 @@ __device__ __forceinline__ uint32_t pt_key(float f) {
 }
 __device__ __forceinline__ float pt_unkey(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k); }
 
+// one CTA per row: the candidates of its nreg regions (capr entries each) are merged and sorted in shared memory
 __global__ void __launch_bounds__(PT_THREADS)
 pairwise_topk_finish_kernel(const int* __restrict__ cnt, const float* __restrict__ cand_val, const int* __restrict__ cand_idx,
-                            int k, int* __restrict__ out_idx, float* __restrict__ out_val, int ldo, int* __restrict__ status) {
+                            int nreg, int capr, int k, int* __restrict__ out_idx, float* __restrict__ out_val, int ldo,
+                            int* __restrict__ status) {
   pdl_grid_sync();
   __shared__ unsigned long long s[PT_CAP];
+  __shared__ int s_total, s_bad;
   const int row = blockIdx.x;
-  int c4[4], off[5];
-  off[0] = 0;
-  bool bad = false;
-  for (int r = 0; r < 4; ++r) {
-    c4[r] = cnt[row * 4 + r];
-    if (c4[r] > PT_CAPR) bad = true;
-    off[r + 1] = off[r] + min(c4[r], PT_CAPR);
-  }
-  const int c = off[4];
-  if (bad || c < k) { if (threadIdx.x == 0) atomicOr(status, 1); return; }
+  const int* rc = cnt + (long long)row * nreg;
+  if (threadIdx.x == 0) { s_total = 0; s_bad = 0; }
+  __syncthreads();
+  int part = 0, over = 0;
+  for (int r = threadIdx.x; r < nreg; r += PT_THREADS) { const int c = rc[r]; part += min(c, capr); over |= c > capr; }
+  part = __reduce_add_sync(0xffffffffu, part);
+  over = __reduce_or_sync(0xffffffffu, over);
+  if ((threadIdx.x & 31) == 0) { atomicAdd(&s_total, part); if (over) s_bad = 1; }
+  __syncthreads();
+  const int c = s_total;
+  if (s_bad || c < k || c > PT_CAP) { if (threadIdx.x == 0) atomicOr(status, 1); return; }
   int npad = 1;
   while (npad < c) npad <<= 1;
-  for (int i = threadIdx.x; i < npad; i += PT_THREADS) {
-    unsigned long long w = ~0ull;
-    if (i < c) {
-      const int r = (i >= off[1]) + (i >= off[2]) + (i >= off[3]);
-      const long long src = ((long long)row * 4 + r) * PT_CAPR + (i - off[r]);
-      w = ((unsigned long long)pt_key(cand_val[src]) << 32) | (unsigned)cand_idx[src];
-    }
-    s[i] = w;
+  // regions in order; every region's entries are copied by the whole CTA
+  for (int r = 0, off = 0; r < nreg; ++r) {
+    const int m = min(rc[r], capr);
+    const long long src = ((long long)row * nreg + r) * capr;
+    for (int i = threadIdx.x; i < m; i += PT_THREADS)
+      s[off + i] = ((unsigned long long)pt_key(cand_val[src + i]) << 32) | (unsigned)cand_idx[src + i];
+    off += m;
   }
+  for (int i = c + threadIdx.x; i < npad; i += PT_THREADS) s[i] = ~0ull;
   __syncthreads();
   for (int kk = 2; kk <= npad; kk <<= 1) {
     for (int j = kk >> 1; j >= 1; j >>= 1) {
@@ -470,29 +535,142 @@ pairwise_topk_finish_kernel(const int* __restrict__ cnt, const float* __restrict
   }
 }
 
+// the sweep's grid and regions.  All-pairs (split = false): at most one CTA per row block starts inside it, so nparts = 2
+// (the fixed layout of se_pairwise_topk).  Two sets (split = true): every SM, and nparts = the most CTAs that share a
+// row block; regions shrink (down to PT_MIN_CAPR) so that a row's regions hold about twice the sort's capacity.
+struct PtShape { int grid, nparts, capr; };
+static PtShape pt_sweep_shape(int rows, int ncols, bool split) {
+  const int tiles_m = ceil_div(rows, PW_BM), tiles_n = ceil_div(ncols, PW_BN);
+  PtShape sh;
+  sh.grid = min(sm_count(), tiles_m * tiles_n);
+  if (!split) { sh.grid = max(1, min(sh.grid, tiles_m)); sh.nparts = 2; sh.capr = PT_CAPR; return sh; }
+  const int per = ceil_div(tiles_m * tiles_n, sh.grid);
+  sh.nparts = 2;
+  for (int tm = 0; tm < tiles_m; ++tm) {
+    const int first = tm * tiles_n / per, last = ((tm + 1) * tiles_n - 1) / per;
+    sh.nparts = max(sh.nparts, last - first + 1);
+  }
+  sh.capr = min(PT_CAPR, max(PT_MIN_CAPR, ceil_div(PT_CAP, sh.nparts) / 32 * 32));
+  return sh;
+}
+
 // extra workspace of the fused path, carved behind the matrix path's (all regions 256-byte aligned)
 struct PtWs {
   __half* Sh; __half* Sl; float* sq_s; float* tau_sum; int* cnt; float* cv; int* ci; long long bytes;
   int S;
 };
-static PtWs pt_carve(void* base, int N, int KW, int rows) {
+static PtWs pt_carve(void* base, int N, int KW, int rows, const PtShape& sh) {
   PtWs w;
   w.S = min(N, PT_SAMPLE);
+  const long long nreg = 2LL * sh.nparts;
   uintptr_t p0 = (reinterpret_cast<uintptr_t>(base) + 255) & ~(uintptr_t)255, p = p0;
   auto take = [&](long long bytes) { uintptr_t r = p; p += (bytes + 255) & ~255LL; return r; };
   w.Sh = reinterpret_cast<__half*>(take((long long)(w.S + 256) * KW * 2));     // + one spare tile of rows for clipped reads
   w.Sl = reinterpret_cast<__half*>(take((long long)(w.S + 256) * KW * 2));
   w.sq_s = reinterpret_cast<float*>(take((long long)(w.S + 512) * 4));
   w.tau_sum = reinterpret_cast<float*>(take((long long)rows * 4));
-  w.cnt = reinterpret_cast<int*>(take((long long)rows * 4 * 4));
-  w.cv = reinterpret_cast<float*>(take((long long)rows * PT_CAP * 4));
-  w.ci = reinterpret_cast<int*>(take((long long)rows * PT_CAP * 4));
+  w.cnt = reinterpret_cast<int*>(take((long long)rows * nreg * 4));
+  w.cv = reinterpret_cast<float*>(take((long long)rows * nreg * sh.capr * 4));
+  w.ci = reinterpret_cast<int*>(take((long long)rows * nreg * sh.capr * 4));
   w.bytes = (long long)(p - p0) + 256;
   return w;
 }
 
 long long pairwise_topk_extra_bytes(int N, int D, int rows) {
-  return pt_carve(nullptr, N, ceil_div(D, 16) * 16, rows).bytes;
+  return pt_carve(nullptr, N, ceil_div(D, 16) * 16, rows, pt_sweep_shape(rows, N, false)).bytes;
+}
+
+// the nested threshold pass's workspace behind the sweep's: the sample's split operands and norms, the k2 first ranks of
+// every row against it, a status word, then the nested call's own PtWs
+struct PtNest { __half* Sh; __half* Sl; float* sq; int* idx; float* val; int* status; void* extra; long long bytes; };
+static PtNest pt_nest_carve(void* base, int KW, int rows) {
+  PtNest n;
+  uintptr_t p0 = (reinterpret_cast<uintptr_t>(base) + 255) & ~(uintptr_t)255, p = p0;
+  auto take = [&](long long bytes) { uintptr_t r = p; p += (bytes + 255) & ~255LL; return r; };
+  n.Sh = reinterpret_cast<__half*>(take((long long)(PT_NEST_S + 256) * KW * 2));
+  n.Sl = reinterpret_cast<__half*>(take((long long)(PT_NEST_S + 256) * KW * 2));
+  n.sq = reinterpret_cast<float*>(take((long long)(PT_NEST_S + 512) * 4));
+  n.idx = reinterpret_cast<int*>(take((long long)rows * PT_NEST_MAXK * 4));
+  n.val = reinterpret_cast<float*>(take((long long)rows * PT_NEST_MAXK * 4));
+  n.status = reinterpret_cast<int*>(take(256));
+  n.extra = reinterpret_cast<void*>(p);
+  n.bytes = (long long)(p - p0) + 256 + pt_carve(nullptr, PT_NEST_S, KW, rows, pt_sweep_shape(rows, PT_NEST_S, true)).bytes;
+  return n;
+}
+
+long long cross_topk_extra_bytes(int Nd, int D, int rows) {
+  const int KW = ceil_div(D, 16) * 16;
+  const PtWs w = pt_carve(nullptr, Nd, KW, rows, pt_sweep_shape(rows, Nd, true));
+  return w.bytes + (Nd > PT_NEST_S ? pt_nest_carve(nullptr, KW, rows).bytes : 0);
+}
+
+// row r's threshold = the k2-th smallest sample distance; a failed nested pass fails the call
+__global__ void __launch_bounds__(256)
+pairwise_nest_threshold_kernel(const float* __restrict__ val, int k2, int rows, const int* __restrict__ nest_status,
+                               float* __restrict__ tau, int* __restrict__ status) {
+  pdl_grid_sync();
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < rows) tau[r] = val[(long long)r * k2 + k2 - 1];
+  if (r == 0 && *nest_status) atomicOr(status, 2);
+}
+
+// sample pass, sweep and finishing sort of rows [row0, row0+rows) of the A operand against the ncols items of B;
+// `extra` is the fused path's own workspace
+static int pt_run(const PwLayout& A, int Na, const PwLayout& B, int ncols, bool split, int row0, int rows, int pmode, int k,
+                  int* out_idx, float* out_val, int ldo, void* extra, int* status, cudaStream_t st) {
+  const PtShape sh = pt_sweep_shape(rows, ncols, split);
+  const PtWs w = pt_carve(extra, ncols, A.KW, rows, sh);
+  const int S = w.S, stride = ncols / S;
+  if (cudaMemsetAsync(w.cnt, 0, (size_t)rows * 2 * sh.nparts * 4, st) != cudaSuccess || cudaMemsetAsync(status, 0, 4, st) != cudaSuccess ||
+      cudaMemsetAsync(w.sq_s, 0, (size_t)(S + 512) * 4, st) != cudaSuccess ||
+      cudaMemsetAsync(w.tau_sum, 0, (size_t)rows * 4, st) != cudaSuccess) {
+    set_error("pairwise_topk: memset failed");
+    return SE_ERR_CUDA;
+  }
+  int rc;
+  if (split && ncols > PT_NEST_S) {
+    PtNest n = pt_nest_carve(reinterpret_cast<uint8_t*>(extra) + w.bytes, A.KW, rows);
+    launch(pairwise_sample_kernel, dim3(min(sm_count() * 4, ceil_div(PT_NEST_S * A.KW, 256))), dim3(256), 0, st, B.Fh, B.Fl, B.sq,
+           B.KW, PT_NEST_S, ncols / PT_NEST_S, n.Sh, n.Sl, n.sq);
+    rc = check_launch("pairwise_sample_kernel");
+    if (rc) return rc;
+    PwLayout Bs = B;
+    Bs.Fh = n.Sh; Bs.Fl = n.Sl; Bs.sq = n.sq;
+    const long long k2l = ceil_div<long long>(3LL * k * PT_NEST_S, ncols);
+    const int k2 = (int)(k2l < 1 ? 1 : (k2l > PT_NEST_MAXK ? PT_NEST_MAXK : k2l));
+    rc = pt_run(A, Na, Bs, PT_NEST_S, true, row0, rows, pmode, k2, n.idx, n.val, k2, n.extra, n.status, st);
+    if (rc) return rc;
+    launch(pairwise_nest_threshold_kernel, dim3(ceil_div(rows, 256)), dim3(256), 0, st, (const float*)n.val, k2, rows,
+           (const int*)n.status, w.tau_sum, status);
+    rc = check_launch("pairwise_nest_threshold_kernel");
+    if (rc) return rc;
+    PwEpi e1 = {1, w.tau_sum, 1.f, w.cnt, w.cv, w.ci, sh.capr, 0, sh.grid, sh.nparts};
+    rc = pw_launch(A, Na, row0, rows, B.Fh, B.Fl, B.sq, ncols, pmode, nullptr, 0, &e1, st);
+    if (rc) return rc;
+    launch(pairwise_topk_finish_kernel, dim3(rows), dim3(PT_THREADS), 0, st, w.cnt, w.cv, w.ci, 2 * sh.nparts, sh.capr, k,
+           out_idx, out_val, ldo, status);
+    return check_launch("pairwise_topk_finish_kernel");
+  }
+  launch(pairwise_sample_kernel, dim3(min(sm_count() * 4, ceil_div(S * A.KW, 256))), dim3(256), 0, st, B.Fh, B.Fl, B.sq, B.KW, S,
+         stride, w.Sh, w.Sl, w.sq_s);
+  rc = check_launch("pairwise_sample_kernel");
+  if (rc) return rc;
+  // thresholds: mean over the sample's half tiles (64 distances each) of the j-th smallest distance, j chosen so that
+  // ~3k of the row's N entries are expected below it (j / 65 of the row).  j > 8 is not tracked: such shapes (k large
+  // against N) simply find fewer than k candidates, report status != 0 and take the matrix path.
+  int j = (int)((3LL * k * (PW_BN / 2 + 1) + ncols / 2) / ncols);
+  j = max(2, min(8, j));
+  PwEpi e2 = {2, w.tau_sum, 0.f, nullptr, nullptr, nullptr, 0, j - 1, 0, 0};
+  rc = pw_launch(A, Na, row0, rows, w.Sh, w.Sl, w.sq_s, S, pmode, nullptr, 0, &e2, st);
+  if (rc) return rc;
+  // the mean over the half tiles that fed the thresholds: those with >= 8 sample columns (a ragged last one may have fewer)
+  const int halves = S / (PW_BN / 2) + (S % (PW_BN / 2) >= 8 ? 1 : 0);
+  PwEpi e1 = {1, w.tau_sum, 1.f / (float)halves, w.cnt, w.cv, w.ci, sh.capr, 0, sh.grid, sh.nparts};
+  rc = pw_launch(A, Na, row0, rows, B.Fh, B.Fl, B.sq, ncols, pmode, nullptr, 0, &e1, st);
+  if (rc) return rc;
+  launch(pairwise_topk_finish_kernel, dim3(rows), dim3(PT_THREADS), 0, st, w.cnt, w.cv, w.ci, 2 * sh.nparts, sh.capr, k, out_idx,
+         out_val, ldo, status);
+  return check_launch("pairwise_topk_finish_kernel");
 }
 
 int pairwise_tc_topk(const float* F, int ldF, int N, int D, int row0, int rows, int pmode, int k, int* out_idx, float* out_val,
@@ -501,33 +679,17 @@ int pairwise_tc_topk(const float* F, int ldF, int N, int D, int row0, int rows, 
   PwLayout L;
   int rc = pw_prepare(F, ldF, N, D, ws, st, &L);
   if (rc) return rc;
-  const PtWs w = pt_carve(L.Fl + (long long)N * L.KW + 2048, N, L.KW, rows);
-  const int S = w.S, stride = N / S;
-  if (cudaMemsetAsync(w.cnt, 0, (size_t)rows * 16, st) != cudaSuccess || cudaMemsetAsync(status, 0, 4, st) != cudaSuccess ||
-      cudaMemsetAsync(w.sq_s, 0, (size_t)(S + 512) * 4, st) != cudaSuccess ||
-      cudaMemsetAsync(w.tau_sum, 0, (size_t)rows * 4, st) != cudaSuccess) {
-    set_error("pairwise_topk: memset failed");
-    return SE_ERR_CUDA;
-  }
-  launch(pairwise_sample_kernel, dim3(min(sm_count() * 4, ceil_div(S * L.KW, 256))), dim3(256), 0, st, L.Fh, L.Fl, L.sq, L.KW, S, stride,
-         w.Sh, w.Sl, w.sq_s);
-  rc = check_launch("pairwise_sample_kernel");
+  return pt_run(L, N, L, N, false, row0, rows, pmode, k, out_idx, out_val, ldo, L.Fl + (long long)N * L.KW + 2048, status, st);
+}
+
+int pairwise_tc_cross_topk(const float* Q, int ldQ, int Nq, const float* X, int ldX, int Nd, int D, int row0, int rows,
+                           int pmode, int k, int* out_idx, float* out_val, int ldo, float* ws_q, float* ws_x, void* extra,
+                           int* status, cudaStream_t st) {
+  if (k < 1 || k > 1024 || k > Nd) return SE_ERR_UNSUPPORTED;
+  PwLayout A, B;
+  int rc = cw_prepare(Q, ldQ, Nq, X, ldX, Nd, D, ws_q, ws_x, st, &A, &B);
   if (rc) return rc;
-  // thresholds: mean over the sample's half tiles (64 distances each) of the j-th smallest distance, j chosen so that
-  // ~3k of the row's N entries are expected below it (j / 65 of the row).  j > 8 is not tracked: such shapes (k large
-  // against N) simply find fewer than k candidates, report status != 0 and take the matrix path.
-  int j = (int)((3LL * k * (PW_BN / 2 + 1) + N / 2) / N);
-  j = max(2, min(8, j));
-  PwEpi e2 = {2, w.tau_sum, 0.f, nullptr, nullptr, nullptr, 0, j - 1};
-  rc = pw_launch(L, N, row0, rows, w.Sh, w.Sl, w.sq_s, S, pmode, nullptr, 0, &e2, st);
-  if (rc) return rc;
-  // the mean over the half tiles that fed the thresholds: those with >= 8 sample columns (a ragged last one may have fewer)
-  const int halves = S / (PW_BN / 2) + (S % (PW_BN / 2) >= 8 ? 1 : 0);
-  PwEpi e1 = {1, w.tau_sum, 1.f / (float)halves, w.cnt, w.cv, w.ci, PT_CAPR, 0};
-  rc = pw_launch(L, N, row0, rows, L.Fh, L.Fl, L.sq, N, pmode, nullptr, 0, &e1, st);
-  if (rc) return rc;
-  launch(pairwise_topk_finish_kernel, dim3(rows), dim3(PT_THREADS), 0, st, w.cnt, w.cv, w.ci, k, out_idx, out_val, ldo, status);
-  return check_launch("pairwise_topk_finish_kernel");
+  return pt_run(A, Nq, B, Nd, true, row0, rows, pmode, k, out_idx, out_val, ldo, extra, status, st);
 }
 
 }  // namespace se

@@ -97,23 +97,24 @@ __device__ __forceinline__ int slot_of(const unsigned long long* s, int P, unsig
 
 __global__ void __launch_bounds__(RP_THREADS, 4)    // 4 CTAs per SM: 128 KB of shared memory, 56 registers, no spills
 relevant_positions_kernel(const float* __restrict__ dist, long long ld, int rows, int n, int q0,
-                          const int32_t* __restrict__ labels, int C, const int32_t* __restrict__ offsets,
-                          const int32_t* __restrict__ members, const int64_t* __restrict__ out_offsets,
-                          int32_t* __restrict__ out) {
+                          const int32_t* __restrict__ query_labels, const int32_t* __restrict__ labels, int C,
+                          const int32_t* __restrict__ offsets, const int32_t* __restrict__ members,
+                          const int64_t* __restrict__ out_offsets, int32_t* __restrict__ out) {
   pdl_grid_sync();
   __shared__ unsigned long long s[RP_CHUNK];
   __shared__ int pos[RP_CHUNK];                // slot histogram -> positions
   __shared__ int rnk[RP_CHUNK];                // member histogram -> ranks among the members
   __shared__ int warp_tot[RP_THREADS / 32];
-  const int i = blockIdx.x, q = q0 + i;
-  const int c = labels[q];
+  // with query_labels (se_relevant_positions_q) the query is no database item: q = -1 removes nothing
+  const int i = blockIdx.x, q = query_labels ? -1 : q0 + i;
+  const int c = query_labels ? query_labels[i] : labels[q];
   if (c < 0 || c >= C) return;                 // se_class_index has rejected such labels
   const float* row = dist + (long long)i * ld;
   const int32_t* mem = members + offsets[c];
-  const int nrel = offsets[c + 1] - offsets[c] - 1;
+  const int nrel = offsets[c + 1] - offsets[c] - (q >= 0 ? 1 : 0);
   int32_t* o = out + out_offsets[i];
-  int qpos = 0;                                // q's place in its class list (ascending indices)
-  for (int lo = 0, hi = nrel; lo <= hi;) {
+  int qpos = q >= 0 ? 0 : nrel;                // q's place in its class list (ascending indices)
+  for (int lo = 0, hi = q >= 0 ? nrel : -1; lo <= hi;) {
     const int mid = (lo + hi) >> 1;
     if (mem[mid] < q) lo = mid + 1; else if (mem[mid] > q) hi = mid - 1; else { qpos = mid; break; }
   }
@@ -211,6 +212,17 @@ extern "C" int se_relevant_positions(const float* dist, int64_t ld, int rows, in
   SE_REQUIRE((int64_t)q0 + rows <= n, "query rows outside the database");
   if (rows == 0) return SE_OK;
   launch(relevant_positions_kernel, dim3(rows), dim3(RP_THREADS), 0, as_stream(stream), dist, (long long)ld, rows, n, q0,
-         labels, C, offsets, members, out_offsets, out);
+         (const int32_t*)nullptr, labels, C, offsets, members, out_offsets, out);
+  return check_launch("relevant_positions_kernel");
+}
+
+extern "C" int se_relevant_positions_q(const float* dist, int64_t ld, int rows, int n, const int32_t* query_labels,
+                                       const int32_t* labels, int C, const int32_t* offsets, const int32_t* members,
+                                       const int64_t* out_offsets, int32_t* out, void* stream) {
+  SE_REQUIRE(dist && query_labels && labels && offsets && members && out_offsets && out, "null pointer");
+  SE_REQUIRE(rows >= 0 && n >= 0 && C > 0 && ld >= n, "bad sizes");
+  if (rows == 0) return SE_OK;
+  launch(relevant_positions_kernel, dim3(rows), dim3(RP_THREADS), 0, as_stream(stream), dist, (long long)ld, rows, n, 0,
+         query_labels, labels, C, offsets, members, out_offsets, out);
   return check_launch("relevant_positions_kernel");
 }

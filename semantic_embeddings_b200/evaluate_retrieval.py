@@ -8,6 +8,8 @@ hierarchical-precision metrics are hand-written kernels (se_pairwise_dist, se_ro
 se_hier_metrics); `retrieval_metrics` chains them per block of query rows without a host round trip.
 `recall_precision` is plot_recall_precision.py's curve and mAP: distance rows, then the positions of each query's
 relevant items (se_class_index, se_relevant_positions), then the curve from those positions on the host.
+The database_* functions do the same for queries against a separate database (se_cross_dist, se_cross_topk,
+se_hier_metrics_q, se_relevant_positions_q): nothing is removed from a ranking, and queries need not be database items.
 """
 import pickle
 
@@ -381,3 +383,276 @@ def hierarchical_precision_topk(topk_idx, labels, wup_lut, lcs_height_lut, ks=(1
         per['AHP@%d (WUP)' % clip] = res[:, 2 * len(ks)]
         per['AHP@%d (LCS_HEIGHT)' % clip] = res[:, 2 * len(ks) + 1]
     return {m: float(v.mean()) for m, v in per.items()}, per
+
+
+# ------------------------------------------------------------------------------------ queries against a separate database
+def _to_device(a, device=None):
+    import torch
+    f = np.ascontiguousarray(np.asarray(a, dtype=np.float32))
+    if f.ndim != 2:
+        raise ValueError('Feature matrix must be 2-dimensional. Actual shape: {}'.format(f.shape))
+    return torch.from_numpy(f).to(torch.device(device or 'cuda'))
+
+
+def _check_sets(q_dev, x_dev):
+    if q_dev.shape[1] != x_dev.shape[1]:
+        raise ValueError('queries and database differ in dimension: {} vs {}'.format(q_dev.shape[1], x_dev.shape[1]))
+    if q_dev.shape[0] == 0 or x_dev.shape[0] == 0:
+        raise ValueError('need at least one query and one database item')
+
+
+def _dist_buffer(rows, n, device):
+    """A [rows, n] float32 device matrix whose rows start on 16-byte boundaries (row pitch a multiple of 4): the
+    tensor-core distance kernels store 16-byte vectors and take the fp32 tiles for any other layout."""
+    import torch
+    return torch.empty((rows, (n + 3) // 4 * 4), dtype=torch.float32, device=device)[:, :n]
+
+
+def cross_distances(queries=None, database=None, normalize=False, row0=0, rows=None, mode=None, device=None, out=None,
+                    q_dev=None, x_dev=None):
+    """Rows [row0, row0+rows) of the Nq x Nd distance matrix of the queries against the database (se_cross_dist) as a
+    CUDA tensor, with the semantics of pairwise_distances (evaluate_retrieval.py:56-63): normalize=True gives -Q^ X^T
+    of the L2-normalised sets, normalize=False sq_q + sq_x - 2 Q X^T.  Neither input is modified.  The result's rows
+    are padded to a multiple of 4 floats (its stride(0)), so that the tensor-core modes store with their own kernel;
+    an `out` with another row pitch gets the fp32 tiles, as in pairwise_distances."""
+    import torch
+    q_dev = _to_device(queries, device) if q_dev is None else q_dev
+    x_dev = _to_device(database, q_dev.device) if x_dev is None else x_dev
+    _check_sets(q_dev, x_dev)
+    Nq, D = q_dev.shape
+    Nd = x_dev.shape[0]
+    rows = Nq - row0 if rows is None else rows
+    mode = _lib.SE_MODE_TF32 if mode is None else mode
+    ws = torch.empty(int(_lib.load().se_cross_workspace_bytes(Nq, Nd, D, mode)), dtype=torch.uint8, device=q_dev.device)
+    if out is None:
+        out = _dist_buffer(rows, Nd, q_dev.device)
+    pmode = _lib.SE_PDIST_NEGDOT if normalize else _lib.SE_PDIST_SQEUCLID
+    with torch.cuda.device(q_dev.device):
+        _lib.call('se_cross_dist', q_dev.data_ptr(), q_dev.stride(0), Nq, x_dev.data_ptr(), x_dev.stride(0), Nd, D, row0, rows,
+                  pmode, 1 if normalize else 0, out.data_ptr(), out.stride(0), ws.data_ptr(), mode, _lib.stream_ptr())
+    return out
+
+
+def _matrix_topk(d, k, want_values):
+    """The first k entries of every row's ranking of a device distance block (se_row_topk, or the se_row_argsort prefix
+    beyond se_row_topk's limits)."""
+    n = d.shape[1]
+    if k <= TOPK_MAX and n <= TOPK_MAX_N:
+        return row_topk(d, k, want_values)
+    idx = row_argsort(d)[:, :k].contiguous()
+    return idx, (d.gather(1, idx.long()) if want_values else None)
+
+
+def cross_topk(queries=None, database=None, k=251, normalize=False, row0=0, rows=None, q_dev=None, x_dev=None, device=None,
+               want_values=False, allow_fallback=True, block_rows=4096):
+    """The k nearest database items of query rows [row0, row0+rows) (ascending distance, ties by index) without the
+    distance matrix in memory: se_cross_topk.  Where the fused path cannot run (D > 128, k > min(1024, Nd)) or reports
+    that some row's candidate list was too short or too long (status != 0), the matrix path gives the same ranking:
+    cross_distances, then se_row_topk or the se_row_argsort prefix.
+    Returns (int32 [rows, k] device tensor, float32 values or None, fused: bool)."""
+    import torch
+    q_dev = _to_device(queries, device) if q_dev is None else q_dev
+    x_dev = _to_device(database, q_dev.device) if x_dev is None else x_dev
+    _check_sets(q_dev, x_dev)
+    Nq, D = q_dev.shape
+    Nd = x_dev.shape[0]
+    rows = Nq - row0 if rows is None else rows
+    if not 1 <= k <= Nd:
+        raise ValueError('k = {} outside 1 .. {} (the database size)'.format(k, Nd))
+    dev = q_dev.device
+    idx = torch.empty((rows, k), dtype=torch.int32, device=dev)
+    val = torch.empty((rows, k), dtype=torch.float32, device=dev) if want_values else None
+    pmode = _lib.SE_PDIST_NEGDOT if normalize else _lib.SE_PDIST_SQEUCLID
+    fused = False
+    if D <= 128 and k <= 1024:
+        ws = torch.empty(int(_lib.load().se_cross_topk_workspace_bytes(Nq, Nd, D, rows)), dtype=torch.uint8, device=dev)
+        status = torch.zeros(1, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.call('se_cross_topk', q_dev.data_ptr(), q_dev.stride(0), Nq, x_dev.data_ptr(), x_dev.stride(0), Nd, D, row0,
+                      rows, pmode, 1 if normalize else 0, k, idx.data_ptr(), _lib.ptr(val), k, ws.data_ptr(), status.data_ptr(),
+                      _lib.stream_ptr())
+        fused = int(status.item()) == 0
+        del ws
+    if not fused:
+        if not allow_fallback:
+            raise _lib.SeError('se_cross_topk: candidate lists out of range (status != 0)')
+        block = max(1, min(block_rows, rows))
+        buf = _dist_buffer(block, Nd, dev)
+        for r0 in range(0, rows, block):
+            r = min(block, rows - r0)
+            d = cross_distances(None, None, normalize, row0 + r0, r, None, out=buf[:r], q_dev=q_dev, x_dev=x_dev)
+            i2, v2 = _matrix_topk(d, k, want_values)
+            idx[r0:r0 + r] = i2
+            if want_values:
+                val[r0:r0 + r] = v2
+    return idx, val, fused
+
+
+def database_ranking(queries, database, normalize=False, block_rows=4096, mode=None, device=None, topk=None):
+    """int64 ndarray (Nq, Nd) -- or (Nq, topk) -- of database indices sorted by ascending distance per query."""
+    import torch
+    q_dev = _to_device(queries, device)
+    x_dev = _to_device(database, q_dev.device)
+    _check_sets(q_dev, x_dev)
+    Nq, Nd = q_dev.shape[0], x_dev.shape[0]
+    k = Nd if topk is None else min(topk, Nd)
+    if k < Nd:
+        return cross_topk(None, None, k, normalize, q_dev=q_dev, x_dev=x_dev)[0].cpu().numpy().astype(np.int64)
+    ranking = np.empty((Nq, k), dtype=np.int64)
+    block = max(1, min(block_rows, Nq, _rows_fitting(Nd, 3)))
+    buf = _dist_buffer(block, Nd, q_dev.device)
+    for r0 in range(0, Nq, block):
+        r = min(block, Nq - r0)
+        d = cross_distances(None, None, normalize, r0, r, mode, out=buf[:r], q_dev=q_dev, x_dev=x_dev)
+        ranking[r0:r0 + r] = row_argsort(d).cpu().numpy()
+    return ranking
+
+
+def database_retrieval(queries, database, normalize=False, return_generator=True, topk=None):
+    """pairwise_retrieval for queries against a separate database: yields (query id, ranked list of database ids).
+    queries / database: anything _features_to_array accepts (2-d array, dict id -> vector, {'feat': dict}, pickle
+    path); ids are the dict keys, or row numbers for arrays.  topk: only the first `topk` database items of every query
+    (se_cross_topk) instead of the full ranking.  Neither input is modified, also with normalize=True."""
+    qf, q_ids = _features_to_array(queries)
+    xf, x_ids = _features_to_array(database)
+    ranking = database_ranking(qf, xf, normalize, topk=topk)
+    q_ids = np.arange(len(ranking)) if q_ids is None else q_ids
+    if x_ids is not None:
+        gen = ((q_ids[i], x_ids[ret].tolist()) for i, ret in enumerate(ranking))
+    else:
+        gen = ((q_ids[i], ret.tolist()) for i, ret in enumerate(ranking))
+    return gen if return_generator else dict(gen)
+
+
+def _rows_fitting(n, words_per_entry, budget=None):
+    """How many rows of n entries of `words_per_entry` 4-byte words fit the memory budget (default: a quarter of the
+    free device memory)."""
+    import torch
+    if budget is None:
+        budget = torch.cuda.mem_get_info()[0] // 4
+    return max(1, int(budget // (4 * words_per_entry * max(n, 1))))
+
+
+def _class_lists(labels_dev, C, query_labels):
+    """Class index of the database and, per query, how many database items share its class."""
+    offsets, members = class_index(labels_dev, C)
+    sizes = np.diff(offsets.cpu().numpy().astype(np.int64))
+    return offsets, members, sizes[np.asarray(query_labels, dtype=np.int64)]
+
+
+def _relevant_positions_q(dist, q_lab_dev, labels_dev, offsets, members, nrel):
+    """se_relevant_positions_q of a device distance block: the positions of every query's class members, concatenated."""
+    import torch
+    rows, n = dist.shape
+    starts = np.cumsum(nrel) - nrel
+    total = int(np.sum(nrel))
+    out_off = torch.from_numpy(starts.astype(np.int64)).to(dist.device)
+    out = torch.empty(max(total, 1), dtype=torch.int32, device=dist.device)
+    with torch.cuda.device(dist.device):
+        _lib.call('se_relevant_positions_q', _lib.ptr(dist), dist.stride(0), rows, n, _lib.ptr(q_lab_dev), _lib.ptr(labels_dev),
+                  offsets.shape[0] - 1, _lib.ptr(offsets), _lib.ptr(members), _lib.ptr(out_off), _lib.ptr(out), _lib.stream_ptr())
+    return out[:total]
+
+
+def _check_labels(lab, n, what):
+    lab = np.asarray(lab, dtype=np.int64)
+    if lab.shape != (n,):
+        raise ValueError('need one {} label per row: {} labels for {} rows'.format(what, lab.shape, n))
+    if n and (lab.min() < 0 or lab.max() >= 2 ** 31 - 1):
+        raise ValueError('{} labels must be non-negative int32 class indices'.format(what))
+    return lab
+
+
+def database_metrics(queries, query_labels_ix, database, labels_ix, wup_lut, lcs_height_lut, kcurve=250, clip_ahp=None,
+                     compute_ap=True, normalize=False, block_rows=2048, mode=None, device=None, rank=0, world=1):
+    """retrieval_metrics for queries against a separate database: hierarchical_precision(..., ignore_qids=False) of the
+    rankings of the database for every query, nothing removed from them.
+    query_labels_ix / labels_ix: class indices of the queries / the database items in the tables wup_lut, lcs_height_lut.
+    clip_ahp = K: P@k (k <= kcurve) and AHP@K from the first max(kcurve, K) ranks of se_cross_topk -- nothing is fully
+    sorted.  clip_ahp None / 0: AHP over the whole list, from full rankings (se_row_argsort, row blocks sized to the free
+    memory).  AP: from the positions of each query's class members in its distance row (se_relevant_positions_q), the
+    mean of k / pos_k over the hits; it needs the distance rows but no sort.
+    Query rows are sharded over `world` processes; returns ({'curve' [rows, 2, kcurve], 'ahp' [rows, 2], 'ap' [rows]},
+    (row0, rows)) for this rank's rows."""
+    import torch
+    from .class_hierarchy import hierarchical_metrics
+    from .parallel import shard_rows
+    q_dev = _to_device(queries, device)
+    x_dev = _to_device(database, q_dev.device)
+    _check_sets(q_dev, x_dev)
+    Nq, Nd = q_dev.shape[0], x_dev.shape[0]
+    q_lab = _check_labels(query_labels_ix, Nq, 'query')
+    x_lab = _check_labels(labels_ix, Nd, 'database')
+    C = np.asarray(wup_lut).shape[0]
+    if max(q_lab.max(), x_lab.max()) >= C:
+        raise ValueError('class index outside the {} classes of the look-up tables'.format(C))
+    clip = int(clip_ahp) if clip_ahp else -1
+    n_ret = Nd if clip < 0 else min(Nd, max(kcurve, clip))
+    kcurve = min(kcurve, n_ret)
+    row0, rows = shard_rows(Nq, world, rank)
+    dev = q_dev.device
+    x_lab_d = torch.from_numpy(x_lab.astype(np.int32)).to(dev)
+    if compute_ap:
+        offsets, members, nrel_all = _class_lists(x_lab_d, C, q_lab)
+    # full rankings: dist + argsort words + indices per row; otherwise only the distance rows of the AP
+    block = max(1, min(block_rows, max(rows, 1), _rows_fitting(Nd, 4 if clip < 0 else 1)))
+    need_dist = clip < 0 or compute_ap
+    buf = _dist_buffer(block, Nd, dev) if need_dist and rows else None
+    outs = []
+    for r0 in range(row0, row0 + rows, block):
+        r = min(block, row0 + rows - r0)
+        d = cross_distances(None, None, normalize, r0, r, mode, out=buf[:r], q_dev=q_dev, x_dev=x_dev) if need_dist else None
+        if clip < 0:
+            idx = row_argsort(d)
+        else:
+            idx = cross_topk(None, None, n_ret, normalize, r0, r, q_dev=q_dev, x_dev=x_dev)[0]
+        res = hierarchical_metrics(idx, None, x_lab, wup_lut, lcs_height_lut, kcurve, clip, False,
+                                   query_labels=q_lab[r0:r0 + r])
+        if compute_ap:
+            nrel = nrel_all[r0:r0 + r]
+            q_lab_d = torch.from_numpy(q_lab[r0:r0 + r].astype(np.int32)).to(dev)
+            pos = _relevant_positions_q(d, q_lab_d, x_lab_d, offsets, members, nrel).cpu().numpy()
+            res['ap'] = recall_precision_points(pos, nrel)[0]
+        outs.append(res)
+    out = {k: np.concatenate([o[k] for o in outs]) for k in (outs[0] if outs else {})}
+    return out, (row0, rows)
+
+
+def database_recall_precision(queries, query_labels, database, labels, normalize=False, bins=None, block_rows=2048, mode=None,
+                              device=None):
+    """recall_precision for queries against a separate database: the loop of plot_recall_precision.py:59-77 without its
+    `r != qid` filter -- the relevant items of a query are the database items of its class, and nothing is removed from
+    its ranking.  Same host arithmetic for the curve and the APs (recall_precision_points); a query whose class has no
+    database item counts as AP 0 and adds no curve point.
+    Returns (recall levels float64 [L], mean precision per level float64 [L], mAP, per-query AP float64 [Nq])."""
+    import torch
+    q_dev = _to_device(queries, device)
+    x_dev = _to_device(database, q_dev.device)
+    _check_sets(q_dev, x_dev)
+    for t in (q_dev, x_dev):
+        if not torch.isfinite(t).all():
+            raise ValueError('features must be finite')
+    Nq, Nd = q_dev.shape[0], x_dev.shape[0]
+    q_lab = _check_labels(query_labels, Nq, 'query')
+    x_lab = _check_labels(labels, Nd, 'database')
+    if bins is not None and int(bins) <= 0:
+        raise ValueError('bins must be positive')
+    dev = q_dev.device
+    C = int(max(q_lab.max(), x_lab.max())) + 1
+    x_lab_d = torch.from_numpy(x_lab.astype(np.int32)).to(dev)
+    offsets, members, nrel_all = _class_lists(x_lab_d, C, q_lab)
+    ap = np.empty(Nq)
+    acc = {}
+    block = max(1, min(block_rows, Nq, _rows_fitting(Nd, 1)))
+    buf = _dist_buffer(block, Nd, dev)
+    for r0 in range(0, Nq, block):
+        r = min(block, Nq - r0)
+        d = cross_distances(None, None, normalize, r0, r, mode, out=buf[:r], q_dev=q_dev, x_dev=x_dev)
+        nrel = nrel_all[r0:r0 + r]
+        q_lab_d = torch.from_numpy(q_lab[r0:r0 + r].astype(np.int32)).to(dev)
+        pos = _relevant_positions_q(d, q_lab_d, x_lab_d, offsets, members, nrel).cpu().numpy()
+        ap[r0:r0 + r], q, lvl, val = recall_precision_points(pos, nrel, bins)
+        _collect_levels(acc, q + r0, lvl, val)
+    levels = np.array(sorted(acc), dtype=np.float64)
+    prec = np.array([np.mean(np.concatenate(acc[level])) for level in levels.tolist()], dtype=np.float64)
+    return levels, prec, float(np.mean(ap)), ap
