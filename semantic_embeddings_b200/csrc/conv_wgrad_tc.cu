@@ -193,7 +193,13 @@ conv_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dy, 
   }
 }
 
-// dW[i] += sum over the slices in slice order; dbias likewise (when given)
+// dW[i] += sum over the slices in slice order; dbias likewise (when given).  Each thread adds its element's slices one
+// after the other, starting from 0, so the result does not depend on the launch configuration.  The slices' loads do
+// not depend on the sum: a thread issues WG_RED_BATCH of them before it adds the first, so that a long reduction (684
+// slices for ResNet-110's 16-channel layers at B = 128) waits for splits / WG_RED_BATCH round trips to L2 instead of
+// one per slice or per few slices.  Fewer slices than a batch take the plain loop.
+constexpr int WG_RED_BATCH = 32;
+
 __global__ void __launch_bounds__(256)
 conv_wgrad_reduce_kernel(const float* __restrict__ ws, int splits, long long T, int Cout, float* __restrict__ dw,
                          float* __restrict__ dbias) {
@@ -204,7 +210,15 @@ conv_wgrad_reduce_kernel(const float* __restrict__ ws, int splits, long long T, 
     const float* src = b ? ws + (long long)splits * T + (i - T) : ws + i;
     const long long stride = b ? Cout : T;
     float v = 0.f;
-    for (int k = 0; k < splits; ++k) v += src[k * stride];
+    int k = 0;
+    for (; k + WG_RED_BATCH <= splits; k += WG_RED_BATCH) {
+      float s[WG_RED_BATCH];
+#pragma unroll
+      for (int j = 0; j < WG_RED_BATCH; ++j) s[j] = __ldg(src + (k + j) * stride);
+#pragma unroll
+      for (int j = 0; j < WG_RED_BATCH; ++j) v += s[j];
+    }
+    for (; k < splits; ++k) v += src[k * stride];
     if (b) dbias[i - T] += v;
     else dw[i] += v;
   }
@@ -262,8 +276,11 @@ long long wgrad_fit_splits(long long want, long long T, int Cout) {
 
 int wgrad_reduce(const float* ws, int splits, long long T, int Cout, float* dw, float* dbias, cudaStream_t st) {
   const long long n = T + (dbias ? Cout : 0);
-  const long long blocks = std::min(ceil_div<long long>(n, 256), 4LL * sm_count());
-  launch(conv_wgrad_reduce_kernel, dim3((unsigned)blocks), dim3(256), 0, st, ws, splits, T, Cout, dw, dbias);
+  // fewer elements than 256 per SM (ResNet-110's 16- and 32-channel layers: 2 304 and 9 216): blocks of 64 threads,
+  // so that the reduction spreads over more SMs and more of its loads are in flight at once
+  const int threads = n < 256LL * sm_count() ? 64 : 256;
+  const long long blocks = std::min(ceil_div<long long>(n, threads), 4LL * sm_count());
+  launch(conv_wgrad_reduce_kernel, dim3((unsigned)blocks), dim3(threads), 0, st, ws, splits, T, Cout, dw, dbias);
   return check_launch("conv_wgrad_reduce_kernel");
 }
 
