@@ -33,6 +33,7 @@ struct WgTcParams {
   int npx;                     // N * Ho * Wo
   int chunks;                  // ceil(npx / 32)
   int per_cta;                 // chunks per CTA (even)
+  int box_tiles;               // > 0: 3x3 / stride 1 with X staged once per CTA, this many 64-row tiles per CTA
   float* ws;                   // [2 * gridDim.x][KK * Cout] partial dW, then [2 * gridDim.x][Cout] partial dbias
   float* dw;                   // direct mode (ws == nullptr): atomics straight into dW / dbias
   float* dbias;

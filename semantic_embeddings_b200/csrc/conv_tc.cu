@@ -55,14 +55,6 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a, uint6
   else wgmma_tf32_n128(d, a, b, acc);
 }
 
-template <int BN>
-__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t b, int acc) {
-  if constexpr (BN == 16) wgmma_tf32_rs_n16(d, a, b, acc);
-  else if constexpr (BN == 32) wgmma_tf32_rs_n32(d, a, b, acc);
-  else if constexpr (BN == 64) wgmma_tf32_rs_n64(d, a, b, acc);
-  else wgmma_tf32_rs_n128(d, a, b, acc);
-}
-
 // The A words of k-steps 0..nks-1 for this thread's two rows: a[ks] = (row0, 8ks + t), (row1, 8ks + t),
 // (row0, 8ks + 4 + t), (row1, 8ks + 4 + t) -- the register fragment of wgmma_tf32_rs_n*.  Rows are numbered in the
 // tile `base` (a stage, or one channel block of the resident box); channel 8ks + 4c + t of a row lies in its 16-byte

@@ -65,6 +65,198 @@ __device__ __forceinline__ void put_t(uint8_t* hi, uint8_t* lo, int c4, int px, 
   }
 }
 
+// The 3x3 / stride 1 / 'same' layers with at most 64 input channels (p.box_tiles > 0): 9 * Cin rows of dW take only
+// ceil(9 * Cin / 64) <= 9 row tiles, and the tiles above re-read and re-transpose X once per tile and dY once per row
+// tile.  Here a CTA stages the X pixels its range touches once -- the range plus one image row and one pixel on either
+// side, as [pixel][Cin + WG_BOX_PAD floats] -- and its warpgroups read A straight from that box into registers (the
+// wgmma_tf32_rs fragment), at the pixel shifted by the row's filter tap; taps that fall outside the image read 0 through
+// a per-pixel mask of the nine taps.  dY is transposed once per chunk and serves all box_tiles row tiles of the CTA.
+// The sums are those of the tiled path bit for bit: the same slices (warpgroup wg takes chunks c_begin + wg + 2j), the
+// same TF32 words (hi / lo split of X in registers, of dY by put_t), the same chain of MMAs per chunk and tile, and the
+// same per-thread dbias sums.
+//   Bank conflicts: one A load of a warp reads 8 consecutive channels (g = lane / 4) of 4 pixels (lane % 4); a pixel
+//   stride of Cin + 8 floats puts the 4 pixels 8 banks apart for every Cin % 16 == 0, so the 32 lanes hit 32 banks.
+constexpr int WG_BOX_PAD = 8;
+constexpr size_t WG_BOX_MAX_SMEM = 200 * 1024;
+
+constexpr int wg_box_tiles(int bn) { return bn >= 64 ? 1 : 3; }   // accumulators: 2 * tiles * BN / 2 registers in X3
+
+template <int BN, int X3>
+__device__ __forceinline__ void wgrad_box(const float* __restrict__ x, const float* __restrict__ dy, const WgTcParams& p,
+                                          uint8_t* smem) {
+  constexpr int TPW = wg_box_tiles(BN);
+  constexpr int YQ = WG_PX * BN / 4 / 128;
+  constexpr int Y_BYTES = BN * 128, WG_BYTES = Y_BYTES * (X3 ? 2 : 1);
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, lane = t & 31;
+  uint8_t* sy = smem + wg * WG_BYTES;
+  uint8_t* syl = sy + Y_BYTES;
+  const int PS = p.Cin + WG_BOX_PAD, halo = p.W + 1;
+  const int c_begin = blockIdx.x * p.per_cta, c_end = min(p.chunks, c_begin + p.per_cta), p0 = c_begin * WG_PX;
+  const int box_px = p.per_cta * WG_PX + 2 * halo;
+  float* box = reinterpret_cast<float*>(smem + 2 * WG_BYTES);
+  uint16_t* mask = reinterpret_cast<uint16_t*>(box + box_px * PS);
+
+  // box pixel b is X pixel p0 - halo + b (stride 1 / 'same': X and dY have the same pixel list)
+  const int c4n = p.Cin / 4;
+#pragma unroll 4
+  for (int i = threadIdx.x; i < box_px * c4n; i += WG_THREADS) {
+    const int b = i / c4n, c4 = i - b * c4n, g = p0 - halo + b;
+    if (g >= 0 && g < p.npx)
+      *reinterpret_cast<float4*>(box + b * PS + 4 * c4) = __ldg(reinterpret_cast<const float4*>(x + (long long)g * p.Cin) + c4);
+  }
+  // bit 3r + s of mask[k]: filter tap (r, s) of output pixel p0 + k lies inside its image
+  const int hw = p.H * p.W;
+  for (int k = threadIdx.x; k < p.per_cta * WG_PX; k += WG_THREADS) {
+    const int g = p0 + k;
+    uint32_t m = 0;
+    if (g < p.npx) {
+      const int n = g / hw, rem = g - n * hw, ho = rem / p.W, wo = rem - ho * p.W;
+#pragma unroll
+      for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int s = 0; s < 3; ++s)
+          if (ho + r - 1 >= 0 && ho + r - 1 < p.H && wo + s - 1 >= 0 && wo + s - 1 < p.W) m |= 1u << (3 * r + s);
+    }
+    mask[k] = (uint16_t)m;
+  }
+  __syncthreads();
+
+  // this thread's two A rows (m and m + 8: channels ci and ci + 8 of one tap, Cin % 16 == 0) in each of its row tiles
+  const int gy = (p.KK + WG_MT - 1) / WG_MT, ty0 = blockIdx.y * TPW;
+  int aoff[TPW], abit[TPW];
+#pragma unroll
+  for (int i = 0; i < TPW; ++i) {
+    const int m = (ty0 + i) * WG_MT + fragment_row(0, t);
+    const int tap = m / p.Cin, ci = m - tap * p.Cin, r = tap / 3, s = tap - 3 * r;
+    aoff[i] = (halo + (r - 1) * p.W + (s - 1)) * PS + ci;
+    abit[i] = m < p.KK ? tap : 16;                 // rows past 9 * Cin: always 0
+  }
+  const int do_bias = blockIdx.y == 0;
+  const long long split = 2LL * blockIdx.x + wg, T = (long long)p.KK * p.Cout;
+  const int co0 = blockIdx.z * BN;
+  const int yc4 = t % (BN / 4), yp0 = t / (BN / 4);
+  float4 yv[YQ];
+  auto load = [&](int chunk) {
+#pragma unroll
+    for (int q = 0; q < YQ; ++q) {
+      const int g = chunk * WG_PX + yp0 + q * (128 / (BN / 4));
+      yv[q] = g < p.npx ? __ldg(reinterpret_cast<const float4*>(dy + (long long)g * p.Cout + co0) + yc4)
+                        : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  };
+
+  float acc[TPW][BN / 2], part[TPW][BN / 2];
+#pragma unroll
+  for (int i = 0; i < TPW; ++i)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[i][j] = 0.f;
+  float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
+  int c = c_begin + wg;
+  if (c < c_end) load(c);
+  int first = 1;
+  for (; c < c_end; c += 2) {
+#pragma unroll
+    for (int q = 0; q < YQ; ++q) {
+      put_t<X3>(sy, syl, yc4, yp0 + q * (128 / (BN / 4)), yv[q]);
+      if (do_bias) { bsum.x += yv[q].x; bsum.y += yv[q].y; bsum.z += yv[q].z; bsum.w += yv[q].w; }
+    }
+    fence_proxy_async();
+    named_bar_sync(1 + wg, 128);
+    if (c + 2 < c_end) load(c + 2);
+    // pixel 4j + lane % 4 of the chunk: k-step j / 2, fragment words 2 * (j & 1) (row m) and 2 * (j & 1) + 1 (row m + 8)
+    int kb[8];
+    uint32_t km[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int k = (c - c_begin) * WG_PX + 4 * j + (lane & 3);
+      kb[j] = k * PS;
+      km[j] = mask[k];
+    }
+#pragma unroll
+    for (int i = 0; i < TPW; ++i) {
+      if (ty0 + i >= gy) break;
+      uint32_t a[4][4], lo[4][4];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const bool ok = (km[j] >> abit[i]) & 1;
+        const float* src = box + kb[j] + aoff[i];
+        a[j >> 1][2 * (j & 1)] = ok ? __float_as_uint(src[0]) : 0u;
+        a[j >> 1][2 * (j & 1) + 1] = ok ? __float_as_uint(src[8]) : 0u;
+      }
+      if (X3) {
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+          for (int w = 0; w < 4; ++w) {
+            const float v = __uint_as_float(a[ks][w]);
+            a[ks][w] = __float_as_uint(tf32_hi(v));
+            lo[ks][w] = __float_as_uint(tf32_lo(v));
+          }
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < WG_PX / 8; ++ks) {
+        const uint64_t db = wgmma_desc(smem_u32(sy) + ks * 32, 128);
+        if (X3) {
+          wgmma_tf32_rs<BN>(part[i], a[ks], db, ks > 0);
+          wgmma_tf32_rs<BN>(part[i], a[ks], wgmma_desc(smem_u32(syl) + ks * 32, 128), 1);
+          wgmma_tf32_rs<BN>(part[i], lo[ks], db, 1);
+        } else {
+          wgmma_tf32_rs<BN>(acc[i], a[ks], db, first == 0 || ks > 0);
+        }
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (X3) {
+#pragma unroll
+      for (int i = 0; i < TPW; ++i)
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) acc[i][j] += part[i][j];
+    }
+    named_bar_sync(1 + wg, 128);
+    first = 0;
+  }
+  float* dwt = p.ws ? p.ws + split * T : p.dw;
+#pragma unroll
+  for (int i = 0; i < TPW; ++i) {
+    if (ty0 + i >= gy) break;
+#pragma unroll
+    for (int j = 0; j < BN / 2; j += 2) {
+      const int row = (ty0 + i) * WG_MT + fragment_row(j, t), co = co0 + fragment_col(j, t);
+      if (row >= p.KK) continue;
+      float2* o = reinterpret_cast<float2*>(dwt + (long long)row * p.Cout + co);
+      if (p.ws) *o = make_float2(acc[i][j], acc[i][j + 1]);
+      else atomicAdd(o, make_float2(acc[i][j], acc[i][j + 1]));
+    }
+  }
+  if (do_bias) {
+    float4* sb = reinterpret_cast<float4*>(sy);       // 128 float4 <= BN * 128 bytes; free after the loop's barrier
+    sb[t] = bsum;
+    named_bar_sync(1 + wg, 128);
+    if (t < BN / 4) {
+      float4 v = sb[t];
+      for (int k = t + BN / 4; k < 128; k += BN / 4) { v.x += sb[k].x; v.y += sb[k].y; v.z += sb[k].z; v.w += sb[k].w; }
+      if (p.ws) reinterpret_cast<float4*>(p.ws + 2LL * gridDim.x * T + split * p.Cout + co0)[t] = v;
+      else if (p.dbias) atomicAdd(reinterpret_cast<float4*>(p.dbias + co0) + t, v);
+    }
+  }
+}
+
+// The staged-box path (p.box_tiles > 0, NP = 1): an overload of the kernel below, so that each path gets the registers
+// it needs (one kernel with both would give the tiled path the box path's accumulators)
+struct WgBox {};
+template <int BN, int X3, int NP>
+__global__ void __launch_bounds__(WG_THREADS, 1)
+conv_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dy, WgTcParams p, WgBox) {
+  static_assert(NP == 1, "the box path keeps one accumulator tile per chunk");
+  pdl_grid_sync();
+  extern __shared__ uint8_t smem_raw[];
+  wgrad_box<BN, X3>(x, dy, p, smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023));
+}
+using WgTiledKernel = void (*)(const float*, const float*, WgTcParams);
+using WgBoxKernel = void (*)(const float*, const float*, WgTcParams, WgBox);
+
 template <int BN, int X3, int NP>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 conv_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dy, WgTcParams p) {
@@ -227,9 +419,13 @@ conv_wgrad_reduce_kernel(const float* __restrict__ ws, int splits, long long T, 
 // ---------------------------------------------------------------------------------------- host side
 template <int BN>
 static bool set_smem_limit() {
-  return cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, 0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess &&
-         cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, 1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess &&
-         cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, 1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) == cudaSuccess;
+  const WgTiledKernel tiled[3] = {conv_wgrad_tc_kernel<BN, 0, 1>, conv_wgrad_tc_kernel<BN, 1, 1>, conv_wgrad_tc_kernel<BN, 1, 4>};
+  const WgBoxKernel box[2] = {conv_wgrad_tc_kernel<BN, 0, 1>, conv_wgrad_tc_kernel<BN, 1, 1>};
+  for (WgTiledKernel k : tiled)
+    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) return false;
+  for (WgBoxKernel k : box)
+    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) return false;
+  return true;
 }
 
 int init_conv_wgrad_tc() {
@@ -334,6 +530,9 @@ bool wgrad_config(const se_conv_desc* d, int x3, int sms, ConvPlan* pl) {
   p.KK = (int)KK;
   p.npx = (int)npx;
   p.chunks = (int)ceil_div<long long>(npx, WG_PX);
+  // The split plan below (gx, per_cta, and the chunks of each slice) fixes the order in which dW and dbias are summed;
+  // it must not change, not even with the kernel path: adding the partial sums in another order moves ResNet-110's
+  // embeddings by about 4 % within three training steps (DESIGN §5.1).
   // about eight CTAs per SM over all row / column tiles, each with at least 4 chunks: a warpgroup's chunks are
   // latency-bound round trips (load, transpose, MMA), so the pixel range is cut finely
   long long gx = ceil_div<long long>(8LL * sms, (long long)gy * gz);
@@ -346,6 +545,20 @@ bool wgrad_config(const se_conv_desc* d, int x3, int sms, ConvPlan* pl) {
   pl->wg_bn = BN;
   pl->wg_np = x3 && npx >= WG_LONG_PX ? 4 : 1;
   pl->smem = 1024 + 2 * (size_t)(WG_MT * 128 + BN * 128) * (x3 ? 2 : 1);
+  // 3x3 / stride 1 with Cin <= 64 and one accumulator tile per chunk: X staged once per CTA (wgrad_box) when the box
+  // fits.  ResNet-50's 64-channel layers at 56 px (28 chunks per CTA: about 290 KB) keep the tiled path.
+  p.box_tiles = 0;
+  if (conv3x3_wgrad_tc_ok(d) && d->Cin <= 64 && pl->wg_np == 1) {
+    const int tiles = wg_box_tiles(BN);
+    const size_t box_px = (size_t)p.per_cta * WG_PX + 2 * (d->W + 1);
+    const size_t smem = 1024 + 2 * (size_t)BN * 128 * (x3 ? 2 : 1) + box_px * (d->Cin + WG_BOX_PAD) * 4 +
+                        (size_t)p.per_cta * WG_PX * 2;
+    if (smem <= WG_BOX_MAX_SMEM) {
+      p.box_tiles = tiles;
+      pl->grid.y = (unsigned)ceil_div(gy, tiles);
+      pl->smem = smem;
+    }
+  }
   return true;
 }
 
@@ -361,9 +574,16 @@ bool conv_wgrad_tc_fixed_order(const se_conv_desc* d, cudaStream_t st) {
 
 template <int BN>
 static void wgrad_go(const ConvPlan& pl, cudaStream_t st, const float* x, const float* dy, const WgTcParams& p) {
-  if (pl.wg_np == 4) launch(conv_wgrad_tc_kernel<BN, 1, 4>, pl.grid, dim3(WG_THREADS), pl.smem, st, x, dy, p);
-  else if (pl.x3) launch(conv_wgrad_tc_kernel<BN, 1, 1>, pl.grid, dim3(WG_THREADS), pl.smem, st, x, dy, p);
-  else launch(conv_wgrad_tc_kernel<BN, 0, 1>, pl.grid, dim3(WG_THREADS), pl.smem, st, x, dy, p);
+  if (p.box_tiles) {
+    WgBoxKernel k = conv_wgrad_tc_kernel<BN, 0, 1>;
+    if (pl.x3) k = conv_wgrad_tc_kernel<BN, 1, 1>;
+    launch(k, pl.grid, dim3(WG_THREADS), pl.smem, st, x, dy, p, WgBox());
+    return;
+  }
+  WgTiledKernel k = conv_wgrad_tc_kernel<BN, 0, 1>;
+  if (pl.wg_np == 4) k = conv_wgrad_tc_kernel<BN, 1, 4>;
+  else if (pl.x3) k = conv_wgrad_tc_kernel<BN, 1, 1>;
+  launch(k, pl.grid, dim3(WG_THREADS), pl.smem, st, x, dy, p);
 }
 
 int conv_wgrad_tc(const ConvPlan& pl, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st) {

@@ -213,6 +213,13 @@ __device__ __forceinline__ void wgmma_tf32_rs_n128(float (&d)[64], const uint32_
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc)
       : "memory");
 }
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t b, int acc) {
+  if constexpr (BN == 16) wgmma_tf32_rs_n16(d, a, b, acc);
+  else if constexpr (BN == 32) wgmma_tf32_rs_n32(d, a, b, acc);
+  else if constexpr (BN == 64) wgmma_tf32_rs_n64(d, a, b, acc);
+  else wgmma_tf32_rs_n128(d, a, b, acc);
+}
 __device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t da, uint64_t db, int acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
