@@ -11,8 +11,9 @@ import argparse, ctypes, json, os, subprocess, sys, tempfile
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-# (N, H=W, Cin, Cout): ResNet-110 stages 1-3 at batch 128, WRN-28-10 stage 1, a ResNet-50 stage-2 3x3 layer
-SHAPES = [(128, 32, 16, 16), (128, 16, 32, 32), (128, 8, 64, 64), (128, 32, 160, 160), (32, 56, 64, 64)]
+# (N, H=W, Cin, Cout): ResNet-110 stages 1-3 at batch 128, WRN-28-10 stage 1, ResNet-50's stage-2 and stage-5 3x3
+# layers at batch 32
+SHAPES = [(128, 32, 16, 16), (128, 16, 32, 32), (128, 8, 64, 64), (128, 32, 160, 160), (32, 56, 64, 64), (32, 7, 512, 512)]
 MODES = {'tf32x3': 2, 'tf32': 1}
 
 

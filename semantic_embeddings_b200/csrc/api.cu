@@ -124,6 +124,7 @@ extern "C" int se_conv2d_fwd_aux(const se_conv_desc* d, const float* x, const fl
   c.w_t = aux && aux->w_t;
   c.w_t_lo = aux && aux->w_t_lo;
   c.stats = stats != nullptr;
+  c.sms = sm_count();
   ConvPlan pl;
   const ConvFamily f = conv_plan(d, 0, mode, c, &pl);
   if (f == CONV_FP32) return conv_fwd_simt(d, x, w, bias, residual, y, relu, stats, as_stream(stream));
@@ -181,6 +182,7 @@ extern "C" int se_conv2d_dgrad_aux(const se_conv_desc* d, const float* dy, const
   ConvCall c;
   c.w_lo = aux && aux->w_lo;
   c.beta = beta;
+  c.sms = sm_count();
   ConvPlan pl;
   const ConvFamily f = conv_plan(d, 1, mode, c, &pl);
   if (f == CONV_FP32) return conv_dgrad_simt(d, dy, w, dx, beta, as_stream(stream));

@@ -76,7 +76,7 @@ struct ConvCall {
   bool stats = false;                             // forward: BatchNorm statistics requested
   float beta = 0.f;                               // backward data: dx = beta * dx + dX
   bool aligned = true;                            // weight gradient: dw and dbias 16-byte aligned
-  int sms = 0;                                    // weight gradient: SMs of the device; sizes the split-K grid only
+  int sms = 0;                                    // SMs of the device (0: unknown); sizes the grid, never a result
 };
 
 struct ConvPlan {

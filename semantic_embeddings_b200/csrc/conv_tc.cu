@@ -15,9 +15,9 @@
 //   1x1 / stride 1 layers are the same GEMM over the flat pixel list (tiles of 128 consecutive pixels), 1x1 / stride 2
 //   layers address the input (forward) or the output (backward data) through the sub-sampled view x[:, ::2, ::2, :].
 //
-// Warp-specialised (384 threads): warp 0 issues the TMA loads of a ring of stages, the two consumer warpgroups
-// (threads 128..383) each own 64 rows of the tile and issue m64nBNk8 wgmma on them; the epilogue (bias / residual /
-// ReLU / BatchNorm sums, or the accumulate of the data gradient) runs on the accumulator registers.
+// Warp-specialised (288 threads): the two consumer warpgroups (warps 0..7) each own 64 rows of the tile and issue
+// m64nBNk8 wgmma on them, two stages in flight; warp 8 issues the TMA loads of a ring of stages.  The epilogue (bias /
+// residual / ReLU / BatchNorm sums, or the accumulate of the data gradient) runs on the accumulator registers.
 //
 // Stages.  A stage is one (filter tap, channel block) pair, in that order (tap-major).  3x3 layers whose channels fit
 // ("resident box", ConvTcParams::res): TMA loads the (Wb + 2) x (Hb + 2) x Nb pixels around the tile -- every channel
@@ -43,8 +43,9 @@ namespace se {
 using namespace tc;
 
 constexpr int CT_BM = 128;
-constexpr int CT_THREADS = 384;        // warpgroup 0: TMA producer (one thread), warpgroups 1 and 2: MMA + epilogue
-constexpr int CT_MAX_STAGES = 6;
+constexpr int CT_CONSUMERS = 256;      // warpgroups 0 and 1 (warps 0..7): MMA + epilogue
+constexpr int CT_THREADS = CT_CONSUMERS + 32;   // warp 8: the TMA producer (one thread)
+constexpr int CT_MAX_STAGES = 4;       // two stages in flight per warpgroup, two loading
 constexpr int CT_SMEM_LIMIT = 227 * 1024;
 
 template <int BN>
@@ -84,8 +85,43 @@ __device__ __forceinline__ void load_a(uint32_t (&a)[4][4], const uint8_t* base,
   }
 }
 
+// CTAs per SM each instantiation is compiled for: the most whose register budget (__launch_bounds__) leaves the
+// kernel without spills and with its wgmma pipeline intact (ptxas -v; see DESIGN §5.1)
+constexpr int ct_min_blocks(int BN, int X3, int NKS) {
+  return BN == 16 ? (NKS == 2 ? 3 : 2) : BN == 32 ? (X3 && NKS == 4 ? 1 : 2) : 1;
+}
+
+// The registers of one stage in flight: its A words (hi, and lo in X3) and, in X3, its partial tile.  The two slots of
+// the consumer loop are separate objects indexed only by constants, so that each stays in registers of its own.
 template <int BN, int X3>
-__global__ void __launch_bounds__(CT_THREADS, (X3 && BN == 16) ? 2 : 1)
+struct CtSlot {
+  uint32_t a[4][4];
+  uint32_t lo[X3 ? 4 : 1][4];
+  float part[X3 ? BN / 2 : 1];
+  int stage;                                // the ring stage this slot's MMAs read
+};
+
+// An empty asm that claims to read and rewrite `v`: the compiler keeps v in its registers up to this point and reads
+// it again only after it.  At the wgmma_wait that covers a slot's MMAs this pins the A registers they read until the
+// tensor core is done with them, and keeps the partial-tile reads after the wait.
+__device__ __forceinline__ void reg_fence(uint32_t& v) { asm volatile("" : "+r"(v)); }
+__device__ __forceinline__ void reg_fence(float& v) { asm volatile("" : "+f"(v)); }
+template <typename T, int N>
+__device__ __forceinline__ void reg_fence(T (&v)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) reg_fence(v[i]);
+}
+template <typename T, int N, int M>
+__device__ __forceinline__ void reg_fence(T (&v)[N][M]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) reg_fence(v[i]);
+}
+
+// NKS = cblk / 8 k-steps per stage, known at compile time: a stage's MMAs then form one straight run, which the
+// tensor core tracks as one group (a run split by branches is closed at every branch, and wgmma_wait<1> would then
+// wait for nearly the whole stage)
+template <int BN, int X3, int NKS>
+__global__ void __launch_bounds__(CT_THREADS, ct_min_blocks(BN, X3, NKS))
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                const __grid_constant__ CUtensorMap map_bl, ConvTcParams p) {
   pdl_trigger();
@@ -104,10 +140,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   const int tm = blockIdx.x, tn = blockIdx.y;
   const int tw_i = tm % p.tw, rest = tm / p.tw;
   const int w0 = tw_i * p.Wb, h0 = (rest % p.th) * p.Hb, n0 = (rest / p.th) * p.Nb;
-  const int row_bytes = p.cblk * 4;
+  constexpr int row_bytes = NKS * 32;     // p.cblk * 4
   const int nk = p.taps * p.taps * p.kblocks;
 
-  if (tid == 0) {
+  if (tid == CT_CONSUMERS) {
     prefetch_tmap(&map_a); prefetch_tmap(&map_b);
     if (X3) prefetch_tmap(&map_bl);
     for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
@@ -117,9 +153,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   __syncthreads();
   pdl_wait();                               // nothing above touches global memory (see common.cuh)
 
-  if (tid < 128) {
-    // ===================== TMA producer
-    if (tid == 0) {
+  if (tid >= CT_CONSUMERS) {
+    // ===================== TMA producer: one thread of warp 8
+    if (tid == CT_CONSUMERS) {
       if (p.res) {
         // the resident box: every channel block of the (Wb + 2) x (Hb + 2) x Nb pixels around the tile, once
         mbar_expect_tx(abar, p.kblocks * p.a_tx);
@@ -148,8 +184,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   }
 
   // ===================== consumers: warpgroup wg owns rows 64*wg .. 64*wg+63 of the tile
-  const int wg = (tid >> 7) - 1, tid_wg = tid & 127, lane = tid & 31;
-  const int nks = p.cblk / 8;
+  const int wg = tid >> 7, tid_wg = tid & 127, lane = tid & 31;
   // the tile rows of this thread's two A rows (output pixels m and m + 8): in a per-tap stage the pixel index itself,
   // in the resident box the pixel's row for filter tap (0, 0); tap (r, s) is r * (Wb + 2) + s rows further on
   int arow[2];
@@ -162,62 +197,99 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   // X3: each stage's MMAs start a fresh register tile `part` that is then added into `acc` -- the tensor core's own
   // accumulation loses low bits with every instruction, which over the 3 x 9 x Kc / 8 MMAs of a wide layer exceeds the
   // fp32-level error budget of this mode
-  float acc[BN / 2], part[BN / 2];
+  float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   if (p.res) mbar_wait(abar, 0);
-  // stage it = (filter tap (r, s), channel block kb), counted along instead of divided out: the A addresses of a
-  // stage are on its critical path
+  // The stage loop keeps two stages in registers, in the slots s0 (even stages) and s1 (odd stages).
+  //   tf32: two stages in flight.  Stage it + 1's MMAs are issued before the wait for stage it's (wgmma_wait<1>), so the
+  //     tensor core works on one while the warpgroup releases the other and loads the next; the MMAs chain into acc in
+  //     the same order as one stage at a time.
+  //   X3: stage it + 1's A is read and split while stage it's MMAs run, and its MMAs are issued right after the wait.
+  //     Stage it's `part` is added into acc only once no MMA is in flight: ptxas serialises every wgmma of a kernel that
+  //     reads one accumulator tile while the MMAs of another are outstanding.
+  // Every MMA and every `acc += part` keeps its place in the order of a one-stage loop; only the waits move.  Stage it =
+  // (filter tap (r, s), channel block kb), counted along at load instead of divided out: the A addresses of a stage are
+  // on its critical path.
   int stage = 0, phase = 0, kb = 0, r = 0, s = 0;
-  for (int it = 0; it < nk; ++it) {
+  const int b_off = p.res ? 0 : p.a_bytes;
+  auto load = [&](CtSlot<BN, X3>& sl) {
     mbar_wait(&full[stage], phase);
     const uint8_t* sst = ring + (size_t)stage * p.stage_bytes;
     const uint8_t* abase = p.res ? smem + (size_t)kb * p.a_bytes : sst;
     const int aoff = p.res ? r * (p.Wb + 2) + s : 0;
-    const uint32_t b0 = smem_u32(p.res ? sst : sst + p.a_bytes), bl0 = b0 + p.b_bytes;
-    uint32_t a[4][4];
-    load_a(a, abase, arow[0] + aoff, arow[1] + aoff, nks, row_bytes, lane & 3);
-    if (X3) {
+    load_a(sl.a, abase, arow[0] + aoff, arow[1] + aoff, NKS, row_bytes, lane & 3);
+    if constexpr (X3 != 0) {
       // A is split here: hi = the TF32 truncation, lo = x - hi (exact in fp32).  B is fed as TMA delivered it: the
       // tensor core reads the TF32 truncation of each fp32 word (test_tf32_operands_are_truncated_by_the_tensor_core),
       // i.e. B_hi of w, and of the low parts w - trunc(w) that se_split_filters wrote
-      uint32_t lo[4][4];
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks)
+      for (int ks = 0; ks < NKS; ++ks)
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          if (ks >= nks) break;
-          const uint32_t hi = a[ks][i] & 0xFFFFE000u;
-          lo[ks][i] = __float_as_uint(__uint_as_float(a[ks][i]) - __uint_as_float(hi));
-          a[ks][i] = hi;
+          const uint32_t hi = sl.a[ks][i] & 0xFFFFE000u;
+          sl.lo[ks][i] = __float_as_uint(__uint_as_float(sl.a[ks][i]) - __uint_as_float(hi));
+          sl.a[ks][i] = hi;
         }
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        if (ks < nks) {
-          const uint64_t db = wgmma_desc(b0 + ks * 32, row_bytes);
-          wgmma_tf32_rs<BN>(part, a[ks], db, ks != 0);
-          wgmma_tf32_rs<BN>(part, a[ks], wgmma_desc(bl0 + ks * 32, row_bytes), 1);
-          wgmma_tf32_rs<BN>(part, lo[ks], db, 1);
-        }
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
-    } else {
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks)
-        if (ks < nks) wgmma_tf32_rs<BN>(acc, a[ks], wgmma_desc(b0 + ks * 32, row_bytes), (it | ks) != 0);
-      wgmma_commit();
-      wgmma_wait<0>();
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[stage]);
+    sl.stage = stage;
     if (++stage == p.stages) { stage = 0; phase ^= 1; }
     if (++kb == p.kblocks) { kb = 0; if (++s == p.taps) { s = 0; ++r; } }
+  };
+  auto mma = [&](CtSlot<BN, X3>& sl, int it) {
+    const uint32_t b0 = smem_u32(ring + (size_t)sl.stage * p.stage_bytes + b_off), bl0 = b0 + p.b_bytes;
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < NKS; ++ks) {
+      const uint64_t db = wgmma_desc(b0 + ks * 32, row_bytes);
+      if constexpr (X3 != 0) {
+        wgmma_tf32_rs<BN>(sl.part, sl.a[ks], db, ks != 0);
+        wgmma_tf32_rs<BN>(sl.part, sl.a[ks], wgmma_desc(bl0 + ks * 32, row_bytes), 1);
+        wgmma_tf32_rs<BN>(sl.part, sl.lo[ks], db, 1);
+      } else {
+        wgmma_tf32_rs<BN>(acc, sl.a[ks], db, (it | ks) != 0);
+      }
+    }
+    wgmma_commit();
+  };
+  // after the wgmma_wait that covers sl's MMAs: its registers may be reused, its partial tile added, its stage released
+  auto retire = [&](CtSlot<BN, X3>& sl) {
+    reg_fence(sl.a);
+    if constexpr (X3 != 0) {
+      reg_fence(sl.lo);
+      reg_fence(sl.part);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] += sl.part[i];
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[sl.stage]);
+  };
+  // cur holds stage it (loaded; tf32: also issued), and stage it + 1 exists: move it on into nxt
+  auto step = [&](CtSlot<BN, X3>& cur, CtSlot<BN, X3>& nxt, int it) {
+    if constexpr (X3 != 0) { mma(cur, it); load(nxt); wgmma_wait<0>(); }
+    else { load(nxt); mma(nxt, it + 1); wgmma_wait<1>(); }
+    retire(cur);
+  };
+  auto last = [&](CtSlot<BN, X3>& cur, int it) {
+    if constexpr (X3 != 0) mma(cur, it);
+    wgmma_wait<0>();
+    retire(cur);
+  };
+  CtSlot<BN, X3> s0, s1;
+  load(s0);
+  if constexpr (X3 == 0) mma(s0, 0);
+  int it = 0;
+  for (; it + 2 < nk; it += 2) {
+    step(s0, s1, it);
+    step(s1, s0, it + 1);
   }
+  if (it + 1 < nk) {
+    step(s0, s1, it);
+    last(s1, it + 1);
+  } else {
+    last(s0, it);
+  }
+  if (!X3) reg_fence(acc);
 
   // ===================== epilogue on the registers: the two rows of this thread, BN/8 column pairs each
   long long off[2];
@@ -265,7 +337,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         csq[j] += __shfl_xor_sync(0xffffffffu, csq[j], o);
       }
     }
-    float* sw = s_stats + ((tid - 128) >> 5) * 2 * BN;
+    float* sw = s_stats + (tid >> 5) * 2 * BN;
     if (lane < 4) {
 #pragma unroll
       for (int j = 0; j < BN / 4; ++j) {
@@ -274,8 +346,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         sw[BN + c] = csq[j];
       }
     }
-    named_bar_sync(2, 256);
-    for (int i = tid - 128; i < 2 * BN; i += 256) {
+    named_bar_sync(2, CT_CONSUMERS);
+    for (int i = tid; i < 2 * BN; i += CT_CONSUMERS) {
       double v = 0.0;
 #pragma unroll
       for (int w = 0; w < 8; ++w) v += (double)s_stats[w * 2 * BN + i];
@@ -348,8 +420,8 @@ static int pick_bn(int Nc, int x3) {
 }
 
 // The launch configuration of conv_tc_kernel for family f (of one tap, for the nine-tap data gradient): false when the
-// tiles, the grid or the shared memory do not fit.  flip: data gradient.
-static bool tc_config(const se_conv_desc* d, ConvFamily f, int Kc, int Nc, int flip, int x3, ConvPlan* pl) {
+// tiles, the grid or the shared memory do not fit.  flip: data gradient; sms: SMs of the device (0: unknown).
+static bool tc_config(const se_conv_desc* d, ConvFamily f, int Kc, int Nc, int flip, int x3, int sms, ConvPlan* pl) {
   ConvTcParams& p = pl->tc;
   const int taps = f == CONV_TC_3X3 ? 3 : 1;
   const bool s2 = f == CONV_TC_1X1_S2 || f == CONV_TC_DGRAD_3X3S2;
@@ -369,6 +441,9 @@ static bool tc_config(const se_conv_desc* d, ConvFamily f, int Kc, int Nc, int f
   p.tw = ceil_div(p.W, p.Wb); p.th = ceil_div(p.H, p.Hb);
   const long long tiles_m = (long long)p.tw * p.th * ceil_div(p.N, p.Nb);
   p.BN = pick_bn(Nc, x3);
+  // a grid of at most half the SMs leaves SMs idle: split the output channels once more, so that it still runs in one
+  // wave (each column of the wgmma tile is computed on its own, so the result does not change)
+  if (p.BN > 16 && sms > 0 && 2 * tiles_m * (Nc / p.BN) <= sms) p.BN >>= 1;
   if (p.BN == 0 || tiles_m > 0x7fffffffLL || Nc / p.BN > 65535) return false;
   p.cblk = Kc >= 32 ? 32 : 16;
   p.kblocks = Kc / p.cblk;
@@ -427,7 +502,7 @@ static ConvFamily conv_plan_wide(const se_conv_desc* d, int dir, int mode, const
     d1.kh = 1; d1.kw = 1;
     f = tc_family(&d1, Kc, Nc) == CONV_TC_1X1_S2 ? CONV_TC_DGRAD_3X3S2 : CONV_FP32;
   }
-  if (f == CONV_FP32 || !tc_config(d, f, Kc, Nc, dir, x3, pl)) return CONV_FP32;
+  if (f == CONV_FP32 || !tc_config(d, f, Kc, Nc, dir, x3, c.sms, pl)) return CONV_FP32;
   pl->tc.beta = f == CONV_TC_DGRAD_3X3S2 ? 1.f : c.beta;
   // wide layers (640 output channels): the per-warp statistics slots of the fused epilogue do not fit in shared memory,
   // the BatchNorm sums come from a separate pass over y
@@ -450,12 +525,18 @@ ConvFamily conv_plan(const se_conv_desc* d, int dir, int mode, const ConvCall& c
   return pl->family = CONV_TC_ODD_3X3;
 }
 
-template <int BN>
+template <int BN, int NKS>
 static void conv_tc_go(int x3, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& ma, const CUtensorMap& mb,
                        const CUtensorMap& mbl, const ConvTcParams& p) {
   if constexpr (BN <= 64)       // pick_bn: <= 64 channels per tile in the error-compensated mode
-    if (x3) return launch(conv_tc_kernel<BN, 1>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
-  launch(conv_tc_kernel<BN, 0>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
+    if (x3) return launch(conv_tc_kernel<BN, 1, NKS>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
+  launch(conv_tc_kernel<BN, 0, NKS>, grid, dim3(CT_THREADS), smem, st, ma, mb, mbl, p);
+}
+template <int BN>
+static void conv_tc_go(int x3, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& ma, const CUtensorMap& mb,
+                       const CUtensorMap& mbl, const ConvTcParams& p) {
+  if (p.cblk == 32) conv_tc_go<BN, 4>(x3, grid, smem, st, ma, mb, mbl, p);
+  else conv_tc_go<BN, 2>(x3, grid, smem, st, ma, mb, mbl, p);
 }
 
 // conv_tc_kernel with the planned configuration and the pointers of p: A = a_tensor (x, or dy for the data gradient),
@@ -488,13 +569,15 @@ static int conv_tc_launch(const ConvPlan& pl, const ConvTcParams& p, const se_co
   return check_launch("conv_tc_kernel");
 }
 
-template <int BN>
+template <int BN, int NKS>
 static bool set_smem_limit() {
   if constexpr (BN <= 64)
-    if (cudaFuncSetAttribute(conv_tc_kernel<BN, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM_LIMIT) != cudaSuccess)
+    if (cudaFuncSetAttribute(conv_tc_kernel<BN, 1, NKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM_LIMIT) != cudaSuccess)
       return false;
-  return cudaFuncSetAttribute(conv_tc_kernel<BN, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM_LIMIT) == cudaSuccess;
+  return cudaFuncSetAttribute(conv_tc_kernel<BN, 0, NKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM_LIMIT) == cudaSuccess;
 }
+template <int BN>
+static bool set_smem_limit() { return set_smem_limit<BN, 2>() && set_smem_limit<BN, 4>(); }
 
 int init_conv_tc() {
   if (!set_smem_limit<16>() || !set_smem_limit<32>() || !set_smem_limit<64>() || !set_smem_limit<128>()) {
