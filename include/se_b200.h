@@ -129,9 +129,20 @@ int se_conv2d_wgrad(const se_conv_desc* d, const float* x, const float* dy, floa
 /* Which kernel family takes this layer in `mode` (pure host-side planning: no device work, callable without a GPU):
  * 1 = a tensor-core kernel, 0 = an fp32 kernel; direction 0 forward, 1 backward data, 2 weight gradient.  (Forward: given the
  * auxiliary kernel copies of se_conv_aux; with BatchNorm statistics wider than 384 channels the sums come from a separate
- * se_bn_stats pass, see se_conv2d_fwd_aux.)  The plan sees the descriptor only, not the buffers: a weight gradient whose
- * dw or dbias is not 16-byte aligned runs on the fp32 kernels even where this returns 1. */
+ * se_bn_stats pass, see se_conv2d_fwd_aux.)  The answer of se_conv2d_plan's tensor_core. */
 int se_conv2d_path(const se_conv_desc* d, int mode, int direction);
+/* The plan of one convolution on a device with `sms` SMs, as se_conv2d_fwd_aux / se_conv2d_dgrad_aux / se_conv2d_wgrad
+ * make it (pure host-side planning, callable without a GPU; given every auxiliary kernel copy).  Like se_conv2d_path it
+ * sees the descriptor only, not the buffers: it assumes 16-byte aligned buffers and no residual, so a call with
+ * misaligned buffers (or a residual) can run another kernel than it reports. */
+typedef struct {
+  int32_t tensor_core;  /* 1: a tensor-core kernel (se_conv2d_path) */
+  int32_t workspace;    /* weight gradient: 1 = the split-K slices fit the workspace, 0 = direct mode (float atomics) */
+  int64_t splits;       /* weight gradient: split-K slices (0 in the other directions) */
+  int64_t split_px;     /* weight gradient: pixels of each CTA's range of the split, 0 where CTAs stride over image tiles */
+  char kernel[160];     /* the kernel as torch.profiler names it: its demangled signature without the return type */
+} se_conv_plan_info;
+int se_conv2d_plan(const se_conv_desc* d, int mode, int direction, int sms, se_conv_plan_info* info);
 /* Dense (models/cifar_resnet.py:233, plainnet.py:67,76, wide_residual_network.py:96, utils.py:242,
  * learn_image_embeddings.py:44): y = x W + b as a 1x1 convolution over a (B,1,1,Cin) tensor. */
 int se_dense_fwd(const float* x, const float* w, const float* bias, float* y, int B, int Cin, int Cout,

@@ -18,27 +18,17 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SHAPES = [('r110 16->16 @32', (128, 32, 32, 16, 16, 3)), ('r110 32->32 @16', (128, 16, 16, 32, 32, 3)),
           ('r110 64->64 @8', (128, 8, 8, 64, 64, 3)), ('wrn 160->160 @32', (64, 32, 32, 160, 160, 3)),
           ('r50 64->64 @56', (32, 56, 56, 64, 64, 3))]
-WG_WS_FLOATS = 8 << 20         # conv_wgrad_tc.cu: the split-K workspace
 
 
-def wgrad_plan(N, Ho, Wo, Cin, Cout, k, sms=132):
-    """wgrad_config (conv_wgrad_tc.cu) in SE_MODE_TF32X3 for a layer with an N x Ho x Wo output: the grid, the split-K
-    slices (one per warpgroup) and the workspace bytes one launch writes and conv_wgrad_reduce_kernel reads back"""
-    npx, KK = N * Ho * Wo, k * k * Cin
-    BN = 64
-    while Cout % BN:
-        BN //= 2
-    chunks = -(-npx // 32)
-    gy, gz = -(-KK // 64), Cout // BN
-    T = KK * Cout
-    fit = WG_WS_FLOATS // (T + Cout)
-    gx = -(-8 * sms // (gy * gz))
-    gx = max(1, min(gx, -(-chunks // 4)))
-    gx = max(1, (min(2 * gx, fit) if fit >= 1 else 2 * gx) // 2)
-    per = -(-chunks // gx)
-    per += per & 1
-    gx = -(-chunks // per)
-    return dict(grid=[gx, gy, gz], slices=2 * gx, workspace_bytes=2 * 2 * gx * (T + Cout) * 4)
+def wgrad_plan(N, H, W, Cin, Cout, k, sms=132):
+    """se_conv2d_plan (SE_MODE_TF32X3) of the library in the source tree: the split-K slices (one per warpgroup) and the
+    workspace bytes one launch writes and conv_wgrad_reduce_kernel reads back"""
+    import ctypes
+    sys.path.insert(0, ROOT)
+    from semantic_embeddings_b200 import _lib as L
+    info = L.ConvPlanInfo()
+    L.call('se_conv2d_plan', L.ConvDesc(N, H, W, Cin, Cout, k, k, 1, 1, 1, H, W), 2, 2, sms, ctypes.byref(info))
+    return dict(slices=info.splits, workspace_bytes=2 * info.splits * (k * k * Cin * Cout + Cout) * 4)
 
 
 REPS = 200
@@ -132,7 +122,7 @@ def main():
     rows = []
     for name, (N, H, W, C, Co, k) in SHAPES:
         p = wgrad_plan(N, H, W, C, Co, k)
-        row = {'layer': name, 'B': N, 'grid': p['grid'], 'slices': p['slices'],
+        row = {'layer': name, 'B': N, 'slices': p['slices'],
                'workspace_MB': round(p['workspace_bytes'] / 1e6, 2), 'x_dy_MB': round(4 * N * H * W * (C + Co) / 1e6, 2)}
         for i, lib in enumerate(libs):
             for kname, short in (('conv_wgrad_tc_kernel', 'tc'), ('conv_wgrad_reduce_kernel', 'reduce')):

@@ -49,6 +49,12 @@ class Residual(ctypes.Structure):
     _fields_ = [('ptr', c_void_p), ('C', c_int32), ('pad_lo', c_int32), ('pool', c_int32), ('H', c_int32), ('W', c_int32)]
 
 
+class ConvPlanInfo(ctypes.Structure):
+    """se_conv_plan_info: what se_conv2d_plan reports."""
+    _fields_ = [('tensor_core', c_int32), ('workspace', c_int32), ('splits', c_int64), ('split_px', c_int64),
+                ('kernel', ctypes.c_char * 160)]
+
+
 class ConvAux(ctypes.Structure):
     _fields_ = [('w_t', c_void_p), ('w_t_lo', c_void_p), ('w_lo', c_void_p)]
 
@@ -115,6 +121,7 @@ _SIGS = {
     'se_conv2d_dgrad': (c_int, [POINTER(ConvDesc), _P, _P, _P, c_float, c_int, _P]),
     'se_conv2d_wgrad': (c_int, [POINTER(ConvDesc), _P, _P, _P, _P, c_int, _P]),
     'se_conv2d_path': (c_int, [POINTER(ConvDesc), c_int, c_int]),
+    'se_conv2d_plan': (c_int, [POINTER(ConvDesc), c_int, c_int, c_int, POINTER(ConvPlanInfo)]),
     'se_dense_fwd': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, _P]),
     'se_dense_bwd': (c_int, [_P, _P, _P, _P, c_float, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'se_bn_stats': (c_int, [_P, c_int64, c_int, _P, _P]),

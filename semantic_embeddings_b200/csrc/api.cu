@@ -39,11 +39,6 @@ int sm_count() {
   return g_sms;
 }
 
-// conv_simt.cu
-int conv_fwd_simt(const se_conv_desc*, const float*, const float*, const float*, const float*, float*, int, double*, cudaStream_t);
-int conv_dgrad_simt(const se_conv_desc*, const float*, const float*, float*, float, cudaStream_t);
-int conv_wgrad_simt(const se_conv_desc*, const float*, const float*, float*, float*, cudaStream_t);
-
 static int check_desc(const se_conv_desc* d) {
   if (!d) { set_error("null conv descriptor"); return SE_ERR_ARG; }
   if (d->N <= 0 || d->H <= 0 || d->W <= 0 || d->Cin <= 0 || d->Cout <= 0 || d->kh <= 0 || d->kw <= 0 ||
@@ -114,22 +109,34 @@ extern "C" int se_init(void) { return ensure_setup(); }
 namespace se { int tc_capabilities(); }
 extern "C" int se_tc_capabilities(void) { return se::tc_capabilities(); }
 
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 extern "C" int se_conv2d_fwd_aux(const se_conv_desc* d, const float* x, const float* w, const se_conv_aux* aux,
                                  const float* bias, const float* residual, float* y, int relu, double* stats, int mode,
                                  void* stream) {
   int rc = check_desc(d);
   if (rc) return rc;
   SE_REQUIRE(x && w && y, "null pointer");
+  if ((rc = ensure_setup())) return rc;
   ConvCall c;
   c.w_t = aux && aux->w_t;
   c.w_t_lo = aux && aux->w_t_lo;
   c.stats = stats != nullptr;
+  c.x_aligned = aligned16(x);
+  c.y_aligned = aligned16(y);
+  c.residual = residual != nullptr;
   c.sms = sm_count();
   ConvPlan pl;
-  const ConvFamily f = conv_plan(d, 0, mode, c, &pl);
-  if (f == CONV_FP32) return conv_fwd_simt(d, x, w, bias, residual, y, relu, stats, as_stream(stream));
-  rc = f == CONV_TC_ODD_3X3 ? conv_fwd_odd_tc(pl, x, aux->w_t, aux->w_t_lo, bias, residual, y, relu, as_stream(stream))
-                            : conv_fwd_tc(pl, d, x, aux->w_t, aux->w_t_lo, bias, residual, y, relu, pl.fused_stats ? stats : nullptr, as_stream(stream));
+  conv_plan(d, 0, mode, c, &pl);
+  const cudaStream_t st = as_stream(stream);
+  double* const fused = pl.fused_stats ? stats : nullptr;
+  switch (pl.family) {
+    case CONV_TC_3X3: case CONV_TC_1X1: case CONV_TC_1X1_S2:
+      rc = conv_fwd_tc(pl, d, x, aux->w_t, aux->w_t_lo, bias, residual, y, relu, fused, st);
+      break;
+    case CONV_TC_ODD_3X3: rc = conv_fwd_odd_tc(pl, x, aux->w_t, aux->w_t_lo, bias, residual, y, relu, st); break;
+    default: rc = conv_fwd_simt(pl, d, x, w, bias, residual, y, relu, fused, st); break;
+  }
   if (rc || !stats || pl.fused_stats) return rc;
   return se_bn_stats(y, (int64_t)d->N * d->Ho * d->Wo, d->Cout, stats, stream);
 }
@@ -179,27 +186,84 @@ extern "C" int se_conv2d_dgrad_aux(const se_conv_desc* d, const float* dy, const
   int rc = check_desc(d);
   if (rc) return rc;
   SE_REQUIRE(dy && w && dx, "null pointer");
+  if ((rc = ensure_setup())) return rc;
   ConvCall c;
   c.w_lo = aux && aux->w_lo;
   c.beta = beta;
   c.sms = sm_count();
   ConvPlan pl;
-  const ConvFamily f = conv_plan(d, 1, mode, c, &pl);
-  if (f == CONV_FP32) return conv_dgrad_simt(d, dy, w, dx, beta, as_stream(stream));
-  if (f == CONV_TC_ODD_3X3) return conv_dgrad_odd_tc(pl, dy, w, c.w_lo ? aux->w_lo : nullptr, dx, beta, as_stream(stream));
-  return conv_dgrad_tc(pl, d, dy, w, c.w_lo ? aux->w_lo : nullptr, dx, beta, as_stream(stream));
+  const cudaStream_t st = as_stream(stream);
+  switch (conv_plan(d, 1, mode, c, &pl)) {
+    case CONV_TC_3X3: case CONV_TC_1X1: case CONV_TC_1X1_S2: case CONV_TC_DGRAD_3X3S2:
+      return conv_dgrad_tc(pl, d, dy, w, c.w_lo ? aux->w_lo : nullptr, dx, beta, st);
+    case CONV_TC_ODD_3X3: return conv_dgrad_odd_tc(pl, dy, w, c.w_lo ? aux->w_lo : nullptr, dx, beta, st);
+    default: return conv_dgrad_simt(pl, d, dy, w, dx, beta, st);
+  }
 }
 extern "C" int se_conv2d_dgrad(const se_conv_desc* d, const float* dy, const float* w, float* dx, float beta, int mode,
                                void* stream) {
   return se_conv2d_dgrad_aux(d, dy, w, nullptr, dx, beta, mode, stream);
 }
 
-extern "C" int se_conv2d_path(const se_conv_desc* d, int mode, int direction) {
+// The kernel a plan launches, as torch.profiler names it: its demangled signature without the return type
+static void kernel_name(const ConvPlan& pl, int dir, char* out, size_t n) {
+  const SimtParams& f = pl.fp;
+  const char* tile = f.bn == 16 ? "128, 16, 4, 2" : f.bn == 32 ? "128, 32, 4, 4" : "64, 64, 4, 4";
+  const char* simt_w = "(se::ConvP, float const*, float const*, float*, float*, int, int, int, int)";
+  switch (pl.family) {
+    case CONV_FP32_TILES:
+      snprintf(out, n, dir ? "se::conv_dgrad_kernel<%s, %s>(se::ConvP, float const*, float const*, float*, float, int)"
+                           : "se::conv_fwd_kernel<%s, %s>(se::ConvP, float const*, float const*, float const*, float const*, "
+                             "float*, int, double*)", tile, f.vec ? "true" : "false");
+      break;
+    case CONV_FP32_DENSE_SMALL:
+      snprintf(out, n, "se::dense_small_fwd_kernel(float const*, float const*, float const*, float*, int, int, int, int)");
+      break;
+    case CONV_FP32_FWD_STEM:
+      snprintf(out, n, "se::conv_fwd_stem_kernel(se::ConvP, float const*, float const*, float const*, float*, int, double*, int)");
+      break;
+    case CONV_FP32_WGRAD:
+      snprintf(out, n, "se::conv_wgrad_kernel<64, 64, 4, 4>(se::ConvP, float const*, float const*, float*, float*, long long, int)");
+      break;
+    case CONV_FP32_WGRAD_STEM: snprintf(out, n, "se::conv_wgrad_stem_kernel%s", simt_w); break;
+    case CONV_FP32_WGRAD_3X3: snprintf(out, n, "se::conv_wgrad3x3_kernel<%d, %d>%s", f.nci, f.nco, simt_w); break;
+    case CONV_TC_WGRAD:
+      snprintf(out, n, "se::conv_wgrad_tc_kernel<%d, %d, %d>(float const*, float const*, se::WgTcParams%s)", pl.wg_bn, pl.x3,
+               pl.wg_np, pl.wg.box_tiles ? ", se::WgBox" : "");
+      break;
+    case CONV_TC_ODD_3X3:
+      snprintf(out, n, dir == 2 ? "se::conv_odd_wgrad_tc_kernel<%d, %d>(float const*, float const*, se::OddWgParams)"
+                                : "se::conv_odd_tc_kernel<%d, %d>(float const*, float const*, float const*, se::OddTcParams)",
+               pl.od_bn, pl.x3);
+      break;
+    default:
+      snprintf(out, n, "se::conv_tc_kernel<%d, %d, %d>(CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, se::ConvTcParams)",
+               pl.tc.BN, pl.x3, pl.tc.cblk / 8);
+  }
+}
+
+extern "C" int se_conv2d_plan(const se_conv_desc* d, int mode, int direction, int sms, se_conv_plan_info* info) {
   int rc = check_desc(d);
   if (rc) return rc;
   SE_REQUIRE(direction >= 0 && direction <= 2, "direction: 0 forward, 1 backward data, 2 weight gradient");
+  SE_REQUIRE(info && sms >= 0, "bad arguments");
+  ConvCall c;
+  c.sms = sms;
   ConvPlan pl;
-  return conv_plan(d, direction, mode, ConvCall(), &pl) == CONV_FP32 ? 0 : 1;
+  conv_plan(d, direction, mode, c, &pl);
+  const long long T = (long long)d->kh * d->kw * d->Cin * d->Cout;
+  info->tensor_core = conv_is_tc(pl.family);
+  info->splits = pl.splits;
+  info->workspace = direction == 2 && pl.splits * (T + d->Cout) <= WG_WS_FLOATS;
+  info->split_px = pl.split_px;
+  kernel_name(pl, direction, info->kernel, sizeof(info->kernel));
+  return SE_OK;
+}
+
+extern "C" int se_conv2d_path(const se_conv_desc* d, int mode, int direction) {
+  se_conv_plan_info info;
+  const int rc = se_conv2d_plan(d, mode, direction, 0, &info);
+  return rc ? rc : info.tensor_core;
 }
 
 extern "C" int se_conv2d_wgrad(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias, int mode,
@@ -207,15 +271,26 @@ extern "C" int se_conv2d_wgrad(const se_conv_desc* d, const float* x, const floa
   int rc = check_desc(d);
   if (rc) return rc;
   SE_REQUIRE(x && dy && dw, "null pointer");
-  // the kernel stores dW / dbias as float2 / float4
+  if ((rc = ensure_setup())) return rc;
   ConvCall c;
-  c.aligned = (reinterpret_cast<uintptr_t>(dw) & 15) == 0 && (reinterpret_cast<uintptr_t>(dbias) & 15) == 0;
+  c.aligned = aligned16(dw) && aligned16(dbias);    // the tensor-core kernels store dW / dbias as float2 / float4
+  c.dy_aligned = aligned16(dy);
   c.sms = sm_count();
   ConvPlan pl;
-  const ConvFamily f = conv_plan(d, 2, mode, c, &pl);
-  if (f == CONV_FP32) return conv_wgrad_simt(d, x, dy, dw, dbias, as_stream(stream));
-  if (f == CONV_TC_ODD_3X3) return conv_wgrad_odd_tc(pl, x, dy, dw, dbias, as_stream(stream));
-  return conv_wgrad_tc(pl, x, dy, dw, dbias, as_stream(stream));
+  conv_plan(d, 2, mode, c, &pl);
+  // Split-K: the kernel writes its partial sums into pl.splits slices of the workspace, and wgrad_reduce adds them into
+  // dW / dbias in slice order; when they do not fit, the kernel adds them itself with atomics (direct mode)
+  const cudaStream_t st = as_stream(stream);
+  const long long T = (long long)d->kh * d->kw * d->Cin * d->Cout;
+  float* ws = nullptr;
+  if ((rc = wgrad_workspace(pl.splits * (T + d->Cout), st, &ws))) return rc;
+  const WgOut o = ws ? WgOut{ws, ws, dbias ? ws + pl.splits * T : nullptr} : WgOut{nullptr, dw, dbias};
+  switch (pl.family) {
+    case CONV_TC_WGRAD: rc = conv_wgrad_tc(pl, x, dy, o, st); break;
+    case CONV_TC_ODD_3X3: rc = conv_wgrad_odd_tc(pl, x, dy, o, st); break;
+    default: rc = conv_wgrad_simt(pl, d, x, dy, o, st); break;
+  }
+  return (rc || !ws) ? rc : wgrad_reduce(ws, (int)pl.splits, T, d->Cout, dw, dbias, st);
 }
 
 static se_conv_desc dense_desc(int B, int Cin, int Cout) {

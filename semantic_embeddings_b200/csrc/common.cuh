@@ -26,6 +26,7 @@ int ensure_setup();
 // [splits][Cout].  wgrad_workspace sets *ws = nullptr when `floats` do not fit (or the stream first appears inside a graph
 // capture): the kernels then add their partial sums into dW / dbias with atomics ("direct mode").
 int wgrad_workspace(long long floats, cudaStream_t st, float** ws);
+constexpr long long WG_WS_FLOATS = 8LL << 20;                         // 32 MB per workspace
 long long wgrad_fit_splits(long long want, long long T, int Cout);   // split count whose slices fit (want if none fit)
 int wgrad_reduce(const float* ws, int splits, long long T, int Cout, float* dw, float* dbias, cudaStream_t st);
 

@@ -359,6 +359,8 @@ bool odd_config(const se_conv_desc* d, int dir, int sms, ConvPlan* pl) {
   p.per_split = (int)(ceil_div<long long>(ceil_div<long long>(npx, splits), OD_BK) * OD_BK);
   splits = ceil_div<long long>(npx, p.per_split);
   pl->grid = dim3((unsigned)ceil_div<long long>(KK, OD_BM), (unsigned)ceil_div(d->Cout, pl->od_bn), (unsigned)splits);
+  pl->splits = splits;
+  pl->split_px = p.per_split;
   return true;
 }
 
@@ -388,14 +390,9 @@ int conv_dgrad_odd_tc(const ConvPlan& pl, const float* dy, const float* w, const
   return odd_launch(pl, p, dy, w, pl.x3 ? w_lo : w, st);
 }
 
-int conv_wgrad_odd_tc(const ConvPlan& pl, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st) {
-  int rc = ensure_setup();
-  if (rc) return rc;
+int conv_wgrad_odd_tc(const ConvPlan& pl, const float* x, const float* dy, const WgOut& o, cudaStream_t st) {
   OddWgParams p = pl.owg;
-  p.dw = dw; p.dbias = dbias;
-  const long long T = 9LL * p.Cin * p.Cout, splits = pl.grid.z;
-  rc = wgrad_workspace(splits * (T + p.Cout), st, &p.ws);
-  if (rc) return rc;
+  p.ws = o.ws; p.dw = o.dw; p.dbias = o.dbias;
   if (pl.od_bn == 64) {
     if (pl.x3) launch(conv_odd_wgrad_tc_kernel<64, 1>, pl.grid, dim3(OD_THREADS), 0, st, x, dy, p);
     else launch(conv_odd_wgrad_tc_kernel<64, 0>, pl.grid, dim3(OD_THREADS), 0, st, x, dy, p);
@@ -403,9 +400,7 @@ int conv_wgrad_odd_tc(const ConvPlan& pl, const float* x, const float* dy, float
     if (pl.x3) launch(conv_odd_wgrad_tc_kernel<32, 1>, pl.grid, dim3(OD_THREADS), 0, st, x, dy, p);
     else launch(conv_odd_wgrad_tc_kernel<32, 0>, pl.grid, dim3(OD_THREADS), 0, st, x, dy, p);
   }
-  rc = check_launch("conv_odd_wgrad_tc_kernel");
-  if (rc || !p.ws) return rc;
-  return wgrad_reduce(p.ws, (int)splits, T, p.Cout, dw, dbias, st);
+  return check_launch("conv_odd_wgrad_tc_kernel");
 }
 
 }  // namespace se

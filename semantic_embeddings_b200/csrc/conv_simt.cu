@@ -12,6 +12,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "conv_plan.cuh"
 
 namespace se {
 
@@ -558,19 +559,6 @@ int init_conv_simt() {
   return SE_OK;
 }
 
-template <int BM, int BN, int TM, int TN>
-static int launch_fwd(const ConvP& p, const float* x, const float* w, const float* bias, const float* residual,
-                      float* y, int relu, double* stats, cudaStream_t st) {
-  long long M = (long long)p.N * p.Ho * p.Wo;
-  dim3 grid((unsigned)ceil_div<long long>(M, BM), (unsigned)ceil_div(p.Cout, BN));
-  bool vec = (p.Cin % 4 == 0) && (p.Cout % 4 == 0);
-  if (vec)
-    launch(conv_fwd_kernel<BM, BN, TM, TN, true>, dim3(grid), dim3((BM / TM) * (BN / TN)), 0, st, p, x, w, bias, residual, y, relu, stats);
-  else
-    launch(conv_fwd_kernel<BM, BN, TM, TN, false>, dim3(grid), dim3((BM / TM) * (BN / TN)), 0, st, p, x, w, bias, residual, y, relu, stats);
-  return check_launch("conv_fwd_kernel");
-}
-
 // Forward of the RGB stem (3x3 / stride 1 / 'same', Cin <= 4, Cout == 16; models/cifar_resnet.py:218 `conv0`): one thread
 // per output pixel keeps all 16 output channels in registers; the 8-row input tile (with its zero halo), the filter
 // and the bias sit in shared memory.  The tiled-GEMM kernel above spends a 16-deep K step on K = 27 and measured
@@ -645,17 +633,6 @@ conv_fwd_stem_kernel(ConvP p, const float* __restrict__ x, const float* __restri
   }
 }
 
-static int launch_fwd_stem(const ConvP& p, const float* x, const float* w, const float* bias, float* y, int relu, double* stats,
-                           cudaStream_t st) {
-  if (p.Cin > 4 || p.Cout != 16 || (p.W % 32) != 0 || p.W > 64) return SE_ERR_UNSUPPORTED;
-  if ((reinterpret_cast<uintptr_t>(y) & 15) != 0) return SE_ERR_UNSUPPORTED;
-  const int TH = (p.H % 8 == 0) ? 8 : ((p.H % 4 == 0) ? 4 : 1);
-  const size_t smem = ((size_t)9 * p.Cin * 16 + 16 + (((TH + 2) * (p.W + 2) * p.Cin + 3) & ~3) + 8 * 32) * sizeof(float);
-  if (smem > 48 * 1024) return SE_ERR_UNSUPPORTED;
-  launch(conv_fwd_stem_kernel, dim3(p.N * (p.H / TH)), dim3(256), smem, st, p, x, w, bias, y, relu, stats, TH);
-  return check_launch("conv_fwd_stem_kernel");
-}
-
 // Dense layer on a skinny batch (the 2048 -> 555 'embedding' layer of config 4 at 32 rows: utils.py:242): the generic
 // tile kernel has 9 CTAs walking K = 2048 serially (0.42 ms).  Here a CTA owns 8 output columns and splits K over 32
 // thread groups (each thread 4 consecutive k per step: one 16-byte load of x per row, four of w), 32 rows of fp32
@@ -702,71 +679,6 @@ dense_small_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w,
       }
     }
   }
-}
-
-int conv_fwd_simt(const se_conv_desc* d, const float* x, const float* w, const float* bias, const float* residual,
-                  float* y, int relu, double* stats, cudaStream_t st) {
-  ConvP p = to_p(d);
-  if (p.kh == 1 && p.kw == 1 && p.H == 1 && p.W == 1 && p.Ho == 1 && p.Wo == 1 && p.N <= 64 && p.Cin >= 512 && p.Cin % 4 == 0 &&
-      !residual && !stats && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
-    launch(dense_small_fwd_kernel, dim3(ceil_div(p.Cout, DS_COLS)), dim3(DS_COLS * DS_KL), 0, st, x, w, bias, y, p.N, p.Cin,
-           p.Cout, relu);
-    return check_launch("dense_small_fwd_kernel");
-  }
-  if (p.kh == 3 && p.kw == 3 && p.stride == 1 && p.pad_t == 1 && p.pad_l == 1 && p.Ho == p.H && p.Wo == p.W && p.Cin <= 4 &&
-      !residual) {
-    int rc = launch_fwd_stem(p, x, w, bias, y, relu, stats, st);
-    if (rc != SE_ERR_UNSUPPORTED) return rc;
-  }
-  if (p.Cout <= 16) return launch_fwd<128, 16, 4, 2>(p, x, w, bias, residual, y, relu, stats, st);
-  if (p.Cout <= 32) return launch_fwd<128, 32, 4, 4>(p, x, w, bias, residual, y, relu, stats, st);
-  return launch_fwd<64, 64, 4, 4>(p, x, w, bias, residual, y, relu, stats, st);
-}
-
-template <int BM, int BN, int TM, int TN>
-static int launch_dgrad(const ConvP& p, const float* dy, const float* w, float* dx, float beta, cudaStream_t st) {
-  long long M = (long long)p.N * p.H * p.W;
-  dim3 grid((unsigned)ceil_div<long long>(M, BM), (unsigned)ceil_div(p.Cin, BN));
-  bool vec = (p.Cout % 4 == 0);
-  const int par = (p.stride == 2 && p.H % 2 == 0 && p.W % 2 == 0 && (((long long)p.N * (p.H / 2) * (p.W / 2)) % BM) == 0) ? 1 : 0;
-  if (vec)
-    launch(conv_dgrad_kernel<BM, BN, TM, TN, true>, dim3(grid), dim3((BM / TM) * (BN / TN)), 0, st, p, dy, w, dx, beta, par);
-  else
-    launch(conv_dgrad_kernel<BM, BN, TM, TN, false>, dim3(grid), dim3((BM / TM) * (BN / TN)), 0, st, p, dy, w, dx, beta, par);
-  return check_launch("conv_dgrad_kernel");
-}
-
-int conv_dgrad_simt(const se_conv_desc* d, const float* dy, const float* w, float* dx, float beta, cudaStream_t st) {
-  ConvP p = to_p(d);
-  if (p.Cin <= 16) return launch_dgrad<128, 16, 4, 2>(p, dy, w, dx, beta, st);
-  if (p.Cin <= 32) return launch_dgrad<128, 32, 4, 4>(p, dy, w, dx, beta, st);
-  return launch_dgrad<64, 64, 4, 4>(p, dy, w, dx, beta, st);
-}
-
-template <int NCI, int NCO>
-static int launch_wgrad3x3(const ConvP& p, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st) {
-  constexpr int CIT = 2 * NCI, COT = 2 * NCO, RG = 256 / (NCI * NCO);
-  int TH = max(1, 128 / p.W);
-  if (TH > p.H) TH = p.H;
-  size_t tile_bytes = ((size_t)(TH + 2) * (p.W + 2) * CIT + (size_t)TH * p.W * COT) * sizeof(float);
-  size_t red_bytes = RG > 1 ? ((size_t)RG * 36 * NCI * NCO + (size_t)RG * 2 * NCO) * sizeof(float) : 0;
-  size_t smem = max(tile_bytes, red_bytes);
-  int tiles_per_img = ceil_div(p.H, TH);
-  int num_tiles = p.N * tiles_per_img;
-  int cy = p.Cin / CIT, cz = p.Cout / COT;
-  const long long T = 9LL * p.Cin * p.Cout;
-  int gx = (int)wgrad_fit_splits(min(num_tiles, max(1, (2 * sm_count()) / (cy * cz))), T, p.Cout);
-  auto kern = conv_wgrad3x3_kernel<NCI, NCO>;
-  if (smem > WGRAD3X3_MAX_SMEM) return SE_ERR_UNSUPPORTED;
-  int rc = ensure_setup();
-  if (rc) return rc;
-  float* ws = nullptr;
-  rc = wgrad_workspace(gx * (T + p.Cout), st, &ws);
-  if (rc) return rc;
-  launch(kern, dim3(gx, cy, cz), dim3(256), smem, st, p, x, dy, ws ? ws : dw, ws ? (dbias ? ws + gx * T : nullptr) : dbias, TH,
-         tiles_per_img, num_tiles, ws ? 0 : 1);
-  rc = check_launch("conv_wgrad3x3_kernel");
-  return (rc || !ws) ? rc : wgrad_reduce(ws, gx, T, p.Cout, dw, dbias, st);
 }
 
 // Weight gradient of a 3x3 / stride 1 / 'same' convolution with very few input channels (the RGB stem,
@@ -833,70 +745,166 @@ conv_wgrad_stem_kernel(ConvP p, const float* __restrict__ x, const float* __rest
   }
 }
 
-static int launch_wgrad_stem(const ConvP& p, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st) {
-  if (p.Cin > 4 || (p.Cout & 3) != 0 || p.Cout > 64 || (p.W & (p.W - 1)) != 0 || p.W > 64) return SE_ERR_UNSUPPORTED;
-  if ((reinterpret_cast<uintptr_t>(dy) & 15) != 0) return SE_ERR_UNSUPPORTED;
-  const int TH = (p.H % 8 == 0) ? 8 : ((p.H % 4 == 0) ? 4 : 1);
-  const int per_pg = (9 * p.Cin + 1) * (p.Cout >> 2);
-  if (per_pg > 512) return SE_ERR_UNSUPPORTED;
-  int PG = 1;
-  while (2 * PG * per_pg <= 512 && (TH * p.W) % (2 * PG) == 0) PG *= 2;
-  const int threads = ceil_div(PG * per_pg, 32) * 32;
-  const size_t smem = ((size_t)(((TH + 2) * (p.W + 2) * p.Cin + 3) & ~3) + (size_t)TH * p.W * p.Cout +
-                       (size_t)max(PG - 1, 1) * per_pg * 4) * sizeof(float);
-  if (smem > 48 * 1024) return SE_ERR_UNSUPPORTED;
-  const int num_tiles = p.N * (p.H / TH);
-  const long long T = 9LL * p.Cin * p.Cout;
-  const int grid = (int)wgrad_fit_splits(min(num_tiles, 2 * sm_count()), T, p.Cout);
-  float* ws = nullptr;
-  int rc = wgrad_workspace(grid * (T + p.Cout), st, &ws);
-  if (rc) return rc;
-  launch(conv_wgrad_stem_kernel, dim3(grid), dim3(threads), smem, st, p, x, dy, ws ? ws : dw, ws ? (dbias ? ws + grid * T : nullptr) : dbias,
-         TH, PG, num_tiles, ws ? 0 : 1);
-  rc = check_launch("conv_wgrad_stem_kernel");
-  return (rc || !ws) ? rc : wgrad_reduce(ws, grid, T, p.Cout, dw, dbias, st);
-}
-
+// ---------------------------------------------------------------------------------------- host side
 constexpr long long WGRAD_LONG_PX = 1LL << 18, WGRAD_SPLIT_PX = 2048;   // see the split count below
 
-int conv_wgrad_simt(const se_conv_desc* d, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st) {
-  ConvP p = to_p(d);
-  if (p.kh == 3 && p.kw == 3 && p.stride == 1 && p.pad_t == 1 && p.pad_l == 1 && p.Ho == p.H && p.Wo == p.W && p.Cin <= 4) {
-    int rc = launch_wgrad_stem(p, x, dy, dw, dbias, st);
-    if (rc != SE_ERR_UNSUPPORTED) return rc;
+static int stem_rows(int H) { return (H % 8 == 0) ? 8 : ((H % 4 == 0) ? 4 : 1); }
+
+// The fp32 kernel of a call that no tensor-core family takes, and its launch configuration (conv_plan)
+void simt_config(const se_conv_desc* d, int dir, const ConvCall& c, ConvPlan* pl) {
+  SimtParams& f = pl->fp;
+  const bool same3x3 = d->kh == 3 && d->kw == 3 && d->stride == 1 && d->pad_t == 1 && d->pad_l == 1 && d->Ho == d->H &&
+                       d->Wo == d->W;
+  pl->block = dim3(256);
+  if (dir == 0) {
+    pl->fused_stats = c.stats;                      // every fp32 forward kernel sums them in its epilogue
+    if (d->kh == 1 && d->kw == 1 && d->H == 1 && d->W == 1 && d->Ho == 1 && d->Wo == 1 && d->N <= 64 && d->Cin >= 512 &&
+        d->Cin % 4 == 0 && !c.residual && !c.stats && c.x_aligned) {
+      pl->grid = dim3(ceil_div(d->Cout, DS_COLS));
+      pl->block = dim3(DS_COLS * DS_KL);
+      pl->family = CONV_FP32_DENSE_SMALL;
+      return;
+    }
+    if (same3x3 && d->Cin <= 4 && !c.residual && d->Cout == 16 && d->W % 32 == 0 && d->W <= 64 && c.y_aligned) {
+      f.TH = stem_rows(d->H);
+      const size_t smem = ((size_t)9 * d->Cin * 16 + 16 + (((f.TH + 2) * (d->W + 2) * d->Cin + 3) & ~3) + 8 * 32) * sizeof(float);
+      if (smem <= 48 * 1024) {
+        pl->grid = dim3(d->N * (d->H / f.TH));
+        pl->smem = smem;
+        pl->family = CONV_FP32_FWD_STEM;
+        return;
+      }
+    }
   }
-  const bool same3x3 = p.kh == 3 && p.kw == 3 && p.stride == 1 && p.pad_t == 1 && p.pad_l == 1 && p.Ho == p.H &&
-                       p.Wo == p.W && (p.Cin % 16 == 0) && (p.Cout % 16 == 0);
-  if (same3x3) {
-    int rc;
-    if (p.Cin % 32 == 0 && p.Cout % 32 == 0) rc = launch_wgrad3x3<16, 16>(p, x, dy, dw, dbias, st);
-    else if (p.Cout % 32 == 0) rc = launch_wgrad3x3<8, 16>(p, x, dy, dw, dbias, st);
-    else if (p.Cin % 32 == 0) rc = launch_wgrad3x3<16, 8>(p, x, dy, dw, dbias, st);
-    else rc = launch_wgrad3x3<8, 8>(p, x, dy, dw, dbias, st);
-    if (rc != SE_ERR_UNSUPPORTED) return rc;
+  if (dir < 2) {
+    // conv_fwd_kernel / conv_dgrad_kernel: the tile by the GEMM's N channels (forward Cout, data gradient Cin)
+    const int Nc = dir == 0 ? d->Cout : d->Cin;
+    f.bn = Nc <= 16 ? 16 : Nc <= 32 ? 32 : 64;
+    const int BM = f.bn == 64 ? 64 : 128;
+    const long long M = dir == 0 ? (long long)d->N * d->Ho * d->Wo : (long long)d->N * d->H * d->W;
+    f.vec = dir == 0 ? d->Cin % 4 == 0 && d->Cout % 4 == 0 : d->Cout % 4 == 0;
+    f.par = dir == 1 && d->stride == 2 && d->H % 2 == 0 && d->W % 2 == 0 &&
+            ((long long)d->N * (d->H / 2) * (d->W / 2)) % BM == 0;
+    pl->grid = dim3((unsigned)ceil_div<long long>(M, BM), (unsigned)ceil_div(Nc, f.bn));
+    pl->family = CONV_FP32_TILES;
+    return;
   }
-  constexpr int BM = 64, BN = 64, TM = 4, TN = 4;
-  const int KK = p.kh * p.kw * p.Cin;
-  long long P = (long long)p.N * p.Ho * p.Wo;
-  int gx = ceil_div(KK, BM), gy = ceil_div(p.Cout, BN);
+  const long long T = (long long)d->kh * d->kw * d->Cin * d->Cout;
+  if (same3x3 && d->Cin <= 4 && (d->Cout & 3) == 0 && d->Cout <= 64 && (d->W & (d->W - 1)) == 0 && d->W <= 64 &&
+      c.dy_aligned) {
+    f.TH = stem_rows(d->H);
+    const int per_pg = (9 * d->Cin + 1) * (d->Cout >> 2);
+    f.PG = 1;
+    while (2 * f.PG * per_pg <= 512 && (f.TH * d->W) % (2 * f.PG) == 0) f.PG *= 2;
+    const size_t smem = ((size_t)(((f.TH + 2) * (d->W + 2) * d->Cin + 3) & ~3) + (size_t)f.TH * d->W * d->Cout +
+                         (size_t)max(f.PG - 1, 1) * per_pg * 4) * sizeof(float);
+    if (per_pg <= 512 && smem <= 48 * 1024) {
+      f.num_tiles = d->N * (d->H / f.TH);
+      pl->splits = wgrad_fit_splits(min(f.num_tiles, 2 * c.sms), T, d->Cout);   // one slice per CTA
+      pl->grid = dim3((unsigned)pl->splits);
+      pl->block = dim3(ceil_div(f.PG * per_pg, 32) * 32);
+      pl->smem = smem;
+      pl->family = CONV_FP32_WGRAD_STEM;
+      return;
+    }
+  }
+  if (same3x3 && d->Cin % 16 == 0 && d->Cout % 16 == 0) {
+    f.nci = d->Cin % 32 == 0 ? 16 : 8;
+    f.nco = d->Cout % 32 == 0 ? 16 : 8;
+    const int CIT = 2 * f.nci, COT = 2 * f.nco, RG = 256 / (f.nci * f.nco);
+    f.TH = min(max(1, 128 / d->W), d->H);
+    const size_t tile_bytes = ((size_t)(f.TH + 2) * (d->W + 2) * CIT + (size_t)f.TH * d->W * COT) * sizeof(float);
+    const size_t red_bytes = RG > 1 ? ((size_t)RG * 36 * f.nci * f.nco + (size_t)RG * 2 * f.nco) * sizeof(float) : 0;
+    const size_t smem = max(tile_bytes, red_bytes);
+    if (smem <= WGRAD3X3_MAX_SMEM) {
+      f.tiles_per_img = ceil_div(d->H, f.TH);
+      f.num_tiles = d->N * f.tiles_per_img;
+      const int cy = d->Cin / CIT, cz = d->Cout / COT;
+      pl->splits = wgrad_fit_splits(min(f.num_tiles, max(1, (2 * c.sms) / (cy * cz))), T, d->Cout);   // one per CTA column
+      pl->grid = dim3((unsigned)pl->splits, cy, cz);
+      pl->smem = smem;
+      pl->family = CONV_FP32_WGRAD_3X3;
+      return;
+    }
+  }
+  // conv_wgrad_kernel<64, 64, 4, 4>
+  const int KK = d->kh * d->kw * d->Cin;
+  const long long P = (long long)d->N * d->Ho * d->Wo;
+  const int gx = ceil_div(KK, 64), gy = ceil_div(d->Cout, 64);
   // split the pixel reduction so that the grid fills the machine about twice
-  long long want = max(1LL, (long long)(2 * sm_count()) / ((long long)gx * gy));
+  long long want = max(1LL, (long long)(2 * c.sms) / ((long long)gx * gy));
   long long splits = min(want, ceil_div<long long>(P, 4 * BK));
   // and on long reductions each split sums at most WGRAD_SPLIT_PX pixels in fp32 when the workspace holds the slices:
   // ResNet-50's stem at 448 px sums 1.6 M pixels (B = 32), which 88 splits of 18 000 took to 2.6e-6 of the largest dW
   // (8e-7 in splits of 2048)
   if (P >= WGRAD_LONG_PX) splits = max(splits, ceil_div<long long>(P, WGRAD_SPLIT_PX));
-  const long long T = (long long)KK * p.Cout;
-  splits = max(1LL, wgrad_fit_splits(splits, T, p.Cout));
-  long long per = ceil_div<long long>(ceil_div<long long>(P, splits), BK) * BK;
-  splits = ceil_div<long long>(P, per);
-  float* ws = nullptr;
-  int rc = wgrad_workspace(splits * (T + p.Cout), st, &ws);
-  if (rc) return rc;
-  launch(conv_wgrad_kernel<BM, BN, TM, TN>, dim3(gx, gy, (unsigned)splits), dim3((BM / TM) * (BN / TN)), 0, st, p, x, dy,
-         ws ? ws : dw, ws ? (dbias ? ws + splits * T : nullptr) : dbias, per, ws ? 0 : 1);
-  rc = check_launch("conv_wgrad_kernel");
-  return (rc || !ws) ? rc : wgrad_reduce(ws, (int)splits, T, p.Cout, dw, dbias, st);
+  splits = max(1LL, wgrad_fit_splits(splits, T, d->Cout));
+  f.per = ceil_div<long long>(ceil_div<long long>(P, splits), BK) * BK;
+  pl->splits = ceil_div<long long>(P, f.per);
+  pl->split_px = f.per;
+  pl->grid = dim3((unsigned)gx, (unsigned)gy, (unsigned)pl->splits);
+  pl->family = CONV_FP32_WGRAD;
+}
+
+template <int BM, int BN, int TM, int TN>
+static void fwd_go(const ConvPlan& pl, const ConvP& p, const float* x, const float* w, const float* bias,
+                   const float* residual, float* y, int relu, double* stats, cudaStream_t st) {
+  if (pl.fp.vec) launch(conv_fwd_kernel<BM, BN, TM, TN, true>, pl.grid, pl.block, 0, st, p, x, w, bias, residual, y, relu, stats);
+  else launch(conv_fwd_kernel<BM, BN, TM, TN, false>, pl.grid, pl.block, 0, st, p, x, w, bias, residual, y, relu, stats);
+}
+
+int conv_fwd_simt(const ConvPlan& pl, const se_conv_desc* d, const float* x, const float* w, const float* bias,
+                  const float* residual, float* y, int relu, double* stats, cudaStream_t st) {
+  const ConvP p = to_p(d);
+  switch (pl.family) {
+    case CONV_FP32_DENSE_SMALL:
+      launch(dense_small_fwd_kernel, pl.grid, pl.block, 0, st, x, w, bias, y, p.N, p.Cin, p.Cout, relu);
+      return check_launch("dense_small_fwd_kernel");
+    case CONV_FP32_FWD_STEM:
+      launch(conv_fwd_stem_kernel, pl.grid, pl.block, pl.smem, st, p, x, w, bias, y, relu, stats, pl.fp.TH);
+      return check_launch("conv_fwd_stem_kernel");
+    default:
+      if (pl.fp.bn == 16) fwd_go<128, 16, 4, 2>(pl, p, x, w, bias, residual, y, relu, stats, st);
+      else if (pl.fp.bn == 32) fwd_go<128, 32, 4, 4>(pl, p, x, w, bias, residual, y, relu, stats, st);
+      else fwd_go<64, 64, 4, 4>(pl, p, x, w, bias, residual, y, relu, stats, st);
+      return check_launch("conv_fwd_kernel");
+  }
+}
+
+template <int BM, int BN, int TM, int TN>
+static void dgrad_go(const ConvPlan& pl, const ConvP& p, const float* dy, const float* w, float* dx, float beta, cudaStream_t st) {
+  if (pl.fp.vec) launch(conv_dgrad_kernel<BM, BN, TM, TN, true>, pl.grid, pl.block, 0, st, p, dy, w, dx, beta, pl.fp.par);
+  else launch(conv_dgrad_kernel<BM, BN, TM, TN, false>, pl.grid, pl.block, 0, st, p, dy, w, dx, beta, pl.fp.par);
+}
+
+int conv_dgrad_simt(const ConvPlan& pl, const se_conv_desc* d, const float* dy, const float* w, float* dx, float beta,
+                    cudaStream_t st) {
+  const ConvP p = to_p(d);
+  if (pl.fp.bn == 16) dgrad_go<128, 16, 4, 2>(pl, p, dy, w, dx, beta, st);
+  else if (pl.fp.bn == 32) dgrad_go<128, 32, 4, 4>(pl, p, dy, w, dx, beta, st);
+  else dgrad_go<64, 64, 4, 4>(pl, p, dy, w, dx, beta, st);
+  return check_launch("conv_dgrad_kernel");
+}
+
+int conv_wgrad_simt(const ConvPlan& pl, const se_conv_desc* d, const float* x, const float* dy, const WgOut& o,
+                    cudaStream_t st) {
+  const ConvP p = to_p(d);
+  const SimtParams& f = pl.fp;
+  const int direct = o.ws ? 0 : 1;
+  switch (pl.family) {
+    case CONV_FP32_WGRAD_STEM:
+      launch(conv_wgrad_stem_kernel, pl.grid, pl.block, pl.smem, st, p, x, dy, o.dw, o.dbias, f.TH, f.PG, f.num_tiles, direct);
+      return check_launch("conv_wgrad_stem_kernel");
+    case CONV_FP32_WGRAD_3X3: {
+      auto kern = f.nci == 16 ? (f.nco == 16 ? conv_wgrad3x3_kernel<16, 16> : conv_wgrad3x3_kernel<16, 8>)
+                              : (f.nco == 16 ? conv_wgrad3x3_kernel<8, 16> : conv_wgrad3x3_kernel<8, 8>);
+      launch(kern, pl.grid, pl.block, pl.smem, st, p, x, dy, o.dw, o.dbias, f.TH, f.tiles_per_img, f.num_tiles, direct);
+      return check_launch("conv_wgrad3x3_kernel");
+    }
+    default:
+      launch(conv_wgrad_kernel<64, 64, 4, 4>, pl.grid, pl.block, 0, st, p, x, dy, o.dw, o.dbias, f.per, direct);
+      return check_launch("conv_wgrad_kernel");
+  }
 }
 
 }  // namespace se

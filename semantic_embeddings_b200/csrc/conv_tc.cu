@@ -385,6 +385,8 @@ transpose_filters_kernel(const float* __restrict__ P, float* __restrict__ PT, fl
 }
 
 // ---------------------------------------------------------------------------------------- host side
+constexpr ConvFamily DECLINED = CONV_FP32_TILES;   // no tensor-core family takes the call: simt_config picks an fp32 one
+
 static int pow2_ge(int v) { int q = 1; while (q < v) q <<= 1; return q; }
 
 // image sizes the 3x3 tiles take: rows of 4..56 pixels (every layer of the reference networks at their input sizes)
@@ -395,20 +397,20 @@ static bool channels_ok(int Kc, int Nc) { return Kc % 16 == 0 && Nc % 16 == 0 &&
 
 // The conv_tc_kernel family of a forward or data-gradient layer with GEMM channels Kc x Nc, by shape alone
 static ConvFamily tc_family(const se_conv_desc* d, int Kc, int Nc) {
-  if (!channels_ok(Kc, Nc)) return CONV_FP32;
+  if (!channels_ok(Kc, Nc)) return DECLINED;
   if (d->kh == 3 && d->kw == 3 && d->stride == 1 && d->pad_t == 1 && d->pad_l == 1 && d->Ho == d->H && d->Wo == d->W)
-    return geometry_ok(d->W) ? CONV_TC_3X3 : CONV_FP32;
-  if (d->kh != 1 || d->kw != 1 || d->pad_t != 0 || d->pad_l != 0) return CONV_FP32;
+    return geometry_ok(d->W) ? CONV_TC_3X3 : DECLINED;
+  if (d->kh != 1 || d->kw != 1 || d->pad_t != 0 || d->pad_l != 0) return DECLINED;
   // 1x1 / stride 1: a GEMM over the flat pixel list, any image size
   if (d->stride == 1 && d->Ho == d->H && d->Wo == d->W)
-    return (long long)d->N * d->H * d->W >= CT_BM ? CONV_TC_1X1 : CONV_FP32;
+    return (long long)d->N * d->H * d->W >= CT_BM ? CONV_TC_1X1 : DECLINED;
   // 1x1 / stride 2 (the first convolution and the projection shortcut of a ResNet-50 stage, the shortcuts of
   // wide_residual_network.py:28): the GEMM of the 1x1 case over the (Ho, Wo) grid, the input (forward) or the output
   // (backward data) addressed through a tensor map of the sub-sampled VIEW x[:, ::2, ::2, :] (pixel and row strides
   // doubled) -- no gather pass.
   if (d->stride == 2 && d->Ho == (d->H + 1) / 2 && d->Wo == (d->W + 1) / 2)
-    return d->Wo <= 32 && geometry_ok(d->Wo) ? CONV_TC_1X1_S2 : CONV_FP32;
-  return CONV_FP32;
+    return d->Wo <= 32 && geometry_ok(d->Wo) ? CONV_TC_1X1_S2 : DECLINED;
+  return DECLINED;
 }
 
 // output channels per tile: the widest wgmma N that divides the channel count (<= 128; <= 64 in the error-compensated
@@ -487,22 +489,22 @@ bool odd_config(const se_conv_desc* d, int dir, int sms, ConvPlan* pl);     // c
 // The families of conv_tc_kernel and conv_wgrad_tc_kernel
 static ConvFamily conv_plan_wide(const se_conv_desc* d, int dir, int mode, const ConvCall& c, ConvPlan* pl) {
   *pl = ConvPlan();
-  if (mode != SE_MODE_TF32 && mode != SE_MODE_TF32X3) return CONV_FP32;
+  if (mode != SE_MODE_TF32 && mode != SE_MODE_TF32X3) return DECLINED;
   const int x3 = pl->x3 = mode == SE_MODE_TF32X3;
-  if (dir == 2) return c.aligned && wgrad_config(d, x3, c.sms, pl) ? (pl->family = CONV_TC_WGRAD) : CONV_FP32;
+  if (dir == 2) return c.aligned && wgrad_config(d, x3, c.sms, pl) ? (pl->family = CONV_TC_WGRAD) : DECLINED;
   // the B operands: the transposed kernel copy (forward) or the kernel itself (data gradient), and their low parts
-  if (dir == 0 && (!c.w_t || (x3 && !c.w_t_lo))) return CONV_FP32;
-  if (dir == 1 && x3 && !c.w_lo) return CONV_FP32;
-  if (dir == 1 && c.beta != 0.f && c.beta != 1.f) return CONV_FP32;     // overwrite or accumulate only
+  if (dir == 0 && (!c.w_t || (x3 && !c.w_t_lo))) return DECLINED;
+  if (dir == 1 && x3 && !c.w_lo) return DECLINED;
+  if (dir == 1 && c.beta != 0.f && c.beta != 1.f) return DECLINED;     // overwrite or accumulate only
   const int Kc = dir == 0 ? d->Cin : d->Cout, Nc = dir == 0 ? d->Cout : d->Cin;
   ConvFamily f = tc_family(d, Kc, Nc);
   if (dir == 1 && conv3x3s2_tc_ok(d)) {
     // every filter tap is a 1x1 / stride 2 data gradient over the same grid, added into its own view of dx
     se_conv_desc d1 = *d;
     d1.kh = 1; d1.kw = 1;
-    f = tc_family(&d1, Kc, Nc) == CONV_TC_1X1_S2 ? CONV_TC_DGRAD_3X3S2 : CONV_FP32;
+    f = tc_family(&d1, Kc, Nc) == CONV_TC_1X1_S2 ? CONV_TC_DGRAD_3X3S2 : DECLINED;
   }
-  if (f == CONV_FP32 || !tc_config(d, f, Kc, Nc, dir, x3, c.sms, pl)) return CONV_FP32;
+  if (f == DECLINED || !tc_config(d, f, Kc, Nc, dir, x3, c.sms, pl)) return DECLINED;
   pl->tc.beta = f == CONV_TC_DGRAD_3X3S2 ? 1.f : c.beta;
   // wide layers (640 output channels): the per-warp statistics slots of the fused epilogue do not fit in shared memory,
   // the BatchNorm sums come from a separate pass over y
@@ -510,19 +512,27 @@ static ConvFamily conv_plan_wide(const se_conv_desc* d, int dir, int mode, const
   return pl->family = f;
 }
 
-ConvFamily conv_plan(const se_conv_desc* d, int dir, int mode, const ConvCall& c, ConvPlan* pl) {
-  const ConvFamily f = conv_plan_wide(d, dir, mode, c, pl);
-  if (f != CONV_FP32 || !conv_odd_tc_ok(d)) return f;
-  // only shapes every family above declines: channel counts that are not all multiples of 8 (see conv_odd_tc_ok)
+// The family of conv_odd_tc.cu: only shapes every family above declines, channel counts that are not all multiples of
+// 8 (see conv_odd_tc_ok)
+static ConvFamily conv_plan_odd(const se_conv_desc* d, int dir, int mode, const ConvCall& c, ConvPlan* pl) {
   *pl = ConvPlan();
-  if (mode != SE_MODE_TF32 && mode != SE_MODE_TF32X3) return CONV_FP32;
+  if (mode != SE_MODE_TF32 && mode != SE_MODE_TF32X3) return DECLINED;
   const int x3 = pl->x3 = mode == SE_MODE_TF32X3;
-  if (dir == 0 && (!c.w_t || (x3 && !c.w_t_lo))) return CONV_FP32;
-  if (dir == 1 && ((x3 && !c.w_lo) || (c.beta != 0.f && c.beta != 1.f))) return CONV_FP32;
-  if (dir == 2 && !c.aligned) return CONV_FP32;
-  if (!odd_config(d, dir, c.sms, pl)) return CONV_FP32;
+  if (dir == 0 && (!c.w_t || (x3 && !c.w_t_lo))) return DECLINED;
+  if (dir == 1 && ((x3 && !c.w_lo) || (c.beta != 0.f && c.beta != 1.f))) return DECLINED;
+  if (dir == 2 && !c.aligned) return DECLINED;
+  if (!odd_config(d, dir, c.sms, pl)) return DECLINED;
   pl->fused_stats = false;                // se_bn_stats sums the BatchNorm statistics after the forward launch
   return pl->family = CONV_TC_ODD_3X3;
+}
+
+ConvFamily conv_plan(const se_conv_desc* d, int dir, int mode, const ConvCall& c, ConvPlan* pl) {
+  ConvFamily f = conv_plan_wide(d, dir, mode, c, pl);
+  if (f == DECLINED && conv_odd_tc_ok(d)) f = conv_plan_odd(d, dir, mode, c, pl);
+  if (conv_is_tc(f)) return f;
+  *pl = ConvPlan();
+  simt_config(d, dir, c, pl);
+  return pl->family;
 }
 
 template <int BN, int NKS>
@@ -590,8 +600,6 @@ int init_conv_tc() {
 // w_t = the transposed kernel copy [tap][co][ci], w_t_lo its low parts (error-compensated mode)
 int conv_fwd_tc(const ConvPlan& pl, const se_conv_desc* d, const float* x, const float* w_t, const float* w_t_lo,
                 const float* bias, const float* residual, float* y, int relu, double* stats, cudaStream_t st) {
-  int rc = ensure_setup();
-  if (rc) return rc;
   ConvTcParams p = pl.tc;
   p.relu = relu; p.bias = bias; p.residual = residual; p.out = y; p.stats = stats;
   return conv_tc_launch(pl, p, d, x, w_t, w_t_lo, st);
@@ -602,8 +610,6 @@ int conv_fwd_tc(const ConvPlan& pl, const se_conv_desc* d, const float* x, const
 // conv3x3s2_tc_ok) adds dY W[r, s]^T into dx[:, r::2, s::2, :], whose last column / row may not exist.
 int conv_dgrad_tc(const ConvPlan& pl, const se_conv_desc* d, const float* dy, const float* w, const float* w_lo, float* dx,
                   float beta, cudaStream_t st) {
-  int rc = ensure_setup();
-  if (rc) return rc;
   const bool nine = pl.family == CONV_TC_DGRAD_3X3S2;
   if ((nine || pl.family == CONV_TC_1X1_S2) && beta == 0.f &&
       cudaMemsetAsync(dx, 0, (size_t)d->N * d->H * d->W * d->Cin * sizeof(float), st) != cudaSuccess) {
@@ -618,7 +624,7 @@ int conv_dgrad_tc(const ConvPlan& pl, const se_conv_desc* d, const float* dy, co
       const long long woff = (long long)(r * 3 + s) * d->Cin * d->Cout;
       p.out = dx + ((long long)r * d->W + s) * d->Cin;
       p.ovw = d->Wo - (s == 2); p.ovh = d->Ho - (r == 2);
-      rc = conv_tc_launch(pl, p, d, dy, w + woff, w_lo ? w_lo + woff : nullptr, st);
+      const int rc = conv_tc_launch(pl, p, d, dy, w + woff, w_lo ? w_lo + woff : nullptr, st);
       if (rc != SE_OK) return rc;
     }
   return SE_OK;

@@ -34,7 +34,6 @@ constexpr int WG_THREADS = 256;
 // Workspaces of the split-K partial sums: one per (device, stream), 32 MB each, allocated outside graph captures (se_init
 // prepares the one of se_run_ops' side stream).  A request that does not fit, or a stream that first appears inside a
 // capture, runs in direct mode instead: the partial sums go into dW with float atomics (correct, not bit-reproducible).
-constexpr long long WG_WS_FLOATS = 8LL << 20;
 struct WgWorkspace { int dev; cudaStream_t st; float* ptr; };
 constexpr int WG_MAX_WS = 32;
 static WgWorkspace g_wg_ws[WG_MAX_WS];
@@ -542,6 +541,8 @@ bool wgrad_config(const se_conv_desc* d, int x3, int sms, ConvPlan* pl) {
   p.per_cta += p.per_cta & 1;
   gx = ceil_div<long long>(p.chunks, p.per_cta);
   pl->grid = dim3((unsigned)gx, (unsigned)gy, (unsigned)gz);
+  pl->splits = 2 * gx;                      // one slice per warpgroup
+  pl->split_px = (long long)p.per_cta * WG_PX;
   pl->wg_bn = BN;
   pl->wg_np = x3 && npx >= WG_LONG_PX ? 4 : 1;
   pl->smem = 1024 + 2 * (size_t)(WG_MT * 128 + BN * 128) * (x3 ? 2 : 1);
@@ -563,13 +564,13 @@ bool wgrad_config(const se_conv_desc* d, int x3, int sms, ConvPlan* pl) {
 }
 
 // se_linear_svm_fit: does the tensor-core kernel take this shape on stream `st` and add its split-K slices in a fixed
-// order, i.e. does at least one pair of slices fit a workspace that exists or can be allocated now?
+// order, i.e. do its slices fit a workspace that exists or can be allocated now?
 bool conv_wgrad_tc_fixed_order(const se_conv_desc* d, cudaStream_t st) {
   ConvPlan pl;
   if (conv_plan(d, 2, SE_MODE_TF32X3, ConvCall(), &pl) != CONV_TC_WGRAD) return false;
   const long long T = (long long)d->kh * d->kw * d->Cin * d->Cout;
   float* ws = nullptr;
-  return wgrad_workspace(2 * (T + d->Cout), st, &ws) == SE_OK && ws != nullptr;
+  return wgrad_workspace(pl.splits * (T + d->Cout), st, &ws) == SE_OK && ws != nullptr;
 }
 
 template <int BN>
@@ -586,23 +587,16 @@ static void wgrad_go(const ConvPlan& pl, cudaStream_t st, const float* x, const 
   launch(k, pl.grid, dim3(WG_THREADS), pl.smem, st, x, dy, p);
 }
 
-int conv_wgrad_tc(const ConvPlan& pl, const float* x, const float* dy, float* dw, float* dbias, cudaStream_t st) {
-  int rc = ensure_setup();
-  if (rc) return rc;
+int conv_wgrad_tc(const ConvPlan& pl, const float* x, const float* dy, const WgOut& o, cudaStream_t st) {
   WgTcParams p = pl.wg;
-  p.dw = dw; p.dbias = dbias;
-  const long long T = (long long)p.KK * p.Cout, splits = 2LL * pl.grid.x;
-  rc = wgrad_workspace(splits * (T + p.Cout), st, &p.ws);
-  if (rc) return rc;
+  p.ws = o.ws; p.dw = o.dw; p.dbias = o.dbias;
   switch (pl.wg_bn) {
     case 16: wgrad_go<16>(pl, st, x, dy, p); break;
     case 32: wgrad_go<32>(pl, st, x, dy, p); break;
     case 64: wgrad_go<64>(pl, st, x, dy, p); break;
     default: wgrad_go<128>(pl, st, x, dy, p); break;
   }
-  rc = check_launch("conv_wgrad_tc_kernel");
-  if (rc || !p.ws) return rc;
-  return wgrad_reduce(p.ws, (int)splits, T, p.Cout, dw, dbias, st);
+  return check_launch("conv_wgrad_tc_kernel");
 }
 
 }  // namespace se

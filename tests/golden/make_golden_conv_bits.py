@@ -1,7 +1,7 @@
-"""Writes tests/golden/conv_bits_ref.npz: for every case of tests/test_gpu_conv_bits.py in SE_MODE_TF32 and
-SE_MODE_TF32X3, the SHA-256 of the output words and a seeded sample of them, of the forward (bias, residual, ReLU) and
-the data gradient (beta 0 and 1), from the library in the source tree (or the one given with --lib), with the name of
-the device it ran on.  Needs a GPU.
+"""Writes tests/golden/conv_bits_ref.npz: for every call of tests/test_gpu_conv_bits.py (RUNS), the SHA-256 of the
+output words and a seeded sample of them, of the forward (bias, residual, ReLU) and the data gradient (beta 0 and 1),
+from the library in the source tree (or the one given with --lib), with the name of the device it ran on.  Needs a
+GPU.
 
     python tests/golden/make_golden_conv_bits.py [--lib OTHER/libse_b200.so]"""
 import argparse
@@ -29,15 +29,14 @@ def main():
     _lib.check(_lib.load().se_init())
     prop = torch.cuda.get_device_properties(0)
     out = {'device': np.array(prop.name)}
-    for i, (name, shape) in enumerate(tb.CASES):
-        for mode, _ in tb.MODES:
-            outs = tb.run(_lib, shape, mode, tb.seed_of(i, mode))
-            for o in tb.OUTPUTS:
-                key = '%s_%d_%s' % (name, mode, o)
-                h, words = tb.digest(outs[o])
-                out[key + '_sha256'], out[key + '_words'] = np.array(h), words
+    for name, shape, mode, seed in tb.RUNS:
+        outs = tb.run(_lib, shape, mode, seed, name not in tb.NO_RESIDUAL)
+        for o in tb.OUTPUTS:
+            key = '%s_%d_%s' % (name, mode, o)
+            h, words = tb.digest(outs[o])
+            out[key + '_sha256'], out[key + '_words'] = np.array(h), words
     np.savez_compressed(args.out, **out)
-    print('%s: %d cases on %s' % (args.out, len(tb.CASES) * len(tb.MODES), prop.name))
+    print('%s: %d cases on %s' % (args.out, len(tb.RUNS), prop.name))
 
 
 if __name__ == '__main__':

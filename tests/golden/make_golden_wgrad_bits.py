@@ -1,6 +1,6 @@
-"""Writes tests/golden/wgrad_bits_ref.npz: dW and dbias (as uint32 words) of se_conv2d_wgrad over the cases of
-tests/test_gpu_wgrad_bits.py, in SE_MODE_TF32 and SE_MODE_TF32X3, from the library in the source tree (or the one given
-with --lib), with the name and SM count of the device it ran on.  Needs a GPU.
+"""Writes tests/golden/wgrad_bits_ref.npz: for every call of se_conv2d_wgrad in tests/test_gpu_wgrad_bits.py (RUNS),
+the dbias words and a SHA-256 of the dW words with a seeded sample of them, from the library in the source tree (or the
+one given with --lib), with the name and SM count of the device it ran on.  Needs a GPU.
 
     python tests/golden/make_golden_wgrad_bits.py [--lib OTHER/libse_b200.so]"""
 import argparse
@@ -28,12 +28,13 @@ def main():
     _lib.check(_lib.load().se_init())
     prop = torch.cuda.get_device_properties(0)
     out = {'device': np.array(prop.name), 'sm_count': np.array(prop.multi_processor_count)}
-    for i, (name, shape) in enumerate(tb.CASES):
-        for mode, _ in tb.MODES:
-            dw, db = tb.run(_lib, shape, mode, tb.seed_of(i, mode))
-            out['%s_%d_dw' % (name, mode)], out['%s_%d_db' % (name, mode)] = dw.reshape(-1), db
+    for name, shape, mode, seed in tb.RUNS:
+        dw, db = tb.run(_lib, shape, mode, seed)
+        key = '%s_%d' % (name, mode)
+        h, words = tb.digest(dw)
+        out[key + '_dw_sha256'], out[key + '_dw_words'], out[key + '_db'] = np.array(h), words, db
     np.savez_compressed(args.out, **out)
-    print('%s: %d cases on %s (%d SMs)' % (args.out, len(tb.CASES) * len(tb.MODES), prop.name, prop.multi_processor_count))
+    print('%s: %d cases on %s (%d SMs)' % (args.out, len(tb.RUNS), prop.name, prop.multi_processor_count))
 
 
 if __name__ == '__main__':

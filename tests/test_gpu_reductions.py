@@ -8,11 +8,11 @@ cond_errors: err_cond = |got - ref| / M elementwise, 0/0 = 0, x/0 = inf), which 
 Each case runs in three seeded input regimes (reduction_oracle.inputs): 'gauss', 'network' and 'spread' (network with
 each image's dY scaled by 2^k, k in [-8, 8]), in SE_MODE_F32 and SE_MODE_TF32X3.
 
-KERNEL names the kernel each case is meant to run: 'tc' is conv_wgrad_tc_kernel<BN, 1, NP> (se_conv2d_path says
-tensor core; BN and NP follow wgrad_config); the fp32 kernels follow the shape rule of conv_wgrad_simt ('stem' =
-conv_wgrad_stem_kernel, 'w3x3<NCI,NCO>' = conv_wgrad3x3_kernel, 'generic' = conv_wgrad_kernel); BatchNorm cases name
-their se_bn_bwd_path.  Every case asserts, from the kernel names torch.profiler records, that the library launched that
-kernel (so no fall-back inside the library goes unnoticed) and the split-K reduction exactly in workspace mode, and test_cases_cover_every_cell requires every (kernel,
+KERNEL names the kernel each case is meant to run: 'tc' is conv_wgrad_tc_kernel<BN, 1, NP>, 'stem' =
+conv_wgrad_stem_kernel, 'w3x3<NCI,NCO>' = conv_wgrad3x3_kernel, 'generic' = conv_wgrad_kernel; BatchNorm cases name
+their se_bn_bwd_path.  Every case asserts that the library's plan (se_conv2d_plan) names that kernel, that the plan's
+kernel is the one torch.profiler records (so no fall-back inside the library goes unnoticed), and that the split-K
+reduction runs exactly when the plan's slices fit the workspace.  test_cases_cover_every_cell requires every (kernel,
 mode, length >= 2^18) cell and every (BN, NP) form of the tensor-core kernel.
 
 BOUNDS holds one bound per cell, about 2x the largest value measured over the sweep (all regimes) on an H100 80GB
@@ -24,6 +24,7 @@ workspace: float atomics) has its own cells.  The four partial tiles per chunk t
 the ACT_LAYERS cases run the kernels on the X and dY of a real 448 px training step.  There one tile per chunk gives
 1.1e-7 .. 1.2e-7 against the cell's 5.5e-8 bound (four tiles: 2.2e-8 .. 2.7e-8)."""
 import math
+import re
 
 import pytest
 import torch
@@ -35,7 +36,6 @@ gpu = pytest.mark.gpu
 
 LONG = 1 << 18                 # both long-sum switches: WG_LONG_PX (conv_wgrad_tc.cu), WGRAD_LONG_PX (conv_simt.cu)
 MODES = {'f32': 0, 'tf32x3': 2}
-WG_WS_FLOATS = 8 << 20         # conv_wgrad_tc.cu: the split-K workspace
 
 # (id, (N, H, W, Cin, Cout, k, stride, padding), {mode: kernel}).  N = None: chosen at run time (_edge_n)
 CONV_CASES = [
@@ -169,57 +169,40 @@ def bound(cell, qty):
     return BOUNDS[cell][qty]
 
 
-# ------------------------------------------------------------------------------------------------ planning mirrors
+# ------------------------------------------------------------------------------------------------ the plan
 def _geometry(shape):
     from test_gpu_ops import conv_geometry
     return conv_geometry(shape + (False,))
 
 
-def fp32_kernel(shape):
-    """conv_wgrad_simt's choice (conv_simt.cu) for an NHWC weight gradient of this shape"""
-    N, H, W, Cin, Cout, k, stride = shape[:7]
-    pt, pl, Ho, Wo = _geometry(shape)
-    same3 = k == 3 and stride == 1 and pt == 1 and pl == 1 and Ho == H and Wo == W
-    if same3 and Cin <= 4:
-        TH = 8 if H % 8 == 0 else 4 if H % 4 == 0 else 1
-        per_pg = (9 * Cin + 1) * (Cout // 4)
-        PG = 1
-        while 2 * PG * per_pg <= 512 and (TH * W) % (2 * PG) == 0:
-            PG *= 2
-        smem = 4 * ((((TH + 2) * (W + 2) * Cin + 3) & ~3) + TH * W * Cout + max(PG - 1, 1) * per_pg * 4)
-        if Cout % 4 == 0 and Cout <= 64 and W & (W - 1) == 0 and W <= 64 and per_pg <= 512 and smem <= 48 * 1024:
-            return 'stem'
-    if same3 and Cin % 16 == 0 and Cout % 16 == 0:
-        nci, nco = (16 if Cin % 32 == 0 else 8), (16 if Cout % 32 == 0 else 8)
-        TH = min(max(1, 128 // W), H)
-        rg = 256 // (nci * nco)
-        smem = 4 * max((TH + 2) * (W + 2) * 2 * nci + TH * W * 2 * nco,
-                       (rg * 36 * nci * nco + rg * 2 * nco) if rg > 1 else 0)
-        if smem <= 160 * 1024:
-            return 'w3x3<%d,%d>' % (nci, nco)
-    return 'generic'
+def wgrad_plan(L, shape, mode, sms):
+    """se_conv2d_plan of the weight gradient of this shape"""
+    import ctypes
+    info = L.ConvPlanInfo()
+    L.call('se_conv2d_plan', conv_desc(L, shape), mode, 2, sms, ctypes.byref(info))
+    return info
 
 
-def tc_plan(shape, sms):
-    """wgrad_config (conv_wgrad_tc.cu) in SE_MODE_TF32X3: BN, NP, the workspace mode, and the chunks of the last CTA"""
-    N, H, W, Cin, Cout, k, stride = shape[:7]
-    _, _, Ho, Wo = _geometry(shape)
-    npx, KK = N * Ho * Wo, k * k * Cin
-    BN = 64
-    while Cout % BN:
-        BN //= 2
-    chunks = -(-npx // 32)
-    gy, gz = -(-KK // 64), Cout // BN
-    T = KK * Cout
-    fit = WG_WS_FLOATS // (T + Cout)
-    gx = -(-8 * sms // (gy * gz))
-    gx = max(1, min(gx, -(-chunks // 4)))
-    gx = max(1, (min(2 * gx, fit) if fit >= 1 else 2 * gx) // 2)
-    per = -(-chunks // gx)
-    per += per & 1
-    gx = -(-chunks // per)
-    return dict(BN=BN, NP=4 if npx >= LONG else 1, workspace=2 * gx * (T + Cout) <= WG_WS_FLOATS,
-                last_chunks=chunks - (gx - 1) * per)
+def case_kernel(info):
+    """the name the cases give the kernel of a plan"""
+    k = info.kernel.decode()
+    for prefix, name in (('se::conv_wgrad_tc_kernel<', 'tc'), ('se::conv_wgrad_stem_kernel(', 'stem'),
+                         ('se::conv_wgrad_kernel<', 'generic')):
+        if k.startswith(prefix):
+            return name
+    m = re.match(r'se::conv_wgrad3x3_kernel<(\d+), (\d+)>', k)
+    assert m, k
+    return 'w3x3<%s,%s>' % m.groups()
+
+
+def tc_form(info):
+    """(BN, NP) of a conv_wgrad_tc_kernel<BN, 1, NP> plan"""
+    return tuple(int(v) for v in re.match(r'se::conv_wgrad_tc_kernel<(\d+), 1, (\d+)>', info.kernel.decode()).groups())
+
+
+def last_cta_chunks(shape, info):
+    """the 32-pixel chunks of the last CTA of a conv_wgrad_tc_kernel plan (two slices per CTA)"""
+    return -(-_npx(shape) // 32) - (info.splits // 2 - 1) * (info.split_px // 32)
 
 
 def _edge_n(case_id, sms):
@@ -227,7 +210,8 @@ def _edge_n(case_id, sms):
     (its second warpgroup writes a zero slice) or at least two"""
     idle = case_id == 'edge-last-wg-idle'
     for n in range(8191, 8191 + 4096):
-        last = tc_plan((n, 1, 32, 64, 64, 1, 1, 'valid'), sms)['last_chunks']
+        shape = (n, 1, 32, 64, 64, 1, 1, 'valid')
+        last = last_cta_chunks(shape, wgrad_plan(_lib(), shape, MODES['tf32x3'], sms))
         if (last == 1) == idle:
             return n
     raise AssertionError('no %s batch found' % case_id)
@@ -246,16 +230,10 @@ def _cell(kernel, mode, n, direct=False, suffix=''):
     return '%s/%s/%s%s%s' % (kernel, mode, 'long' if n >= LONG else 'short', '/direct' if direct else '', suffix)
 
 
-def kernel_name(kernel, plan=None):
-    """what the profiler calls the kernel a case names (tc: with the BN and NP of its plan)"""
-    if kernel == 'tc':
-        return 'conv_wgrad_tc_kernel<%d, 1, %d>' % (plan['BN'], plan['NP'])
-    if kernel.startswith('w3x3'):
-        return 'conv_wgrad3x3_kernel<%s>' % kernel[5:-1].replace(',', ', ')
-    if kernel.startswith('bn:'):
-        return {'reg': 'bn_bwd_reg_kernel', 'quad': 'bn_bwd_fused_kernel', 'atomic': 'bn_bwd_fused_kernel',
-                'vec': 'bn_bwd_reduce_kernel', 'scalar': 'bn_bwd_reduce_kernel'}[kernel[3:]]
-    return {'stem': 'conv_wgrad_stem_kernel', 'generic': 'conv_wgrad_kernel<'}[kernel]
+def kernel_name(kernel):
+    """what the profiler calls the kernel of a BatchNorm path"""
+    return {'reg': 'bn_bwd_reg_kernel', 'quad': 'bn_bwd_fused_kernel', 'atomic': 'bn_bwd_fused_kernel',
+            'vec': 'bn_bwd_reduce_kernel', 'scalar': 'bn_bwd_reduce_kernel'}[kernel[3:]]
 
 
 def launched_kernels(fn):
@@ -328,19 +306,16 @@ def _check_wgrad(case_id, kernels, shape, regime, dense=False, tensors=None, suf
         ref, M, rb, Mb = ro.conv_wgrad_ref(xd, dyd, d.kh, d.stride, d.pad_t, d.pad_l)
     for mname, mode in MODES.items():
         kernel = kernels[mname]
-        tc = conv_paths(L, d, mode)[2]
-        assert tc == (kernel == 'tc'), (case_id, mname, kernel, 'se_conv2d_path', tc)
-        plan = tc_plan(cshape, sms) if tc else None
-        if not tc:
-            assert fp32_kernel(cshape) == kernel, (case_id, mname, kernel, fp32_kernel(cshape))
+        plan = wgrad_plan(L, cshape, mode, sms)
+        assert case_kernel(plan) == kernel, (case_id, mname, kernel, plan.kernel)
+        assert conv_paths(L, d, mode)[2] == plan.tensor_core, (case_id, mname, 'se_conv2d_path')
         dw, db, launches = _run_wgrad(L, d, xd, dyd, Cout, mode, B if dense else None)
         names = launched_kernels(lambda: _run_wgrad(L, d, xd, dyd, Cout, mode, B if dense else None))
         direct = launches == 1
-        if tc:
-            assert direct == (not plan['workspace']), (case_id, launches, plan)
-        # the library ran the kernel the case names (no fall-back inside it), with its reduction in workspace mode
-        assert_ran(case_id, names, kernel_name(kernel, plan))
-        assert direct == (not any('conv_wgrad_reduce_kernel' in n for n in names)), (case_id, names)
+        # the library ran the kernel its plan names (no fall-back inside it), with its reduction in workspace mode
+        assert_ran(case_id, names, plan.kernel.decode())
+        assert direct == (not plan.workspace) == (not any('conv_wgrad_reduce_kernel' in n for n in names)), \
+            (case_id, launches, plan.splits, names)
         cell = _cell(kernel, mname, npx, direct, suffix)
         errs = {'dw': ro.cond_errors(dw, ref, M), 'db': ro.cond_errors(db, rb, Mb)}
         same = True
@@ -350,8 +325,8 @@ def _check_wgrad(case_id, kernels, shape, regime, dense=False, tensors=None, suf
             same = torch.equal(dw, dw2) and torch.equal(db, db2)
             del dw2, db2
         report('reductions', case=case_id, regime=regime, mode=mname, kernel=kernel, cell=cell, npx=npx,
-               launches=launches, same_bits=same, kernels=names,
-               **({'BN': plan['BN'], 'NP': plan['NP'], 'last_cta_chunks': plan['last_chunks']} if tc else {}),
+               launches=launches, same_bits=same, kernels=names, splits=plan.splits,
+               **({'last_cta_chunks': last_cta_chunks(cshape, plan)} if kernel == 'tc' else {}),
                **{'%s_%s' % (q, k): v for q, e in errs.items() for k, v in e.items()})
         del dw, db
         _assert_bounds(case_id, cell, errs)
@@ -461,27 +436,20 @@ def test_bn_dgamma_dbeta(case, regime):
 def test_cases_cover_every_cell():
     """Every kernel runs at both lengths in both modes (the tensor-core kernel in SE_MODE_TF32X3 only, BatchNorm in
     no mode), every (BN, NP) form of the tensor-core kernel runs, and every cell has a bound.  Host-side planning only
-    (se_conv2d_path, se_bn_bwd_path at the device's SM count, or an H100 SXM's 132 without a device)."""
+    (se_conv2d_plan, se_bn_bwd_path at the device's SM count, or an H100 SXM's 132 without a device)."""
     L = _lib()
     sms = _sms()
     cells, forms = set(), set()
     for cases, dense in ((CONV_CASES, False), (DENSE_CASES, True)):
         for case_id, shape, kernels in cases:
             cshape = (shape[0], 1, 1, shape[1], shape[2], 1, 1, 'valid') if dense else _shape(case_id, shape, sms)
-            d = conv_desc(L, cshape)
             for mname, mode in MODES.items():
                 k = kernels[mname]
-                tc = int(L.load().se_conv2d_path(d, mode, 2))
-                assert tc == (k == 'tc'), (case_id, mname, k)
-                direct = False
-                if tc:
-                    p = tc_plan(cshape, sms)
-                    forms.add((p['BN'], p['NP']))
-                    direct = not p['workspace']
-                else:
-                    assert fp32_kernel(cshape) == k, (case_id, mname, k, fp32_kernel(cshape))
-                    direct = 9 * cshape[3] * cshape[4] + cshape[4] > WG_WS_FLOATS and k.startswith('w3x3')
-                cells.add(_cell(k, mname, _npx(cshape), direct))
+                p = wgrad_plan(L, cshape, mode, sms)
+                assert case_kernel(p) == k, (case_id, mname, k, p.kernel)
+                if k == 'tc':
+                    forms.add(tc_form(p))
+                cells.add(_cell(k, mname, _npx(cshape), not p.workspace))
     for layer, cin, cout in (('res2a_branch2a', 64, 64), ('res2a_branch1', 64, 256), ('res2b_branch2a', 256, 64)):
         assert layer in ACT_LAYERS
         cshape = (32, 111, 111, cin, cout, 1, 1, 'valid')
