@@ -639,7 +639,8 @@ int se_relevant_positions_q(const float* dist, int64_t ld, int rows, int n, cons
  * (sklearn's defaults: tol 1e-4, max_iter 1000).  The row sums are se_dense_fwd / se_dense_bwd in SE_MODE_TF32X3 with D
  * padded to a multiple of 4 and C to a multiple of 16 (zero columns); the weight gradient must add its split-K slices in
  * a fixed order, so (D+1) x C is limited by the library's workspace (about 4M elements: 2048 x 2048 fits) and
- * SE_ERR_UNSUPPORTED names the shape otherwise.  No float atomics: reruns give the same bits.
+ * SE_ERR_UNSUPPORTED names the shape otherwise.  Where N x D or N x C reaches 2^31 the GEMMs run in equal row blocks
+ * (N padded to whole blocks; X^T R adds the blocks in order).  No float atomics: reruns give the same bits.
  * X [N, ldx] float32 features; labels [N] int32 in [0, C) (else SE_ERR_ARG); outputs W [D, C] (Dense layout), b [C],
  * iters [C] int32 accepted Newton steps, gnorm [C] float32 = final |grad f_c| / |grad f_c(0)| (b, iters, gnorm may be
  * NULL).  workspace: se_linear_svm_workspace_bytes(N, D, C) bytes of device memory, 256-byte aligned.
@@ -648,6 +649,20 @@ int se_relevant_positions_q(const float* dist, int64_t ld, int rows, int n, cons
 int64_t se_linear_svm_workspace_bytes(int N, int D, int C);
 int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, const int32_t* labels, int C, float penalty, float tol,
                       int max_iter, float* W, float* b, int32_t* iters, float* gnorm, void* workspace, void* stream);
+/* One block of classes of the same problem: classes [c0, min(c0 + cb, C)) of a C-class problem (rows of every other class
+ * are negatives; 0 < cb <= C), on a workspace of se_linear_svm_classes_workspace_bytes(N, D, cb) bytes.  W [D, C], b, iters, gnorm
+ * [C] as above; only the block's columns are written.  A class's bits depend on its position in a block of width cb, not
+ * on c0.  packed != 0: the workspace already holds X packed by an earlier call with the same N, D and cb (X may be NULL),
+ * so a C-class problem is fitted block after block with X packed once.  se_linear_svm_block_classes(N, D, C): the widest
+ * block (C, or a multiple of 16 below it) whose weight gradient fits the fixed-order workspace; 0 if none does.
+ * se_linear_svm_last_cg_steps(): the CG steps (Hessian products, all classes of the call together) of the last
+ * se_linear_svm_fit or se_linear_svm_fit_classes that completed on the calling thread. */
+int64_t se_linear_svm_classes_workspace_bytes(int N, int D, int cb);
+int se_linear_svm_block_classes(int N, int D, int C);
+int64_t se_linear_svm_last_cg_steps(void);
+int se_linear_svm_fit_classes(const float* X, int64_t ldx, int N, int D, const int32_t* labels, int C, int c0, int cb,
+                              float penalty, float tol, int max_iter, float* W, float* b, int32_t* iters, float* gnorm,
+                              void* workspace, int packed, void* stream);
 /* Feature scaling of train_and_predict (:33-38) with numpy's float32 results bit for bit, and score negation:
  *   SE_SCALE_ROW_L2      y = x / ||x||_2 per row (float32 squares summed in numpy's pairwise order, true division)
  *   SE_SCALE_COL_MAXABS  colmax[j] = max_i |x_ij|          (y is not written)

@@ -154,6 +154,11 @@ _SIGS = {
     'se_center_loss_fwd_bwd': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_float, _P, _P, _P, _P]),
     'se_linear_svm_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'se_linear_svm_fit': (c_int, [_P, c_int64, c_int, c_int, _P, c_int, c_float, c_float, c_int, _P, _P, _P, _P, _P, _P]),
+    'se_linear_svm_classes_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
+    'se_linear_svm_block_classes': (c_int, [c_int, c_int, c_int]),
+    'se_linear_svm_last_cg_steps': (c_int64, []),
+    'se_linear_svm_fit_classes': (c_int, [_P, c_int64, c_int, c_int, _P, c_int, c_int, c_int, c_float, c_float, c_int, _P, _P,
+                                          _P, _P, _P, c_int, _P]),
     'se_scale_features': (c_int, [_P, c_int64, c_int, c_int, c_int, _P, c_float, _P, c_int64, _P]),
     'se_sgd_schedule': (c_int, [_P, _P]),
     'se_pairwise_topk_workspace_bytes': (c_int64, [c_int, c_int, c_int]),

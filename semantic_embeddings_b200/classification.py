@@ -79,9 +79,37 @@ def check_training_labels(labels, num_classes):
                          'indices)'.format(missing[:10].tolist()))
 
 
-def linear_svm_fit(X, labels, num_classes, C=0.1, tol=1e-4, max_iter=1000):
+# Device memory linear_svm_fit leaves to everything but its workspace (the library's weight-gradient workspace, the
+# outputs, the CUDA context's own allocations)
+SVM_MEMORY_MARGIN = 1 << 30
+
+
+def svm_block_classes(num_classes, fixed_max, workspace_bytes, budget, max_block_classes=None):
+    """Classes per block of linear_svm_fit: the widest block -- num_classes, else a multiple of 16 -- that is at most
+    max_block_classes, at most fixed_max (the widest block whose weight gradient adds its split-K slices in a fixed order,
+    se_linear_svm_block_classes) and whose workspace, workspace_bytes(cb), fits in `budget` bytes.  0 when none does."""
+    cb = min(num_classes, fixed_max, max_block_classes or num_classes)
+    while cb > 0 and not 0 < workspace_bytes(cb) <= budget:
+        cb = (cb - 1) // 16 * 16
+    return max(cb, 0)
+
+
+def _memory_budget(device):
+    """Bytes a new workspace can take on `device`: free memory plus what torch's allocator holds unused, less the margin."""
+    import torch
+    free, _ = torch.cuda.mem_get_info(device)
+    return free + torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device) - SVM_MEMORY_MARGIN
+
+
+def linear_svm_fit(X, labels, num_classes, C=0.1, tol=1e-4, max_iter=1000, max_block_classes=None, info=None):
     """One-vs-rest LinearSVC(C, tol, max_iter) on the device (se_linear_svm_fit).  X [N, D] float32, labels [N] in
-    [0, num_classes).  Returns CUDA tensors (W [D, C], b [C], iters [C] int32, gnorm [C] = final |grad| / |grad(0)|)."""
+    [0, num_classes).  Returns CUDA tensors (W [D, C], b [C], iters [C] int32, gnorm [C] = final |grad| / |grad(0)|).
+
+    A problem whose weight gradient does not fit the fixed-order workspace, or whose workspace does not fit in free
+    device memory, is fitted in blocks of classes (se_linear_svm_fit_classes; svm_block_classes picks the width), with X
+    packed once and kept in the one workspace.  max_block_classes caps the classes per block.  A dict passed as `info`
+    receives the fit's classes_per_block, blocks, workspace_bytes and cg_steps (Hessian products, summed over the
+    blocks)."""
     import torch
     x = _device_matrix(X)
     N, D = x.shape
@@ -89,16 +117,49 @@ def linear_svm_fit(X, labels, num_classes, C=0.1, tol=1e-4, max_iter=1000):
         else labels.to(device=x.device, dtype=torch.int32).contiguous()
     if lab.numel() != N:
         raise ValueError('{} labels for {} feature rows'.format(lab.numel(), N))
+    if max_block_classes is not None and max_block_classes < 1:
+        raise ValueError('max_block_classes must be positive, got {}'.format(max_block_classes))
     lib = _lib.load()
-    ws = torch.empty(int(lib.se_linear_svm_workspace_bytes(N, D, num_classes)), dtype=torch.uint8, device=x.device)
-    W = torch.empty((D, num_classes), dtype=torch.float32, device=x.device)
-    b = torch.empty(num_classes, dtype=torch.float32, device=x.device)
-    iters = torch.empty(num_classes, dtype=torch.int32, device=x.device)
-    gnorm = torch.empty(num_classes, dtype=torch.float32, device=x.device)
+    whole = int(lib.se_linear_svm_workspace_bytes(N, D, num_classes))
+    fixed = int(lib.se_linear_svm_block_classes(N, D, num_classes))
     with torch.cuda.device(x.device):
-        _lib.call('se_linear_svm_fit', x.data_ptr(), x.stride(0), N, D, lab.data_ptr(), num_classes, float(C), float(tol),
-                  int(max_iter), W.data_ptr(), b.data_ptr(), iters.data_ptr(), gnorm.data_ptr(), ws.data_ptr(),
-                  _lib.stream_ptr())
+        budget = _memory_budget(x.device)
+        one_block = (max_block_classes is None or max_block_classes >= num_classes) and fixed >= num_classes
+        if one_block and 0 < whole <= budget:
+            ws = torch.empty(whole, dtype=torch.uint8, device=x.device)
+            cb = num_classes
+        else:
+            ws_bytes = lambda c: int(lib.se_linear_svm_classes_workspace_bytes(N, D, c))
+            cb = svm_block_classes(num_classes, fixed, ws_bytes, budget, max_block_classes)
+            if cb <= 0:
+                if fixed <= 0:
+                    raise ValueError('linear SVM: D = {} features are too many for the fixed-order weight gradient even '
+                                     'with 16 classes per block'.format(D))
+                need = ws_bytes(min(16, num_classes))
+                raise MemoryError('linear SVM: N x D = {} x {} with {} classes needs {:.3g} GB of device memory for a '
+                                  'block of {} classes (X packed: {:.3g} GB); {:.3g} GB are available'.format(
+                                      N, D, num_classes, need / 1e9, min(16, num_classes), 4.0 * N * D / 1e9,
+                                      max(budget, 0) / 1e9) if need > 0 else
+                                  'linear SVM: N = {} rows are too many for the solver\'s workspace'.format(N))
+            ws = torch.empty(ws_bytes(cb), dtype=torch.uint8, device=x.device)
+        W = torch.empty((D, num_classes), dtype=torch.float32, device=x.device)
+        b = torch.empty(num_classes, dtype=torch.float32, device=x.device)
+        iters = torch.empty(num_classes, dtype=torch.int32, device=x.device)
+        gnorm = torch.empty(num_classes, dtype=torch.float32, device=x.device)
+        cg_steps = 0
+        if cb == num_classes and one_block:
+            _lib.call('se_linear_svm_fit', x.data_ptr(), x.stride(0), N, D, lab.data_ptr(), num_classes, float(C), float(tol),
+                      int(max_iter), W.data_ptr(), b.data_ptr(), iters.data_ptr(), gnorm.data_ptr(), ws.data_ptr(),
+                      _lib.stream_ptr())
+            cg_steps = int(lib.se_linear_svm_last_cg_steps())
+        else:
+            for c0 in range(0, num_classes, cb):
+                _lib.call('se_linear_svm_fit_classes', x.data_ptr(), x.stride(0), N, D, lab.data_ptr(), num_classes, c0, cb,
+                          float(C), float(tol), int(max_iter), W.data_ptr(), b.data_ptr(), iters.data_ptr(),
+                          gnorm.data_ptr(), ws.data_ptr(), int(c0 > 0), _lib.stream_ptr())
+                cg_steps += int(lib.se_linear_svm_last_cg_steps())
+    if info is not None:
+        info.update(classes_per_block=cb, blocks=-(-num_classes // cb), workspace_bytes=ws.numel(), cg_steps=cg_steps)
     return W, b, iters, gnorm
 
 
@@ -116,19 +177,30 @@ def _rank_ascending(scores, k):
     return idx.cpu().numpy()
 
 
+# Each se_dense_fwd call of the rankings takes fewer than this many elements of the test features and of the scores
+_GEMM_ELEMS = 1 << 31
+
+
 def svm_decision_ranks(X_test, W, b, k=5):
-    """The first k classes of decision_function(X_test).argsort(-1)[:, ::-1], ties by lower class index."""
+    """The first k classes of decision_function(X_test).argsort(-1)[:, ::-1], ties by lower class index.  Test sets whose
+    features or scores reach 2^31 elements are scored in row blocks (each row's scores are computed alike)."""
     x = _device_matrix(X_test, W.device)
     nW, nb = _scale(W.clone(), _lib.SE_SCALE_MUL, scale=-1.0), _scale(b.clone()[None], _lib.SE_SCALE_MUL, scale=-1.0)[0]
-    return _rank_ascending(_dense(x, nW, nb), min(k, W.shape[1]))
+    k = min(k, W.shape[1])
+    wide = max(x.shape[1], W.shape[1])
+    if x.shape[0] * wide < _GEMM_ELEMS:
+        return _rank_ascending(_dense(x, nW, nb), k)
+    rows = (_GEMM_ELEMS - 1) // wide // 64 * 64
+    return np.concatenate([_rank_ascending(_dense(x[r:r + rows], nW, nb), k) for r in range(0, x.shape[0], rows)])
 
 
-def svm_predict(X_train, labels_train, X_test, num_classes, normalize=False, C=0.1, k=5, tol=1e-4, max_iter=1000):
+def svm_predict(X_train, labels_train, X_test, num_classes, normalize=False, C=0.1, k=5, tol=1e-4, max_iter=1000,
+                max_block_classes=None):
     """train_and_predict (:20-48) on extracted features: scaling, the one-vs-rest fit, the ranking of the test rows.
     Returns (ranks [n_test, min(k, C)] int32, the fit's iters and gnorm as numpy arrays)."""
     check_training_labels(labels_train, num_classes)
     xtr, xte = scale_features(X_train, X_test, normalize)
-    W, b, iters, gnorm = linear_svm_fit(xtr, labels_train, num_classes, C, tol, max_iter)
+    W, b, iters, gnorm = linear_svm_fit(xtr, labels_train, num_classes, C, tol, max_iter, max_block_classes)
     return svm_decision_ranks(xte, W, b, k), iters.cpu().numpy(), gnorm.cpu().numpy()
 
 

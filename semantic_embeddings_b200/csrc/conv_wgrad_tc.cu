@@ -563,8 +563,16 @@ bool wgrad_config(const se_conv_desc* d, int x3, int sms, ConvPlan* pl) {
   return true;
 }
 
-// se_linear_svm_fit: does the tensor-core kernel take this shape on stream `st` and add its split-K slices in a fixed
-// order, i.e. do its slices fit a workspace that exists or can be allocated now?
+// se_linear_svm_fit: does the tensor-core kernel take this shape and are its split-K slices small enough for the
+// workspace, so that they are added in a fixed order?  (Host only: no device is needed.)
+bool conv_wgrad_tc_fixed_order_shape(const se_conv_desc* d) {
+  ConvPlan pl;
+  if (conv_plan(d, 2, SE_MODE_TF32X3, ConvCall(), &pl) != CONV_TC_WGRAD) return false;
+  const long long T = (long long)d->kh * d->kw * d->Cin * d->Cout;
+  return pl.splits * (T + d->Cout) <= WG_WS_FLOATS;
+}
+
+// ... and does that workspace exist on stream `st` or can it be allocated now?
 bool conv_wgrad_tc_fixed_order(const se_conv_desc* d, cudaStream_t st) {
   ConvPlan pl;
   if (conv_plan(d, 2, SE_MODE_TF32X3, ConvCall(), &pl) != CONV_TC_WGRAD) return false;

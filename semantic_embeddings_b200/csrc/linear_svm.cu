@@ -12,6 +12,15 @@
 // order.  No float atomics anywhere, and the weight gradient is only run where it adds its split-K slices in a fixed
 // order: reruns give the same bits.
 //
+// Large problems: each GEMM call takes fewer than 2^31 elements of X, S and R.  Where N x D or N x C reaches 2^31, the
+// rows are cut into equal blocks of rb rows (Np padded to a whole number of blocks with zero rows): S = X W + b runs
+// block by block (column-wise, so the blocks do not change its arithmetic), and X^T R adds the blocks' sums into one
+// accumulator in block order (each block's split-K slices in their own fixed order), so reruns still give the same bits.
+// Problems below that size run as one block, the calls they always made.  se_linear_svm_fit_classes solves the classes
+// [c0, c0 + cb) of a C-class problem: class c's problem depends only on which labels equal c, so a problem whose (D+1) x C
+// weight gradient or state matrices are too large is solved block of classes after block of classes, with the packed X
+// kept in the workspace between the blocks.
+//
 // se_scale_features: the feature normalisation of evaluate_classification_accuracy.py:33-38 with numpy's float32 results
 // bit for bit (row norms summed in numpy's pairwise order, true division), and the negation of score matrices that lets
 // se_row_topk (ascending) rank in descending order.
@@ -24,6 +33,7 @@
 namespace se {
 
 bool conv_wgrad_tc_fixed_order(const se_conv_desc* d, cudaStream_t st);   // conv_wgrad_tc.cu
+bool conv_wgrad_tc_fixed_order_shape(const se_conv_desc* d);
 
 namespace {
 
@@ -42,6 +52,7 @@ struct SvmClass {
 struct SvmDims {
   int N, Np, Dp, P, C, Cp, nrb, max_cg;
   float penalty;
+  int c0;                                   // class c of the state matrices is label c0 + c
 };
 
 // fixed-order sum over the 32 warps of one value per (warp, lane): result valid in warp 0
@@ -67,13 +78,15 @@ __global__ void __launch_bounds__(256) svm_pack_kernel(const float* __restrict__
   }
 }
 
-// counts[c] = rows with label c; bad = 1 when a label lies outside [0, C).  Integer atomics: exact in any order.
-__global__ void __launch_bounds__(256) svm_count_kernel(const int32_t* __restrict__ labels, int N, int C, int* counts, int* bad) {
+// counts[c] = rows with label c0 + c for c < nc; bad = 1 when a label lies outside [0, C).  Integer atomics: exact in
+// any order.
+__global__ void __launch_bounds__(256) svm_count_kernel(const int32_t* __restrict__ labels, int N, int C, int c0, int nc,
+                                                        int* counts, int* bad) {
   pdl_grid_sync();
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < N; i += gridDim.x * blockDim.x) {
     const int y = labels[i];
     if (y < 0 || y >= C) atomicOr(bad, 1);
-    else atomicAdd(&counts[y], 1);
+    else if (y >= c0 && y - c0 < nc) atomicAdd(&counts[y - c0], 1);
   }
 }
 
@@ -113,7 +126,7 @@ __global__ void __launch_bounds__(HB_THREADS) svm_hinge_kernel(float* __restrict
       if (take) { s = S_new[o]; S[o] = s; }
       float r = 0.f;
       if (i < dm.N && c < dm.C) {
-        const float y = labels[i] == c ? 1.f : -1.f;
+        const float y = labels[i] == dm.c0 + c ? 1.f : -1.f;
         const float m = 1.f - y * s;
         if (m > 0.f) {
           acc += (double)m * (double)m;
@@ -145,7 +158,7 @@ __global__ void __launch_bounds__(256) svm_hess_mask_kernel(float* __restrict__ 
     const int c = (int)(e - i * dm.Cp);
     float v = 0.f;
     if (i < dm.N && c < dm.C) {
-      const float y = labels[i] == c ? 1.f : -1.f;
+      const float y = labels[i] == dm.c0 + c ? 1.f : -1.f;
       if (1.f - y * S[e] > 0.f) v = 2.f * dm.penalty * T[e];
     }
     T[e] = v;
@@ -396,8 +409,9 @@ __global__ void __launch_bounds__(SV_THREADS) svm_tr_kernel(const float* __restr
     }
 }
 
+// W [D, ldw], b, iters, gnorm: columns c0 .. c0 + C - 1
 __global__ void __launch_bounds__(256) svm_out_kernel(const float* __restrict__ Wv, const SvmClass* __restrict__ st, SvmDims dm,
-                                                      int D, float* __restrict__ W, float* __restrict__ b,
+                                                      int D, int ldw, float* __restrict__ W, float* __restrict__ b,
                                                       int32_t* __restrict__ iters, float* __restrict__ gnorm) {
   pdl_grid_sync();
   const long long n = (long long)D * dm.C;
@@ -405,12 +419,12 @@ __global__ void __launch_bounds__(256) svm_out_kernel(const float* __restrict__ 
     if (e < n) {
       const long long j = e / dm.C;
       const int c = (int)(e - j * dm.C);
-      W[e] = Wv[j * dm.Cp + c];
+      W[j * ldw + dm.c0 + c] = Wv[j * dm.Cp + c];
     } else {
-      const int c = (int)(e - n);
-      if (b) b[c] = Wv[(long long)dm.Dp * dm.Cp + c];
-      if (iters) iters[c] = st[c].iters;
-      if (gnorm) gnorm[c] = st[c].gnorm0 > 0.0 ? (float)(st[c].gnorm / st[c].gnorm0) : 0.f;
+      const int c = (int)(e - n), o = dm.c0 + c;
+      if (b) b[o] = Wv[(long long)dm.Dp * dm.Cp + c];
+      if (iters) iters[o] = st[c].iters;
+      if (gnorm) gnorm[o] = st[c].gnorm0 > 0.0 ? (float)(st[c].gnorm / st[c].gnorm0) : 0.f;
     }
   }
 }
@@ -507,20 +521,40 @@ __global__ void __launch_bounds__(256) scale_cols_kernel(const float* x, long lo
 
 inline long long align_up(long long v, long long a) { return (v + a - 1) / a * a; }
 
+// Every GEMM call of the solver takes fewer than this many elements of X (rows x Dp) and of S / R (rows x Cp)
+constexpr long long SV_GEMM_ELEMS = 1LL << 31;
+
 struct SvmLayout {
   SvmDims dm;
+  int rb, nblk;                                  // GEMM row blocks: nblk blocks of rb rows, Np = rb nblk
+  bool ok;                                       // false: Np does not fit an int (no workspace)
   long long off_xp, off_scur, off_strial, off_r, off_vec[7], off_partial, off_state, off_counts, off_ctr, total;
 };
 
 SvmLayout svm_layout(int N, int D, int C) {
   SvmLayout L = {};
   SvmDims& d = L.dm;
+  if (D > 0x7fffffff - 3 || C > 0x7fffffff - 15) return L;     // Dp, Cp must fit an int
   d.N = N;
-  d.Np = std::max(N, 32);                             // the tensor-core weight gradient wants >= 32 rows
   d.Dp = (int)align_up(D, 4);                    // float4 rows of X
   d.P = d.Dp + 1;
   d.C = C;
   d.Cp = (int)align_up(C, 16);                   // output-channel tiles of the weight gradient
+  long long np = std::max(N, 32);                // the tensor-core weight gradient wants >= 32 rows
+  const long long wide = std::max(d.Dp, d.Cp);
+  L.nblk = 1;
+  if (np * wide >= SV_GEMM_ELEMS) {              // equal blocks of whole hinge-pass row blocks
+    const long long rb_max = (SV_GEMM_ELEMS - 1) / wide / HB_ROWS * HB_ROWS;
+    L.ok = rb_max >= HB_ROWS;
+    if (!L.ok) return L;
+    const long long nblk = (np + rb_max - 1) / rb_max, rb = align_up((np + nblk - 1) / nblk, HB_ROWS);
+    L.nblk = (int)nblk;
+    np = rb * nblk;
+  }
+  L.ok = np <= 0x7fffffffLL - HB_ROWS;
+  if (!L.ok) return L;
+  d.Np = (int)np;
+  L.rb = (int)(np / L.nblk);
   d.nrb = (d.Np + HB_ROWS - 1) / HB_ROWS;
   d.max_cg = 2 * d.P;
   long long o = 0;
@@ -538,38 +572,36 @@ SvmLayout svm_layout(int N, int D, int C) {
   return L;
 }
 
+// Hessian products (CG steps, all classes together) of the last fit on the calling thread
+thread_local long long g_last_cg_steps = 0;
+
 int grid_for(long long n, int threads) { return (int)std::min<long long>(std::max<long long>(1, (n + threads - 1) / threads), 8LL * sm_count()); }
 
-}  // namespace
-}  // namespace se
+se_conv_desc gemm_desc(const SvmLayout& L) { return {L.rb, 1, 1, L.dm.Dp, L.dm.Cp, 1, 1, 1, 0, 0, 1, 1}; }
 
-using namespace se;
-
-extern "C" int64_t se_linear_svm_workspace_bytes(int N, int D, int C) {
-  if (N <= 0 || D <= 0 || C <= 0) return 0;
-  return svm_layout(N, D, C).total;
-}
-
-extern "C" int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, const int32_t* labels, int C, float penalty, float tol,
-                                 int max_iter, float* W, float* b, int32_t* iters, float* gnorm, void* workspace, void* stream) {
-  SE_REQUIRE(X && labels && W && workspace, "null pointer");
-  SE_REQUIRE(N > 0 && D > 0 && C > 0 && ldx >= D, "N, D, C > 0 and ldx >= D");
-  SE_REQUIRE(penalty > 0.f && tol > 0.f && max_iter > 0, "penalty > 0, tol > 0, max_iter > 0");
-  SE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
-  const SvmLayout L = svm_layout(N, D, C);
+// The solver on the workspace of layout L (whose dm.C real classes are labels c0 .. c0 + dm.C - 1 of a Ctot-class problem).
+// X is packed into the workspace unless `packed` (an earlier call on the same workspace packed the same X).  Outputs are
+// columns c0 .. of W [D, Ctot], b, iters, gnorm.
+int svm_fit(const char* who, const SvmLayout& L, const float* X, long long ldx, int N, int D, const int32_t* labels, int Ctot,
+            int c0, float penalty, float tol, int max_iter, float* W, float* b, int32_t* iters, float* gnorm, void* workspace,
+            int packed, void* stream) {
   SvmDims dm = L.dm;
   dm.penalty = penalty;
-  SE_REQUIRE((long long)dm.Np * dm.Cp < (1LL << 31) && (long long)dm.Np * dm.Dp < (1LL << 31), "N x D and N x C must stay below 2^31");
+  dm.c0 = c0;
+  // the gradient / Hessian sums X^T R must add their split-K slices in a fixed order (no float atomics)
+  se_conv_desc gd = gemm_desc(L);
+  if (!conv_wgrad_tc_fixed_order_shape(&gd)) {
+    se::set_error("%s: (D+1) x C = %d x %d does not fit the fixed-order weight-gradient workspace", who, dm.Dp, dm.Cp);
+    return SE_ERR_UNSUPPORTED;
+  }
   cudaStream_t st = as_stream(stream);
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   if (cudaStreamIsCapturing(st, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) {
-    se::set_error("se_linear_svm_fit: the solver synchronises with its stream and cannot be captured");
+    se::set_error("%s: the solver synchronises with its stream and cannot be captured", who);
     return SE_ERR_ARG;
   }
-  // the gradient / Hessian sums X^T R must add their split-K slices in a fixed order (no float atomics)
-  se_conv_desc gd = {dm.Np, 1, 1, dm.Dp, dm.Cp, 1, 1, 1, 0, 0, 1, 1};
   if (!conv_wgrad_tc_fixed_order(&gd, st)) {
-    se::set_error("se_linear_svm_fit: (D+1) x C = %d x %d does not fit the fixed-order weight-gradient workspace", dm.Dp, dm.Cp);
+    se::set_error("%s: (D+1) x C = %d x %d does not fit the fixed-order weight-gradient workspace", who, dm.Dp, dm.Cp);
     return SE_ERR_UNSUPPORTED;
   }
   char* ws = static_cast<char*>(workspace);
@@ -591,6 +623,7 @@ extern "C" int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, cons
   int* ctr = reinterpret_cast<int*>(ws + L.off_ctr);
   const long long vec_bytes = (long long)dm.P * dm.Cp * 4;
   const long long wdw = (long long)dm.Dp * dm.Cp;               // intercept row offset
+  const long long xblk = (long long)L.rb * dm.Dp, sblk = (long long)L.rb * dm.Cp;
   const int cls_blocks = (dm.Cp + SV_COLS - 1) / SV_COLS;
   int rc = SE_OK;
 #define SV_CHECK(call)           \
@@ -600,31 +633,46 @@ extern "C" int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, cons
 #define SV_CUDA(call, what)                                                   \
   do {                                                                        \
     cudaError_t e_ = (call);                                                  \
-    if (e_ != cudaSuccess) { se::set_error("%s: %s", what, cudaGetErrorString(e_)); return SE_ERR_CUDA; } \
+    if (e_ != cudaSuccess) { se::set_error("%s: %s: %s", who, what, cudaGetErrorString(e_)); return SE_ERR_CUDA; } \
   } while (0)
 
-  // gradient sums: XtR = X^T R (rows < Dp), column sums of R (intercept row)
+  // scores: S = X Wm + bm, row block by row block
+  auto x_w = [&](const float* Wm, float* S) -> int {
+    for (int k = 0; k < L.nblk; ++k) {
+      const int r = se_dense_fwd(xp + k * xblk, Wm, Wm + wdw, S + k * sblk, L.rb, dm.Dp, dm.Cp, 0, nullptr, SE_MODE_TF32X3, stream);
+      if (r != SE_OK) return r;
+    }
+    return SE_OK;
+  };
+  // gradient sums: XtR = X^T R (rows < Dp), column sums of R (intercept row); the row blocks add into XtR in order
   auto xt_r = [&](const float* Rm) -> int {
-    if (cudaMemsetAsync(XtR, 0, vec_bytes, st) != cudaSuccess) { se::set_error("se_linear_svm_fit: memset"); return SE_ERR_CUDA; }
-    return se_dense_bwd(xp, nullptr, Rm, nullptr, 0.f, XtR, XtR + wdw, dm.Np, dm.Dp, dm.Cp, SE_MODE_TF32X3, stream);
+    if (cudaMemsetAsync(XtR, 0, vec_bytes, st) != cudaSuccess) { se::set_error("%s: memset", who); return SE_ERR_CUDA; }
+    for (int k = 0; k < L.nblk; ++k) {
+      const int r = se_dense_bwd(xp + k * xblk, nullptr, Rm + k * sblk, nullptr, 0.f, XtR, XtR + wdw, L.rb, dm.Dp, dm.Cp,
+                                 SE_MODE_TF32X3, stream);
+      if (r != SE_OK) return r;
+    }
+    return SE_OK;
   };
   auto read_counters = [&](int* host) -> int {
-    SV_CUDA(cudaMemcpyAsync(host, ctr, 2 * sizeof(int), cudaMemcpyDeviceToHost, st), "se_linear_svm_fit: counters");
-    SV_CUDA(cudaStreamSynchronize(st), "se_linear_svm_fit");
+    SV_CUDA(cudaMemcpyAsync(host, ctr, 2 * sizeof(int), cudaMemcpyDeviceToHost, st), "counters");
+    SV_CUDA(cudaStreamSynchronize(st), "synchronise");
     return SE_OK;
   };
 
-  SV_CUDA(cudaMemsetAsync(counts, 0, (size_t)dm.Cp * 4 + 4, st), "se_linear_svm_fit: memset");
-  for (int k = 0; k < 7; ++k) SV_CUDA(cudaMemsetAsync(ws + L.off_vec[k], 0, vec_bytes, st), "se_linear_svm_fit: memset");
-  SV_CUDA(cudaMemsetAsync(s_cur, 0, (size_t)dm.Np * dm.Cp * 4, st), "se_linear_svm_fit: memset");
-  launch(svm_pack_kernel, dim3(grid_for((long long)dm.Np * dm.Dp, 256)), dim3(256), 0, st, X, (long long)ldx, N, D, dm.Np, dm.Dp, xp);
-  SV_CHECK(check_launch("svm_pack_kernel"));
-  launch(svm_count_kernel, dim3(grid_for(N, 256)), dim3(256), 0, st, labels, N, C, counts, bad);
+  SV_CUDA(cudaMemsetAsync(counts, 0, (size_t)dm.Cp * 4 + 4, st), "memset");
+  for (int k = 0; k < 7; ++k) SV_CUDA(cudaMemsetAsync(ws + L.off_vec[k], 0, vec_bytes, st), "memset");
+  SV_CUDA(cudaMemsetAsync(s_cur, 0, (size_t)dm.Np * dm.Cp * 4, st), "memset");
+  if (!packed) {
+    launch(svm_pack_kernel, dim3(grid_for((long long)dm.Np * dm.Dp, 256)), dim3(256), 0, st, X, ldx, N, D, dm.Np, dm.Dp, xp);
+    SV_CHECK(check_launch("svm_pack_kernel"));
+  }
+  launch(svm_count_kernel, dim3(grid_for(N, 256)), dim3(256), 0, st, labels, N, Ctot, c0, dm.C, counts, bad);
   SV_CHECK(check_launch("svm_count_kernel"));
   int host_bad = 0;
-  SV_CUDA(cudaMemcpyAsync(&host_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st), "se_linear_svm_fit: labels");
-  SV_CUDA(cudaStreamSynchronize(st), "se_linear_svm_fit");
-  if (host_bad) { se::set_error("se_linear_svm_fit: a label lies outside [0, C)"); return SE_ERR_ARG; }
+  SV_CUDA(cudaMemcpyAsync(&host_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st), "labels");
+  SV_CUDA(cudaStreamSynchronize(st), "synchronise");
+  if (host_bad) { se::set_error("%s: a label lies outside [0, C)", who); return SE_ERR_ARG; }
   launch(svm_init_kernel, dim3((dm.Cp + 255) / 256), dim3(256), 0, st, state, (const int*)counts, dm, tol);
   SV_CHECK(check_launch("svm_init_kernel"));
 
@@ -634,8 +682,10 @@ extern "C" int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, cons
   SV_CHECK(check_launch("svm_hinge_kernel"));
   SV_CHECK(xt_r(R));
   int host[2] = {0, 0};
+  long long cg_steps = 0;
+  g_last_cg_steps = 0;
   for (;;) {
-    SV_CUDA(cudaMemsetAsync(ctr, 0, 16, st), "se_linear_svm_fit: memset");
+    SV_CUDA(cudaMemsetAsync(ctr, 0, 16, st), "memset");
     launch(svm_newton_kernel, dim3(cls_blocks), dim3(SV_THREADS), 0, st, (const float*)Wv, (const float*)XtR, G, Sv, Rv, Dv, state,
            (const double*)partial, dm, max_iter, ctr);
     SV_CHECK(check_launch("svm_newton_kernel"));
@@ -643,11 +693,12 @@ extern "C" int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, cons
     if (host[0] == 0) break;
     // conjugate gradient on H s = -g inside the trust region, one Hessian product per step for all classes
     while (host[1] > 0) {
-      SV_CHECK(se_dense_fwd(xp, Dv, Dv + wdw, R, dm.Np, dm.Dp, dm.Cp, 0, nullptr, SE_MODE_TF32X3, stream));
+      ++cg_steps;
+      SV_CHECK(x_w(Dv, R));
       launch(svm_hess_mask_kernel, dim3(grid_for((long long)dm.Np * dm.Cp, 256)), dim3(256), 0, st, R, (const float*)s_cur, labels, dm);
       SV_CHECK(check_launch("svm_hess_mask_kernel"));
       SV_CHECK(xt_r(R));
-      SV_CUDA(cudaMemsetAsync(ctr, 0, 16, st), "se_linear_svm_fit: memset");
+      SV_CUDA(cudaMemsetAsync(ctr, 0, 16, st), "memset");
       launch(svm_cg_kernel, dim3(cls_blocks), dim3(SV_THREADS), 0, st, (const float*)XtR, Sv, Rv, Dv, state, dm, ctr);
       SV_CHECK(check_launch("svm_cg_kernel"));
       SV_CHECK(read_counters(host));
@@ -656,7 +707,7 @@ extern "C" int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, cons
     launch(svm_trial_kernel, dim3(cls_blocks), dim3(SV_THREADS), 0, st, (const float*)Wv, (const float*)G, (const float*)Sv,
            (const float*)Rv, Wt, state, dm);
     SV_CHECK(check_launch("svm_trial_kernel"));
-    SV_CHECK(se_dense_fwd(xp, Wt, Wt + wdw, s_trial, dm.Np, dm.Dp, dm.Cp, 0, nullptr, SE_MODE_TF32X3, stream));
+    SV_CHECK(x_w(Wt, s_trial));
     launch(svm_hinge_kernel, dim3(dm.nrb), dim3(HB_THREADS), 0, st, s_trial, (const float*)nullptr, (const SvmClass*)state, labels, dm,
            (float*)nullptr, partial);
     SV_CHECK(check_launch("svm_hinge_kernel"));
@@ -667,13 +718,70 @@ extern "C" int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, cons
     SV_CHECK(check_launch("svm_hinge_kernel"));
     SV_CHECK(xt_r(R));
   }
-  launch(svm_out_kernel, dim3(grid_for((long long)D * C + C, 256)), dim3(256), 0, st, (const float*)Wv, (const SvmClass*)state, dm, D,
-         W, b, iters, gnorm);
+  launch(svm_out_kernel, dim3(grid_for((long long)D * dm.C + dm.C, 256)), dim3(256), 0, st, (const float*)Wv, (const SvmClass*)state,
+         dm, D, Ctot, W, b, iters, gnorm);
   SV_CHECK(check_launch("svm_out_kernel"));
-  SV_CUDA(cudaStreamSynchronize(st), "se_linear_svm_fit");
+  SV_CUDA(cudaStreamSynchronize(st), "synchronise");
+  g_last_cg_steps = cg_steps;
 #undef SV_CHECK
 #undef SV_CUDA
   return SE_OK;
+}
+
+}  // namespace
+}  // namespace se
+
+using namespace se;
+
+extern "C" int64_t se_linear_svm_workspace_bytes(int N, int D, int C) {
+  if (N <= 0 || D <= 0 || C <= 0) return 0;
+  const SvmLayout L = svm_layout(N, D, C);
+  return L.ok ? L.total : 0;
+}
+
+extern "C" int64_t se_linear_svm_last_cg_steps(void) { return g_last_cg_steps; }
+
+extern "C" int64_t se_linear_svm_classes_workspace_bytes(int N, int D, int cb) { return se_linear_svm_workspace_bytes(N, D, cb); }
+
+extern "C" int se_linear_svm_block_classes(int N, int D, int C) {
+  if (N <= 0 || D <= 0 || C <= 0) return 0;
+  for (int cb = (int)align_up(C, 16); cb > 0; cb -= 16) {
+    const SvmLayout L = svm_layout(N, D, cb);
+    if (!L.ok) continue;
+    se_conv_desc gd = gemm_desc(L);
+    if (conv_wgrad_tc_fixed_order_shape(&gd)) return std::min(cb, C);
+  }
+  return 0;
+}
+
+extern "C" int se_linear_svm_fit(const float* X, int64_t ldx, int N, int D, const int32_t* labels, int C, float penalty, float tol,
+                                 int max_iter, float* W, float* b, int32_t* iters, float* gnorm, void* workspace, void* stream) {
+  SE_REQUIRE(X && labels && W && workspace, "null pointer");
+  SE_REQUIRE(N > 0 && D > 0 && C > 0 && ldx >= D, "N, D, C > 0 and ldx >= D");
+  SE_REQUIRE(penalty > 0.f && tol > 0.f && max_iter > 0, "penalty > 0, tol > 0, max_iter > 0");
+  SE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
+  const SvmLayout L = svm_layout(N, D, C);
+  SE_REQUIRE(L.ok, "N rows padded to whole GEMM row blocks must stay below 2^31");
+  return svm_fit("se_linear_svm_fit", L, X, ldx, N, D, labels, C, 0, penalty, tol, max_iter, W, b, iters, gnorm, workspace, 0, stream);
+}
+
+extern "C" int se_linear_svm_fit_classes(const float* X, int64_t ldx, int N, int D, const int32_t* labels, int C, int c0, int cb,
+                                         float penalty, float tol, int max_iter, float* W, float* b, int32_t* iters, float* gnorm,
+                                         void* workspace, int packed, void* stream) {
+  SE_REQUIRE(labels && W && workspace && (X || packed), "null pointer");
+  SE_REQUIRE(N > 0 && D > 0 && C > 0 && (packed || ldx >= D), "N, D, C > 0 and ldx >= D");
+  if (c0 < 0 || c0 >= C || cb <= 0 || cb > C) {
+    se::set_error("se_linear_svm_fit_classes: requirement failed: 0 <= c0 < C and 0 < cb <= C (c0 = %d, cb = %d, C = %d)", c0, cb,
+                  C);
+    return SE_ERR_ARG;
+  }
+  SE_REQUIRE(penalty > 0.f && tol > 0.f && max_iter > 0, "penalty > 0, tol > 0, max_iter > 0");
+  SE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
+  SvmLayout L = svm_layout(N, D, cb);
+  SE_REQUIRE(L.ok, "N rows padded to whole GEMM row blocks must stay below 2^31");
+  L.dm.C = std::min(cb, C - c0);                // the last block may be narrower: its other columns are padding
+  return svm_fit("se_linear_svm_fit_classes", L, X, ldx, N, D, labels, C, c0, penalty, tol, max_iter, W, b, iters, gnorm, workspace,
+                 packed, stream);
 }
 
 extern "C" int se_scale_features(const float* x, int64_t ldx, int rows, int D, int op, float* colmax, float scale, float* y,
