@@ -15,9 +15,10 @@
  *     never allocates or frees device memory.  Kernels that need scratch take it explicitly.
  *   - `stream` is a cudaStream_t; all calls are asynchronous w.r.t. the host and capturable
  *     into a CUDA graph.
- *   - process-wide state is limited to what se_init() / se_comm_init() create: the low-priority
- *     side stream and the fork/join events se_run_ops uses for weight gradients, and the NCCL
- *     communicator with its stream and event.  Kernels keep no state between calls.
+ *   - process-wide state is limited to what se_init() / se_comm_init() / se_runner_create() create:
+ *     the plan runners (each a low-priority side stream for weight gradients, its fork/join
+ *     events and its split-K workspace), and the NCCL communicator with its stream and event.
+ *     Kernels keep no state between calls.
  *   - activations are float32 NHWC; conv kernels are float32 HWIO (Keras layout); dense
  *     kernels are (in,out).  `mode` selects the arithmetic of contraction kernels:
  *     SE_MODE_F32 = fp32 FFMA; SE_MODE_TF32 = TF32 wgmma (operands read with a
@@ -729,6 +730,23 @@ typedef struct {
   void* p[16];
 } se_op;
 int se_run_ops(const se_op* ops, int n, int mode, void* stream);
+/* Plan runners, for plans that run at the same time (CUDA graphs captured from them and replayed concurrently on
+ * different streams).  se_run_ops runs every plan on the library's default runner, whose side stream and split-K
+ * workspace all its plans share: two of its graphs replayed at once would write the same workspace.
+ *   se_runner_create:  a runner of its own: side stream, fork/join events and a split-K workspace of the default
+ *                      runner's size (so every split plan, and every result, is the same on any runner).  Everything is
+ *                      allocated here, never during a capture; call it outside captures.  SE_ERR_CUDA when no
+ *                      workspace can be had: the library keeps at most 32 (one per device and stream, the default
+ *                      runner's and those of eager se_conv2d_wgrad streams included).
+ *   se_runner_destroy: waits for the runner's side stream and frees it all.  No graph captured on the runner may be
+ *                      replayed afterwards.  NULL is accepted.
+ *   se_run_ops_runner: se_run_ops on `runner`.  The BatchNorm kernels with a grid-wide barrier are launched
+ *                      cooperatively, so that another plan's kernels cannot keep part of their grid off the GPU (same
+ *                      kernels, grids and bits).  SE_ERR_ARG for a plan with SE_OP_ALLREDUCE: the communication stream
+ *                      is process-wide. */
+int se_runner_create(void** runner);
+int se_runner_destroy(void* runner);
+int se_run_ops_runner(const se_op* ops, int n, int mode, void* stream, void* runner);
 /* profiling variant (bench.py): eager, a CUDA-event pair around every op, per-op device milliseconds */
 int se_run_ops_timed(const se_op* ops, int n, int mode, void* stream, float* ms_out);
 

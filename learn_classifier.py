@@ -88,6 +88,7 @@ def build_parser():
                    help='Do not display training progress, but just the final performance.')
     g.add_argument('--arith', type=str, default='tf32x3', choices=['tf32x3', 'f32', 'tf32'],
                    help='(new) arithmetic of the convolution kernels, see learn_image_embeddings.py')
+    trainer.add_lr_sweep_argument(g)
     utils.add_lr_schedule_arguments(parser)
     return parser
 
@@ -96,6 +97,7 @@ def main(argv=None):
     args = build_parser().parse_args(argv)
     if args.val_batch_size is None:
         args.val_batch_size = args.batch_size
+    sweep = trainer.lr_sweep_runs(args)
 
     from semantic_embeddings_b200.engine import Engine
     from semantic_embeddings_b200.parallel import broadcast_parameters
@@ -112,14 +114,22 @@ def main(argv=None):
     mode = trainer.arith_mode(args, say)
     callbacks, epochs, decay = trainer.schedule(args, data)        # learn_classifier.py:128,142-145
     pb = args.batch_size // world
-    eng = Engine(graph, pb, objective='softmax', label_smoothing=args.label_smoothing, num_classes=data.num_classes,
-                 mode=mode, device='cuda:%d' % local, nesterov=args.nesterov, clipnorm=args.clipgrad, world_size=world,
-                 decay=decay)
-    trainer.resume(eng, args.snapshot, say)
-    broadcast_parameters([eng.P, eng.S, eng.V, eng.lr_dev])
+
+    def make_engine(run, **kw):
+        return Engine(graph, pb, objective='softmax', label_smoothing=run.label_smoothing, num_classes=data.num_classes,
+                      mode=mode, device='cuda:%d' % local, nesterov=run.nesterov, clipnorm=run.clipgrad, world_size=world,
+                      decay=decay, **kw)
 
     ks = tuple(args.top_k_acc)
     rng = np.random.RandomState(1234)          # identical stream on every rank: the permutation is shared, slices differ
+    if sweep:
+        return trainer.lr_sweep(args, sweep, make_engine, graph.input.shape, data, 'cuda:%d' % local, rng, ks, say,
+                                lambda eng: {graph.output.producer.name},
+                                lambda eng, run, tag: final_evaluation(eng, run, graph, data, ks, say, 0, tag),
+                                'Pre-training last layer', train_ks=ks)
+    eng = make_engine(args)
+    trainer.resume(eng, args.snapshot, say)
+    broadcast_parameters([eng.P, eng.S, eng.V, eng.lr_dev])
 
     # Load pre-trained weights and train the last layer for a few epochs (learn_classifier.py:109-125)
     if args.finetune:
@@ -134,16 +144,22 @@ def main(argv=None):
             say('Full model training')
 
     trainer.fit(eng, data, args, callbacks[0], epochs, rng, rank, world, ks, say, train_ks=ks)
-
-    # Evaluate final performance (learn_classifier.py:157-163): evaluate_generator's [loss, acc, acc<k>...]
-    val, pred = trainer.run_validation(eng, data, ks, None)
-    if rank == 0:
-        say([val['loss'], val['acc']] + [val['acc%d' % k] for k in ks])
-        say('Average Accuracy: {:.4f}'.format(trainer.average_accuracy(pred, data.labels_test)))
-        trainer.dump_weights(eng, args)
-        if args.feature_dump:                                  # learn_classifier.py:178-182
-            trainer.dump_features(eng, data, utils.feature_layer(graph).name, args.feature_dump)
+    final_evaluation(eng, args, graph, data, ks, say, rank)
     return 0
+
+
+def final_evaluation(eng, args, graph, data, ks, say, rank=0, tag=''):
+    """Final performance (learn_classifier.py:157-163), evaluate_generator's [loss, acc, acc<k>...], on every rank;
+    rank 0 prints it and writes the weight, model and feature dumps."""
+    val, pred = trainer.run_validation(eng, data, ks, None)
+    if rank != 0:
+        return
+    scores = [val['loss'], val['acc']] + [val['acc%d' % k] for k in ks]
+    say(tag + str(scores) if tag else scores)
+    say(tag + 'Average Accuracy: {:.4f}'.format(trainer.average_accuracy(pred, data.labels_test)))
+    trainer.dump_weights(eng, args)
+    if args.feature_dump:                                  # learn_classifier.py:178-182
+        trainer.dump_features(eng, data, utils.feature_layer(graph).name, args.feature_dump)
 
 
 if __name__ == '__main__':

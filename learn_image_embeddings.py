@@ -78,6 +78,7 @@ def build_parser():
     g.add_argument('--top_k_acc', type=int, nargs='+', default=[])
     g.add_argument('--arith', type=str, default='tf32x3', choices=['tf32x3', 'f32', 'tf32'],
                    help='(new) arithmetic of the convolution kernels, see the module docstring')
+    trainer.add_lr_sweep_argument(g)
     utils.add_lr_schedule_arguments(parser)
     return parser
 
@@ -89,6 +90,7 @@ def main(argv=None):
     if args.cls_base is not None and args.cls_base.lstrip('-').isdigit():
         raise ValueError('--cls_base takes a layer NAME here (e.g. avg_pool): Keras layer indices count Activation / Add / '
                          'Lambda layers that this graph fuses into their producers')
+    sweep = trainer.lr_sweep_runs(args)
 
     from semantic_embeddings_b200.engine import Engine
     from semantic_embeddings_b200.parallel import broadcast_parameters
@@ -114,14 +116,22 @@ def main(argv=None):
     mode = trainer.arith_mode(args, say)
     callbacks, epochs, decay = trainer.schedule(args, data)        # learn_image_embeddings.py:224-227
     pb = args.batch_size // world
-    eng = Engine(graph, pb, embedding, loss=args.loss, cls_weight=args.cls_weight, num_classes=data.num_classes, mode=mode,
-                 device='cuda:%d' % local, nesterov=args.nesterov, clipnorm=args.clipgrad, world_size=world, decay=decay,
-                 cls_base=args.cls_base if args.cls_weight > 0 else None)
-    trainer.resume(eng, args.snapshot, say)
-    broadcast_parameters([eng.P, eng.S, eng.V, eng.lr_dev])
+
+    def make_engine(run, **kw):
+        return Engine(graph, pb, embedding, loss=run.loss, cls_weight=run.cls_weight, num_classes=data.num_classes,
+                      mode=mode, device='cuda:%d' % local, nesterov=run.nesterov, clipnorm=run.clipgrad, world_size=world,
+                      decay=decay, cls_base=run.cls_base if run.cls_weight > 0 else None, **kw)
 
     ks = tuple(args.top_k_acc)
     rng = np.random.RandomState(1234)          # identical stream on every rank: the permutation is shared, slices differ
+    if sweep:
+        return trainer.lr_sweep(args, sweep, make_engine, graph.input.shape, data, 'cuda:%d' % local, rng, ks, say,
+                                lambda eng: new_layers(graph, eng),
+                                lambda eng, run, tag: final_evaluation(eng, run, data, ks, say, 0, tag),
+                                'Pre-training new layers')
+    eng = make_engine(args)
+    trainer.resume(eng, args.snapshot, say)
+    broadcast_parameters([eng.P, eng.S, eng.V, eng.lr_dev])
 
     # Load pre-trained weights and train the new layers for a few epochs (learn_image_embeddings.py:183-207)
     if args.finetune:
@@ -131,27 +141,37 @@ def main(argv=None):
         broadcast_parameters([eng.P, eng.S])
         if args.finetune_init > 0:
             say('Pre-training new layers')
-            last = [n for n in graph.nodes if any(k.startswith(n.name + '/') for k in eng.offsets)][-1].name
-            new_layers = {'embedding', 'prob', last}      # :188-190 (the embedding model's last layer stays trainable)
             # this phase's optimizer: SGD(lr=sgd_lr) without decay (:192-199); the full-model phase compiles a new one
-            trainer.pretrain_new_layers(eng, data, args, new_layers, rng, rank, world, ks, say)
+            trainer.pretrain_new_layers(eng, data, args, new_layers(graph, eng), rng, rank, world, ks, say)
             say('Full model training')
 
     trainer.fit(eng, data, args, callbacks[0], epochs, rng, rank, world, ks, say)
-
-    # final performance (learn_image_embeddings.py:245-254)
-    val, pred = run_validation(eng, data, ks, True if args.embedding == 'onehot' else None)
-    if rank == 0:
-        order = ['total'] if 'total' in val else []
-        order += [k for k in ('loss', 'cls_loss', 'acc') if k in val] + sorted(k for k in val if k.startswith('acc') and k != 'acc')
-        order += [k for k in ('cls_acc',) if k in val] + sorted(k for k in val if k.startswith('cls_acc') and k != 'cls_acc')
-        say([val[k] for k in order])
-        if pred is not None and (args.cls_weight > 0 or args.embedding == 'onehot'):
-            say('Average Accuracy: {:.4f}'.format(trainer.average_accuracy(pred, data.labels_test)))
-        trainer.dump_weights(eng, args)
-        if args.feature_dump:                                  # learn_image_embeddings.py:270-275
-            trainer.dump_features(eng, data, 'head_out', args.feature_dump)
+    final_evaluation(eng, args, data, ks, say, rank)
     return 0
+
+
+def new_layers(graph, eng):
+    """The layers --finetune_init trains (learn_image_embeddings.py:188-190): the embedding model's last layer stays
+    trainable."""
+    last = [n for n in graph.nodes if any(k.startswith(n.name + '/') for k in eng.offsets)][-1].name
+    return {'embedding', 'prob', last}
+
+
+def final_evaluation(eng, args, data, ks, say, rank=0, tag=''):
+    """Final performance (learn_image_embeddings.py:245-254) on every rank; rank 0 prints it and writes the weight,
+    model and feature dumps."""
+    val, pred = run_validation(eng, data, ks, True if args.embedding == 'onehot' else None)
+    if rank != 0:
+        return
+    order = ['total'] if 'total' in val else []
+    order += [k for k in ('loss', 'cls_loss', 'acc') if k in val] + sorted(k for k in val if k.startswith('acc') and k != 'acc')
+    order += [k for k in ('cls_acc',) if k in val] + sorted(k for k in val if k.startswith('cls_acc') and k != 'cls_acc')
+    say(tag + str([val[k] for k in order]) if tag else [val[k] for k in order])
+    if pred is not None and (args.cls_weight > 0 or args.embedding == 'onehot'):
+        say(tag + 'Average Accuracy: {:.4f}'.format(trainer.average_accuracy(pred, data.labels_test)))
+    trainer.dump_weights(eng, args)
+    if args.feature_dump:                                  # learn_image_embeddings.py:270-275
+        trainer.dump_features(eng, data, 'head_out', args.feature_dump)
 
 
 if __name__ == '__main__':

@@ -208,6 +208,9 @@ _SIGS = {
     'se_embedding_deviation_f64': (c_int, [_P, c_int64, c_int, c_int, _P, c_int64, c_int, _P, _P, _P]),
     'se_run_ops': (c_int, [POINTER(Op), c_int, c_int, _P]),
     'se_run_ops_timed': (c_int, [POINTER(Op), c_int, c_int, _P, POINTER(c_float)]),
+    'se_runner_create': (c_int, [POINTER(_P)]),
+    'se_runner_destroy': (c_int, [_P]),
+    'se_run_ops_runner': (c_int, [POINTER(Op), c_int, c_int, _P, _P]),
 }
 
 _lib = None

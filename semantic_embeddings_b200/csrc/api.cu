@@ -22,9 +22,11 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
+// set while se_run_ops_runner issues a plan: its grid-barrier kernels are launched cooperatively (see there)
+static thread_local bool t_runner_plan = false;
 bool coop_enabled() {
   static const bool on = getenv("SE_BN_COOP") != nullptr;
-  return on;
+  return on || t_runner_plan;
 }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int sm_count() {
@@ -66,13 +68,49 @@ extern "C" int se_device_sm_count(void) { return sm_count(); }
 // multi-op plan issues them on a second, lowest-priority stream (see Streams below).  Inside a CUDA-graph capture this
 // becomes a parallel branch.  The backward-data / BatchNorm-backward chain and the wgrad kernels can share an SM (shared
 // memory, registers; see conv_tc.cu / conv_wgrad_tc.cu), so the side branch fills the latency bubbles of the main chain.
-static cudaStream_t g_side = nullptr;
-static cudaEvent_t g_ev_fork = nullptr, g_ev_join = nullptr;
+// A plan runner owns that side stream, its fork / join events and, through the side stream, a weight-gradient workspace
+// (wgrad_workspace is keyed by stream).  se_run_ops runs on the default runner that se_init creates; se_runner_create
+// makes one more for every plan that runs at the same time as another (see se_run_ops_runner).
+struct se_runner {
+  cudaStream_t side = nullptr;
+  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+};
+static se_runner g_default_runner;
 
 namespace se {
 int init_conv_simt(); int init_pairwise_tc(); int init_conv_tc(); int init_conv_wgrad_tc(); int init_head();
 int init_bn_bwd(); int init_row_topk(); int init_resample_crop();
 int wgrad_workspace_prepare(cudaStream_t st);
+void wgrad_workspace_release(cudaStream_t st);
+
+static void runner_free(se_runner* r) {
+  if (r->side) {
+    cudaStreamSynchronize(r->side);
+    wgrad_workspace_release(r->side);
+    cudaStreamDestroy(r->side);
+  }
+  if (r->ev_fork) cudaEventDestroy(r->ev_fork);
+  if (r->ev_join) cudaEventDestroy(r->ev_join);
+  *r = se_runner();
+}
+
+// the side stream (lowest priority), its events and its weight-gradient workspace: all allocated here, never inside a
+// capture
+static int runner_init(se_runner* r) {
+  int lo = 0, hi = 0;
+  cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&r->side, cudaStreamNonBlocking, lo);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&r->ev_fork, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&r->ev_join, cudaEventDisableTiming);
+  if (e != cudaSuccess) {
+    set_error("cannot create the side stream of a plan runner: %s", cudaGetErrorString(e));
+    runner_free(r);
+    return SE_ERR_CUDA;
+  }
+  const int rc = wgrad_workspace_prepare(r->side);
+  if (rc) runner_free(r);
+  return rc;
+}
 
 static int setup() {
   sm_count();
@@ -81,16 +119,7 @@ static int setup() {
     const int rc = init();
     if (rc) return rc;
   }
-  int lo = 0, hi = 0;
-  cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
-  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&g_side, cudaStreamNonBlocking, lo);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g_ev_fork, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g_ev_join, cudaEventDisableTiming);
-  if (e != cudaSuccess) {
-    set_error("se_init: cannot create the side stream of se_run_ops: %s", cudaGetErrorString(e));
-    return SE_ERR_CUDA;
-  }
-  return wgrad_workspace_prepare(g_side);
+  return runner_init(&g_default_runner);
 }
 
 int ensure_setup() {
@@ -350,26 +379,27 @@ static void wait_for(cudaStream_t waiter, cudaStream_t st, cudaEvent_t ev) {
 //   - the end of the call joins everything, on every path (an unjoined fork would invalidate an ongoing capture).
 struct Streams {
   cudaStream_t main;
-  bool use_side;              // a multi-op plan
+  const se_runner* r;
+  bool use_side;              // a multi-op plan, or any plan of a runner of its own
   bool side_open = false;     // side-stream work not yet joined
   bool transposing = false;   // ... and it is the filter transposition
   bool comm_pending = false;  // all-reduces not yet joined
 
   cudaStream_t fork_side() {
     if (!use_side) return main;
-    wait_for(g_side, main, g_ev_fork);
+    wait_for(r->side, main, r->ev_fork);
     side_open = true;
-    return g_side;
+    return r->side;
   }
   void join_side() {
     if (!side_open) return;
-    wait_for(main, g_side, g_ev_join);
+    wait_for(main, r->side, r->ev_join);
     side_open = transposing = false;
   }
   cudaStream_t fork_comm() {
     const cudaStream_t cs = comm_stream();
     wait_for(cs, main, comm_event());
-    if (side_open) wait_for(cs, g_side, comm_event());
+    if (side_open) wait_for(cs, r->side, comm_event());
     comm_pending = true;
     return cs;
   }
@@ -393,8 +423,58 @@ extern "C" int se_run_ops(const se_op* ops, int n, int mode, void* stream) {
   SE_REQUIRE(ops && n >= 0, "bad arguments");
   int rc = ensure_setup();
   if (rc) return rc;
-  Streams st{as_stream(stream), n > 1};
+  Streams st{as_stream(stream), &g_default_runner, n > 1};
   rc = run_ops_impl(ops, n, mode, stream, st);
+  st.join_all();
+  return rc;
+}
+
+extern "C" int se_runner_create(void** runner) {
+  SE_REQUIRE(runner, "null pointer");
+  *runner = nullptr;
+  int rc = ensure_setup();
+  if (rc) return rc;
+  se_runner* r = new se_runner();
+  if ((rc = runner_init(r))) {
+    delete r;
+    return rc;
+  }
+  *runner = r;
+  return SE_OK;
+}
+
+extern "C" int se_runner_destroy(void* runner) {
+  if (!runner) return SE_OK;
+  SE_REQUIRE(runner != &g_default_runner, "the default runner belongs to the library");
+  se_runner* r = static_cast<se_runner*>(runner);
+  runner_free(r);
+  delete r;
+  return SE_OK;
+}
+
+// Plans that run at the same time -- CUDA graphs captured from them and replayed on different streams -- must not share a
+// side stream: the side stream names the split-K workspace of their weight gradients.  A runner's side stream is its own,
+// so its plans write their own workspace; the workspace has the default runner's size, so every split plan, and every
+// bit, is the same on any runner.  Two more rules keep concurrent plans apart:
+//   - the BatchNorm kernels with a grid-wide barrier are launched cooperatively: their CTAs are co-resident only if the
+//     grid is launched as a whole, which another plan's kernels holding SMs (another such barrier above all) do not
+//     otherwise guarantee.  The kernels, grids and results are the same; only the programmatic dependent launch of those
+//     kernels is lost;
+//   - the communication stream is process-wide, so a runner refuses plans with SE_OP_ALLREDUCE.
+extern "C" int se_run_ops_runner(const se_op* ops, int n, int mode, void* stream, void* runner) {
+  SE_REQUIRE(ops && n >= 0 && runner, "bad arguments");
+  for (int k = 0; k < n; ++k)
+    if (ops[k].opcode == SE_OP_ALLREDUCE) {
+      set_error("se_run_ops_runner: SE_OP_ALLREDUCE at index %d: all-reduces run on the process-wide communication "
+                "stream, with se_run_ops only", k);
+      return SE_ERR_ARG;
+    }
+  int rc = ensure_setup();
+  if (rc) return rc;
+  Streams st{as_stream(stream), static_cast<const se_runner*>(runner), true};
+  t_runner_plan = true;
+  rc = run_ops_impl(ops, n, mode, stream, st);
+  t_runner_plan = false;
   st.join_all();
   return rc;
 }

@@ -17,8 +17,8 @@ int bn_bwd(const float* x, const float* y, const float* dout, int64_t rows, int 
 void count_launch(int n = 1);
 int sm_count();
 // The library's one-time set-up (api.cu), run by se_init and by every entry point that depends on it: the shared-memory
-// limits of the kernels that need more than 48 KB, and se_run_ops' side stream with its events and weight-gradient
-// workspace.  Runs once per process, thread-safe; a failure is returned, with its message, by every later call.
+// limits of the kernels that need more than 48 KB, and se_run_ops' default plan runner: its side stream with its events
+// and weight-gradient workspace.  Runs once per process, thread-safe; a failure is returned, with its message, by every later call.
 int ensure_setup();
 // weight gradients without atomics (conv_wgrad_tc.cu): split-K partial sums go to slices of a workspace of the library
 // (one per device and stream) and wgrad_reduce adds the slices into dW / dbias in slice order, so the result is the same
@@ -77,9 +77,9 @@ inline void launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, c
   cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);   // errors surface through check_launch()
 }
 
-// Kernels with a grid-wide barrier (bn.cu): SE_BN_COOP=1 launches them with the cooperative attribute -- the runtime then
-// guarantees that all CTAs are co-resident (or fails the launch) instead of relying on "grid <= #SMs and nothing else
-// holds the SMs".  Cooperative launches cannot be programmatic dependents, so the PDL attribute is dropped for them.
+// Kernels with a grid-wide barrier (bn.cu): SE_BN_COOP=1, and every plan of se_run_ops_runner, launch them with the
+// cooperative attribute -- the runtime then guarantees that all CTAs are co-resident (or fails the launch) instead of
+// relying on "grid <= #SMs and nothing else holds the SMs".  Cooperative launches cannot be programmatic dependents, so the PDL attribute is dropped for them.
 bool coop_enabled();
 template <typename... KArgs, typename... Args>
 inline void launch_grid_barrier(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {

@@ -32,7 +32,7 @@ constexpr int WG_MT = 64;              // rows of dW ((filter tap, input channel
 constexpr int WG_THREADS = 256;
 
 // Workspaces of the split-K partial sums: one per (device, stream), 32 MB each, allocated outside graph captures (se_init
-// prepares the one of se_run_ops' side stream).  A request that does not fit, or a stream that first appears inside a
+// prepares the one of se_run_ops' side stream, se_runner_create the one of each runner's).  A request that does not fit, or a stream that first appears inside a
 // capture, runs in direct mode instead: the partial sums go into dW with float atomics (correct, not bit-reproducible).
 struct WgWorkspace { int dev; cudaStream_t st; float* ptr; };
 constexpr int WG_MAX_WS = 32;
@@ -459,9 +459,26 @@ int wgrad_workspace(long long floats, cudaStream_t st, float** ws) {
   return SE_OK;
 }
 
+// a plan runner's workspace: an error, not direct mode, when it cannot be had (the table is full), so that no runner
+// runs its weight gradients with atomics
 int wgrad_workspace_prepare(cudaStream_t st) {
   float* ws = nullptr;
-  return wgrad_workspace(1, st, &ws);
+  const int rc = wgrad_workspace(1, st, &ws);
+  if (rc == SE_OK && ws == nullptr) {
+    set_error("wgrad_workspace: all %d weight-gradient workspaces are taken (destroy a plan runner first)", WG_MAX_WS);
+    return SE_ERR_CUDA;
+  }
+  return rc;
+}
+
+// se_runner_destroy: frees the workspace of a runner's side stream (the stream has drained)
+void wgrad_workspace_release(cudaStream_t st) {
+  std::lock_guard<std::mutex> lock(g_wg_mu);
+  for (int i = 0; i < g_wg_nws; ++i)
+    if (g_wg_ws[i].st == st) {
+      cudaFree(g_wg_ws[i].ptr);
+      g_wg_ws[i--] = g_wg_ws[--g_wg_nws];
+    }
 }
 
 long long wgrad_fit_splits(long long want, long long T, int Cout) {

@@ -47,6 +47,28 @@ LABELEMBED_TABLE = 'labelembeddings/embeddings'
 CENTROIDS = 'cls_centroids/embeddings'
 
 
+class Runner:
+    """A plan runner of the library's own (se_runner_create): a weight-gradient side stream, its events and a split-K
+    workspace.  Engines whose captured steps replay at the same time on different streams each need one (Engine(...,
+    runner=Runner())): on the library's default runner their weight gradients would share one workspace.  Each engine
+    keeps a reference to its runner, so the runner outlives the graphs captured on it."""
+    WORKSPACE_BYTES = 32 << 20        # the split-K workspace (WG_WS_FLOATS floats, csrc/common.cuh)
+
+    def __init__(self):
+        self.lib = _lib.load()
+        h = ctypes.c_void_p()
+        _lib.check(self.lib.se_runner_create(ctypes.byref(h)), 'se_runner_create')
+        self.handle = h
+
+    def close(self):
+        if getattr(self, 'handle', None):
+            self.lib.se_runner_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        self.close()
+
+
 class Engine:
     """objective='embedding' (learn_image_embeddings.py): the graph's output is the embedding, the fused head compares it
     with the rows of `embedding` under `loss`, optionally with the softmax classifier branch of `cls_weight`.
@@ -75,6 +97,10 @@ class Engine:
     set_trainable, which set_trainable(None) undoes.  The metrics are 'loss' (prob cross-entropy + w * center loss),
     'prob_loss', 'center_loss' (unweighted) and 'acc'.  The infer plan ends at the class probabilities.
 
+    runner: a Runner, for engines whose steps replay concurrently (trainer.fit_lr_sweep); None runs on the library's
+    default runner.  input_buffer: a (batch,) + input shape float32 device tensor the plans read instead of an input
+    buffer of the engine's own, so that several engines read one composed batch.
+
     optimizer='sgd': Keras SGD(lr, momentum (0.9 by default), decay, nesterov, clipnorm).  optimizer='adagrad': Keras
     Adagrad(lr, epsilon, decay) with the same optional clipnorm; its accumulators live where SGD keeps its velocity
     (get_velocity / set_velocity), and it takes no momentum.
@@ -92,7 +118,7 @@ class Engine:
                  world_size=1, fuse_stats=True, use_cuda_graph=True, seed=0, decay=0.0,
                  grad_buckets=3, comm='auto', cls_base=None, objective='embedding', label_smoothing=0.0,
                  margin=None, optimizer='sgd', epsilon=1e-7, tau=None, alpha=None, beta=None, center_loss_weight=None,
-                 centroids=None):
+                 centroids=None, runner=None, input_buffer=None):
         if loss not in LOSS_KINDS:
             raise ValueError('unknown loss %r' % loss)
         if margin is not None and loss != 'devise_rank':
@@ -157,6 +183,10 @@ class Engine:
         self.comm_native = False
         if self.world > 1 and comm == 'native' and self.dev.type == 'cuda':
             self.comm_native = self._init_native_comm(required=True)
+        if runner is not None and self.comm_native:
+            raise ValueError("a plan runner takes no all-reduce ops: comm='native' runs on the library's default runner")
+        self.runner = runner
+        self.input_buffer = input_buffer
         self.fuse_stats = fuse_stats
         self.use_cuda_graph = use_cuda_graph
         if objective == 'softmax':
@@ -360,7 +390,15 @@ class Engine:
         # activations and their gradients
         g = self.g
         self.act, self.grad = {}, {}
-        self.x = torch.zeros((B,) + g.input.shape, **f32)
+        if self.input_buffer is None:
+            self.x = torch.zeros((B,) + g.input.shape, **f32)
+        else:
+            x = self.input_buffer
+            if tuple(x.shape) != (B,) + tuple(g.input.shape) or x.dtype != torch.float32 or x.device != dev or \
+                    not x.is_contiguous():
+                raise ValueError('input_buffer is %s %s on %s, the plans need a contiguous float32 %s on %s'
+                                 % (tuple(x.shape), x.dtype, x.device, (B,) + tuple(g.input.shape), dev))
+            self.x = x
         self.act[g.input.name] = self.x
         for n in self.nodes:
             self.act[n.output.name] = torch.zeros((B,) + n.output.shape, **f32)
@@ -443,6 +481,18 @@ class Engine:
     def get_velocity(self):
         torch.cuda.synchronize(self.dev)
         return OrderedDict((n, self._pview(n, self.V).detach().cpu().numpy().copy()) for n in self.offsets)
+
+    def device_bytes(self):
+        """Bytes of the device buffers this engine allocated: parameters and optimizer state, activations and their
+        gradients, metric and BatchNorm scratch.  Not counted: an input_buffer given to the constructor, the class
+        embedding matrix, and the split-K workspace of a plan runner (Runner.WORKSPACE_BYTES)."""
+        own = [self.P, self.G, self.V, self.PT, self.PL, self.PTL, self.S, self.labels, self.le_work, self.stats,
+               self.saved, self.sgd_out, self.lr_dev, self.loss_buf, self.acc_buf, self.cls_loss_buf, self.cls_acc_buf,
+               self.rank_buf, self.cls_rank_buf, self.center_buf]
+        own += list(self.act.values()) + list(self.grad.values())
+        sizes = {t.data_ptr(): t.numel() * t.element_size() for t in own
+                 if t is not None and not (self.input_buffer is not None and t is self.x)}
+        return int(sum(sizes.values()))
 
     # ------------------------------------------------------------------ plan construction
     def _op(self, opcode, i=(), f=(), p=()):
@@ -869,11 +919,16 @@ class Engine:
         return _lib.launch_count() - before
 
     # ------------------------------------------------------------------ execution
+    def _run_ops(self, arr):
+        if self.runner is None:
+            return self.lib.se_run_ops(arr, len(arr), self.mode, _lib.stream_ptr())
+        return self.lib.se_run_ops_runner(arr, len(arr), self.mode, _lib.stream_ptr(), self.runner.handle)
+
     def _run(self, which, graph=None):
         arr = self.plans[which]
         use_graph = self.use_cuda_graph if graph is None else graph
         if not use_graph:
-            _lib.check(self.lib.se_run_ops(arr, len(arr), self.mode, _lib.stream_ptr()), 'se_run_ops(%s)' % which)
+            _lib.check(self._run_ops(arr), 'se_run_ops(%s)' % which)
             return
         cg = self._graphs.get(which)
         if cg is None:
@@ -882,7 +937,7 @@ class Engine:
             torch.cuda.synchronize(self.dev)
             cg = torch.cuda.CUDAGraph()
             with torch.cuda.graph(cg):
-                _lib.check(self.lib.se_run_ops(arr, len(arr), self.mode, _lib.stream_ptr()), 'se_run_ops(%s) capture' % which)
+                _lib.check(self._run_ops(arr), 'se_run_ops(%s) capture' % which)
             self._graphs[which] = cg
         cg.replay()
 
